@@ -5,7 +5,7 @@
 
 Same flags, log records and checkpoint files as the reference chapter
 (LambdaLabsML/distributed-training-guide ``01-single-gpu/train_llm.py``); the step itself
-runs on this repository's sm_100a kernels (see README.md in this directory).
+runs on this repository's sm_90a kernels (see README.md in this directory).
 """
 import os
 import sys

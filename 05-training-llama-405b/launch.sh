@@ -19,7 +19,7 @@ REMOTE_CMD="cd $WORKDIR && \
       --experiment-name $EXPERIMENT_NAME \
       --dataset-name Skylion007/openwebtext \
       --model-name meta-llama/Llama-3.1-405B \
-      --batch-size 1 --seq-length 4096 \
+      --batch-size 1 --seq-length 2048 \
       --cpu-offload --checkpoint-activations --prefetch-layers --log-freq 1"
 
 xargs -a "$HOSTS_FILE" -I {} ssh {} tmux new-session -d -s dtg-405b "bash -lc '$REMOTE_CMD'"

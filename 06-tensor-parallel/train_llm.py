@@ -2,7 +2,7 @@
 
     torchrun --standalone --nproc-per-node gpu train_llm.py -d synthetic -m meta-llama/Llama-3.1-8B -b 16 -s 1024
 
-Column-parallel q/k/v/gate/up and row-parallel o/down projections run as single tcgen05 kernels that
+Column-parallel q/k/v/gate/up and row-parallel o/down projections run as single wgmma kernels that
 fetch / scatter their sequence-sharded operand over NVLink (all-gather->GEMM, GEMM->reduce-scatter);
 the loss is vocab-parallel (parallel/tp.py).  Flags follow the reference chapter."""
 import os

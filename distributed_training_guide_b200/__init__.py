@@ -1,4 +1,4 @@
-"""distributed_training_guide_b200 — a B200-native (sm_100a) distributed causal-LM training
+"""distributed_training_guide_b200 — a H100-native (sm_90a) distributed causal-LM training
 runtime with the capabilities of LambdaLabsML/distributed-training-guide.
 
 Layout:  ``models/`` (Llama / GPT-2), ``ops/`` (autograd wrappers over the hand-written

@@ -1,7 +1,7 @@
-"""Loader for the in-tree sm_100a extension ``distributed_training_guide_b200/_C*.so``.
+"""Loader for the in-tree sm_90a extension ``distributed_training_guide_b200/_C*.so``.
 
 The extension is built by ``build.py`` (``__graft_entry__.build()``) with
-``nvcc -gencode arch=compute_100a,code=sm_100a``.  On a machine with a CUDA device the
+``nvcc -gencode arch=compute_90a,code=sm_90a``.  On a machine with a CUDA device the
 ops *require* it (there is no silent PyTorch fallback on the GPU hot path): a missing
 or unloadable extension raises at first use.  On CPU-only machines the pure-PyTorch
 reference ops in ``ops/reference.py`` are used.
@@ -35,7 +35,7 @@ def load(required: bool = False):
                 _load_error = e
     if _C is None and required:
         raise RuntimeError(
-            "the sm_100a extension distributed_training_guide_b200/_C.so is not available "
+            "the sm_90a extension distributed_training_guide_b200/_C.so is not available "
             f"({_load_error!r}); run `python -c 'import __graft_entry__ as g; g.build()'` "
             "(or `python -m distributed_training_guide_b200.build`) first"
         )
@@ -50,7 +50,7 @@ _forced = {s.strip() for s in os.environ.get("DTG_FORCE_REFERENCE", "").split(",
 
 
 def use_cuda_kernel(op: str, *tensors) -> bool:
-    """True when ``op`` must run through the sm_100a extension for these tensors."""
+    """True when ``op`` must run through the sm_90a extension for these tensors."""
     if not tensors or not all(t.is_cuda for t in tensors if t is not None):
         return False
     if op in _forced or "all" in _forced:

@@ -1,8 +1,8 @@
-"""In-tree build of the sm_100a extension ``distributed_training_guide_b200/_C.so``.
+"""In-tree build of the sm_90a extension ``distributed_training_guide_b200/_C.so``.
 
     python -m distributed_training_guide_b200.build [--force] [--verbose]
 
-Every ``csrc/*.cu`` is compiled by nvcc for ``-gencode arch=compute_100a,code=sm_100a
+Every ``csrc/*.cu`` is compiled by nvcc for ``-gencode arch=compute_90a,code=sm_90a
 -lineinfo`` (cross-compiles without a GPU), ``csrc/*.cpp`` by g++ against the torch headers,
 and everything is linked into one shared object next to this file so that it travels with
 the repository snapshot to the GPU box (a JIT cache under ~/.cache would not).  The kernels
@@ -26,7 +26,7 @@ OBJ = HERE / "build" / "obj"
 TARGET = HERE / "_C.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "--expt-extended-lambda", "-Xcompiler", "-fPIC",
     "-Xptxas", "-v", "-DNDEBUG",
 ]

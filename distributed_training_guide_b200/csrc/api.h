@@ -1,4 +1,4 @@
-// Host-side launcher API of the sm_100a kernels (raw pointers + stream; no torch types so the
+// Host-side launcher API of the sm_90a kernels (raw pointers + stream; no torch types so the
 // .cu files compile in seconds).  bind.cpp adapts torch tensors onto these.
 #pragma once
 #include <cuda_runtime.h>
@@ -34,15 +34,15 @@ void cross_entropy_fwd_bwd(void* logits, const long long* targets, float* row_lo
 void adamw_flat(void* p, const void* g, void* m, void* v, long long n, float lr, float beta1, float beta2, float eps,
                 float wd, int step, float grad_scale, bool state_fp32, cudaStream_t s);
 
-// ---- gemm_tcgen05.cu -----------------------------------------------------------------------
-// out[M,N] (+)= op(A) @ op(B), bf16 in / fp32 TMEM accumulate / bf16 out, row-major storage:
+// ---- gemm_wgmma.cu -------------------------------------------------------------------------
+// out[M,N] (+)= op(A) @ op(B), bf16 in / fp32 register accumulate / bf16 out, row-major storage:
 //   a_kmajor: A stored [M,K] (else [K,M]);  b_kmajor: B stored [N,K] (else [K,N]).
-// lda/ldb/ldc are row strides in elements.  variant: 0 = auto, 1 = 1-CTA 128x256, 2 = 2-CTA 256x256
+// lda/ldb/ldc are row strides in elements.  variant: 0 = auto, 1 = 1-CTA 128x256, 2 = 2-CTA cluster 256x256
 void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
                bool a_kmajor, bool b_kmajor, bool accumulate, int variant, cudaStream_t s);
 
 int gemm_max_active_clusters(int cg);
-// tensor-parallel variants over symmetric buffers (see gemm_tcgen05.cu)
+// tensor-parallel variants over symmetric buffers (see gemm_wgmma.cu)
 void gemm_bf16_dist(int mode, const void* const* a_srcs, const void* const* b_srcs, void* const* c_dsts, int M, int N,
                     int K, long long lda, long long ldb, long long ldc, bool b_kmajor, bool accumulate, int nranks,
                     int rank, int rows_per_peer, cudaStream_t s);
@@ -55,8 +55,9 @@ void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int 
                   bool b_kmajor, int nranks, int rank, int rows_per_peer, uint32_t* flags, uint32_t ag_epoch,
                   uint32_t* const* pads, uint32_t bar_epoch, int n_comm, cudaStream_t s);
 
-// ---- attention.cu --------------------------------------------------------------------------
+// ---- attention_fwd.cu / attention_bwd.cu ---------------------------------------------------
 // qkv: [B,S,nh+2*nkv,128] bf16 (q heads | k heads | v heads); o: [B,S,nh,128]; lse: [B,nh,S] fp32
+// attn_fwd: P through shared memory; attn_fwd2: P kept in registers
 void attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s);
 void attn_fwd2(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s);
 void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* dq_acc,

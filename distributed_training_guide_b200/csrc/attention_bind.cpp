@@ -1,4 +1,4 @@
-// Python bindings for the tcgen05 flash-attention kernels.
+// Python bindings for the wgmma flash-attention kernels.
 #include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
@@ -19,8 +19,8 @@ void check_qkv(const Tensor& qkv, int64_t nh, int64_t nkv) {
               "qkv must be [B, S, nh+2*nkv, 128]");
 }
 
-// version: 0 = default (DTG_ATTN_FWD env, else 2), 1 = one query tile per CTA (attention_fwd.cu),
-// 2 = two tiles per CTA, P kept in tensor memory (attention_fwd2.cu)
+// version: 0 = default (DTG_ATTN_FWD env, else 2), 1 = P through shared memory, 2 = P kept in registers
+// (both in attention_fwd.cu)
 int default_fwd_version() {
   static int v = -1;
   if (v < 0) {
@@ -69,6 +69,6 @@ void bind_attention(pybind11::module_& m) {
         pybind11::arg("version") = 0);
   m.def("attn_bwd", &py_attn_bwd, pybind11::arg("d_o"), pybind11::arg("qkv"), pybind11::arg("o"), pybind11::arg("lse"),
         pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("scale"), pybind11::arg("trace") = pybind11::none(),
-        pybind11::arg("mode") = 0);   // 0 = default (DTG_ATTN_BWD), 1 = P/dS through shared memory, 2 = P/dS in TMEM
+        pybind11::arg("mode") = 0);   // 0 = default (DTG_ATTN_BWD), 1 = P/dS through shared memory, 2 = P/dS in registers
 }
 }  // namespace dtg

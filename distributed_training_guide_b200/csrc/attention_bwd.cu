@@ -1,21 +1,20 @@
-// Causal flash-attention backward on tcgen05 (head_dim 128, GQA).
+// Causal flash-attention backward on wgmma (head_dim 128, GQA).
 //
 // Two passes of ONE kernel template, each owning a 128-row block R and streaming 64-wide column
 // blocks C of the opposite kind (no atomics, deterministic):
 //
 //   KV pass  R = 128 keys of a kv head, C = 64-query blocks of every q head in its GQA group
-//            S^T = K_R Q_C^T,  dP^T = V_R dO_C^T          (tcgen05.mma 128x64x128, fp32 in TMEM)
-//            P^T = exp2(S^T*c - lse_q),  dS^T = P^T o (dP^T - delta_q) * scale     (softmax warps)
-//            dV_R += P^T dO_C,   dK_R += dS^T Q_C         (A from shared memory, B MN-major)
+//            S^T = K_R Q_C^T,  dP^T = V_R dO_C^T          (wgmma m64n64k16 per warpgroup, fp32 in registers)
+//            P^T = exp2(S^T*c - lse_q),  dS^T = P^T o (dP^T - delta_q) * scale
+//            dV_R += P^T dO_C,   dK_R += dS^T Q_C         (wgmma m64n128k16, B = the C tile, MN-major)
 //   Q pass   R = 128 queries of a q head, C = 64-key blocks
 //            S = Q_R K_C^T,  dP = dO_R V_C^T,  dS = P o (dP - delta_q) * scale,   dQ_R += dS K_C
 //
-// Warp roles as in the forward kernel: warp 0 TMA producer (resident R tiles once, C tiles in a
-// 2-stage ring), warp 1 MMA issuer (score MMAs of block t+1 are issued before the gradient MMAs of
-// block t, the S/dP TMEM buffers are double-buffered), warp 2 TMEM allocator, warps 4-7 one row each.
-// delta = rowsum(dO o O) is produced by a small preprocess kernel.  Gradients are written into a
-// dqkv buffer with the same fused layout as qkv, so the RoPE-backward kernel and the fused
-// qkv dgrad/wgrad GEMMs consume it directly.
+// 256 threads = two math warpgroups that own 64 rows of R each and keep their gradient accumulators in
+// registers for the whole pass (up to 255 registers a thread: two warps per SM sub-partition); thread 0 also
+// issues the TMA loads (resident R tiles once, C tiles into a 3-stage ring two blocks ahead).  delta = rowsum(dO o O) is produced by a small preprocess
+// kernel.  Gradients are written into a dqkv buffer with the same fused layout as qkv, so the
+// RoPE-backward kernel and the fused qkv dgrad/wgrad GEMMs consume it directly.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -36,17 +35,14 @@ constexpr int R_HALF = R_TILE / 2;
 constexpr int C_TILE = 64 * 128 * 2;   // 16 KB streamed tile (two 8 KB halves)
 constexpr int C_HALF = C_TILE / 2;
 constexpr int OFF_R1 = 0, OFF_R2 = R_TILE;
-constexpr int Y_STAGES = 3;                   // TMA ring depth for the streamed tiles: a stage is only
-                                              // released by the gradient MMAs of its block, two stages left
-                                              // the next block's load exposed (~1 TMA latency per block)
+constexpr int Y_STAGES = 3;                   // TMA ring depth for the streamed tiles
 constexpr int OFF_Y = 2 * R_TILE;             // [stage][Y1 | Y2]
-constexpr int OFF_P = OFF_Y + Y_STAGES * 2 * C_TILE;  // 16 KB: [128 rows x 64] bf16, K-major
+constexpr int OFF_P = OFF_Y + Y_STAGES * 2 * C_TILE;  // 16 KB: [128 rows x 64] bf16, K-major (SS form only)
 constexpr int OFF_DS = OFF_P + 128 * 128;     // 16 KB
 constexpr int OFF_BAR = OFF_DS + 128 * 128;
 constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-constexpr uint32_t TM_S = 0, TM_DP = 128, TM_ACC_A = 256, TM_ACC_B = 384;
 constexpr float LOG2E = 1.4426950408889634f;
-constexpr int THREADS = 384;  // 4 control warps + 8 compute warps (two threads per row)
+constexpr int THREADS = 256;
 }  // namespace bwd
 
 // delta[b, h, s] = sum_d dO * O   (one warp per (token, head) row)
@@ -72,10 +68,10 @@ __global__ void attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ d_o, con
   }
 }
 
-// TS = true: P^T / dS^T (KV pass) and dS (Q pass) never go through shared memory — the softmax threads write them as
-// packed bf16 over the S / dP scores they were computed from (tcgen05.st) and the gradient MMAs read their A operand
-// from tensor memory (TS form).  Per 128x64 block that removes 32 KB of shared-memory stores and 32 KB of A-operand
-// reads out of ~192 KB: the N=64 MMAs of this kernel are shared-memory-bandwidth-bound (profiles/prof_attn_bwd.md).
+// TS = true: P^T / dS^T (KV pass) and dS (Q pass) never go through shared memory — they are packed to bf16 in the
+// registers they were computed in and feed the gradient MMAs as their A operand (RS form).  Per 128x64 block that
+// removes 32 KB of shared-memory stores and 32 KB of A-operand reads.  TS = false stages them through
+// 128B-swizzled shared memory (SS form).
 template <bool KV_MODE, bool TS>
 __global__ void __launch_bounds__(bwd::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_constant__ CUtensorMap tm_qkv_c,
@@ -83,8 +79,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
                 const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv,
                 int S, int nh, int nkv, float scale, int num_r_blocks, long long* __restrict__ trace) {
   using namespace bwd;
-  // optional in-kernel timeline (tools/prof_attn.py --trace): CTA (0,0) records clock64() at the
-  // pipeline hand-over points; columns: [iter][0..3] softmax warp 4, [4..6] MMA thread
+  // optional in-kernel timeline (attn_bwd(..., trace=int64[1024])): CTA (0,0) records clock64() per column block:
+  // [iter][0] scores ready, [1] P / dS computed, [3] gradient MMAs retired (thread 0)
   const bool tracing = trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -92,13 +88,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
   uint64_t* res_full = bars + 0;
   uint64_t* y_full = bars + 1;     // [Y_STAGES]
   uint64_t* y_empty = bars + 5;    // [Y_STAGES]
-  uint64_t* sdp_full = bars + 9;   // [2]
-  uint64_t* sdp_empty = bars + 11; // [2]
-  uint64_t* pds_full = bars + 13;
-  uint64_t* pds_empty = bars + 14;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 16);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int group = nh / nkv;
   const int nht = nh + 2 * nkv;
   // KV pass: blockIdx.x = (batch, kv head), early key blocks (most work) first.
@@ -114,266 +105,217 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
   const int n_c = KV_MODE ? (S / 64 - c_start) : (R0 + 128) / 64;
   const int n_iter = KV_MODE ? n_c * group : n_c;
 
-  if (warp == 0 && elect_one()) {
+  if (threadIdx.x == 0) {
     prefetch_tensormap(&tm_qkv_r);
     prefetch_tensormap(&tm_qkv_c);
     prefetch_tensormap(&tm_do_r);
     prefetch_tensormap(&tm_do_c);
-  }
-  if (warp == 1 && elect_one()) {
     mbar_init(res_full, 1);
     for (int i = 0; i < Y_STAGES; ++i) {
       mbar_init(&y_full[i], 1);
-      mbar_init(&y_empty[i], 1);
+      mbar_init(&y_empty[i], 2);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&sdp_full[i], 1);
-      mbar_init(&sdp_empty[i], 8);
-    }
-    mbar_init(pds_full, 8);
-    mbar_init(pds_empty, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc<1>(tmem_ptr_smem, 512);
-    tmem_relinquish<1>();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
-    if (elect_one()) {
-      // resident tiles: KV pass -> K_R, V_R ; Q pass -> Q_R, dO_R
-      mbar_arrive_expect_tx(res_full, 2 * R_TILE);
-      if (KV_MODE) {
-        tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1, 0, nh + kv_head, R0, batch);
-        tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1 + R_HALF, 64, nh + kv_head, R0, batch);
-        tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R2, 0, nh + nkv + kv_head, R0, batch);
-        tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R2 + R_HALF, 64, nh + nkv + kv_head, R0, batch);
-      } else {
-        tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1, 0, head_r, R0, batch);
-        tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1 + R_HALF, 64, head_r, R0, batch);
-        tma_load_4d(&tm_do_r, res_full, smem + OFF_R2, 0, head_r, R0, batch);
-        tma_load_4d(&tm_do_r, res_full, smem + OFF_R2 + R_HALF, 64, head_r, R0, batch);
-      }
-      for (int t = 0; t < n_iter; ++t) {
-        const int st = t % Y_STAGES;
-        const uint32_t ph = (uint32_t)((t / Y_STAGES) & 1);
-        const int c = c_start + (KV_MODE ? t % n_c : t);
-        const int C0 = c * 64;
-        uint8_t* y1 = smem + OFF_Y + st * 2 * C_TILE;
-        uint8_t* y2 = y1 + C_TILE;
-        mbar_wait(&y_empty[st], ph ^ 1);
-        mbar_arrive_expect_tx(&y_full[st], 2 * C_TILE);
-        if (KV_MODE) {
-          const int qh = kv_head * group + t / n_c;
-          tma_load_4d(&tm_qkv_c, &y_full[st], y1, 0, qh, C0, batch);
-          tma_load_4d(&tm_qkv_c, &y_full[st], y1 + C_HALF, 64, qh, C0, batch);
-          tma_load_4d(&tm_do_c, &y_full[st], y2, 0, qh, C0, batch);
-          tma_load_4d(&tm_do_c, &y_full[st], y2 + C_HALF, 64, qh, C0, batch);
-        } else {
-          tma_load_4d(&tm_qkv_c, &y_full[st], y1, 0, nh + kv_head, C0, batch);
-          tma_load_4d(&tm_qkv_c, &y_full[st], y1 + C_HALF, 64, nh + kv_head, C0, batch);
-          tma_load_4d(&tm_qkv_c, &y_full[st], y2, 0, nh + nkv + kv_head, C0, batch);
-          tma_load_4d(&tm_qkv_c, &y_full[st], y2 + C_HALF, 64, nh + nkv + kv_head, C0, batch);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 64, false, false);    // scores: both operands K-major
-      constexpr uint32_t idesc_g = make_idesc_bf16(128, 128, false, true);    // gradients: B (C tile) MN-major
-      const uint32_t r1 = smem_u32(smem + OFF_R1), r2 = smem_u32(smem + OFF_R2);
-      const uint32_t sp = smem_u32(smem + OFF_P), sds = smem_u32(smem + OFF_DS);
-      auto issue_scores = [&](int t) {
-        const int st = t & 1;                       // S / dP TMEM buffer
-        const uint32_t ph = (uint32_t)((t >> 1) & 1);
-        const int ys = t % Y_STAGES;                // shared-memory stage of the streamed tiles
-        mbar_wait(&y_full[ys], (uint32_t)((t / Y_STAGES) & 1));
-        // TS: buffer st is free once the gradient MMAs of block t-2 (which read P / dS from it) have been issued —
-        // they were, in this thread's program order, and tcgen05.mma executes in issue order
-        if (!TS) mbar_wait(&sdp_empty[st], ph ^ 1);
-        tc_fence_after();
-        const uint32_t y1 = smem_u32(smem + OFF_Y + ys * 2 * C_TILE), y2 = y1 + C_TILE;
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint32_t ra = (uint32_t)((kk >> 2) * R_HALF + (kk & 3) * 32);
-          const uint32_t cb = (uint32_t)((kk >> 2) * C_HALF + (kk & 3) * 32);
-          mma_f16_ss<1>(tmem_base + TM_S + st * 64, desc_kmajor_sw128(r1 + ra), desc_kmajor_sw128(y1 + cb), idesc_s,
-                        kk ? 1u : 0u);
-        }
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint32_t ra = (uint32_t)((kk >> 2) * R_HALF + (kk & 3) * 32);
-          const uint32_t cb = (uint32_t)((kk >> 2) * C_HALF + (kk & 3) * 32);
-          mma_f16_ss<1>(tmem_base + TM_DP + st * 64, desc_kmajor_sw128(r2 + ra), desc_kmajor_sw128(y2 + cb), idesc_s,
-                        kk ? 1u : 0u);
-        }
-        mma_commit(&sdp_full[st]);
-      };
-      mbar_wait(res_full, 0);
-      issue_scores(0);
-      for (int t = 0; t < n_iter; ++t) {
-        if (t + 1 < n_iter) issue_scores(t + 1);
-        if (tracing && t < 64) trace[t * 8 + 4] = clock64();
-        const int ys = t % Y_STAGES;
-        mbar_wait(pds_full, (uint32_t)(t & 1));
-        if (tracing && t < 64) trace[t * 8 + 5] = clock64();
-        tc_fence_after();
-        const uint32_t y1 = smem_u32(smem + OFF_Y + ys * 2 * C_TILE), y2 = y1 + C_TILE;
-        const uint32_t st_g = (uint32_t)(t & 1);
-        if (KV_MODE) {
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {  // dV += P^T dO_C
-            if (TS)
-              mma_f16_ts(tmem_base + TM_ACC_A, tmem_base + TM_S + st_g * 64 + kk * 8,
-                         desc_mnmajor_sw128(y2 + kk * 2048, C_HALF), idesc_g, (t | kk) ? 1u : 0u);
-            else
-              mma_f16_ss<1>(tmem_base + TM_ACC_A, desc_kmajor_sw128(sp + kk * 32),
-                            desc_mnmajor_sw128(y2 + kk * 2048, C_HALF), idesc_g, (t | kk) ? 1u : 0u);
-          }
-        }
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {  // dK += dS^T Q_C   /   dQ += dS K_C
-          if (TS)
-            mma_f16_ts(tmem_base + TM_ACC_B, tmem_base + TM_DP + st_g * 64 + kk * 8,
-                       desc_mnmajor_sw128(y1 + kk * 2048, C_HALF), idesc_g, (t | kk) ? 1u : 0u);
-          else
-            mma_f16_ss<1>(tmem_base + TM_ACC_B, desc_kmajor_sw128(sds + kk * 32),
-                          desc_mnmajor_sw128(y1 + kk * 2048, C_HALF), idesc_g, (t | kk) ? 1u : 0u);
-        }
-        mma_commit(pds_empty);
-        mma_commit(&y_empty[ys]);
-        if (tracing && t < 64) trace[t * 8 + 6] = clock64();
-      }
-    }
-  } else if (warp >= 4) {
-    // two threads per row: each owns 32 of the 64 columns of a block (and 64 of the 128 output columns)
-    const int q = warp & 3;
-    const int half = (warp - 4) >> 2;
-    const int r = q * 32 + lane;  // row inside R == TMEM lane
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    const float sl2 = scale * LOG2E;
-    float lse_r = 0.f, delta_r = 0.f;
-    if (!KV_MODE) {
-      const long long idx = ((long long)batch * nh + head_r) * S + R0 + r;
-      lse_r = lse[idx] * LOG2E;
-      delta_r = delta[idx];
-    }
-    uint8_t* sp = smem + OFF_P + r * 128;
-    uint8_t* sds = smem + OFF_DS + r * 128;
-    for (int t = 0; t < n_iter; ++t) {
-      const int st = t & 1;
-      const int c = c_start + (KV_MODE ? t % n_c : t);
-      const int C0 = c * 64 + half * 32;  // first column I own
-      float lq[32], dq[32];
-      if (KV_MODE) {  // per-column statistics of the 32 queries I own (same addresses across the warp)
-        const int qh = kv_head * group + t / n_c;
-        const float4* lp = reinterpret_cast<const float4*>(lse + ((long long)batch * nh + qh) * S + C0);
-        const float4* dp = reinterpret_cast<const float4*>(delta + ((long long)batch * nh + qh) * S + C0);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 a = __ldg(lp + i), b = __ldg(dp + i);
-          lq[4 * i] = a.x * LOG2E; lq[4 * i + 1] = a.y * LOG2E; lq[4 * i + 2] = a.z * LOG2E; lq[4 * i + 3] = a.w * LOG2E;
-          dq[4 * i] = b.x; dq[4 * i + 1] = b.y; dq[4 * i + 2] = b.z; dq[4 * i + 3] = b.w;
-        }
-      }
-      const bool tr = tracing && warp == 4 && lane == 0 && t < 64;
-      mbar_wait(&sdp_full[st], (uint32_t)((t >> 1) & 1));
-      if (tr) trace[t * 8 + 0] = clock64();
-      tc_fence_after();
-      uint32_t rs[32], rd[32];
-      tmem_ld_32x32b_x32(lane_addr + TM_S + st * 64 + half * 32, rs);
-      tmem_ld_32x32b_x32(lane_addr + TM_DP + st * 64 + half * 32, rd);
-      tmem_ld_wait();
-      if (!TS) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&sdp_empty[st]);
-      }
-      // causal: query index >= key index.  Only blocks that touch the diagonal need the compare.
-      const bool need_mask = KV_MODE ? (C0 < R0 + 127) : (C0 + 31 > R0);
-      uint32_t pk_p[16], pk_ds[16];  // 32 bf16 each
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        float pv[2], dv[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float l2 = KV_MODE ? lq[i + e] : lse_r;
-          const float dl = KV_MODE ? dq[i + e] : delta_r;
-          float p = fast_exp2(fmaf(__uint_as_float(rs[i + e]), sl2, -l2));
-          if (need_mask) {
-            const bool ok = KV_MODE ? (C0 + i + e >= R0 + r) : (R0 + r >= C0 + i + e);
-            p = ok ? p : 0.f;
-          }
-          pv[e] = p;
-          dv[e] = p * (__uint_as_float(rd[i + e]) - dl) * scale;
-        }
-        __nv_bfloat162 a = __floats2bfloat162_rn(pv[0], pv[1]);
-        __nv_bfloat162 b = __floats2bfloat162_rn(dv[0], dv[1]);
-        pk_p[i >> 1] = *reinterpret_cast<uint32_t*>(&a);
-        pk_ds[i >> 1] = *reinterpret_cast<uint32_t*>(&b);
-      }
-      if (tr) trace[t * 8 + 1] = clock64();
-      if (TS) {
-        // over the scores just read: P^T -> S buffer, dS -> dP buffer of this stage, my 16 packed columns each.
-        // (The other half-row thread may still be loading ITS 32 score columns: disjoint from the 16 packed columns
-        // [16*half, 16*half+16) only for half 0; so both threads of a row sync on the named barrier first.)
-        named_bar_sync(1 + q, 64);
-        if (KV_MODE) tmem_st_32x32b_x16(lane_addr + TM_S + st * 64 + half * 16, pk_p);
-        tmem_st_32x32b_x16(lane_addr + TM_DP + st * 64 + half * 16, pk_ds);
-        tmem_st_wait();
-      } else {
-        if (t > 0) mbar_wait(pds_empty, (uint32_t)((t - 1) & 1));  // gradient MMAs of t-1 released P / dS
-        if (tr) trace[t * 8 + 2] = clock64();
-#pragma unroll
-        for (int ch = 0; ch < 4; ++ch) {  // my 4 chunks of 8 bf16 inside the 64-wide row, 128B swizzle
-          const uint32_t off = (uint32_t)((((half * 4 + ch) ^ (r & 7))) << 4);
-          if (KV_MODE)
-            *reinterpret_cast<uint4*>(sp + off) = make_uint4(pk_p[ch * 4], pk_p[ch * 4 + 1], pk_p[ch * 4 + 2], pk_p[ch * 4 + 3]);
-          *reinterpret_cast<uint4*>(sds + off) =
-              make_uint4(pk_ds[ch * 4], pk_ds[ch * 4 + 1], pk_ds[ch * 4 + 2], pk_ds[ch * 4 + 3]);
-        }
-        fence_proxy_async();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_full);
-      if (tr) trace[t * 8 + 3] = clock64();
-    }
-    // write the accumulated gradients of this row (my 64 of the 128 columns)
-    mbar_wait(pds_empty, (uint32_t)((n_iter - 1) & 1));
-    tc_fence_after();
-    const long long tok = (long long)batch * S + R0 + r;
-    auto write_row = [&](uint32_t tm_col, int out_head) {
-      __nv_bfloat16* dst = dqkv + (tok * nht + out_head) * (long long)D + half * 64;
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        uint32_t rr[32];
-        tmem_ld_32x32b_x32(lane_addr + tm_col + half * 64 + cc * 32, rr);
-        tmem_ld_wait();
-#pragma unroll
-        for (int v = 0; v < 4; ++v) {
-          float f[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(rr[v * 8 + i]);
-          st8(dst + cc * 32 + v * 8, pack8(f));
-        }
-      }
-    };
+  // TMA issue (thread 0): the resident tiles once, then the streamed tiles Y_STAGES - 1 blocks ahead of the math
+  auto issue_y = [&](int t) {
+    const int st = t % Y_STAGES;
+    const uint32_t ph = (uint32_t)((t / Y_STAGES) & 1);
+    const int c = c_start + (KV_MODE ? t % n_c : t);
+    const int C0 = c * 64;
+    uint8_t* y1 = smem + OFF_Y + st * 2 * C_TILE;
+    uint8_t* y2 = y1 + C_TILE;
+    mbar_wait_mma(&y_empty[st], ph ^ 1);
+    mbar_arrive_expect_tx(&y_full[st], 2 * C_TILE);
     if (KV_MODE) {
-      write_row(TM_ACC_A, nh + nkv + kv_head);  // dV
-      write_row(TM_ACC_B, nh + kv_head);        // dK
+      const int qh = kv_head * group + t / n_c;
+      tma_load_4d(&tm_qkv_c, &y_full[st], y1, 0, qh, C0, batch);
+      tma_load_4d(&tm_qkv_c, &y_full[st], y1 + C_HALF, 64, qh, C0, batch);
+      tma_load_4d(&tm_do_c, &y_full[st], y2, 0, qh, C0, batch);
+      tma_load_4d(&tm_do_c, &y_full[st], y2 + C_HALF, 64, qh, C0, batch);
     } else {
-      write_row(TM_ACC_B, head_r);              // dQ
+      tma_load_4d(&tm_qkv_c, &y_full[st], y1, 0, nh + kv_head, C0, batch);
+      tma_load_4d(&tm_qkv_c, &y_full[st], y1 + C_HALF, 64, nh + kv_head, C0, batch);
+      tma_load_4d(&tm_qkv_c, &y_full[st], y2, 0, nh + nkv + kv_head, C0, batch);
+      tma_load_4d(&tm_qkv_c, &y_full[st], y2 + C_HALF, 64, nh + nkv + kv_head, C0, batch);
+    }
+  };
+  if (threadIdx.x == 0) {
+    // resident tiles: KV pass -> K_R, V_R ; Q pass -> Q_R, dO_R
+    mbar_arrive_expect_tx(res_full, 2 * R_TILE);
+    if (KV_MODE) {
+      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1, 0, nh + kv_head, R0, batch);
+      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1 + R_HALF, 64, nh + kv_head, R0, batch);
+      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R2, 0, nh + nkv + kv_head, R0, batch);
+      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R2 + R_HALF, 64, nh + nkv + kv_head, R0, batch);
+    } else {
+      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1, 0, head_r, R0, batch);
+      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1 + R_HALF, 64, head_r, R0, batch);
+      tma_load_4d(&tm_do_r, res_full, smem + OFF_R2, 0, head_r, R0, batch);
+      tma_load_4d(&tm_do_r, res_full, smem + OFF_R2 + R_HALF, 64, head_r, R0, batch);
+    }
+    for (int t = 0; t < Y_STAGES - 1 && t < n_iter; ++t) issue_y(t);
+  }
+  {
+    const int half = wg;                               // rows [64*half, 64*half + 64) of R
+    const int g = lane >> 2, tq = lane & 3;
+    const int rl0 = half * 64 + (warp & 3) * 16 + g;   // my rows of R: rl0 and rl0 + 8
+    const bool signal = (threadIdx.x & 127) == 0;
+    const bool tr_thread = tracing && threadIdx.x == 0;
+    const float sl2 = scale * LOG2E;
+    float lse_r[2] = {0.f, 0.f}, delta_r[2] = {0.f, 0.f};
+    if (!KV_MODE) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long idx = ((long long)batch * nh + head_r) * S + R0 + rl0 + 8 * h;
+        lse_r[h] = lse[idx] * LOG2E;
+        delta_r[h] = delta[idx];
+      }
+    }
+    [[maybe_unused]] float acc_a[KV_MODE ? 64 : 1];   // dV (KV pass)
+    float acc_b[64];                                  // dK (KV pass) / dQ (Q pass)
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      if constexpr (KV_MODE) acc_a[i] = 0.f;
+      acc_b[i] = 0.f;
+    }
+    const uint32_t r1 = smem_u32(smem + OFF_R1) + (uint32_t)(half * 8192);
+    const uint32_t r2 = smem_u32(smem + OFF_R2) + (uint32_t)(half * 8192);
+    const uint32_t sp = smem_u32(smem + OFF_P) + (uint32_t)(half * 8192);
+    const uint32_t sds = smem_u32(smem + OFF_DS) + (uint32_t)(half * 8192);
+    mbar_wait_mma(res_full, 0);
+    for (int t = 0; t < n_iter; ++t) {
+      // refill the stage block t-1 used (both warpgroups must be done with it; the other one is at most one block
+      // behind)
+      if (threadIdx.x == 0 && t + Y_STAGES - 1 < n_iter) issue_y(t + Y_STAGES - 1);
+      const int ys = t % Y_STAGES;
+      const int c = c_start + (KV_MODE ? t % n_c : t);
+      const int C0 = c * 64;
+      [[maybe_unused]] const float* lq = nullptr;
+      [[maybe_unused]] const float* dq = nullptr;
+      if (KV_MODE) {  // per-column statistics of the queries of this block
+        const int qh = kv_head * group + t / n_c;
+        lq = lse + ((long long)batch * nh + qh) * S + C0;
+        dq = delta + ((long long)batch * nh + qh) * S + C0;
+      }
+      mbar_wait_mma(&y_full[ys], (uint32_t)((t / Y_STAGES) & 1));
+      const uint32_t y1 = smem_u32(smem + OFF_Y + ys * 2 * C_TILE), y2 = y1 + C_TILE;
+      float sc[32], dp[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) sc[i] = dp[i] = 0.f;
+      wgmma_fence();
+      fence_regs(sc);
+      fence_regs(dp);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint32_t ra = (uint32_t)((kk >> 2) * R_HALF + (kk & 3) * 32);
+        const uint32_t cb = (uint32_t)((kk >> 2) * C_HALF + (kk & 3) * 32);
+        wgmma_m64n64k16_ss<0, 0>(sc, desc_kmajor_sw128(r1 + ra), desc_kmajor_sw128(y1 + cb), 1u);
+      }
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+        const uint32_t ra = (uint32_t)((kk >> 2) * R_HALF + (kk & 3) * 32);
+        const uint32_t cb = (uint32_t)((kk >> 2) * C_HALF + (kk & 3) * 32);
+        wgmma_m64n64k16_ss<0, 0>(dp, desc_kmajor_sw128(r2 + ra), desc_kmajor_sw128(y2 + cb), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(sc);
+      fence_regs(dp);
+      if (tr_thread && t < 64) trace[t * 8 + 0] = clock64();
+      // causal: query index >= key index.  Only blocks that touch the diagonal need the compare.
+      const bool need_mask = KV_MODE ? (C0 < R0 + 127) : (C0 + 63 > R0);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int col = 8 * (i >> 2) + 2 * tq + (i & 1);
+        const int h = (i >> 1) & 1;
+        const int row = rl0 + 8 * h;
+        float l2, dl;
+        if constexpr (KV_MODE) {
+          l2 = __ldg(lq + col) * LOG2E;
+          dl = __ldg(dq + col);
+        } else {
+          l2 = lse_r[h];
+          dl = delta_r[h];
+        }
+        float p = fast_exp2(fmaf(sc[i], sl2, -l2));
+        if (need_mask) {
+          const bool ok = KV_MODE ? (C0 + col >= R0 + row) : (R0 + row >= C0 + col);
+          p = ok ? p : 0.f;
+        }
+        sc[i] = p;
+        dp[i] = p * (dp[i] - dl) * scale;
+      }
+      uint32_t pp[4][4], pd[4][4];   // bf16 A fragments of the four k16 steps of the gradient MMAs
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          pp[kk][r] = pack_bf16x2(sc[8 * kk + 2 * r], sc[8 * kk + 2 * r + 1]);
+          pd[kk][r] = pack_bf16x2(dp[8 * kk + 2 * r], dp[8 * kk + 2 * r + 1]);
+        }
+      if (tr_thread && t < 64) trace[t * 8 + 1] = clock64();
+      if constexpr (!TS) {
+        // [128 rows x 64 columns] bf16, 128B swizzle (what TMA would have written)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int row = rl0 + ((r & 1) ? 8 : 0);
+            const int col = 16 * kk + ((r & 2) ? 8 : 0) + 2 * tq;
+            const int off = row * 128 + (((col >> 3) ^ (row & 7)) << 4) + (col & 7) * 2;
+            if (KV_MODE) *reinterpret_cast<uint32_t*>(smem + OFF_P + off) = pp[kk][r];
+            *reinterpret_cast<uint32_t*>(smem + OFF_DS + off) = pd[kk][r];
+          }
+        fence_proxy_async();            // generic-proxy writes -> visible to the async proxy (wgmma)
+        named_bar_sync(1 + half, 128);
+      }
+      wgmma_fence();
+      if constexpr (KV_MODE) fence_regs(acc_a);
+      fence_regs(acc_b);
+      if constexpr (KV_MODE) {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {  // dV += P^T dO_C
+          const uint64_t db = desc_mnmajor_sw128(y2 + kk * 2048, C_HALF);
+          if constexpr (TS) wgmma_m64n128k16_rs<1>(acc_a, pp[kk], db, 1u);
+          else wgmma_m64n128k16_ss<0, 1>(acc_a, desc_kmajor_sw128(sp + kk * 32), db, 1u);
+        }
+      }
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {    // dK += dS^T Q_C   /   dQ += dS K_C
+        const uint64_t db = desc_mnmajor_sw128(y1 + kk * 2048, C_HALF);
+        if constexpr (TS) wgmma_m64n128k16_rs<1>(acc_b, pd[kk], db, 1u);
+        else wgmma_m64n128k16_ss<0, 1>(acc_b, desc_kmajor_sw128(sds + kk * 32), db, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if constexpr (KV_MODE) fence_regs(acc_a);
+      fence_regs(acc_b);
+      if (signal) mbar_arrive(&y_empty[ys]);
+      if constexpr (!TS) named_bar_sync(1 + half, 128);   // every warp's MMAs are done with P / dS
+      if (tr_thread && t < 64) trace[t * 8 + 3] = clock64();
+    }
+    // write the accumulated gradients of my two rows
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const long long tok = (long long)batch * S + R0 + rl0 + 8 * h;
+      auto write_row = [&](const float (&acc)[64], int out_head) {
+        __nv_bfloat16* dst = dqkv + (tok * nht + out_head) * (long long)D;
+#pragma unroll
+        for (int nb = 0; nb < 16; ++nb)
+          *reinterpret_cast<__nv_bfloat162*>(dst + 8 * nb + 2 * tq) =
+              __floats2bfloat162_rn(acc[4 * nb + 2 * h], acc[4 * nb + 2 * h + 1]);
+      };
+      if constexpr (KV_MODE) {
+        write_row(acc_a, nh + nkv + kv_head);  // dV
+        write_row(acc_b, nh + kv_head);        // dK
+      } else {
+        write_row(acc_b, head_r);              // dQ
+      }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<1>(tmem_base, 512);
 }
 
 void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* trace_buf,
@@ -395,11 +337,11 @@ void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse,
     DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
     attr = true;
   }
-  static const bool ts_default = []() {   // DTG_ATTN_BWD=ts (default: P / dS stay in tensor memory) | ss
+  static const bool ts_default = []() {   // DTG_ATTN_BWD=rs (default: P / dS stay in registers) | ss
     const char* e = getenv("DTG_ATTN_BWD");
-    return e ? e[0] == 't' : true;
+    return e ? e[0] != 's' : true;
   }();
-  const bool ts = mode == 0 ? ts_default : mode == 2;   // mode: 0 default, 1 = ss, 2 = ts
+  const bool ts = mode == 0 ? ts_default : mode == 2;   // mode: 0 default, 1 = ss, 2 = rs
   const int nblk = S / 128;
   if (ts) {
     attn_bwd_kernel<true, true><<<dim3(B * nkv, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(

@@ -1,19 +1,16 @@
-// Causal flash-attention forward on tcgen05 (head_dim 128, GQA), reading q/k/v straight out of
+// Causal flash-attention forward on wgmma (head_dim 128, GQA), reading q/k/v straight out of
 // the fused qkv activation [B, S, nh + 2*nkv, 128] through one strided 4-D TMA descriptor (no
-// transposes, no repeat_kv copies).  One CTA = one (batch, q-head, 128-query block):
+// transposes, no repeat_kv copies).  One CTA = one (batch, q-head, 128-query block), 384 threads:
 //
-//   warp 0    TMA producer     Q once; K_j / V_j into 2-stage rings (separate barriers so QK^T
-//                              can start as soon as K lands)
-//   warp 1    MMA issuer       S[j%2] = Q K_j^T  (128x128x128, fp32 in TMEM, double-buffered so
-//                              the next block's scores are computed during this block's softmax)
-//                              O     += P_j V_j  (P from shared memory, V as an MN-major operand)
-//   warp 2    TMEM allocator   512 columns: S0 | S1 | O
-//   warps 4-11 softmax         two threads per query row (64 score columns each; two warps per SM
-//                              sub-partition hide each other's latency): tcgen05.ld of the half row,
-//                              online max (halves combined through shared memory + a 64-thread named
-//                              barrier) / sum in fp32 with ex2.approx, P -> bf16 -> 128B-swizzled shared
-//                              memory, O rescaled in TMEM only when some row's running max moved,
-//                              final O / l and the logsumexp written from registers.
+//   warpgroup 0     TMA producer (one elected lane of warp 0): Q once; K_j / V_j into 2-stage rings
+//                   (separate barriers so Q K^T can start as soon as K lands)
+//   warpgroups 1-2  64 query rows each: S = Q K_j^T (wgmma m64n128k16, fp32 in registers), online
+//                   softmax in registers (a row lives in the 4 threads of a quad), O += P_j V_j
+//                   (V as an MN-major operand), final O / l and the logsumexp written from registers.
+//
+// P_REGS (version 2): P is packed to bf16 in the registers it was computed in and feeds the PV wgmma as its
+// A operand (RS form) — the accumulator fragment of two n8 column blocks is exactly the A fragment of one
+// k16 step.  Version 1 stages P through 128B-swizzled shared memory (SS form).
 //
 // Replaces torch SDPA / flash-attn-2 (mma.sync) that the reference uses (SURVEY.md K2/K3).
 #include <cuda.h>
@@ -32,33 +29,29 @@ constexpr int BM = 128, BN = 128, D = 128;
 constexpr int TILE_BYTES = 128 * 128 * 2;  // 32 KB: two 64-column halves of [128 rows x 128 B]
 constexpr int HALF_BYTES = TILE_BYTES / 2;
 constexpr int OFF_Q = 0, OFF_K = TILE_BYTES, OFF_V = 3 * TILE_BYTES, OFF_P = 5 * TILE_BYTES;
-constexpr int OFF_BAR = 6 * TILE_BYTES;
-constexpr int OFF_RED = OFF_BAR + 256;          // float [3][2][128]: row max exchange (double-buffered by block
-                                                // parity: a fast warp may already publish block j+1) + row sums
-constexpr int SMEM_BYTES = OFF_RED + 3072 + 1024;
 constexpr int THREADS = 384;
-constexpr uint32_t TM_S0 = 0, TM_S1 = 128, TM_O = 256;
+template <bool P_REGS>
+struct Layout {
+  static constexpr int OFF_BAR = P_REGS ? OFF_P : OFF_P + TILE_BYTES;
+  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+};
 }  // namespace fwd
 
+template <bool P_REGS>
 __global__ void __launch_bounds__(fwd::THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __restrict__ o, float* __restrict__ lse,
                 int S, int nh, int nkv, float scale_log2, int num_m_blocks) {
   using namespace fwd;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Layout<P_REGS>::OFF_BAR);
   uint64_t* q_full = bars + 0;
   uint64_t* k_full = bars + 1;    // [2]
   uint64_t* v_full = bars + 3;    // [2]
   uint64_t* k_empty = bars + 5;   // [2]
   uint64_t* v_empty = bars + 7;   // [2]
-  uint64_t* s_full = bars + 9;    // [2]
-  uint64_t* s_empty = bars + 11;  // [2]
-  uint64_t* p_full = bars + 13;
-  uint64_t* pv_done = bars + 14;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 16);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   // longest rows first: CTAs are dispatched in blockIdx order, causal work grows with the q block
   // (grid = (B*nh, num_m_blocks): x varies fastest, so every head's longest block goes out first)
   const int m_block = num_m_blocks - 1 - (int)blockIdx.y;
@@ -68,32 +61,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
   const int n_blocks = m_block + 1;  // causal, BM == BN
   const int q0 = m_block * BM;
 
-  if (warp == 0 && elect_one()) prefetch_tensormap(&tm_qkv);
-  if (warp == 1 && elect_one()) {
+  if (threadIdx.x == 0) {
+    prefetch_tensormap(&tm_qkv);
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&k_full[i], 1);
       mbar_init(&v_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-      mbar_init(&v_empty[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_empty[i], 8);
+      mbar_init(&k_empty[i], 2);
+      mbar_init(&v_empty[i], 2);
     }
-    mbar_init(p_full, 8);
-    mbar_init(pv_done, 1);
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc<1>(tmem_ptr_smem, 512);
-    tmem_relinquish<1>();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
-    if (elect_one()) {
+  if (wg == 0) {
+    if (warp == 0 && elect_one()) {
       // Q tile: two 64-column halves
       mbar_arrive_expect_tx(q_full, TILE_BYTES);
       tma_load_4d(&tm_qkv, q_full, smem + OFF_Q, 0, head, q0, batch);
@@ -102,176 +84,145 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
       for (int j = 0; j < n_blocks; ++j) {
         const int st = j & 1;
         const uint32_t ph = (uint32_t)((j >> 1) & 1);
-        mbar_wait(&k_empty[st], ph ^ 1);
+        mbar_wait_mma(&k_empty[st], ph ^ 1);
         mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
         tma_load_4d(&tm_qkv, &k_full[st], smem + OFF_K + st * TILE_BYTES, 0, kh, j * BN, batch);
         tma_load_4d(&tm_qkv, &k_full[st], smem + OFF_K + st * TILE_BYTES + HALF_BYTES, 64, kh, j * BN, batch);
-        mbar_wait(&v_empty[st], ph ^ 1);
+        mbar_wait_mma(&v_empty[st], ph ^ 1);
         mbar_arrive_expect_tx(&v_full[st], TILE_BYTES);
         tma_load_4d(&tm_qkv, &v_full[st], smem + OFF_V + st * TILE_BYTES, 0, vh, j * BN, batch);
         tma_load_4d(&tm_qkv, &v_full[st], smem + OFF_V + st * TILE_BYTES + HALF_BYTES, 64, vh, j * BN, batch);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc_qk = make_idesc_bf16(128, 128, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 128, false, true);
-      const uint32_t sq = smem_u32(smem + OFF_Q), sp = smem_u32(smem + OFF_P);
-      auto issue_qk = [&](int j) {
-        const int st = j & 1;
+  } else {
+    // ===================== softmax warpgroups =====================
+    const int half = wg - 1;                       // query rows [64*half, 64*half + 64) of the tile
+    const int g = lane >> 2, tq = lane & 3;
+    const int rl0 = half * 64 + (warp & 3) * 16 + g;   // my rows: rl0 and rl0 + 8 (tile-local)
+    const bool signal = (threadIdx.x & 127) == 0;
+    const uint32_t sq = smem_u32(smem + OFF_Q) + (uint32_t)(half * 8192);
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // l_run: this thread's partial row sums
+    mbar_wait_mma(q_full, 0);
+    for (int j = 0; j < n_blocks; ++j) {
+      const int st = j & 1;
+      const uint32_t ph = (uint32_t)((j >> 1) & 1);
+      float s[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) s[i] = 0.f;
+      mbar_wait_mma(&k_full[st], ph);
+      {
         const uint32_t sk = smem_u32(smem + OFF_K + st * TILE_BYTES);
-        const uint32_t d_tm = tmem_base + (st ? TM_S1 : TM_S0);
+        wgmma_fence();
+        fence_regs(s);
 #pragma unroll
         for (int kk = 0; kk < 8; ++kk) {
           const uint32_t off = (uint32_t)((kk >> 2) * HALF_BYTES + (kk & 3) * 32);
-          mma_f16_ss<1>(d_tm, desc_kmajor_sw128(sq + off), desc_kmajor_sw128(sk + off), idesc_qk, kk ? 1u : 0u);
+          wgmma_m64n128k16_ss<0, 0>(s, desc_kmajor_sw128(sq + off), desc_kmajor_sw128(sk + off), 1u);
         }
-        mma_commit(&s_full[st]);
-        mma_commit(&k_empty[st]);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      issue_qk(0);
-      for (int j = 0; j < n_blocks; ++j) {
-        if (j + 1 < n_blocks) {
-          const int st = (j + 1) & 1;
-          const uint32_t ph = (uint32_t)(((j + 1) >> 1) & 1);
-          mbar_wait(&k_full[st], ph);
-          mbar_wait(&s_empty[st], ph ^ 1);  // softmax of block j-1 has drained this score buffer
-          tc_fence_after();
-          issue_qk(j + 1);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(s);
+      }
+      if (signal) mbar_arrive(&k_empty[st]);
+      if (j == n_blocks - 1) {   // diagonal block: mask keys after the query
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+          const int col = 8 * (i >> 2) + 2 * tq + (i & 1);
+          const int row = rl0 + ((i & 2) ? 8 : 0);
+          if (col > row) s[i] = -INFINITY;
         }
-        const int st = j & 1;
-        mbar_wait(p_full, (uint32_t)(j & 1));
-        mbar_wait(&v_full[st], (uint32_t)((j >> 1) & 1));
-        tc_fence_after();
+      }
+      float alpha[2], mb[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) mx = fmaxf(mx, s[4 * (i >> 1) + 2 * h + (i & 1)]);
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        mx = fmaxf(m_run[h], mx);
+        alpha[h] = fast_exp2((m_run[h] - mx) * scale_log2);  // 0 on the first block (m_run = -inf)
+        mb[h] = mx * scale_log2;
+        m_run[h] = mx;
+      }
+      float sum[2] = {0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i < 64; ++i) {
+        const int h = (i >> 1) & 1;
+        s[i] = fast_exp2(fmaf(s[i], scale_log2, -mb[h]));
+        sum[h] += s[i];
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) l_run[h] = l_run[h] * alpha[h] + sum[h];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] *= alpha[(i >> 1) & 1];
+      uint32_t pa[8][4];   // P as bf16 A fragments, one per k16 step of the PV MMA
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) pa[kk][r] = pack_bf16x2(s[8 * kk + 2 * r], s[8 * kk + 2 * r + 1]);
+      uint32_t sp = 0;
+      if constexpr (!P_REGS) {
+        // P -> [128 rows x 128 keys] bf16, two 64-key halves, 128B swizzle (what TMA would have written)
+        uint8_t* pbase = smem + OFF_P;
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk)
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int row = rl0 + ((r & 1) ? 8 : 0);
+            const int key = 16 * kk + ((r & 2) ? 8 : 0) + 2 * tq;
+            const int chunk = (key & 63) >> 3;
+            *reinterpret_cast<uint32_t*>(pbase + (key >> 6) * HALF_BYTES + row * 128 + ((chunk ^ (row & 7)) << 4) +
+                                         (key & 7) * 2) = pa[kk][r];
+          }
+        fence_proxy_async();           // generic-proxy writes of P -> visible to the async proxy (wgmma)
+        named_bar_sync(1 + half, 128);
+        sp = smem_u32(pbase) + (uint32_t)(half * 8192);
+      }
+      mbar_wait_mma(&v_full[st], ph);
+      {
         const uint32_t sv = smem_u32(smem + OFF_V + st * TILE_BYTES);
+        wgmma_fence();
+        fence_regs(acc);
 #pragma unroll
         for (int kk = 0; kk < 8; ++kk) {
-          const uint64_t da = desc_kmajor_sw128(sp + (uint32_t)((kk >> 2) * HALF_BYTES + (kk & 3) * 32));
           const uint64_t db = desc_mnmajor_sw128(sv + (uint32_t)(kk * 2048), HALF_BYTES);
-          mma_f16_ss<1>(tmem_base + TM_O, da, db, idesc_pv, (j | kk) ? 1u : 0u);
+          if constexpr (P_REGS) {
+            wgmma_m64n128k16_rs<1>(acc, pa[kk], db, 1u);
+          } else {
+            const uint64_t da = desc_kmajor_sw128(sp + (uint32_t)((kk >> 2) * HALF_BYTES + (kk & 3) * 32));
+            wgmma_m64n128k16_ss<0, 1>(acc, da, db, 1u);
+          }
         }
-        mma_commit(pv_done);
-        mma_commit(&v_empty[st]);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(acc);
       }
-    }
-  } else if (warp >= 4) {
-    // ===================== softmax / correction / epilogue =====================
-    const int q = warp & 3;             // TMEM lane quarter this warp may touch
-    const int half = (warp - 4) >> 2;   // which 64 score columns (and which 64 output columns) are mine
-    const int row = q * 32 + lane;      // query row within the tile == TMEM lane
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    float* red = reinterpret_cast<float*>(smem + OFF_RED);
-    float m_run = -INFINITY, l_run = 0.f;  // l_run: partial row sum over my columns
-    uint8_t* sp = smem + OFF_P + half * HALF_BYTES + row * 128;
-    for (int j = 0; j < n_blocks; ++j) {
-      const int st = j & 1;
-      mbar_wait(&s_full[st], (uint32_t)((j >> 1) & 1));
-      tc_fence_after();
-      float s[64];
-      {
-        uint32_t r0[32], r1[32];  // both loads in flight before the single wait
-        tmem_ld_32x32b_x32(lane_addr + (st ? TM_S1 : TM_S0) + half * 64, r0);
-        tmem_ld_32x32b_x32(lane_addr + (st ? TM_S1 : TM_S0) + half * 64 + 32, r1);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          s[i] = __uint_as_float(r0[i]);
-          s[32 + i] = __uint_as_float(r1[i]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[st]);  // scores are in registers now
-      if (j == n_blocks - 1) {                   // diagonal block: mask keys after the query
-#pragma unroll
-        for (int i = 0; i < 64; ++i)
-          if (half * 64 + i > row) s[i] = -INFINITY;
-      }
-      float mx4[4] = {s[0], s[1], s[2], s[3]};  // four independent chains instead of one 64-deep one
-#pragma unroll
-      for (int i = 4; i < 64; i += 4) {
-        mx4[0] = fmaxf(mx4[0], s[i]);
-        mx4[1] = fmaxf(mx4[1], s[i + 1]);
-        mx4[2] = fmaxf(mx4[2], s[i + 2]);
-        mx4[3] = fmaxf(mx4[3], s[i + 3]);
-      }
-      float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-      float* redj = red + (j & 1) * 256;
-      redj[half * 128 + row] = mx;
-      named_bar_sync(1 + q, 64);  // the two warps that share these 32 rows
-      mx = fmaxf(m_run, fmaxf(mx, redj[(half ^ 1) * 128 + row]));
-      const float alpha = fast_exp2((m_run - mx) * scale_log2);  // 0 on the first block (m_run = -inf)
-      const float mb = mx * scale_log2;
-      float sum4[4] = {0.f, 0.f, 0.f, 0.f};
-      uint32_t pk[32];
-#pragma unroll
-      for (int i = 0; i < 64; i += 2) {
-        const float p0 = fast_exp2(fmaf(s[i], scale_log2, -mb));
-        const float p1 = fast_exp2(fmaf(s[i + 1], scale_log2, -mb));
-        sum4[(i >> 1) & 3] += p0 + p1;
-        __nv_bfloat162 h = __floats2bfloat162_rn(p0, p1);
-        pk[i >> 1] = *reinterpret_cast<uint32_t*>(&h);
-      }
-      const float sum = (sum4[0] + sum4[1]) + (sum4[2] + sum4[3]);
-      l_run = l_run * alpha + sum;
-      m_run = mx;
-      // P_j may only overwrite the shared buffer / O may only be touched once PV_{j-1} is done
-      if (j > 0) mbar_wait(pv_done, (uint32_t)((j - 1) & 1));
-#pragma unroll
-      for (int c = 0; c < 8; ++c)
-        *reinterpret_cast<uint4*>(sp + ((c ^ (row & 7)) << 4)) =
-            make_uint4(pk[c * 4], pk[c * 4 + 1], pk[c * 4 + 2], pk[c * 4 + 3]);
-      if (j > 0 && __any_sync(0xffffffffu, alpha < 1.f)) {
-        tc_fence_after();
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(lane_addr + TM_O + half * 64 + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(__uint_as_float(r[i]) * alpha);
-          tmem_st_32x32b_x32(lane_addr + TM_O + half * 64 + c * 32, r);
-        }
-        tmem_st_wait();
-      }
-      fence_proxy_async();  // generic-proxy writes of P -> visible to the tensor core's async proxy
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
+      if (signal) mbar_arrive(&v_empty[st]);
+      if constexpr (!P_REGS) named_bar_sync(1 + half, 128);   // every warp's PV MMAs are done with P
     }
     // epilogue: O / l -> bf16 -> global ; logsumexp
-    red[512 + half * 128 + row] = l_run;
-    named_bar_sync(1 + q, 64);
-    const float l_tot = l_run + red[512 + (half ^ 1) * 128 + row];
-    mbar_wait(pv_done, (uint32_t)((n_blocks - 1) & 1));
-    tc_fence_after();
-    const float inv_l = 1.f / l_tot;
-    const long long tok = (long long)batch * S + q0 + row;
-    __nv_bfloat16* orow = o + (tok * nh + head) * (long long)D + half * 64;
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint32_t r[32];
-      tmem_ld_32x32b_x32(lane_addr + TM_O + half * 64 + c * 32, r);
-      tmem_ld_wait();
+    for (int h = 0; h < 2; ++h) {
+      float l = l_run[h];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      const float inv_l = 1.f / l;
+      const int row = rl0 + 8 * h;
+      const long long tok = (long long)batch * S + q0 + row;
+      __nv_bfloat16* orow = o + (tok * nh + head) * (long long)D;
 #pragma unroll
-      for (int v = 0; v < 4; ++v) {
-        float f[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) f[i] = __uint_as_float(r[v * 8 + i]) * inv_l;
-        st8(orow + c * 32 + v * 8, pack8(f));
-      }
+      for (int nb = 0; nb < 16; ++nb)
+        *reinterpret_cast<__nv_bfloat162*>(orow + 8 * nb + 2 * tq) =
+            __floats2bfloat162_rn(acc[4 * nb + 2 * h] * inv_l, acc[4 * nb + 2 * h + 1] * inv_l);
+      // natural-log logsumexp of the scaled scores
+      if (tq == 0)
+        lse[((long long)batch * nh + head) * S + q0 + row] = m_run[h] * scale_log2 * 0.6931471805599453f + __logf(l);
     }
-    // natural-log logsumexp of the scaled scores
-    if (half == 0)
-      lse[((long long)batch * nh + head) * S + q0 + row] = m_run * scale_log2 * 0.6931471805599453f + __logf(l_tot);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc<1>(tmem_base, 512);
 }
 
 CUtensorMap make_tmap_heads(const void* base, int B, int S, int heads, int box_rows) {
@@ -282,20 +233,32 @@ CUtensorMap make_tmap_heads(const void* base, int B, int S, int heads, int box_r
   return make_tmap_bf16(base, 4, dims, strides, box, true);
 }
 
-void attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s) {
+template <bool P_REGS>
+static void launch_attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale,
+                            cudaStream_t s) {
   if (S % 128 != 0) throw std::runtime_error("attn_fwd: sequence length must be a multiple of 128");
   if (nh % nkv != 0) throw std::runtime_error("attn_fwd: nh must be a multiple of nkv");
   const CUtensorMap tm = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 128);
+  constexpr int smem = fwd::Layout<P_REGS>::SMEM_BYTES;
   static bool attr = false;
   if (!attr) {
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fwd::SMEM_BYTES));
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<P_REGS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr = true;
   }
   const int num_m = S / 128;
-  attn_fwd_kernel<<<dim3(B * nh, num_m, 1), fwd::THREADS, fwd::SMEM_BYTES, s>>>(tm, (__nv_bfloat16*)o, lse, S, nh, nkv,
-                                                                      scale * 1.4426950408889634f, num_m);
+  attn_fwd_kernel<P_REGS><<<dim3(B * nh, num_m, 1), fwd::THREADS, smem, s>>>(tm, (__nv_bfloat16*)o, lse, S, nh, nkv,
+                                                                            scale * 1.4426950408889634f, num_m);
   note_launch();
   DTG_LAUNCH_CHECK();
+}
+
+// version 1: P through shared memory
+void attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s) {
+  launch_attn_fwd<false>(qkv, o, lse, B, S, nh, nkv, scale, s);
+}
+// version 2: P stays in registers (RS-form PV MMA)
+void attn_fwd2(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s) {
+  launch_attn_fwd<true>(qkv, o, lse, B, S, nh, nkv, scale, s);
 }
 
 }  // namespace dtg

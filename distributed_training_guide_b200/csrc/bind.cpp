@@ -175,7 +175,7 @@ void adamw_flat(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, double lr, dou
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "distributed_training_guide_b200 sm_100a kernels";
+  m.doc() = "distributed_training_guide_b200 sm_90a kernels";
   m.def("launch_count", []() { return (uint64_t)dtg::launch_count(); });
   m.def("gemm", &gemm, py::arg("a"), py::arg("b"), py::arg("out"), py::arg("trans_a") = false,
         py::arg("trans_b") = false, py::arg("accumulate") = false, py::arg("variant") = 0);

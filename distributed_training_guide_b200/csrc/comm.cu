@@ -1,4 +1,4 @@
-// NVLink 5 / NVSwitch collectives over peer-mapped ("symmetric") memory, fused with the math that
+// NVLink / NVSwitch collectives over peer-mapped ("symmetric") memory, fused with the math that
 // surrounds them in data-parallel training.  Every kernel takes a device table of the N ranks'
 // base pointers to the SAME symmetric buffer plus a table of signal pads, and synchronises
 // device-side (st.release.sys / ld.acquire.sys epoch flags, one channel per CTA) — no host

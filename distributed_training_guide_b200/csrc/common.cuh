@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels: error checks, launch accounting, bf16 vector math.
+// Shared helpers for the sm_90a kernels: error checks, launch accounting, bf16 vector math.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

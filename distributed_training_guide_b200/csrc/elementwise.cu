@@ -1,4 +1,4 @@
-// Memory-bound ops of the Llama step, hand-written for sm_100a:
+// Memory-bound ops of the Llama step, hand-written for sm_90a:
 //   fused (residual add +) RMSNorm fwd / bwd, in-place RoPE on the fused qkv activation,
 //   SwiGLU fwd / bwd, embedding gather / scatter-add, scalar scale.
 // All are pure-bandwidth kernels: 16-byte vector accesses, fp32 math in registers, one pass

@@ -1,6 +1,6 @@
 // Tensor / sequence-parallel support kernels (chapters 06 / 07).  The tensor-core halves of the fused
 // paths — all-gather->GEMM, GEMM->reduce-scatter push, wgrad over a sequence-sharded operand — are the
-// distributed modes of the tcgen05 GEMM in gemm_tcgen05.cu (operand tiles fetched from / stored to peer
+// distributed modes of the wgmma GEMM in gemm_wgmma.cu (operand tiles fetched from / stored to peer
 // GPUs over NVLink inside the kernel).  This file holds the pieces around them:
 //
 //   tp_reduce_parts      out = (residual +) sum of the N partial tiles peers pushed into my staging

@@ -1,4 +1,4 @@
-// Tile configuration shared by the tcgen05 GEMM and the fused GEMM+collective kernels.
+// Tile configuration shared by the wgmma GEMM and the fused GEMM+collective kernels.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -14,19 +14,24 @@ namespace dtg {
 
 template <int CG>
 struct GemmCfg {
-  static constexpr int BM = 128;          // C rows per CTA (UMMA_M = BM * CG)
-  static constexpr int BN = 256;          // C columns per tile (UMMA_N)
+  static constexpr int THREADS = 384;     // producer warpgroup + two consumer warpgroups
+  static constexpr int BM = 128;          // C rows per CTA (a CG-CTA cluster covers BM * CG rows)
+  static constexpr int BN = 256;          // C columns per tile (wgmma N)
   static constexpr int BK = 64;           // one 128-byte swizzle span of bf16 per stage
-  static constexpr int B_ROWS = BN / CG;  // rows of B (N) this CTA stages; the pair shares B
+  static constexpr int B_ROWS = BN / CG;  // rows of B (N) this CTA loads; CG 2 multicasts them to the pair
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = B_ROWS * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (CG == 1) ? 4 : 6;
+  static constexpr int STAGES = 4;
   static constexpr int BAR_BYTES = 256;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;  // +1024: manual alignment slack
-  // B_MODE 3 (operand B gathered from the ranks' FSDP shards by warp 3 of every CTA): a 2-slot bounce ring
+  // A_MODE 3 communication CTAs reuse the pipeline smem as a ring of COMM_SLOTS pieces
+  static constexpr int COMM_PIECE = 32768;
+  static constexpr int COMM_SLOTS = STAGES * STAGE_BYTES / COMM_PIECE;
+  // B_MODE 3 (operand B gathered from the ranks' FSDP shards by warp 1 of every CTA): a 2-slot bounce ring
   static constexpr int GATHER_PIECE = 16384;
   static constexpr int GATHER_BYTES = 2 * GATHER_PIECE;
+  static_assert(2 * STAGES + (COMM_SLOTS > 2 ? COMM_SLOTS : 2) <= BAR_BYTES / 8, "barrier area");
 };
 
 template <int N>
@@ -50,7 +55,7 @@ struct GemmDist {
   int rank, nranks;
   long long tile_bytes;              // bytes of one 256-row tile of A (contiguous: lda == K)
   // B_MODE 3 (FSDP unshard inside the consuming GEMM): operand B is a weight whose bytes [bg_begin, bg_end) of the
-  // group's flat layout are spread over the ranks' shards (rank p owns flat bytes [p*per, (p+1)*per)).  Warp 3 of
+  // group's flat layout are spread over the ranks' shards (rank p owns flat bytes [p*per, (p+1)*per)).  Warp 1 of
   // every CTA bounces 16 KB pieces shard -> smem -> local full buffer and counts them per `1 << bg_chunk_shift`
   // byte chunk; the TMA producer acquires the counters of the chunks under a B box before loading it.
   const char* bg_src[kMaxRanks];     // shard base per rank (NOT rotated; [rank] is my own shard)
@@ -74,8 +79,8 @@ __host__ __device__ __forceinline__ int tile_m(int t, int num_m_tiles, const Gem
   return m >= num_m_tiles ? m - num_m_tiles : m;
 }
 // Tile order.  Default: M fastest (consecutive CTAs share the B tile) within a group of `group_m` row tiles
-// whose slice of A stays L2-resident while B streams past once per group: the ~74 tiles in flight then touch
-// group_m row panels of A and 74/group_m column panels of B instead of every row panel of A, which is what keeps
+// whose slice of A stays L2-resident while B streams past once per group: the ~66 tiles in flight then touch
+// group_m row panels of A and 66/group_m column panels of B instead of every row panel of A, which is what keeps
 // a tall GEMM (wgrad with M = 22016 or 32000) from re-streaming all of A from HBM for every column of tiles.
 // With an in-kernel all-gather
 // (`local_m_tiles` > 0): first every tile of my own rows (pure local work while the communication CTAs
@@ -113,7 +118,7 @@ __host__ __device__ __forceinline__ void tile_mn(int t, int num_m_tiles, const G
 }
 #endif
 
-// TMA descriptor builders (gemm_tcgen05.cu)
+// TMA descriptor builders (gemm_wgmma.cu)
 CUtensorMap make_tmap_bf16(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                            const uint32_t* box, bool swizzle128);
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,

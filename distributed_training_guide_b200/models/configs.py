@@ -87,7 +87,7 @@ REGISTRY = {
     "meta-llama/Llama-3.1-70B": _llama("meta-llama/Llama-3.1-70B", 128256, 8192, 28672, 80, 64, 8, 131072, 5e5, _LLAMA3_SCALING),
     "meta-llama/Llama-3.1-405B": _llama("meta-llama/Llama-3.1-405B", 128256, 16384, 53248, 126, 128, 8, 131072, 5e5, _LLAMA3_SCALING),
     "meta-llama/Meta-Llama-3.1-405B": _llama("meta-llama/Meta-Llama-3.1-405B", 128256, 16384, 53248, 126, 128, 8, 131072, 5e5, _LLAMA3_SCALING),
-    # tiny configs for tests / smoke runs (head_dim 128 so the sm_100a attention kernel applies)
+    # tiny configs for tests / smoke runs (head_dim 128 so the sm_90a attention kernel applies)
     "debug-llama": _llama("debug-llama", 1024, 256, 512, 2, 2, 2, 2048, 1e4),
     "debug-llama-gqa": _llama("debug-llama-gqa", 1024, 512, 1024, 2, 4, 2, 2048, 5e5),
     "debug-llama-tp": _llama("debug-llama-tp", 2048, 1024, 2048, 2, 8, 8, 2048, 1e4),

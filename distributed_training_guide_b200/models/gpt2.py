@@ -3,7 +3,7 @@
 This is the model of the guide's smoke command (``-m openai-community/gpt2``, reference
 ``01-single-gpu/README.md:9-12``) and of BASELINE.json's config 01, which is a CPU
 plumbing configuration.  It is therefore written in plain PyTorch ops (SURVEY.md K4b);
-the sm_100a kernels target the Llama family.  Parameter names follow HF's
+the sm_90a kernels target the Llama family.  Parameter names follow HF's
 ``GPT2LMHeadModel`` (``transformer.wte.weight`` ... ``transformer.h.{i}.attn.c_attn.weight``).
 """
 from __future__ import annotations

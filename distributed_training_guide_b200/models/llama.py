@@ -1,4 +1,4 @@
-"""Llama-family causal LM built on the sm_100a op layer.
+"""Llama-family causal LM built on the sm_90a op layer.
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
 the reference instantiates at e.g. ``02-distributed-data-parallel/train_llm.py:57-58``)
@@ -8,7 +8,7 @@ so checkpoints keep meaningful keys: ``model.embed_tokens.weight``,
 ``model.norm.weight``, ``lm_head.weight``.
 
 What is *different* from the HF module code (SURVEY.md §3.2) is the execution plan:
-  * q/k/v (and gate/up) projections run as ONE tcgen05 GEMM over a fused weight that is
+  * q/k/v (and gate/up) projections run as ONE wgmma GEMM over a fused weight that is
     just the adjacent placement of the three (two) parameters in the layer's flat buffer;
   * RoPE rotates the q and k heads in place inside the fused qkv activation, attention
     reads q/k/v straight out of that buffer through strided TMA descriptors (no

@@ -1,7 +1,7 @@
 """Op layer: every hot op of the Llama training step as an ``autograd.Function``.
 
-On CUDA tensors each op calls a hand-written sm_100a kernel from the in-tree
-extension (``csrc/``): tcgen05/TMEM/TMA GEMM (fwd / dgrad / wgrad), tcgen05
+On CUDA tensors each op calls a hand-written sm_90a kernel from the in-tree
+extension (``csrc/``): wgmma/TMA GEMM (fwd / dgrad / wgrad), wgmma
 flash-attention, fused residual-add+RMSNorm, in-place RoPE on the fused qkv buffer,
 SwiGLU, in-place softmax-cross-entropy, embedding gather / scatter-add and flat
 AdamW.  On CPU tensors the same Functions run the reference math in
@@ -78,7 +78,7 @@ def _emit_weight_grad(param, compute_into, shape_like):
 
 
 def gemm(a, b, out=None, trans_a=False, trans_b=False, accumulate=False):
-    """out[M,N] (+)= op(a) @ op(b) on the tcgen05 GEMM (bf16 in, fp32 accumulate in TMEM).
+    """out[M,N] (+)= op(a) @ op(b) on the wgmma GEMM (bf16 in, fp32 accumulate in registers).
 
     ``op(a)`` is ``a`` ([M,K]) or ``a.T`` when ``trans_a`` (a given as [K,M]);
     ``op(b)`` is ``b`` ([K,N]) or ``b.T`` when ``trans_b`` (b given as [N,K]).
@@ -154,7 +154,7 @@ class _Linear(torch.autograd.Function):
 
 
 def linear(x, w, bias=None):
-    """y = x @ w.T (+ bias).  bf16 CUDA tensors run the tcgen05 GEMM."""
+    """y = x @ w.T (+ bias).  bf16 CUDA tensors run the wgmma GEMM."""
     if bias is None and _ext.use_cuda_kernel("gemm", x, w) and x.dtype == torch.bfloat16:
         return _Linear.apply(x, w, w)
     return ref.linear(x, w, bias)
@@ -306,7 +306,7 @@ def attention_qkv(qkv, nh, nkv, scale=None):
     q, k, v = qkv[:, :, :nh], qkv[:, :, nh:nh + nkv], qkv[:, :, nh + nkv:]
     if qkv.is_cuda:
         # head dims other than 128 (GPT-2 style / toy configs) and sequence lengths that are not a multiple of
-        # the 128-row tile are outside the sm_100a kernel's scope; use the library kernel rather than the
+        # the 128-row tile are outside the sm_90a kernel's scope; use the library kernel rather than the
         # O(S^2)-memory reference
         o = torch.nn.functional.scaled_dot_product_attention(
             q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=True, scale=scale,

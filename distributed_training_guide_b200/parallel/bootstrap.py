@@ -8,7 +8,7 @@ device_count``, ``set_device``, ``init_process_group(rank, world_size, device_id
 (``02:272-280``), local-rank-0-first (``05-training-llama-405b/train_llm.py:415-423``) and
 ``rank_ordered`` (``06-tensor-parallel/train_llm.py:346-353``).
 
-NCCL (over NVLink 5 / NVSwitch) is the backend on GPUs and carries bootstrap, barriers and
+NCCL (over NVLink / NVSwitch) is the backend on GPUs and carries bootstrap, barriers and
 cold-path collectives; the hot-path collectives are this package's own NVLink kernels
 (``parallel/symm.py``, ``csrc/comm.cu``).  ``gloo`` is used on CPU (tests, toy).
 """

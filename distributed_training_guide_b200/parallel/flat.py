@@ -4,7 +4,7 @@ Every engine in this package (single GPU, DDP, ZeRO-1, FSDP, TP, 2-D) keeps a *g
 parameters (one decoder layer, the embedding, the head) in ONE contiguous buffer, with a
 second contiguous buffer for its gradients:
 
-  * the tcgen05 wgrad GEMM writes straight into the gradient view, so there is no autograd
+  * the wgmma wgrad GEMM writes straight into the gradient view, so there is no autograd
     accumulation pass and no bucket copy (what torch DDP needs ``gradient_as_bucket_view``
     and a C++ Reducer for; reference ``02-distributed-data-parallel/train_llm.py:66-68``);
   * q|k|v and gate|up are adjacent in the buffer, so the fused projections cost nothing;

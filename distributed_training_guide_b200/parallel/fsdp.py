@@ -109,12 +109,11 @@ class FSDPEngine:
         self.tied = bool(getattr(model.config, "tie_word_embeddings", False))
         assert self.is_llama or init_fn is None, "tensor-parallel slices are implemented for the Llama family"
         esize = torch.empty((), dtype=dtype).element_size()
-        # Unshard fused into the consuming GEMMs (csrc/gemm_tcgen05.cu, B_MODE 3): the big matrices of a group are
+        # Unshard fused into the consuming GEMMs (csrc/gemm_wgmma.cu, B_MODE 3): the big matrices of a group are
         # gathered by the GEMM kernel that reads them; only the small tail (norm gains) keeps a prefetched copy.
         # Needs every matrix to start and end on a chunk boundary of the flat layout and every shard to be a whole
         # number of chunks.  Selected with DTG_FSDP_GATHER=gemm; the DEFAULT is the copy-engine unshard of whole groups
-        # ("ce"), which measured faster on 8xB200 (Llama-2-7B: 189.2 ms/step vs 228.2 ms fused, profiles/RESULTS.md):
-        # one 16 KB x 2 bounce ring per CTA does not keep enough NVLink bytes in flight to feed a GEMM that consumes
+        # ("ce"): one 16 KB x 2 bounce ring per CTA does not keep enough NVLink bytes in flight to feed a GEMM that consumes
         # 7/8 remote weights, while the copy engines prefetch a whole layer ahead for free.
         self.fused_gather = (self.use_kernels and self.is_llama and world_size > 1 and esize == 2 and init_fn is None
                              and os.environ.get("DTG_FSDP_GATHER", "ce") == "gemm")
@@ -266,7 +265,7 @@ class FSDPEngine:
         Reference: FSDP2's per-layer all-gather in front of the layer's first matmul and again in backward
         (``fully_shard(layer, reshard_after_forward=True)``, ``04-fully-sharded-data-parallel/train_llm.py:83-90``) and
         the root ``model.unshard()`` prefetch (``04:187-188``): there three NCCL-side kernels per gather (copy-in,
-        all_gather_into_tensor, copy-out), here none — the bytes move inside the consuming tcgen05 GEMM."""
+        all_gather_into_tensor, copy-out), here none — the bytes move inside the consuming wgmma GEMM."""
         self.gather_pads = self.symm.new_pad_set()   # these kernels run on the compute stream: own pad + epochs
         self._counters, self._ngather = {}, {}
         esize = 2

@@ -331,7 +331,7 @@ class FullyShardedDataParallel(Strategy):
 
 class TwoDParallel(Strategy):
     """Chapters 06 / 07: tensor parallel + sequence parallel inside a contiguous ``tp`` group
-    (``parallel/tp.py``: collectives fused into the tcgen05 GEMMs), and — when the data-parallel
+    (``parallel/tp.py``: collectives fused into the wgmma GEMMs), and — when the data-parallel
     size is > 1 — FSDP of the TP-local shards over the strided ``dp`` group (``parallel/fsdp.py``),
     i.e. the 2-D mesh of ``07-2d-parallel/train_llm.py:47-53,121-123``.  The sampler is keyed on
     the dp coordinate so TP peers read identical batches (``06-tensor-parallel/train_llm.py:141-147``)."""

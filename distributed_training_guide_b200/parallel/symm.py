@@ -4,7 +4,7 @@ This is the substrate the reference does not have (it only ever calls NCCL, SURV
 each rank ``cudaMalloc``s the same size outside the caching allocator, exports a CUDA-IPC handle,
 handles are exchanged once through ``torch.distributed`` (NCCL/gloo is used for this bootstrap
 only), and every rank maps its peers' buffers.  Collective *kernels* (``csrc/comm.cu``,
-``csrc/fused_tp.cu``) then load/store peer memory over NVLink 5 / NVSwitch and synchronise with
+``csrc/fused_tp.cu``) then load/store peer memory over NVLink / NVSwitch and synchronise with
 device-side epoch flags in a symmetric signal pad — no host round trips, no NCCL on the hot path.
 
 ``SymmGroup`` also runs on a single rank (N = 1: same kernels, no peers), which is how the

@@ -10,7 +10,7 @@ NCCL all-gather / reduce-scatter / all-to-all sitting on the critical path of ev
 Here the activations between blocks are sequence shards ``[T/t, H]`` living in NVLink-symmetric
 buffers, and the collectives disappear into the tensor-core kernels:
 
-  * column-parallel linear = ONE tcgen05 GEMM kernel in which a few communication CTAs bulk-copy the
+  * column-parallel linear = ONE wgmma GEMM kernel in which a few communication CTAs bulk-copy the
     peers' row tiles over NVLink into the local gathered buffer and publish per-tile flags, while the
     GEMM CTAs start on the local rows and acquire a tile's flag before their TMA reads it (all-gather ->
     GEMM, ``gemm_ag``; a variant that TMA-loads every tile from its owner, ``gemm_dist`` mode 1, re-fetches
@@ -106,7 +106,7 @@ class TPContext:
         T, Tl, H = a.shape[0], self.rpp, self.H
         y = torch.empty(Tl, H, dtype=a.dtype, device=a.device)
         if self.mc_rs:
-            # ONE plain tcgen05 GEMM into my copy of the partial buffer + ONE kernel that barriers and reads my
+            # ONE plain wgmma GEMM into my copy of the partial buffer + ONE kernel that barriers and reads my
             # rows through the multicast address (in-switch fp32 sum) fused with the residual add.  Two buffers
             # alternate: a buffer is rewritten two GEMMs later, after a barrier every rank passed in between.
             pb = self.part[self._part_i]

@@ -25,7 +25,7 @@ CHAPTER_EXTRAS = {
 
 def get_parser(chapter: str = "01-single-gpu", require_experiment: bool = False) -> argparse.ArgumentParser:
     extras = CHAPTER_EXTRAS[chapter]
-    p = argparse.ArgumentParser(description=f"{chapter}: causal-LM training on B200")
+    p = argparse.ArgumentParser(description=f"{chapter}: causal-LM training on H100")
     p.add_argument("-e", "--experiment-name", default=None, required=require_experiment,
                    help="enables checkpointing/resume under <save-dir>/<experiment-name>")
     p.add_argument("-d", "--dataset-name", default=None, required=True,

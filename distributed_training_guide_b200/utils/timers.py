@@ -94,7 +94,7 @@ class LocalTimer:
 
 def device_time_ms(fn, warmup=3, iters=10, flush_l2=True):
     """CUDA-event timing of ``fn`` per the profiling recipe: warm-up, L2 flush between
-    iterations (a 256 MiB write > the 126 MB L2), synchronise on both sides."""
+    iterations (a 256 MiB write > the 50 MB L2), synchronise on both sides."""
     for _ in range(warmup):
         fn()
     torch.cuda.synchronize()

@@ -34,7 +34,7 @@ def test_bench_prints_the_contract_json(capsys):
     import bench
 
     args = SimpleNamespace(gpus=1, steps=2, warmup=3, impl="b200", model="debug-llama", seq_len=64, batch=2,
-                           parallelism="ddp", tensor_parallel=None, layers=None)
+                           parallelism="ddp", tensor_parallel=None, layers=None, dump_outputs=None)
     patches = [mock.patch("torch.cuda.Event", _Ev), mock.patch("torch.cuda.synchronize", lambda *a, **k: None),
                mock.patch("torch.cuda.max_memory_allocated", lambda *a, **k: 0),
                mock.patch.dict("os.environ", {"DTG_PHASE_TIMING": "1", "WORLD_SIZE": "1"})]
@@ -60,13 +60,47 @@ def test_bench_prints_the_contract_json(capsys):
     assert abs(line["value"] - 1000.0 * 2 * 64 / line["ms_per_step"]) < 1e-6 * line["value"]
 
 
+def _bench_dump(out_dir, steps):
+    import bench
+
+    args = SimpleNamespace(gpus=1, steps=steps, warmup=1, impl="b200", model="debug-llama", seq_len=64, batch=1,
+                           parallelism="ddp", tensor_parallel=None, layers=None, dump_outputs=str(out_dir))
+    with contextlib.ExitStack() as es:
+        for p in [mock.patch("torch.cuda.Event", _Ev), mock.patch("torch.cuda.synchronize", lambda *a, **k: None),
+                  mock.patch("torch.cuda.max_memory_allocated", lambda *a, **k: 0),
+                  mock.patch.dict("os.environ", {"WORLD_SIZE": "1"})]:
+            es.enter_context(p)
+        with contextlib.redirect_stdout(io.StringIO()) as buf:
+            bench.run_b200(args)
+    import faulthandler
+
+    faulthandler.cancel_dump_traceback_later()
+    return json.loads([l for l in buf.getvalue().splitlines() if l.startswith("{")][-1])
+
+
+def test_bench_dump_outputs_is_reproducible(tmp_path):
+    """--dump-outputs: the last timed step's loss and a seeded weight sample, float32, identical for identical
+    arguments, and different when --steps changes how many timed steps ran."""
+    import numpy as np
+
+    a = _bench_dump(tmp_path / "a", steps=2)
+    _bench_dump(tmp_path / "b", steps=2)
+    c = _bench_dump(tmp_path / "c", steps=3)
+    assert a["steps"] == 2 and c["steps"] == 3
+    for name in ("loss.npy", "params_sample.npy"):
+        x, y = np.load(tmp_path / "a" / name), np.load(tmp_path / "b" / name)
+        assert x.dtype == np.float32 and x.size > 0 and (tmp_path / "a" / name).stat().st_size < 64 << 20
+        assert np.array_equal(x, y), name
+    assert not np.array_equal(np.load(tmp_path / "a" / "params_sample.npy"), np.load(tmp_path / "c" / "params_sample.npy"))
+
+
 def _bench_rank(rank, world):
     import io
 
     import bench
 
     args = SimpleNamespace(gpus=world, steps=2, warmup=3, impl="b200", model="debug-llama", seq_len=64, batch=1,
-                           parallelism="ddp", tensor_parallel=None, layers=None)
+                           parallelism="ddp", tensor_parallel=None, layers=None, dump_outputs=None)
     buf = io.StringIO()
     with contextlib.ExitStack() as es:
         for p in [mock.patch("torch.cuda.Event", _Ev), mock.patch("torch.cuda.synchronize", lambda *a, **k: None),

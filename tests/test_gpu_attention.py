@@ -1,4 +1,4 @@
-"""tcgen05 flash-attention forward/backward vs an fp32 reference (causal, GQA, head_dim 128)."""
+"""wgmma flash-attention forward/backward vs an fp32 reference (causal, GQA, head_dim 128)."""
 import math
 
 import pytest
@@ -20,7 +20,7 @@ def _rel(a, b):
 @pytest.mark.parametrize("B,S,nh,nkv", [(1, 128, 1, 1), (1, 256, 2, 1), (2, 384, 4, 2), (1, 1024, 8, 2), (1, 2048, 4, 4),
                                         (1, 4096, 32, 4), (2, 640, 8, 1)])
 def test_attention_forward_versions(B, S, nh, nkv, version):
-    """Both forward kernels (1: one query tile per CTA; 2: two tiles per CTA, P in tensor memory) against fp32 —
+    """Both forward kernels (1: P through shared memory; 2: P kept in registers) against fp32 —
     including the bench shape (S 4096, 32 heads, GQA 8:1) and odd numbers of 128-row tiles (384, 640)."""
     torch.manual_seed(0)
     C = _ext.load(True)
@@ -42,7 +42,7 @@ def test_attention_forward_versions(B, S, nh, nkv, version):
 @pytest.mark.parametrize("version", [1, 2])
 def test_attention_forward_row_max_jumps_late(version):
     """Scores whose row maximum grows by far more than the lazy-rescale threshold in LATE key blocks, for SOME rows of
-    a warp only (v2 rescales O in tensor memory with warp-collective tcgen05.ld/st: the decision must be warp-uniform;
+    a warp only (the rescale decision is per row, made by the four threads of a quad;
     random-normal inputs never take that branch after the first block)."""
     torch.manual_seed(3)
     C = _ext.load(True)
@@ -86,7 +86,7 @@ def test_attention_fwd_bwd(B, S, nh, nkv):
 @pytest.mark.parametrize("mode", [1, 2])
 @pytest.mark.parametrize("B,S,nh,nkv", [(1, 256, 2, 1), (1, 1024, 8, 2), (1, 2048, 4, 4), (2, 384, 4, 2)])
 def test_attention_backward_modes(B, S, nh, nkv, mode):
-    """Backward with P / dS staged through shared memory (mode 1) and kept in tensor memory (mode 2, TS-form gradient
+    """Backward with P / dS staged through shared memory (mode 1) and kept in registers (mode 2, RS-form gradient
     MMAs) against the fp32 reference."""
     torch.manual_seed(0)
     C = _ext.load(True)

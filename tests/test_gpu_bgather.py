@@ -1,5 +1,5 @@
-"""FSDP unshard fused into the consuming GEMM (gemm_tcgen05.cu, B_MODE 3): the weight lives in the ranks' flat shards,
-warp 3 of every CTA gathers it into the local full buffer while the tensor cores consume the rows that have arrived.
+"""FSDP unshard fused into the consuming GEMM (gemm_wgmma.cu, B_MODE 3): the weight lives in the ranks' flat shards,
+warp 1 of every CTA gathers it into the local full buffer while the tensor cores consume the rows that have arrived.
 Checked against a plain fp32 matmul of the full weight, forward (B K-major) and dgrad (B MN-major) — needs >= 2 GPUs."""
 import pytest
 import torch

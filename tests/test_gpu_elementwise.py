@@ -1,4 +1,4 @@
-"""sm_100a elementwise / reduction kernels vs the fp32 PyTorch reference of the same op."""
+"""sm_90a elementwise / reduction kernels vs the fp32 PyTorch reference of the same op."""
 import math
 
 import pytest

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (all operand layouts, 1-CTA and 2-CTA variants) vs an fp32 reference."""
+"""wgmma GEMM (all operand layouts, 1-CTA and 2-CTA variants) vs an fp32 reference."""
 import os
 
 import pytest

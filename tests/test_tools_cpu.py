@@ -64,31 +64,6 @@ def test_bench_stage_budgets_fit_the_driver_limit():
     assert total < 870, total
 
 
-def test_reference_arm_environment_shim_restores_rope_init_fn():
-    """baseline/run_ref.py runs the UNMODIFIED reference scripts; chapters 04/05/07 call
-    ``LlamaRotaryEmbedding.rope_init_fn`` after ``to_empty()``, which transformers >= 5 dropped.  The shim (outside the
-    reference tree) restores it with the same contract, and reports itself."""
-    import torch
-
-    sys.path.insert(0, str(ROOT / "baseline"))
-    import run_ref
-
-    applied = run_ref._environment_shims()
-    from transformers import AutoConfig, AutoModelForCausalLM
-    from transformers.models.llama.modeling_llama import LlamaRotaryEmbedding
-
-    assert hasattr(LlamaRotaryEmbedding, "rope_init_fn")
-    cfg = AutoConfig.for_model("llama", vocab_size=128, hidden_size=64, intermediate_size=128, num_hidden_layers=1,
-                               num_attention_heads=2, num_key_value_heads=2)
-    with torch.device("meta"):
-        m = AutoModelForCausalLM.from_config(cfg)
-    m.to_empty(device="cpu")
-    rot = m.model.rotary_emb
-    inv_freq, scaling = rot.rope_init_fn(rot.config, "cpu")          # what the reference's reset_rope does
-    assert inv_freq.shape == (cfg.hidden_size // cfg.num_attention_heads // 2,) and float(scaling) == 1.0
-    assert all(isinstance(a, str) for a in applied)
-
-
 def test_both_bench_arms_describe_the_same_config():
     """The driver compares the two arms' ``config`` dicts: same model / batch / sequence / mesh strings from one helper."""
     from types import SimpleNamespace

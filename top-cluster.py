@@ -6,7 +6,7 @@ a dead worker as a drop in the process count (see diagnosing-errors/README.md).
 
     python top-cluster.py hosts [--poll-freq 1000] [--once] [--local]
 
-Same purpose and CLI as the reference's top-cluster.py; written for B200 nodes (1 kW power limit).
+Same purpose and CLI as the reference's top-cluster.py.
 """
 import argparse
 import concurrent.futures as cf
