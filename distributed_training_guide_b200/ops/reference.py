@@ -2,7 +2,9 @@
 
 These serve two roles and are never a second GPU backend:
   * the CPU execution path (chapter 01's GPT-2 plumbing config, all ``gloo`` tests);
-  * the numerics oracle the CUDA kernels are tested against (``tests/test_kernels_gpu.py``).
+  * the numerics oracle the CUDA kernels are tested against (``tests/test_gpu_elementwise.py``,
+    ``tests/test_gpu_attention.py``, ``tests/test_gpu_gemm.py``; ``tests/test_gpu_step_reference.py`` runs a
+    whole fp32 model on them against the training step).
 
 Semantics follow what the reference guide gets from ``transformers`` (SURVEY.md §3.2 /
 K1-K9): RMSNorm with fp32 statistics, half-rotation RoPE, causal softmax attention
@@ -102,8 +104,11 @@ def shift_labels(labels):
 
 
 def cross_entropy(logits, targets, ignore_index=-100):
-    """logits [T, V] (any float dtype), targets [T] already shifted -> mean loss (fp32)."""
-    return F.cross_entropy(logits.float(), targets, ignore_index=ignore_index, reduction="mean")
+    """logits [T, V] (any float dtype), targets [T] already shifted -> mean loss (fp32) over the targets that are
+    not ``ignore_index``.  With none left (a chunk of padding) the loss is 0 with a zero gradient, as in the CUDA
+    kernel, where ``reduction="mean"`` would give NaN."""
+    total = F.cross_entropy(logits.float(), targets, ignore_index=ignore_index, reduction="sum")
+    return total / (targets != ignore_index).sum().clamp(min=1)
 
 
 def embedding(ids, w):

@@ -19,6 +19,23 @@ from torch.distributed.elastic.multiprocessing.errors import record
 STATE = os.environ.get("TOY_STATE_FILE", "./toy-state.json")
 
 
+def init_process_group(timeout):
+    """gloo process group of this attempt, with its store keys under a per-attempt prefix.
+
+    torchrun hands its workers the TCPStore of its own rendezvous and keeps that store across restarts, so the
+    keys a failed attempt wrote (among them the listening address of every gloo peer) are still there when the
+    restarted gang sets up.  A worker can then read a dead peer's address and fail to connect ("Connection
+    refused"; the next attempt may hang on a stale counter instead), which burns the restarts.  Prefixing every
+    key with the restart count gives each attempt a clean namespace."""
+    rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
+    # without the shared store (TORCH_DISABLE_SHARE_RDZV_TCP_STORE=1) rank 0 hosts a fresh store per attempt
+    hosted_by_agent = os.environ.get("TORCHELASTIC_USE_AGENT_STORE") == "True"
+    store = dist.TCPStore(os.environ["MASTER_ADDR"], int(os.environ["MASTER_PORT"]), world,
+                          is_master=not hosted_by_agent and rank == 0, timeout=timeout)
+    store = dist.PrefixStore(f"toy/attempt_{os.environ.get('TORCHELASTIC_RESTART_COUNT', '0')}", store)
+    dist.init_process_group(backend="gloo", store=store, rank=rank, world_size=world, timeout=timeout)
+
+
 @record
 def main():
     ap = argparse.ArgumentParser()
@@ -31,7 +48,7 @@ def main():
 
     import datetime
 
-    dist.init_process_group(backend="gloo", timeout=datetime.timedelta(seconds=120))
+    init_process_group(datetime.timedelta(seconds=120))
     rank, world = dist.get_rank(), dist.get_world_size()
     state = {"num_steps": 0}
     if os.path.exists(STATE):

@@ -1,12 +1,10 @@
-"""The elastic toy under torchrun: state-file resume across launches, and (best effort) an injected
-failure followed by a gang restart."""
+"""The elastic toy under torchrun: state-file resume across launches, and an injected failure followed by a
+gang restart."""
 import json
 import os
 import subprocess
 import sys
 from pathlib import Path
-
-import pytest
 
 ROOT = Path(__file__).resolve().parent.parent
 TOY = str(ROOT / "related-topics" / "elastic-training" / "toy.py")
@@ -32,11 +30,11 @@ def test_toy_resumes_from_state_file(tmp_path):
 
 
 def test_toy_injected_failure_restarts(tmp_path):
-    try:
-        r = _launch(tmp_path, ["--steps", "20", "--fail-at-steps", "7"], 75)
-    except subprocess.TimeoutExpired:
-        pytest.skip("gloo re-rendezvous after a torchrun restart is slow on this host")
+    """One restart must be enough: the restarted gang sets up its process group in a store namespace of its own, so
+    no worker reads an address or counter the failed attempt left behind (which failed or hung about one run in
+    three before)."""
+    r = _launch(tmp_path, ["--steps", "20", "--fail-at-steps", "7"], 300)
     out = r.stdout + r.stderr
-    if r.returncode != 0:
-        pytest.skip("torchrun exhausted its restarts on gloo reconnect errors")
+    assert r.returncode == 0, out[-2000:]
     assert "injected failure" in out and "resuming at step 7" in out and "finished 20 steps" in out
+    assert "restart count=1" in out and "restart count=2" not in out, out[-2000:]

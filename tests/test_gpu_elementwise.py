@@ -108,6 +108,36 @@ def test_cross_entropy(T, V):
     _close(logits.grad * T, 0.5 * lf.grad * T, 2e-3, 3e-2, "dlogits*0.5")
 
 
+@pytest.mark.parametrize("case", ["all_ignored", "first_and_last_column", "one_row", "std20"])
+def test_cross_entropy_edges(case):
+    """Edges against fp64, every element within tolerance (no outlier budget): no valid target at all (loss 0 and
+    zero dlogits, not NaN), targets in the first and last column, a single row, logits with std 20."""
+    T, V, std = {"all_ignored": (64, 1024, 2.0), "first_and_last_column": (128, 32000, 2.0),
+                 "one_row": (1, 128256, 2.0), "std20": (256, 32000, 20.0)}[case]
+    torch.manual_seed(0)
+    logits = (std * torch.randn(T, V, device=DEV)).to(torch.bfloat16)
+    tgt = torch.randint(0, V, (T,), device=DEV)
+    if case == "all_ignored":
+        tgt.fill_(-100)
+    elif case == "first_and_last_column":
+        tgt[0::2], tgt[1::2] = 0, V - 1
+    n_valid = int((tgt != -100).sum())
+    lf = logits.double().requires_grad_(True)
+    want = torch.nn.functional.cross_entropy(lf, tgt, ignore_index=-100, reduction="sum") / max(n_valid, 1)
+    want.backward()
+    x = logits.clone().requires_grad_(True)
+    loss = ops.cross_entropy(x * 1.0, tgt)   # the op overwrites its input with dlogits
+    loss.backward()
+    assert torch.isfinite(loss) and torch.isfinite(x.grad).all(), (loss.item(), case)
+    assert abs(loss.item() - want.item()) <= 1e-4 * max(1.0, abs(want.item())), (loss.item(), want.item())
+    err = (x.grad.double() - lf.grad).abs()
+    tol = 1e-6 / max(n_valid, 1) + 8e-3 * lf.grad.abs()   # 8e-3: two bf16 ulps
+    bad = err > tol
+    assert not bad.any(), f"{case}: {int(bad.sum())} of {err.numel()} dlogits out of tolerance, max err {err.max():.3g}"
+    if case == "all_ignored":
+        assert loss.item() == 0.0 and int(torch.count_nonzero(x.grad)) == 0
+
+
 @pytest.mark.parametrize("T,V,H", [(256, 1000, 256), (4096, 32000, 4096)])
 def test_embedding(T, V, H):
     torch.manual_seed(0)

@@ -62,3 +62,18 @@ def test_registry_parameter_counts():
     assert abs(get_config("meta-llama/Meta-Llama-3-8B").num_parameters() / 1e9 - 8.030) < 0.01
     assert abs(get_config("meta-llama/Meta-Llama-3-70B").num_parameters() / 1e9 - 70.554) < 0.01
     assert abs(get_config("meta-llama/Llama-3.1-405B").num_parameters() / 1e9 - 405.85) < 0.1
+
+
+def test_cross_entropy_without_valid_targets_is_zero():
+    """The CPU path agrees with the CUDA kernel when every target is ignored: loss 0, zero gradient, no NaN; with
+    valid targets it is the usual mean."""
+    from distributed_training_guide_b200 import ops
+
+    torch.manual_seed(0)
+    logits = torch.randn(4, 16, requires_grad=True)
+    loss = ops.cross_entropy(logits, torch.full((4,), -100))
+    loss.backward()
+    assert loss.item() == 0.0 and int(torch.count_nonzero(logits.grad)) == 0
+    tgt = torch.tensor([1, -100, 3, 15])
+    want = torch.nn.functional.cross_entropy(logits, tgt, ignore_index=-100)
+    assert torch.allclose(ops.cross_entropy(logits, tgt), want, rtol=1e-6, atol=0)
