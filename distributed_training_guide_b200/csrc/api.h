@@ -41,6 +41,11 @@ void adamw_flat(void* p, const void* g, void* m, void* v, long long n, float lr,
 void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
                bool a_kmajor, bool b_kmajor, bool accumulate, int variant, cudaStream_t s);
 
+// C[M,N] (+)= scale_a[0] * scale_b[0] * A8[M,K] . B8[N,K]^T with fp8 operands (A e4m3, or e5m2 when a_e5m2; B e4m3),
+// both K-major; scale_a / scale_b are device pointers.  N, lda, ldb and ldc must be multiples of 16.
+void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
+              bool a_e5m2, const float* scale_a, const float* scale_b, bool accumulate, int variant, cudaStream_t s);
+
 int gemm_max_active_clusters(int cg);
 // tensor-parallel variants over symmetric buffers (see gemm_wgmma.cu)
 void gemm_bf16_dist(int mode, const void* const* a_srcs, const void* const* b_srcs, void* const* c_dsts, int M, int N,
@@ -54,6 +59,14 @@ void gemm_bf16_bgather(const void* A, void* full_base, void* C, int M, int N, in
 void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int N, int K, long long ldb, long long ldc,
                   bool b_kmajor, int nranks, int rank, int rows_per_peer, uint32_t* flags, uint32_t ag_epoch,
                   uint32_t* const* pads, uint32_t bar_epoch, int n_comm, cudaStream_t s);
+
+// ---- fp8.cu --------------------------------------------------------------------------------
+// amax[0] = max |x| of a bf16 [R, C] matrix with row stride ld (elements), on the device.
+void fp8_amax(const void* x, long long R, int C, long long ld, float* amax, cudaStream_t s);
+// q = satfinite(x * scale) in e4m3 (or e5m2), scale = amax == 0 ? 1 : FP8_MAX / amax, written row-major to `out`
+// [R, C] and / or transposed to `out_t` [C, R] (either may be null); scale_inv[0] = 1 / scale.
+void fp8_cast_transpose(const void* x, long long ld, int R, int C, bool e5m2, const float* amax, void* out, void* out_t,
+                        float* scale_inv, cudaStream_t s);
 
 // ---- attention_fwd.cu / attention_bwd.cu ---------------------------------------------------
 // qkv: [B,S,nh+2*nkv,128] bf16 (q heads | k heads | v heads); o: [B,S,nh,128]; lse: [B,nh,S] fp32

@@ -38,6 +38,65 @@ void gemm(const Tensor& a, const Tensor& b, Tensor& out, bool trans_a, bool tran
                  /*a_kmajor=*/!trans_a, /*b_kmajor=*/trans_b, accumulate, variant, stream());
 }
 
+void check_fp8_2d(const Tensor& t, const char* name) {
+  TORCH_CHECK(t.is_cuda(), name, " must be a CUDA tensor");
+  TORCH_CHECK(t.scalar_type() == at::kFloat8_e4m3fn || t.scalar_type() == at::kFloat8_e5m2, name,
+              " must be float8_e4m3fn or float8_e5m2");
+  TORCH_CHECK(t.dim() == 2, name, " must be 2-D");
+  TORCH_CHECK(t.stride(1) == 1, name, " must have a contiguous last dimension");
+}
+void check_scalar_f32(const Tensor& t, const char* name) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat && t.numel() == 1, name,
+              " must be a one-element float32 CUDA tensor");
+}
+
+// out[M,N] (+)= scale_a * scale_b * a[M,K] @ b[N,K]^T; a e4m3 or e5m2, b e4m3; the scales stay on the device
+void gemm_fp8(const Tensor& a, const Tensor& b, Tensor& out, const Tensor& scale_a, const Tensor& scale_b,
+              bool accumulate, int variant) {
+  check_fp8_2d(a, "a");
+  check_fp8_2d(b, "b");
+  check_bf16_2d(out, "out");
+  TORCH_CHECK(b.scalar_type() == at::kFloat8_e4m3fn, "gemm_fp8: b must be float8_e4m3fn");
+  check_scalar_f32(scale_a, "scale_a");
+  check_scalar_f32(scale_b, "scale_b");
+  const c10::cuda::CUDAGuard guard(a.device());
+  const int M = (int)a.size(0), K = (int)a.size(1), N = (int)b.size(0);
+  TORCH_CHECK(b.size(1) == K, "gemm_fp8: inner dimensions differ (", K, " vs ", b.size(1), ")");
+  TORCH_CHECK(out.size(0) == M && out.size(1) == N, "gemm_fp8: out has the wrong shape");
+  dtg::gemm_fp8(a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0), out.stride(0),
+                a.scalar_type() == at::kFloat8_e5m2, scale_a.data_ptr<float>(), scale_b.data_ptr<float>(), accumulate,
+                variant, stream());
+}
+
+Tensor fp8_amax(const Tensor& x) {
+  check_bf16_2d(x, "x");
+  const c10::cuda::CUDAGuard guard(x.device());
+  Tensor amax = torch::empty({1}, x.options().dtype(at::kFloat));
+  dtg::fp8_amax(x.data_ptr(), x.size(0), (int)x.size(1), x.stride(0), amax.data_ptr<float>(), stream());
+  return amax;
+}
+
+// (x8 [R,C] or None, x8^T [C,R] or None, scale_inv [1]) of a bf16 [R,C] matrix given its device amax
+std::tuple<c10::optional<Tensor>, c10::optional<Tensor>, Tensor> fp8_cast_transpose(const Tensor& x, const Tensor& amax,
+                                                                                    bool e5m2, bool rowwise,
+                                                                                    bool transposed) {
+  check_bf16_2d(x, "x");
+  check_scalar_f32(amax, "amax");
+  TORCH_CHECK(rowwise || transposed, "fp8_cast_transpose: ask for at least one layout");
+  TORCH_CHECK(x.numel() > 0, "fp8_cast_transpose: empty tensor");
+  const c10::cuda::CUDAGuard guard(x.device());
+  const auto dt = e5m2 ? at::kFloat8_e5m2 : at::kFloat8_e4m3fn;
+  const int64_t R = x.size(0), C = x.size(1);
+  c10::optional<Tensor> out, out_t;
+  if (rowwise) out = torch::empty({R, C}, x.options().dtype(dt));
+  if (transposed) out_t = torch::empty({C, R}, x.options().dtype(dt));
+  Tensor scale_inv = torch::empty({1}, x.options().dtype(at::kFloat));
+  dtg::fp8_cast_transpose(x.data_ptr(), x.stride(0), (int)R, (int)C, e5m2, amax.data_ptr<float>(),
+                          out ? out->data_ptr() : nullptr, out_t ? out_t->data_ptr() : nullptr,
+                          scale_inv.data_ptr<float>(), stream());
+  return {out, out_t, scale_inv};
+}
+
 std::tuple<Tensor, Tensor, c10::optional<Tensor>> rmsnorm_fwd(const Tensor& x, const Tensor& w, double eps,
                                                               const c10::optional<Tensor>& res) {
   check_contig(x, "x", at::kBFloat16);
@@ -179,7 +238,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("launch_count", []() { return (uint64_t)dtg::launch_count(); });
   m.def("gemm", &gemm, py::arg("a"), py::arg("b"), py::arg("out"), py::arg("trans_a") = false,
         py::arg("trans_b") = false, py::arg("accumulate") = false, py::arg("variant") = 0);
-  m.def("gemm_max_active_clusters", [](int cg) { return dtg::gemm_max_active_clusters(cg); });
+  m.def("gemm_fp8", &gemm_fp8, py::arg("a"), py::arg("b"), py::arg("out"), py::arg("scale_a"), py::arg("scale_b"),
+        py::arg("accumulate") = false, py::arg("variant") = 0);
+  m.def("fp8_amax", &fp8_amax);
+  m.def("fp8_cast_transpose", &fp8_cast_transpose, py::arg("x"), py::arg("amax"), py::arg("e5m2"),
+        py::arg("rowwise") = true, py::arg("transposed") = true);
+  m.def("gemm_max_active_clusters",[](int cg) { return dtg::gemm_max_active_clusters(cg); });
   m.def("rmsnorm_fwd", &rmsnorm_fwd);
   m.def("rmsnorm_bwd", &rmsnorm_bwd);
   m.def("rope_inplace", &rope_inplace);

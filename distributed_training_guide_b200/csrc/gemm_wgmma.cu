@@ -52,13 +52,21 @@ __device__ __forceinline__ int bg_rotation_chunks(const GemmDist& d) {   // firs
   return (int)((bg_clamp(d, (long long)(d.rank + 1) * d.bg_per_bytes) - d.bg_begin) >> d.bg_chunk_shift);
 }
 
-template <bool A_K, bool B_K, int CG, int A_MODE = 0, int B_MODE = 0, int C_MODE = 0>
+// ET selects the operand element type: 0 = bf16 (every mode above); 1 = fp8, A e4m3 and B e4m3; 2 = fp8, A e5m2 and B
+// e4m3.  The fp8 forms take both operands K-major and plain (mode 0): the fp8 wgmma has no transposed operands, so
+// the caller passes transposed copies.  A stage then holds a K block of 128 fp8 elements, which is the same 128-byte
+// swizzle span, stage size and descriptor stepping as 64 bf16 elements, and the epilogue multiplies the fp32
+// accumulators by the two per-tensor dequantisation scales `scale_a[0] * scale_b[0]`, read from device memory.
+template <bool A_K, bool B_K, int CG, int A_MODE = 0, int B_MODE = 0, int C_MODE = 0, int ET = 0>
 __global__ void __launch_bounds__(GemmCfg<CG>::THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
                  const __grid_constant__ TmapSet<(B_MODE ? kMaxRanks : 1)> tmBs, const __grid_constant__ GemmDist dist,
                  __nv_bfloat16* __restrict__ C, int M, int N, int K, long long ldc, int accumulate, int num_m_tiles,
-                 int num_tiles) {
+                 int num_tiles, const float* __restrict__ scale_a, const float* __restrict__ scale_b) {
+  static_assert(ET == 0 || (A_K && B_K && A_MODE == 0 && B_MODE == 0 && C_MODE == 0),
+                "the fp8 GEMM takes K-major operands from one tensor map each");
   using Cfg = GemmCfg<CG>;
+  constexpr int BK = ET ? 2 * Cfg::BK : Cfg::BK;   // elements of K per stage: one 128-byte span either way
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
@@ -73,7 +81,7 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
   const bool is_comm = (A_MODE == 3) && (int)(blockIdx.x / CG) < n_comm;
   const int cluster_id = (int)(blockIdx.x / CG) - n_comm;       // index among the GEMM clusters
   const int num_clusters = (int)(gridDim.x / CG) - n_comm;
-  const int num_kb = (K + Cfg::BK - 1) / Cfg::BK;
+  const int num_kb = (K + BK - 1) / BK;
   const int local_m_tiles = (A_MODE == 3) ? dist.rows_per_peer / (Cfg::BM * CG) : 0;
 
   if (threadIdx.x == 0) {
@@ -202,7 +210,7 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
         for (int kbi = 0; kbi < num_kb; ++kbi) {
           // K-gathered operands start with the local rank's slice of K
           const int kb = (A_MODE == 2 || B_MODE == 2 || (B_MODE == 3 && !B_K)) ? (kbi + dist.k_shift) % num_kb : kbi;
-          const int k0 = kb * Cfg::BK;
+          const int k0 = kb * BK;
           int a_k0 = k0, b_k0 = k0;
           const CUtensorMap* tmB_p = &tmBs.m[0];
           if constexpr (A_MODE == 2) {
@@ -347,11 +355,17 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
         const uint32_t b_base = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
         wgmma_fence();
         fence_regs(acc);
+        if constexpr (ET == 0) {
 #pragma unroll
-        for (int k = 0; k < Cfg::BK / 16; ++k) {
-          const uint64_t da = A_K ? desc_kmajor_sw128(a_base + k * 32) : desc_mnmajor_sw128(a_base + k * 2048, 8192);
-          const uint64_t db = B_K ? desc_kmajor_sw128(b_base + k * 32) : desc_mnmajor_sw128(b_base + k * 2048, 8192);
-          wgmma_m64n256k16_ss<A_K ? 0 : 1, B_K ? 0 : 1>(acc, da, db, 1u);
+          for (int k = 0; k < Cfg::BK / 16; ++k) {
+            const uint64_t da = A_K ? desc_kmajor_sw128(a_base + k * 32) : desc_mnmajor_sw128(a_base + k * 2048, 8192);
+            const uint64_t db = B_K ? desc_kmajor_sw128(b_base + k * 32) : desc_mnmajor_sw128(b_base + k * 2048, 8192);
+            wgmma_m64n256k16_ss<A_K ? 0 : 1, B_K ? 0 : 1>(acc, da, db, 1u);
+          }
+        } else {
+#pragma unroll
+          for (int k = 0; k < BK / 32; ++k)
+            wgmma_m64n256k32_fp8_ss<ET>(acc, desc_kmajor_sw128(a_base + k * 32), desc_kmajor_sw128(b_base + k * 32), 1u);
         }
         wgmma_commit();
         wgmma_wait<1>();              // the previous stage's MMAs have retired: hand its buffers back
@@ -363,7 +377,9 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
       wgmma_wait<0>();
       fence_regs(acc);
       if (prev >= 0) release(prev);
-      // epilogue: accumulator fragment -> bf16 pairs -> global
+      // epilogue: accumulator fragment (x dequantisation scale, fp8) -> bf16 pairs -> global
+      [[maybe_unused]] float deq = 1.f;
+      if constexpr (ET != 0) deq = scale_a[0] * scale_b[0];
       const int r0 = m0 + wq * 16 + (lane >> 2);
       const int c0 = n0 + 2 * (lane & 3);
 #pragma unroll
@@ -380,6 +396,10 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
           const int col = c0 + 8 * j;
           if (col < N) {
             float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
+            if constexpr (ET != 0) {
+              x *= deq;
+              y *= deq;
+            }
             __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(crow + col);
             if (accumulate) {
               const float2 g = __bfloat1622float2(*p);
@@ -412,8 +432,8 @@ static PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
   return fn;
 }
 
-CUtensorMap make_tmap_bf16(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                           const uint32_t* box, bool swizzle128) {
+static CUtensorMap make_tmap_typed(CUtensorMapDataType dtype, const void* base, int rank, const uint64_t* dims,
+                                   const uint64_t* strides_bytes, const uint32_t* box, bool swizzle128) {
   // The driver entry point needs a current context; autograd worker threads may reach this before
   // any runtime call has bound the primary context to them.
   static thread_local bool ctx_bound = false;
@@ -434,7 +454,7 @@ CUtensorMap make_tmap_bf16(const void* base, int rank, const uint64_t* dims, con
     estr[i] = 1;
     if (i > 0) gstr[i - 1] = strides_bytes[i - 1];
   }
-  CUresult r = get_encode_fn()(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim,
+  CUresult r = get_encode_fn()(&m, dtype, (cuuint32_t)rank, const_cast<void*>(base), gdim,
                                gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                                swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
                                CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -445,12 +465,26 @@ CUtensorMap make_tmap_bf16(const void* base, int rank, const uint64_t* dims, con
   return m;
 }
 
+CUtensorMap make_tmap_bf16(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                           const uint32_t* box, bool swizzle128) {
+  return make_tmap_typed(CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, base, rank, dims, strides_bytes, box, swizzle128);
+}
+
 CUtensorMap make_tmap_2d(const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes, uint32_t box_inner,
                          uint32_t box_outer) {
   uint64_t dims[2] = {inner, outer};
   uint64_t strides[1] = {row_stride_bytes};
   uint32_t box[2] = {box_inner, box_outer};
   return make_tmap_bf16(base, 2, dims, strides, box, true);
+}
+
+// 2-D map of 1-byte elements (fp8 operands), 128B swizzle
+static CUtensorMap make_tmap_2d_u8(const void* base, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
+                                   uint32_t box_inner, uint32_t box_outer) {
+  uint64_t dims[2] = {inner, outer};
+  uint64_t strides[1] = {row_stride_bytes};
+  uint32_t box[2] = {box_inner, box_outer};
+  return make_tmap_typed(CU_TENSOR_MAP_DATA_TYPE_UINT8, base, 2, dims, strides, box, true);
 }
 
 static int g_gemm_variant = 0;  // 0 = env/default
@@ -467,29 +501,32 @@ int default_gemm_variant() {
 
 // One launcher for the plain and the tensor-parallel GEMMs.  `a_srcs` / `b_srcs`: base pointer of the
 // operand on every rank (only [0] is used in mode 0); `dist.c_ptr` set by the caller for C_MODE 1.
-template <bool A_K, bool B_K, int CG, int A_MODE, int B_MODE, int C_MODE>
+template <bool A_K, bool B_K, int CG, int A_MODE, int B_MODE, int C_MODE, int ET = 0>
 static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, void* C, int M, int N, int K,
                         long long lda, long long ldb, long long ldc, bool accumulate, GemmDist dist, int nranks,
-                        cudaStream_t s) {
+                        cudaStream_t s, const float* scale_a = nullptr, const float* scale_b = nullptr) {
   using Cfg = GemmCfg<CG>;
+  constexpr int ESIZE = ET ? 1 : 2;   // bytes per operand element
   TmapSet<(A_MODE ? kMaxRanks : 1)> tmA;
   TmapSet<(B_MODE ? kMaxRanks : 1)> tmB;
   const int rpp = dist.rows_per_peer;
   for (int p = 0; p < ((A_MODE == 1 || A_MODE == 2) ? nranks : 1); ++p) {
     const int rows = (A_MODE == 1) ? rpp : M;   // M extent of this source (mode 3: the local gathered buffer)
     const int ks = (A_MODE == 2) ? rpp : K;     // K extent of this source
-    tmA.m[p] = A_K ? make_tmap_2d(a_srcs[p], ks, rows, lda * 2, 64, Cfg::BM) : make_tmap_2d(a_srcs[p], rows, ks, lda * 2, 64, 64);
+    if constexpr (ET != 0) tmA.m[p] = make_tmap_2d_u8(a_srcs[p], ks, rows, lda, 128, Cfg::BM);
+    else tmA.m[p] = A_K ? make_tmap_2d(a_srcs[p], ks, rows, lda * 2, 64, Cfg::BM) : make_tmap_2d(a_srcs[p], rows, ks, lda * 2, 64, 64);
   }
   for (int p = 0; p < ((B_MODE == 1 || B_MODE == 2) ? nranks : 1); ++p) {
     const int ks = (B_MODE == 2) ? rpp : K;
-    tmB.m[p] = B_K ? make_tmap_2d(b_srcs[p], ks, N, ldb * 2, 64, Cfg::B_ROWS) : make_tmap_2d(b_srcs[p], N, ks, ldb * 2, 64, 64);
+    if constexpr (ET != 0) tmB.m[p] = make_tmap_2d_u8(b_srcs[p], ks, N, ldb, 128, Cfg::B_ROWS);
+    else tmB.m[p] = B_K ? make_tmap_2d(b_srcs[p], ks, N, ldb * 2, 64, Cfg::B_ROWS) : make_tmap_2d(b_srcs[p], N, ks, ldb * 2, 64, 64);
   }
   for (int p = ((A_MODE == 1 || A_MODE == 2) ? nranks : 1); p < (A_MODE ? kMaxRanks : 1); ++p) tmA.m[p] = tmA.m[0];
   for (int p = ((B_MODE == 1 || B_MODE == 2) ? nranks : 1); p < (B_MODE ? kMaxRanks : 1); ++p) tmB.m[p] = tmB.m[0];
   const int num_m_tiles = (M + Cfg::BM * CG - 1) / (Cfg::BM * CG);
   const int num_n_tiles = (N + Cfg::BN - 1) / Cfg::BN;
   const int num_tiles = num_m_tiles * num_n_tiles;
-  auto kern = gemm_bf16_kernel<A_K, B_K, CG, A_MODE, B_MODE, C_MODE>;
+  auto kern = gemm_bf16_kernel<A_K, B_K, CG, A_MODE, B_MODE, C_MODE, ET>;
   constexpr int kSmem = Cfg::SMEM_BYTES + (B_MODE == 3 ? Cfg::GATHER_BYTES : 0);
   static bool attr_set = false;
   if (!attr_set) {
@@ -498,14 +535,14 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
   }
   dist.num_n_tiles = num_n_tiles;
   if constexpr (A_MODE == 0 && B_MODE == 0 && C_MODE == 0) {
-    // keep one group's panel of A (group_m x TM x K bf16) within ~1/3 of the 50 MB L2; with very long K nothing
+    // keep one group's panel of A (group_m x TM x K elements) within ~1/3 of the 50 MB L2; with very long K nothing
     // fits and a squarish block of 8 row tiles by (tiles in flight / 8) column tiles minimises the bytes each
     // wave touches
     static const long long budget = []() {
       const char* e = getenv("DTG_GEMM_L2_BUDGET_MB");
       return (long long)(e ? atoi(e) : 16) << 20;
     }();
-    const long long panel = (long long)Cfg::BM * CG * K * 2;
+    const long long panel = (long long)Cfg::BM * CG * K * ESIZE;
     long long gm = budget / (panel > 0 ? panel : 1);
     if (gm < 8) gm = 8;
     dist.group_m = gm >= num_m_tiles ? 0 : (int)gm;
@@ -532,7 +569,7 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
   cfg.attrs = attrs;
   cfg.numAttrs = 1;
   DTG_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, dist, (__nv_bfloat16*)C, M, N, K, ldc, accumulate ? 1 : 0,
-                                    num_m_tiles, num_tiles));
+                                    num_m_tiles, num_tiles, scale_a, scale_b));
   note_launch();
 }
 
@@ -586,6 +623,35 @@ void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long 
   DTG_GEMM_CASE(false, false)
   DTG_GEMM_CASE(false, true)
 #undef DTG_GEMM_CASE
+}
+
+// C[M,N] (+)= scale_a[0] * scale_b[0] * A8[M,K] . B8[N,K]^T: per-tensor scaled fp8 operands, both stored row-major
+// with K contiguous (lda / ldb in elements = bytes), fp32 accumulators, bf16 C with row stride ldc.  A is e4m3, or
+// e5m2 when `a_e5m2` (an output gradient); B is e4m3.  The scales are device pointers, so nothing here waits on the
+// kernels that computed them.
+void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
+              bool a_e5m2, const float* scale_a, const float* scale_b, bool accumulate, int variant, cudaStream_t s) {
+  if (M <= 0 || N <= 0 || K <= 0) return;
+  if ((N % 16) || (lda % 16) || (ldb % 16) || (ldc % 16))
+    throw std::runtime_error("gemm_fp8: N and the leading dimensions must be multiples of 16 elements (TMA needs "
+                             "16-byte row strides of the fp8 operands)");
+  if (variant == 0) variant = default_gemm_variant();
+  if (variant == 3) variant = (M > 128) ? 2 : 1;
+  const int cg = (variant == 2) ? 2 : 1;
+  const void* as[1] = {A};
+  const void* bs[1] = {B};
+  GemmDist dist{};
+#define DTG_GEMM_FP8_CASE(ET)                                                                                     \
+  if (cg == 2) launch_gemm<true, true, 2, 0, 0, 0, ET>(as, bs, C, M, N, K, lda, ldb, ldc, accumulate, dist, 1, s,  \
+                                                       scale_a, scale_b);                                        \
+  else launch_gemm<true, true, 1, 0, 0, 0, ET>(as, bs, C, M, N, K, lda, ldb, ldc, accumulate, dist, 1, s, scale_a, \
+                                               scale_b);
+  if (a_e5m2) {
+    DTG_GEMM_FP8_CASE(2)
+  } else {
+    DTG_GEMM_FP8_CASE(1)
+  }
+#undef DTG_GEMM_FP8_CASE
 }
 
 // Tensor-parallel GEMMs over NVLink symmetric buffers (always the CTA-pair kernel).

@@ -186,6 +186,7 @@ class LlamaDecoderLayer(nn.Module):
         self.post_attention_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
         self._fused = {}  # name -> FusedWeight, installed by parallel.flat.FlatParamGroup
         self.tp = None  # installed by parallel.tp.apply_tensor_parallel
+        self.fp8 = False  # set through LlamaForCausalLM.fp8: the four projections run ops.fp8_linear
 
     # fused weights -------------------------------------------------------------------
     def _qkv_weight(self):
@@ -208,16 +209,18 @@ class LlamaDecoderLayer(nn.Module):
         Returns (mlp_out, residual) with the final add again deferred to the consumer."""
         att = self.self_attn
         B, S, _ = x.shape
+        fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
         y, h = self.input_layernorm(x, residual)
         w, owner = self._qkv_weight()
-        qkv = ops.fused_linear(y, w, owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
+        qkv = fused_linear(y, w, owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
         qkv = ops.rope_qkv_(qkv, cos, sin, att.num_heads + att.num_kv_heads)
         a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads).reshape(B, S, att.num_heads * att.head_dim)
-        a = att.o_proj(a)
+        a = ops.fp8_linear(a, att.o_proj.weight) if self.fp8 else att.o_proj(a)
         y, h = self.post_attention_layernorm(a, h)
         w, owner = self._gate_up_weight()
-        act = ops.swiglu(ops.fused_linear(y, w, owner))
-        return self.mlp.down_proj(act), h
+        act = ops.swiglu(fused_linear(y, w, owner))
+        down = ops.fp8_linear(act, self.mlp.down_proj.weight) if self.fp8 else self.mlp.down_proj(act)
+        return down, h
 
 
 class LlamaModel(nn.Module):
@@ -252,6 +255,19 @@ class LlamaForCausalLM(nn.Module):
         self.engine = None
         self.activation_checkpointing = False
         self.tp = None
+        self.fp8 = False
+
+    @property
+    def fp8(self) -> bool:
+        """Run the decoder-layer projections (q|k|v, o, gate|up, down) through ``ops.fp8_linear``: fp8 GEMMs with
+        per-tensor current scaling.  The lm_head, embedding, attention, norms and loss stay bf16."""
+        return self._fp8
+
+    @fp8.setter
+    def fp8(self, on: bool):
+        self._fp8 = bool(on)
+        for layer in self.model.layers:
+            layer.fp8 = self._fp8
 
     # -- initialisation -----------------------------------------------------------------
     @torch.no_grad()

@@ -1,7 +1,8 @@
 """Op layer: every hot op of the Llama training step as an ``autograd.Function``.
 
 On CUDA tensors each op calls a hand-written sm_90a kernel from the in-tree
-extension (``csrc/``): wgmma/TMA GEMM (fwd / dgrad / wgrad), wgmma
+extension (``csrc/``): wgmma/TMA GEMM (fwd / dgrad / wgrad) in bf16 and, for
+``fp8_linear``, in fp8 with its amax and cast-transpose kernels, wgmma
 flash-attention, fused residual-add+RMSNorm, in-place RoPE on the fused qkv buffer,
 SwiGLU, in-place softmax-cross-entropy, embedding gather / scatter-add and flat
 AdamW.  On CPU tensors the same Functions run the reference math in
@@ -27,7 +28,7 @@ from . import reference as ref
 
 __all__ = [
     "linear", "fused_linear", "rms_norm", "add_rms_norm", "rope_qkv_", "attention_qkv", "swiglu", "cross_entropy",
-    "embedding", "gemm", "ref",
+    "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "ref",
 ]
 
 
@@ -167,6 +168,91 @@ def fused_linear(x, w, owner=None):
     if _ext.use_cuda_kernel("gemm", x, w) and x.dtype == torch.bfloat16:
         return _Linear.apply(x, w, owner if owner is not None else w)
     return ref.linear(x, w)
+
+
+# --------------------------------------------------------------------------------------
+# fp8 linear (per-tensor current scaling; x and W in e4m3, dy in e5m2)
+# --------------------------------------------------------------------------------------
+def fp8_amax(t):
+    """max |t| of a 2-D bf16 tensor as a one-element fp32 tensor on its device."""
+    if _ext.use_cuda_kernel("fp8", t):
+        return _ext.load().fp8_amax(t)
+    return t.float().abs().max().reshape(1)
+
+
+def fp8_cast(t, dtype, rowwise=True, transposed=True, amax=None):
+    """``(t8, t8_T, scale_inv)`` of a 2-D bf16 tensor quantised to ``dtype`` (see ``ref.fp8_quantize``): the
+    row-major copy and / or its transpose (None when not asked for) and the one-element fp32 dequantisation scale,
+    which stays on the device.  ``amax`` (from ``fp8_amax``) is computed when not given.  CUDA: the amax and
+    cast-transpose kernels."""
+    if amax is None:
+        amax = fp8_amax(t)
+    if _ext.use_cuda_kernel("fp8", t):
+        return _ext.load().fp8_cast_transpose(t, amax, dtype == torch.float8_e5m2, rowwise, transposed)
+    t8, scale_inv = ref.fp8_quantize(t, dtype, amax)
+    return (t8 if rowwise else None), (t8.t().contiguous() if transposed else None), scale_inv
+
+
+def gemm_fp8(a8, scale_inv_a, b8, scale_inv_b, out=None, accumulate=False, out_dtype=torch.bfloat16):
+    """out[M,N] (+)= scale_inv_a * scale_inv_b * a8[M,K] @ b8[N,K].T with fp32 accumulation.  a8 is e4m3 or e5m2,
+    b8 e4m3, both with K contiguous; ``out`` may be a strided view (of a flat gradient)."""
+    if out is None:
+        out = torch.empty(a8.shape[0], b8.shape[0], dtype=out_dtype, device=a8.device)
+        accumulate = False
+    if _ext.use_cuda_kernel("fp8", a8, b8, out):
+        _ext.load().gemm_fp8(a8, b8, out, scale_inv_a, scale_inv_b, accumulate)
+    else:
+        r = ref.fp8_gemm(a8, scale_inv_a, b8, scale_inv_b)
+        out.copy_((out.float() + r) if accumulate else r)
+    return out
+
+
+class _FP8Linear(torch.autograd.Function):
+    """y = x @ W.T with every GEMM in fp8: forward X8 . W8^T, dgrad dY8 . (W8^T)^T, wgrad (dY8^T) . (X8^T)^T.  The
+    fp8 GEMM takes K-major operands only, so forward casts x into both layouts and keeps the transposed copy (1 byte
+    per element) for backward instead of the bf16 input; backward casts dy into both layouts.  W8^T is cast again in
+    backward from the weight, which does not change before its gradient is computed, with the amax forward measured,
+    so it is bit-identical to the forward's quantisation; keeping it from forward instead would hold 1 byte per
+    parameter through the step (6.5 GB for Llama-2-7B, more than an 80 GB H100 has left at S 4096)."""
+
+    @staticmethod
+    def forward(ctx, x, w, w_param):
+        x2 = x.reshape(-1, x.shape[-1])
+        x8, x8t, sx = fp8_cast(x2, torch.float8_e4m3fn)
+        amax_w = fp8_amax(w)
+        w8, _, sw = fp8_cast(w, torch.float8_e4m3fn, transposed=False, amax=amax_w)
+        y = gemm_fp8(x8, sx, w8, sw, out_dtype=x.dtype)
+        ctx.save_for_backward(x8t, sx, w, amax_w)
+        ctx.w_param = w_param
+        ctx.x_shape = x.shape
+        return y.view(*x.shape[:-1], w.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        x8t, sx, w, amax_w = ctx.saved_tensors
+        dy2 = dy.reshape(-1, dy.shape[-1])
+        if not dy2.is_contiguous():
+            dy2 = dy2.contiguous()
+        dy8, dy8t, sdy = fp8_cast(dy2, torch.float8_e5m2, rowwise=ctx.needs_input_grad[0])
+        dx = None
+        if ctx.needs_input_grad[0]:
+            _, w8t, sw = fp8_cast(w, torch.float8_e4m3fn, rowwise=False, amax=amax_w)
+            dx = gemm_fp8(dy8, sdy, w8t, sw, out_dtype=dy.dtype).view(ctx.x_shape)  # [T,N] . [K,N]^T
+        dw = None
+        if ctx.needs_input_grad[1] or getattr(ctx.w_param, "_dtg_grad", None) is not None:
+            dw = _emit_weight_grad(
+                ctx.w_param,
+                lambda out, acc: gemm_fp8(dy8t, sdy, x8t, sx, out=out, accumulate=acc),  # [N,T] . [K,T]^T
+                ctx.w_param,
+            )
+        return dx, dw, None
+
+
+def fp8_linear(x, w, owner=None):
+    """``linear`` with fp8 GEMMs (forward, dgrad and wgrad).  ``owner`` is what carries the flat-gradient view: the
+    ``models.llama.FusedWeight`` of a fused weight, or the parameter itself; None when ``w`` is an ordinary autograd
+    tensor.  CPU tensors run the same quantisation through ``ops/reference.py``."""
+    return _FP8Linear.apply(x, w, owner if owner is not None else w)
 
 
 # --------------------------------------------------------------------------------------

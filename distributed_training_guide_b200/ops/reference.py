@@ -8,7 +8,8 @@ These serve two roles and are never a second GPU backend:
 
 Semantics follow what the reference guide gets from ``transformers`` (SURVEY.md §3.2 /
 K1-K9): RMSNorm with fp32 statistics, half-rotation RoPE, causal softmax attention
-with GQA, SwiGLU, shifted-label mean cross-entropy with ``ignore_index=-100``.
+with GQA, SwiGLU, shifted-label mean cross-entropy with ``ignore_index=-100``.  The fp8 functions define the
+quantisation of ``ops.fp8_linear`` (per-tensor current scaling) exactly, so the cast kernels are tested bit for bit.
 """
 from __future__ import annotations
 
@@ -113,6 +114,27 @@ def cross_entropy(logits, targets, ignore_index=-100):
 
 def embedding(ids, w):
     return F.embedding(ids, w)
+
+
+def fp8_quantize(t, dtype, amax=None):
+    """Per-tensor current scaling of ``t`` to ``dtype`` (``torch.float8_e4m3fn`` or ``torch.float8_e5m2``), as the
+    fp8 cast kernels compute it: ``amax = max|t|``, ``scale = FP8_MAX / amax`` in fp32 (1 when amax is 0),
+    ``t8 = round_to_nearest_even(t * scale)`` saturated at +-FP8_MAX.  torch's cast of an out-of-range value gives
+    NaN (e4m3) or Inf (e5m2) instead of saturating, hence the clamp, which keeps NaN.  A non-finite amax makes the
+    scale 0 or NaN, so ``t8`` holds NaN and the non-finite value reaches whatever consumes it.
+    ``amax`` (a one-element fp32 tensor) is computed from ``t`` when not given.
+    Returns ``(t8, scale_inv)`` with ``scale_inv = 1 / scale`` as a one-element fp32 tensor."""
+    fp8_max = torch.finfo(dtype).max
+    tf = t.float()
+    amax = tf.abs().max().reshape(1) if amax is None else amax.float().reshape(1)
+    scale = torch.where(amax == 0, torch.ones_like(amax), torch.full_like(amax, fp8_max) / amax)
+    t8 = (tf * scale).clamp(-fp8_max, fp8_max).to(dtype)
+    return t8, torch.ones_like(scale) / scale
+
+
+def fp8_gemm(a8, scale_inv_a, b8, scale_inv_b):
+    """fp32 ``(a8 * scale_inv_a) @ (b8 * scale_inv_b).T`` of fp8 operands stored [M, K] and [N, K]."""
+    return (a8.float() * scale_inv_a) @ (b8.float() * scale_inv_b).t()
 
 
 def adamw_step(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step, grad_scale=1.0):

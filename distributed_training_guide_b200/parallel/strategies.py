@@ -141,6 +141,7 @@ class SingleDevice(Strategy):
         model = build_model(config, dtype=self.dtype(), device=self.env.device)
         self.groups, self.symm, self.registry = _flat_groups_on(self, model, 1)
         _load_pretrained(args, model=model)
+        _apply_fp8(args, model)
         return model
 
     def build_optimizer(self, args, model, lr):
@@ -159,6 +160,27 @@ class SingleDevice(Strategy):
         if enabled or eng is None:
             return contextlib.nullcontext()
         return eng.no_sync()
+
+
+#: engines whose decoder-layer projections can run in fp8 (``--fp8``); the FSDP / TP engines gather their operands
+#: inside bf16 GEMM kernels that have no fp8 form
+FP8_PARALLELISMS = ("single", "ddp", "ddp_allreduce")
+
+
+def _apply_fp8(args, model):
+    """``model.fp8 = args.fp8`` for the engines that support it (Llama models only)."""
+    if not getattr(args, "fp8", False):
+        return
+    from ..models.llama import LlamaForCausalLM
+
+    if not isinstance(model, LlamaForCausalLM):
+        raise ValueError(f"fp8 applies to the Llama models' decoder layers, not {type(model).__name__}")
+    model.fp8 = True
+
+
+def check_fp8_supported(parallelism: str):
+    if parallelism not in FP8_PARALLELISMS:
+        raise ValueError(f"fp8 is supported by the {', '.join(FP8_PARALLELISMS)} engines, not {parallelism!r}")
 
 
 def _load_pretrained(args, model=None, engine=None, default="never"):
@@ -219,6 +241,7 @@ class DataParallelZero1(Strategy):
             if float(flag.item()) > 0:
                 for g in self.groups:
                     dist.broadcast(g.param, src=0)
+        _apply_fp8(args, model)
         self.model = model
         return model
 

@@ -13,8 +13,8 @@ COMMON = ("experiment-name", "dataset-name", "dataset-subset", "model-name", "sa
           "num-epochs", "lr", "batch-size", "log-freq", "ckpt-freq", "seq-length")
 
 CHAPTER_EXTRAS = {
-    "01-single-gpu": (),
-    "02-distributed-data-parallel": (),
+    "01-single-gpu": ("fp8",),
+    "02-distributed-data-parallel": ("fp8",),
     "04-fully-sharded-data-parallel": ("cpu-offload",),
     "05-training-llama-405b": ("cpu-offload", "checkpoint-activations", "prefetch-layers"),
     "06-tensor-parallel": (),
@@ -57,6 +57,10 @@ def get_parser(chapter: str = "01-single-gpu", require_experiment: bool = False)
     p.add_argument("--pretrained", choices=("auto", "require", "never"), default=None,
                    help="load local Hugging Face safetensors for --model-name (chapter 05 defaults to auto: load "
                         "them when they exist on disk; other chapters default to never = random init)")
+    if "fp8" in extras:
+        p.add_argument("--fp8", default=False, action="store_true",
+                       help="run the decoder-layer projections (q|k|v, o, gate|up, down) as fp8 GEMMs with per-tensor "
+                            "current scaling: x and W in e4m3, output gradients in e5m2")
     if "cpu-offload" in extras:
         p.add_argument("--cpu-offload", default=False, action="store_true")
     if "checkpoint-activations" in extras:
