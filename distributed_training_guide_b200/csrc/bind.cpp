@@ -22,6 +22,12 @@ void check_contig(const Tensor& t, const char* name, at::ScalarType dt) {
   TORCH_CHECK(t.is_cuda() && t.is_contiguous(), name, " must be a contiguous CUDA tensor");
   TORCH_CHECK(t.scalar_type() == dt, name, " has the wrong dtype");
 }
+// Operands the kernels read or write in 16-byte vectors: contiguous is not enough, a view may start at any element.
+void check_vec(const Tensor& t, const char* name, at::ScalarType dt) {
+  check_contig(t, name, dt);
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, name,
+              " must start at a 16-byte aligned address (the kernel accesses it in 16-byte vectors)");
+}
 
 void gemm(const Tensor& a, const Tensor& b, Tensor& out, bool trans_a, bool trans_b, bool accumulate, int variant) {
   check_bf16_2d(a, "a");
@@ -99,17 +105,19 @@ std::tuple<c10::optional<Tensor>, c10::optional<Tensor>, Tensor> fp8_cast_transp
 
 std::tuple<Tensor, Tensor, c10::optional<Tensor>> rmsnorm_fwd(const Tensor& x, const Tensor& w, double eps,
                                                               const c10::optional<Tensor>& res) {
-  check_contig(x, "x", at::kBFloat16);
-  check_contig(w, "w", at::kBFloat16);
+  check_vec(x, "x", at::kBFloat16);
+  check_vec(w, "w", at::kBFloat16);
   const c10::cuda::CUDAGuard guard(x.device());
   const int T = (int)x.size(0), H = (int)x.size(1);
+  TORCH_CHECK(w.numel() == H, "rmsnorm: w must have one entry per column of x");
   Tensor y = torch::empty_like(x);
   Tensor rstd = torch::empty({T}, x.options().dtype(at::kFloat));
   c10::optional<Tensor> h;
   const void* rp = nullptr;
   void* hp = nullptr;
   if (res.has_value()) {
-    check_contig(*res, "residual", at::kBFloat16);
+    check_vec(*res, "residual", at::kBFloat16);
+    TORCH_CHECK(res->sizes() == x.sizes(), "rmsnorm: residual and x differ in shape");
     h = torch::empty_like(x);
     rp = res->data_ptr();
     hp = h->data_ptr();
@@ -121,16 +129,20 @@ std::tuple<Tensor, Tensor, c10::optional<Tensor>> rmsnorm_fwd(const Tensor& x, c
 
 std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& h, const Tensor& w, const Tensor& rstd,
                                        const c10::optional<Tensor>& dres) {
-  check_contig(dy, "dy", at::kBFloat16);
-  check_contig(h, "h", at::kBFloat16);
+  check_vec(dy, "dy", at::kBFloat16);
+  check_vec(h, "h", at::kBFloat16);
+  check_vec(w, "w", at::kBFloat16);
+  check_contig(rstd, "rstd", at::kFloat);
   const c10::cuda::CUDAGuard guard(dy.device());
   const int T = (int)dy.size(0), H = (int)dy.size(1);
+  TORCH_CHECK(h.sizes() == dy.sizes() && w.numel() == H && rstd.numel() == T, "rmsnorm_bwd: shapes differ");
   Tensor dx = torch::empty_like(dy);
   Tensor dw = torch::empty({H}, dy.options().dtype(at::kFloat));
   Tensor partial = torch::empty({dtg::rmsnorm_bwd_grid(T), H}, dy.options().dtype(at::kFloat));
   const void* dr = nullptr;
   if (dres.has_value()) {
-    check_contig(*dres, "dres", at::kBFloat16);
+    check_vec(*dres, "dres", at::kBFloat16);
+    TORCH_CHECK(dres->sizes() == dy.sizes(), "rmsnorm_bwd: dres and dy differ in shape");
     dr = dres->data_ptr();
   }
   dtg::rmsnorm_bwd(dy.data_ptr(), h.data_ptr(), w.data_ptr(), rstd.data_ptr<float>(), dr, dx.data_ptr(),
@@ -140,20 +152,22 @@ std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& h, const 
 
 void rope_inplace(Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t n_rot, bool inverse) {
   // qkv: [B, S, heads, d] contiguous; cos/sin fp32 [S, d/2] or [B, S, d/2]
-  check_contig(qkv, "qkv", at::kBFloat16);
-  check_contig(cos, "cos", at::kFloat);
-  check_contig(sin, "sin", at::kFloat);
+  check_vec(qkv, "qkv", at::kBFloat16);
+  check_vec(cos, "cos", at::kFloat);
+  check_vec(sin, "sin", at::kFloat);
   TORCH_CHECK(qkv.dim() == 4, "qkv must be [B,S,heads,d]");
   const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1), NH = qkv.size(2), d = qkv.size(3);
   const bool per_token = cos.dim() == 3;
   TORCH_CHECK(cos.size(-1) == d / 2 && cos.size(per_token ? 1 : 0) == S, "cos/sin table has the wrong shape");
+  TORCH_CHECK(sin.sizes() == cos.sizes(), "cos and sin differ in shape");
+  TORCH_CHECK(n_rot >= 0 && n_rot <= NH, "rope: n_rot must be within [0, heads]");
   dtg::rope_inplace(qkv.data_ptr(), cos.data_ptr<float>(), sin.data_ptr<float>(), B * S, (int)S, (int)NH, (int)n_rot,
                     (int)d, per_token, inverse, stream());
 }
 
 Tensor swiglu_fwd(const Tensor& gu) {
-  check_contig(gu, "gu", at::kBFloat16);
+  check_vec(gu, "gu", at::kBFloat16);
   const c10::cuda::CUDAGuard guard(gu.device());
   const int64_t T = gu.size(0), I = gu.size(1) / 2;
   Tensor h = torch::empty({T, I}, gu.options());
@@ -161,8 +175,8 @@ Tensor swiglu_fwd(const Tensor& gu) {
   return h;
 }
 Tensor swiglu_bwd(const Tensor& dh, const Tensor& gu) {
-  check_contig(dh, "dh", at::kBFloat16);
-  check_contig(gu, "gu", at::kBFloat16);
+  check_vec(dh, "dh", at::kBFloat16);
+  check_vec(gu, "gu", at::kBFloat16);
   const c10::cuda::CUDAGuard guard(gu.device());
   Tensor dgu = torch::empty_like(gu);
   dtg::swiglu_bwd(dh.data_ptr(), gu.data_ptr(), dgu.data_ptr(), gu.size(0), (int)(gu.size(1) / 2), stream());
@@ -170,7 +184,7 @@ Tensor swiglu_bwd(const Tensor& dh, const Tensor& gu) {
 }
 
 Tensor cross_entropy_fwd_bwd(Tensor& logits, const Tensor& targets) {
-  check_contig(logits, "logits", at::kBFloat16);
+  check_vec(logits, "logits", at::kBFloat16);
   check_contig(targets, "targets", at::kLong);
   const c10::cuda::CUDAGuard guard(logits.device());
   const int T = (int)logits.size(0), V = (int)logits.size(1);
@@ -183,7 +197,7 @@ Tensor cross_entropy_fwd_bwd(Tensor& logits, const Tensor& targets) {
 }
 
 void scale_inplace(Tensor& x, const Tensor& scale) {
-  check_contig(x, "x", at::kBFloat16);
+  check_vec(x, "x", at::kBFloat16);
   check_contig(scale, "scale", at::kFloat);
   const c10::cuda::CUDAGuard guard(x.device());
   dtg::scale_inplace(x.data_ptr(), scale.data_ptr<float>(), x.numel(), stream());
@@ -191,7 +205,7 @@ void scale_inplace(Tensor& x, const Tensor& scale) {
 
 Tensor embedding_fwd(const Tensor& ids, const Tensor& w) {
   check_contig(ids, "ids", at::kLong);
-  check_contig(w, "w", at::kBFloat16);
+  check_vec(w, "w", at::kBFloat16);
   const c10::cuda::CUDAGuard guard(w.device());
   Tensor out = torch::empty({ids.numel(), w.size(1)}, w.options());
   dtg::embedding_fwd((const long long*)ids.data_ptr<int64_t>(), w.data_ptr(), out.data_ptr(), ids.numel(),
@@ -199,29 +213,40 @@ Tensor embedding_fwd(const Tensor& ids, const Tensor& w) {
   return out;
 }
 void embedding_bwd_sorted(const Tensor& dout, const Tensor& ids_sorted, const Tensor& perm, Tensor& dw, bool accumulate) {
-  TORCH_CHECK(dout.is_contiguous() && dw.is_contiguous() && ids_sorted.is_contiguous() && perm.is_contiguous(), "contiguous");
-  TORCH_CHECK(dout.scalar_type() == at::kBFloat16 && dw.scalar_type() == at::kBFloat16, "bf16 gradients");
-  TORCH_CHECK(ids_sorted.scalar_type() == at::kLong && perm.scalar_type() == at::kLong && perm.numel() == ids_sorted.numel(),
-              "int64 ids / permutation");
+  check_vec(dout, "dout", at::kBFloat16);
+  check_vec(dw, "dw", at::kBFloat16);
+  check_contig(ids_sorted, "ids_sorted", at::kLong);
+  check_contig(perm, "perm", at::kLong);
+  TORCH_CHECK(perm.numel() == ids_sorted.numel(), "int64 ids / permutation");
   const c10::cuda::CUDAGuard guard(dw.device());
   dtg::embedding_bwd_sorted(dout.data_ptr(), (const long long*)ids_sorted.data_ptr<int64_t>(),
                             (const long long*)perm.data_ptr<int64_t>(), dw.data_ptr(), ids_sorted.numel(),
                             (int)dw.size(1), accumulate, at::cuda::getCurrentCUDAStream().stream());
 }
 
-void embedding_bwd(const Tensor& dout, const Tensor& ids, Tensor& dw) {
-  check_contig(dout, "dout", at::kBFloat16);
+// dw (+)= the per-id sum of dout's rows; the [T, H] fp32 scratch and the [V] slot table live until the call returns
+// (the caching allocator keeps them on this stream)
+void embedding_bwd(const Tensor& dout, const Tensor& ids, Tensor& dw, bool accumulate) {
+  check_vec(dout, "dout", at::kBFloat16);
   check_contig(ids, "ids", at::kLong);
-  check_contig(dw, "dw", at::kBFloat16);
+  check_vec(dw, "dw", at::kBFloat16);
+  TORCH_CHECK(dw.dim() == 2 && dout.dim() == 2 && dout.size(1) == dw.size(1) && dout.size(0) == ids.numel(),
+              "embedding_bwd: dout must be [T, H] for T ids and dw [V, H]");
   const c10::cuda::CUDAGuard guard(dw.device());
-  dtg::embedding_bwd(dout.data_ptr(), (const long long*)ids.data_ptr<int64_t>(), dw.data_ptr(), ids.numel(),
-                     (int)dw.size(1), stream());
+  const int64_t T = ids.numel(), V = dw.size(0), H = dw.size(1);
+  Tensor slot = torch::empty({V}, dw.options().dtype(at::kInt));
+  Tensor sums = torch::empty({T, H}, dw.options().dtype(at::kFloat));
+  dtg::embedding_bwd(dout.data_ptr(), (const long long*)ids.data_ptr<int64_t>(), dw.data_ptr(),
+                     reinterpret_cast<unsigned int*>(slot.data_ptr<int>()), sums.data_ptr<float>(), T, V, (int)H,
+                     accumulate, stream());
 }
 
 void adamw_flat(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, double lr, double b1, double b2, double eps,
                 double wd, int64_t step, double grad_scale) {
-  check_contig(p, "p", at::kBFloat16);
-  check_contig(g, "g", at::kBFloat16);
+  check_vec(p, "p", at::kBFloat16);
+  check_vec(g, "g", at::kBFloat16);
+  check_vec(m, "exp_avg", m.scalar_type());
+  check_vec(v, "exp_avg_sq", v.scalar_type());
   TORCH_CHECK(m.scalar_type() == v.scalar_type(), "exp_avg / exp_avg_sq dtypes differ");
   const bool fp32 = m.scalar_type() == at::kFloat;
   TORCH_CHECK(fp32 || m.scalar_type() == at::kBFloat16, "optimizer state must be bf16 or fp32");
@@ -252,7 +277,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("cross_entropy_fwd_bwd", &cross_entropy_fwd_bwd);
   m.def("scale_inplace", &scale_inplace);
   m.def("embedding_fwd", &embedding_fwd);
-  m.def("embedding_bwd", &embedding_bwd);
+  m.def("embedding_bwd", &embedding_bwd, py::arg("dout"), py::arg("ids"), py::arg("dw"), py::arg("accumulate") = false);
   m.def("embedding_bwd_sorted", &embedding_bwd_sorted);
   m.def("adamw_flat", &adamw_flat);
   dtg::bind_comm(m);

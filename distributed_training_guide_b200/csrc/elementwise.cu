@@ -345,16 +345,55 @@ __global__ void embedding_fwd_kernel(const long long* __restrict__ ids, const __
   }
 }
 
-__global__ void embedding_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const long long* __restrict__ ids,
-                                     __nv_bfloat16* __restrict__ dw, long long T, int H) {
-  const int ppr = H >> 1;  // bf16x2 pairs per row
-  const long long total = T * ppr;
+// Default backward, summed in fp32 with one bf16 rounding per table row (a bf16 atomic per occurrence would round
+// once per token, and the most frequent ids of real text occur hundreds of times per batch):
+//   1. slot[id] = the first token position that holds id (atomicMin over the tokens; the table starts at ~0u);
+//   2. sums[slot[ids[t]]] += dout[t] with fp32 vector atomics, into a zeroed [T, H] fp32 scratch;
+//   3. the token at each id's slot writes dw[id] = bf16(sums[slot] (+ dw[id])).
+// Every shape is fixed by T, H and V, so nothing waits on the host.
+__global__ void embedding_slot_kernel(const long long* __restrict__ ids, unsigned int* __restrict__ slot, long long T) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < T; t += (long long)gridDim.x * blockDim.x)
+    atomicMin(slot + ids[t], (unsigned int)t);
+}
+
+__global__ void embedding_sum_kernel(const __nv_bfloat16* __restrict__ dout, const long long* __restrict__ ids,
+                                     const unsigned int* __restrict__ slot, float* __restrict__ sums, long long T,
+                                     int H) {
+  const int vpr = H >> 3;
+  const long long total = T * vpr;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
-    const long long t = idx / ppr;
-    const int c = (int)(idx % ppr);
-    const __nv_bfloat162 g = reinterpret_cast<const __nv_bfloat162*>(dout + t * H)[c];
-    atomicAdd(reinterpret_cast<__nv_bfloat162*>(dw + ids[t] * H) + c, g);
+    const long long t = idx / vpr;
+    const int v = (int)(idx % vpr);
+    float g[8];
+    unpack8(ld8(dout + t * H + v * 8), g);
+    float4* dst = reinterpret_cast<float4*>(sums + (long long)slot[ids[t]] * H + v * 8);
+    atomicAdd(dst, make_float4(g[0], g[1], g[2], g[3]));
+    atomicAdd(dst + 1, make_float4(g[4], g[5], g[6], g[7]));
+  }
+}
+
+__global__ void embedding_write_kernel(const float* __restrict__ sums, const long long* __restrict__ ids,
+                                       const unsigned int* __restrict__ slot, __nv_bfloat16* __restrict__ dw,
+                                       long long T, int H, int accumulate) {
+  const int vpr = H >> 3;
+  const long long total = T * vpr;
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const long long t = idx / vpr;
+    const long long id = ids[t];
+    if (slot[id] != (unsigned int)t) continue;   // a later occurrence: the first one writes the row
+    const int v = (int)(idx % vpr);
+    const float4* src = reinterpret_cast<const float4*>(sums + t * H + v * 8);
+    const float4 a = src[0], b = src[1];
+    float acc[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    if (accumulate) {
+      float old[8];
+      unpack8(ld8(dw + id * H + v * 8), old);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc[j] += old[j];
+    }
+    st8(dw + id * H + v * 8, pack8(acc));
   }
 }
 
@@ -397,9 +436,19 @@ void embedding_fwd(const long long* ids, const void* w, void* out, long long T, 
   note_launch();
   DTG_LAUNCH_CHECK();
 }
-void embedding_bwd(const void* dout, const long long* ids, void* dw, long long T, int H, cudaStream_t s) {
-  embedding_bwd_kernel<<<ew_grid(T * (H / 2)), 256, 0, s>>>((const __nv_bfloat16*)dout, ids, (__nv_bfloat16*)dw, T, H);
-  note_launch();
+void embedding_bwd(const void* dout, const long long* ids, void* dw, unsigned int* slot, float* sums, long long T,
+                   long long V, int H, bool accumulate, cudaStream_t s) {
+  if (H % 8 != 0) throw std::runtime_error("embedding: hidden size must be a multiple of 8");
+  if (T >= 0xFFFFFFFFLL) throw std::runtime_error("embedding: too many tokens for 32-bit slots");
+  if (!accumulate) DTG_CUDA_CHECK(cudaMemsetAsync(dw, 0, (size_t)V * H * sizeof(__nv_bfloat16), s));
+  if (T <= 0) return;
+  DTG_CUDA_CHECK(cudaMemsetAsync(slot, 0xFF, (size_t)V * sizeof(unsigned int), s));
+  DTG_CUDA_CHECK(cudaMemsetAsync(sums, 0, (size_t)T * H * sizeof(float), s));
+  embedding_slot_kernel<<<ew_grid(T), 256, 0, s>>>(ids, slot, T);
+  embedding_sum_kernel<<<ew_grid(T * (H / 8)), 256, 0, s>>>((const __nv_bfloat16*)dout, ids, slot, sums, T, H);
+  embedding_write_kernel<<<ew_grid(T * (H / 8)), 256, 0, s>>>(sums, ids, slot, (__nv_bfloat16*)dw, T, H,
+                                                             accumulate ? 1 : 0);
+  note_launch(3);
   DTG_LAUNCH_CHECK();
 }
 

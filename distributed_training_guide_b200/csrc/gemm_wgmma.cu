@@ -601,11 +601,28 @@ int gemm_max_active_clusters(int cg) {
   return n;
 }
 
+// TMA operands need 16-byte aligned bases (the tensor-map encoder refuses others); the epilogue stores C in
+// bf16 pairs, and 16 bytes keeps every row of C on a vector boundary as ldc % 8 == 0 does for the rows after it.
+static void check_gemm_bases(const char* who, const void* A, const void* B, const void* C) {
+  const struct { const void* p; const char* name; } ops[3] = {{A, "A"}, {B, "B"}, {C, "C"}};
+  for (const auto& o : ops)
+    if (reinterpret_cast<uintptr_t>(o.p) % 16)
+      throw std::runtime_error(std::string(who) + ": " + o.name + " must start at a 16-byte aligned address");
+}
+
+// K == 0: the product is zero, so overwrite mode writes zeros over the M x N view and accumulate mode leaves it as is
+static void gemm_empty_k(void* C, int M, int N, long long ldc, bool accumulate, cudaStream_t s) {
+  if (!accumulate)
+    DTG_CUDA_CHECK(cudaMemset2DAsync(C, (size_t)ldc * 2, 0, (size_t)N * 2, (size_t)M, s));
+}
+
 void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
                bool a_kmajor, bool b_kmajor, bool accumulate, int variant, cudaStream_t s) {
-  if (M <= 0 || N <= 0 || K <= 0) return;
+  if (M <= 0 || N <= 0) return;
   if ((N % 8) || (ldc % 8) || (lda % 8) || (ldb % 8))
     throw std::runtime_error("gemm_bf16: N and the leading dimensions must be multiples of 8 elements");
+  check_gemm_bases("gemm_bf16", A, B, C);
+  if (K <= 0) return gemm_empty_k(C, M, N, ldc, accumulate, s);
   if (variant == 0) variant = default_gemm_variant();
   if (variant == 3) variant = (M > 128) ? 2 : 1;  // auto: the CTA-pair tile is 256 rows tall
   const int cg = (variant == 2) ? 2 : 1;
@@ -631,10 +648,12 @@ void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long 
 // kernels that computed them.
 void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
               bool a_e5m2, const float* scale_a, const float* scale_b, bool accumulate, int variant, cudaStream_t s) {
-  if (M <= 0 || N <= 0 || K <= 0) return;
+  if (M <= 0 || N <= 0) return;
   if ((N % 16) || (lda % 16) || (ldb % 16) || (ldc % 16))
     throw std::runtime_error("gemm_fp8: N and the leading dimensions must be multiples of 16 elements (TMA needs "
                              "16-byte row strides of the fp8 operands)");
+  check_gemm_bases("gemm_fp8", A, B, C);
+  if (K <= 0) return gemm_empty_k(C, M, N, ldc, accumulate, s);
   if (variant == 0) variant = default_gemm_variant();
   if (variant == 3) variant = (M > 128) ? 2 : 1;
   const int cg = (variant == 2) ? 2 : 1;

@@ -483,9 +483,8 @@ class _Embedding(torch.autograd.Function):
                 srt, perm = torch.sort(flat, stable=True)
                 C.embedding_bwd_sorted(d2, srt.contiguous(), perm.contiguous(), out, True)
                 return
-            if not acc:
-                out.zero_()
-            C.embedding_bwd(d2, flat, out)
+            # each row summed in fp32 and rounded once; overwrite mode zeroes the rows of absent ids too
+            C.embedding_bwd(d2, flat, out, acc)
 
         return None, _emit_weight_grad(w, into, w)
 

@@ -1,0 +1,410 @@
+"""The memory-bound kernels against fp64, element by element, with no outlier budget.
+
+The yardstick is the fp64 result of the same operation on the same bf16 inputs (and the same fp32 tables, for RoPE).
+Each element may be one bf16 ulp of it away, plus, where a reduction or a cancellation makes one ulp unreachable for a
+correct fp32 kernel, a stated term of fp32 size.  Each test prints its worst row or element.
+
+Shapes reach what the launchers do at scale: RoPE and SwiGLU past the grid cap (16 CTAs per SM) so the grid-stride
+loops run, RMSNorm backward with more rows than its persistent grid (8 CTAs per SM), hidden sizes that leave some
+threads a partial share of 16-byte vectors, and every branch of the RMSNorm dispatch.
+"""
+import math
+
+import pytest
+import torch
+
+from distributed_training_guide_b200 import _ext, ops
+from distributed_training_guide_b200.ops import reference as ref
+from test_gpu_step_reference import (CONFIGS, GRAD_FACTOR, GRAD_SLACK, _bf16_spacing, _capture_buckets, _engine,
+                                     _engine_grads, _plain_model_grads)
+
+pytestmark = pytest.mark.gpu
+BF16 = torch.bfloat16
+# fp32 work, relative to the size of the terms it combines: a few fp32 ulps (2^-24 each) of the terms, far below one
+# bf16 ulp (2^-8) of them, so a wrong term still shows
+FP32_TERMS = 2.0 ** -18
+
+
+def _C():
+    return _ext.load(True)
+
+
+def _gen(seed):
+    return torch.Generator(device="cuda").manual_seed(seed)
+
+
+def _ulps(got, want64, extra=None):
+    """|got - want| in bf16 ulps of want, after an allowance ``extra`` (fp64, same shape) is taken off."""
+    err = (got.double() - want64).abs()
+    if extra is not None:
+        err = (err - extra).clamp_min(0)
+    return err / _bf16_spacing(want64.float()).double()
+
+
+def _check_ulps(tag, got, want64, extra=None):
+    u = _ulps(got, want64, extra)
+    u = torch.where(torch.isnan(u), torch.full_like(u, float("inf")), u)
+    flat = u.reshape(u.shape[0], -1) if u.dim() > 1 else u.reshape(1, -1)
+    row_worst = flat.max(1).values
+    r = int(row_worst.argmax())
+    print(f"\n{tag}: worst row {r}: {row_worst[r].item():.3g} ulp; {int((u > 0.5).sum())} of {u.numel()} elements "
+          "more than half an ulp off")
+    assert bool((u <= 1).all()), f"{tag}: {int((u > 1).sum())} elements more than one bf16 ulp off " \
+                                 f"(worst {u.max().item():.3g} in row {r})"
+
+
+def _refused(call, match):
+    torch.cuda.synchronize()
+    n0 = _ext.launch_count()
+    with pytest.raises(RuntimeError, match=match):
+        call()
+    assert _ext.launch_count() == n0, "a refused call launched a kernel"
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# embedding backward
+# ------------------------------------------------------------------------------------------------------------------
+def _zipf_ids(T, V, s, seed):
+    """T ids drawn from a Zipf(s) law over V ids (rank r has probability ~ r^-s), ranks assigned to ids at random."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    p = torch.arange(1, V + 1, device="cuda", dtype=torch.float64).pow(-s)
+    ranks = torch.multinomial(p.float(), T, replacement=True, generator=g)
+    return torch.randperm(V, device="cuda", generator=g)[ranks]
+
+
+def _ids(kind, T, V, seed=0):
+    if kind.startswith("zipf"):
+        return _zipf_ids(T, V, float(kind[4:]), seed)
+    g = _gen(seed)
+    ids = torch.randint(0, V, (T,), device="cuda", generator=g)
+    if kind == "pad":                       # half the batch is one id (padding / EOS runs)
+        ids[torch.randperm(T, device="cuda", generator=g)[:T // 2]] = 7
+    return ids
+
+
+def _row_rel(got, exact):
+    """Relative L2 error of each row."""
+    return (got.double() - exact).norm(dim=1) / exact.norm(dim=1).clamp_min(1e-300)
+
+
+# A row may be this much further from the exact sum than its correctly rounded value (one rounding of the fp32 sum
+# leaves it at 1.00x; one bf16 rounding per occurrence gives 3-20x on the most frequent ids)
+EMB_FACTOR, EMB_SLACK = 1.5, 1e-6
+V_EMB, H_EMB = 32000, 4096
+# Measured on an H100 80GB HBM3 at a 400 W power limit: every row at 1.00x.  The kernel it replaced, which added each
+# occurrence with a bf16 atomic, was at 13.9x on the most frequent id of Zipf(1.0) T 4096 (383 occurrences), 21x on
+# Zipf(1.2), 28x at T 16384 (1549 occurrences) and 32x on the pad id (2048); PyTorch's backward is at 1.00x.
+
+
+@pytest.mark.parametrize("kind,T", [("zipf1.0", 4096), ("zipf1.2", 4096), ("zipf1.0", 16384), ("pad", 4096),
+                                    ("uniform", 4096)])
+def test_embedding_backward_rows_against_fp64(kind, T):
+    V, H = V_EMB, H_EMB
+    ids = _ids(kind, T, V)
+    dout = (1e-3 * torch.randn(T, H, device="cuda", generator=_gen(1))).to(BF16)
+    w = torch.zeros(V, H, device="cuda", dtype=BF16, requires_grad=True)
+    ops.embedding(ids, w).backward(dout)
+    got = w.grad
+    exact = torch.zeros(V, H, device="cuda", dtype=torch.float64).index_add_(0, ids, dout.double())
+    counts = torch.bincount(ids, minlength=V)
+    present = counts > 0
+    rows = present.nonzero().squeeze(1)
+    rel = _row_rel(got[rows], exact[rows])
+    rel_cr = _row_rel(exact[rows].to(BF16), exact[rows])
+    wt = torch.zeros(V, H, device="cuda", dtype=BF16, requires_grad=True)
+    torch.nn.functional.embedding(ids, wt).backward(dout)
+    rel_torch = _row_rel(wt.grad[rows], exact[rows])
+    ratio = rel / rel_cr.clamp_min(1e-30)
+    top = counts[rows].argsort(descending=True)[:5]
+    print(f"\n{kind} T {T}: most frequent ids (occurrences: kernel / PyTorch bf16 / correctly rounded rel err, ratio)")
+    for i in top.tolist():
+        print(f"  {int(counts[rows][i]):6d}: {rel[i]:.3e} / {rel_torch[i]:.3e} / {rel_cr[i]:.3e}  {ratio[i]:.2f}x")
+    worst = int(ratio.argmax())
+    print(f"  worst row (id {int(rows[worst])}, {int(counts[rows][worst])} occurrences): {ratio[worst]:.2f}x")
+    assert int(torch.count_nonzero(got[~present])) == 0, "rows of absent ids are not zero"
+    bad = rel > EMB_FACTOR * rel_cr + EMB_SLACK
+    assert not bad.any(), f"{int(bad.sum())} rows beyond {EMB_FACTOR}x the correctly rounded error " \
+                          f"(worst {ratio.max().item():.2f}x)"
+
+
+@pytest.mark.parametrize("accumulate", [False, True])
+def test_embedding_backward_modes(accumulate):
+    """Overwrite mode writes every row of the table, zeros for absent ids, over whatever the buffer held (a flat
+    gradient still holding the previous step's); accumulate mode (gradient accumulation, the tied lm_head) gives
+    round(old + sum) with one rounding."""
+    V, H, T = 5000, 1032, 4096
+    ids = _ids("zipf1.1", T, V, seed=3)
+    dout = (1e-2 * torch.randn(T, H, device="cuda", generator=_gen(4))).to(BF16)
+    old = torch.randn(V, H, device="cuda", generator=_gen(5)).mul(0.05).to(BF16)
+    dw = old.clone()
+    _C().embedding_bwd(dout, ids, dw, accumulate)
+    exact = torch.zeros(V, H, device="cuda", dtype=torch.float64).index_add_(0, ids, dout.double())
+    if accumulate:
+        exact += old.double()
+    present = torch.bincount(ids, minlength=V) > 0
+    absent = dw[~present]
+    if accumulate:
+        assert torch.equal(absent, old[~present]), "accumulate changed rows of absent ids"
+    else:
+        assert int(torch.count_nonzero(absent)) == 0, "overwrite left rows of absent ids nonzero"
+    rel = _row_rel(dw[present], exact[present])
+    rel_cr = _row_rel(exact[present].to(BF16), exact[present])
+    print(f"\naccumulate={accumulate}: worst row ratio to the correctly rounded {(rel / rel_cr.clamp_min(1e-30)).max():.3f}")
+    assert bool((rel <= EMB_FACTOR * rel_cr + EMB_SLACK).all())
+
+
+@pytest.mark.parametrize("case", ["gqa-b2-s256", "gqa-b2-s256-tied"])
+def test_embedding_gradient_through_engine_zipf_batch(case, monkeypatch):
+    """One engine step on a Zipf batch (real text repeats its frequent ids; ``synthetic_batch`` is uniform): the
+    gradient rows of the 20 most frequent ids against fp32, each within the step test's rule."""
+    cfg = CONFIGS[case]
+    with _engine(monkeypatch, cfg) as eng:
+        rec = _capture_buckets(eng)
+        V = eng.config.vocab_size
+        ids = _zipf_ids(cfg["B"] * cfg["S"], V, 1.1, seed=9).view(cfg["B"], cfg["S"]).cpu()
+        batch = {"input_ids": ids, "labels": ids.clone()}
+        weights = {n: p.detach().clone() for n, p in eng.model.named_parameters()}
+        eng.step(batch)
+        torch.cuda.synchronize()
+        grads = _engine_grads(eng, rec)
+        _, ref_grads = _plain_model_grads(eng.config, {n: w.float() for n, w in weights.items()}, [batch],
+                                          torch.float32, monkeypatch)
+        _, bf16_grads = _plain_model_grads(eng.config, weights, [batch], torch.bfloat16, monkeypatch)
+    name = "model.embed_tokens.weight"
+    counts = torch.bincount(ids.reshape(-1), minlength=V)
+    top = counts.argsort(descending=True)[:20].cuda()
+    rk = _row_rel(grads[name][top], ref_grads[name][top].double())
+    rb = _row_rel(bf16_grads[name][top], ref_grads[name][top].double())
+    print(f"\n{case}: top-20 ids ({int(counts.max())} .. {int(counts[top[-1].cpu()])} occurrences): "
+          f"kernel / PyTorch bf16 row error, worst ratio {(rk / rb.clamp_min(1e-30)).max():.2f}")
+    for i in range(0, 20, 5):
+        print(f"  id {int(top[i])}: {rk[i]:.3e} / {rb[i]:.3e}")
+    bad = rk > GRAD_FACTOR * rb + GRAD_SLACK
+    assert not bad.any(), f"{int(bad.sum())} of the 20 most frequent rows beyond {GRAD_FACTOR}x PyTorch bf16 + " \
+                          f"{GRAD_SLACK}"
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# RMSNorm
+# ------------------------------------------------------------------------------------------------------------------
+NORM_H = [8, 1024, 1032, 2048, 2056, 4096, 4104, 8192, 8200, 16384]
+NORM_T = [1, 17, 2048, 8192]
+
+
+def _norm_inputs(T, H, seed):
+    g = _gen(seed)
+    x = torch.randn(T, H, device="cuda", generator=g)
+    r = torch.randn(T, H, device="cuda", generator=g)
+    if T > 2:
+        r[T // 3] *= 1e3            # an outlier row of the residual stream
+        x[T // 2], r[T // 2] = 0, 0     # an all-zero row
+    w = 1 + 0.1 * torch.randn(H, device="cuda", generator=g)
+    dy = torch.randn(T, H, device="cuda", generator=g)
+    dres = torch.randn(T, H, device="cuda", generator=g)
+    return [t.to(BF16) for t in (x, r, w, dy, dres)]
+
+
+@pytest.mark.parametrize("with_res", [False, True])
+@pytest.mark.parametrize("T", NORM_T)
+@pytest.mark.parametrize("H", NORM_H)
+def test_rmsnorm_against_fp64(H, T, with_res):
+    if T == 8192 and H not in (1032, 4104, 16384):
+        pytest.skip("T 8192 runs at three hidden sizes; T 2048 already exceeds the backward's persistent grid")
+    eps = 1e-5
+    x, r, w, dy, dres = _norm_inputs(T, H, seed=H + T)
+    C = _C()
+    y, rstd, h = C.rmsnorm_fwd(x, w, eps, r if with_res else None)
+    # forward: h = bf16(x + r) (the residual stream is stored in bf16), y = h * rstd * w
+    h64 = (x.double() + r.double()).to(BF16).double() if with_res else x.double()
+    if with_res:
+        _check_ulps(f"H{H} T{T} h", h, x.double() + r.double())
+    rstd64 = 1.0 / (h64.square().mean(1, keepdim=True) + eps).sqrt()
+    assert bool(((rstd.double() - rstd64[:, 0]).abs() <= 1e-5 * rstd64[:, 0]).all()), "rstd"
+    y64 = h64 * rstd64 * w.double()
+    _check_ulps(f"H{H} T{T} res={with_res} y", y, y64, FP32_TERMS * y64.abs())
+    # backward: g = dy * w, xhat = h * rstd; dx = rstd (g - xhat mean(g xhat)) (+ dres); dw = sum_rows dy xhat
+    hh = h if with_res else x
+    dx, dw = C.rmsnorm_bwd(dy, hh, w, rstd, dres if with_res else None)
+    g64, xhat = dy.double() * w.double(), h64 * rstd64
+    dot = (g64 * xhat).mean(1, keepdim=True)
+    dx64 = rstd64 * (g64 - xhat * dot) + (dres.double() if with_res else 0)
+    # the terms dx combines, and the fp32 dot's error (the mean of |g xhat| per row), scaled by what multiplies them
+    terms = rstd64 * (g64.abs() + xhat.abs() * (dot.abs() + (g64 * xhat).abs().mean(1, keepdim=True)))
+    if with_res:
+        terms = terms + dres.double().abs()
+    _check_ulps(f"H{H} T{T} res={with_res} dx", dx, dx64, FP32_TERMS * terms)
+    dw64 = (dy.double() * xhat).sum(0)
+    dw_terms = (dy.double() * xhat).abs().sum(0)
+    err = (dw.double() - dw64).abs()
+    worst = int((err / dw_terms.clamp_min(1e-300)).argmax())
+    print(f"\nH{H} T{T} dw: worst column {worst}: |err| {err[worst]:.3g} of sum |terms| {dw_terms[worst]:.3g}")
+    assert bool((err <= 2.0 ** -16 * dw_terms).all()), f"dw: {int((err > 2.0 ** -16 * dw_terms).sum())} columns off"
+
+
+def test_rmsnorm_rejects_unsupported_hidden_sizes():
+    C = _C()
+    for H in (12, 1028, 16392, 32768):
+        x = torch.randn(4, H, device="cuda").to(BF16)
+        w = torch.ones(H, device="cuda", dtype=BF16)
+        _refused(lambda: C.rmsnorm_fwd(x, w, 1e-5, None), "hidden size")
+        rstd = torch.ones(4, device="cuda")
+        _refused(lambda: C.rmsnorm_bwd(x, x, w, rstd, None), "hidden size")
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# RoPE
+# ------------------------------------------------------------------------------------------------------------------
+def _rope64(x, cos, sin, inverse):
+    """fp64 rotation of bf16 ``x`` [B,S,n,d] with the fp32 tables, and the size of the terms it combines."""
+    d2 = x.shape[-1] // 2
+    xd = x.double()
+    a, b = xd[..., :d2], xd[..., d2:]
+    c = (cos[None, :, None] if cos.dim() == 2 else cos[:, :, None]).double()
+    s = (sin[None, :, None] if sin.dim() == 2 else sin[:, :, None]).double()
+    if inverse:
+        s = -s
+    out = torch.cat([a * c - b * s, b * c + a * s], -1)
+    terms = torch.cat([(a * c).abs() + (b * s).abs(), (b * c).abs() + (a * s).abs()], -1)
+    return out, terms
+
+
+ROPE_CASES = {   # B, S, total heads, rotated heads, d, per-token positions
+    "d16": (2, 64, 6, 4, 16, False),
+    "d32": (2, 128, 5, 3, 32, True),
+    "d64": (1, 256, 8, 6, 64, False),
+    "d128-grid-stride": (1, 4096, 48, 40, 128, False),   # 32 q + 8 k + 8 v heads: 1.3 M vectors
+    "d256": (2, 64, 4, 2, 256, True),
+    "d128-pos131072": (2, 512, 12, 10, 128, True),
+}
+
+
+@pytest.mark.parametrize("case", list(ROPE_CASES))
+def test_rope_against_fp64(case):
+    B, S, NH, n_rot, d, per_token = ROPE_CASES[case]
+    g = _gen(len(case))
+    qkv = torch.randn(B, S, NH, d, device="cuda", generator=g).to(BF16)
+    if per_token:
+        pos = torch.randint(0, 131073, (B, S), device="cuda", generator=g)
+        pos[0, 0] = 131072
+    else:
+        pos = torch.arange(S, device="cuda")
+    cos, sin = ref.rope_tables(pos, d, 5e5)
+    for inverse in (False, True):
+        x = qkv.clone()
+        _C().rope_inplace(x, cos, sin, n_rot, inverse)
+        assert torch.equal(x[:, :, n_rot:].view(torch.int16), qkv[:, :, n_rot:].view(torch.int16)), \
+            "heads at or above n_rot changed"
+        want, terms = _rope64(qkv[:, :, :n_rot], cos, sin, inverse)
+        _check_ulps(f"{case} inverse={inverse}", x[:, :, :n_rot].reshape(B * S, -1), want.reshape(B * S, -1),
+                    FP32_TERMS * terms.reshape(B * S, -1))
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# SwiGLU
+# ------------------------------------------------------------------------------------------------------------------
+# Where exp(-g) overflows fp32 (g < -88.72) the kernel returns the limits h = 0 and dg = 0; the exact values are
+# at most |u| |g| e^g and |dh u| (1 + |g|) e^g in size, below 4e-42 |u| (|dh u|) at g = -100: that is the absolute
+# allowance near zero.  Everywhere else each element is within one bf16 ulp plus FP32_TERMS of the terms it combines;
+# that term matters only for dgate near g = -1.28, where sg + silu (1 - sg) cancels to zero.
+SWIGLU_CASES = [(8, 600_000), (1792, 3000), (11008, 512)]   # (I, T): every case runs the grid-stride loop
+
+
+@pytest.mark.parametrize("I,T", SWIGLU_CASES)
+def test_swiglu_against_fp64(I, T):
+    g = _gen(I)
+    gate = 3 * torch.randn(T * I, device="cuda", generator=g)
+    special = torch.tensor([0.0, 10, -10, 30, -30, 88, -88, 100, -100], device="cuda")
+    idx = torch.randperm(T * I, device="cuda", generator=g)[:4096]
+    gate[idx] = special[torch.arange(4096, device="cuda") % len(special)]
+    gu = torch.cat([gate.view(T, I), torch.randn(T, I, device="cuda", generator=g)], 1).to(BF16)
+    dh = torch.randn(T, I, device="cuda", generator=g).to(BF16)
+    h = _C().swiglu_fwd(gu)
+    dgu = _C().swiglu_bwd(dh, gu)
+    gd, ud, dd = gu[:, :I].double(), gu[:, I:].double(), dh.double()
+    sg = torch.sigmoid(gd)
+    silu = gd * sg
+    overflow = gd < -88.72
+    tail = torch.where(overflow, (1 + gd.abs()) * gd.exp(), torch.zeros_like(gd))
+    h64 = silu * ud
+    _check_ulps(f"I{I} T{T} h", h, h64, FP32_TERMS * h64.abs() + tail * ud.abs())
+    dg64 = dd * ud * (sg + silu * (1 - sg))
+    du64 = dd * silu
+    dg_terms = (dd * ud).abs() * (sg + (silu * (1 - sg)).abs())
+    _check_ulps(f"I{I} T{T} dgate", dgu[:, :I], dg64, FP32_TERMS * dg_terms + tail * (dd * ud).abs())
+    _check_ulps(f"I{I} T{T} dup", dgu[:, I:], du64, FP32_TERMS * du64.abs() + tail * dd.abs())
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# scale_inplace
+# ------------------------------------------------------------------------------------------------------------------
+def test_scale_inplace():
+    n = 8 * 600_000     # past the grid cap
+    x0 = torch.randn(n, device="cuda", generator=_gen(0)).to(BF16)
+    x0[::1000] = float("nan")
+    x0[1::1000] = float("inf")
+    C = _C()
+    x = x0.clone()
+    C.scale_inplace(x, torch.ones(1, device="cuda"))
+    assert torch.equal(x.view(torch.int16), x0.view(torch.int16)), "scale 1 changed bits"
+    fin = torch.isfinite(x0)
+    for s in (0.5, 4.0, 2.0 ** -10):
+        x = x0.clone()
+        C.scale_inplace(x, torch.full((1,), s, device="cuda"))
+        want = (x0.float() * s).to(BF16)
+        assert torch.equal(x[fin].view(torch.int16), want[fin].view(torch.int16)), f"scale {s}: not exact"
+    for s in (0.3, 1.7, 1e-3):
+        x = x0.clone()
+        s32 = torch.tensor(s, dtype=torch.float32)
+        C.scale_inplace(x, s32.reshape(1).cuda())
+        _check_ulps(f"scale {s}", x[fin].reshape(1, -1), (x0[fin].double() * s32.double().item()).reshape(1, -1))
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# alignment: contiguous tensors that do not start on a 16-byte boundary are refused before any launch
+# ------------------------------------------------------------------------------------------------------------------
+def _misaligned(shape, dtype=BF16):
+    n = math.prod(shape)
+    return torch.zeros(n + 16, device="cuda", dtype=dtype)[1:1 + n].view(shape)
+
+
+def test_vector_kernels_reject_misaligned_tensors():
+    C = _C()
+    T, H, V = 64, 256, 512
+    bf = lambda *s: torch.zeros(*s, device="cuda", dtype=BF16)  # noqa: E731
+    f32 = lambda *s: torch.zeros(*s, device="cuda")              # noqa: E731
+    x, w, rstd = bf(T, H), bf(H), f32(T)
+    for t in (_misaligned((T, H)), _misaligned((H,))):
+        assert t.is_contiguous() and t.data_ptr() % 16 != 0
+    _refused(lambda: C.rmsnorm_fwd(_misaligned((T, H)), w, 1e-5, None), "x must start")
+    _refused(lambda: C.rmsnorm_fwd(x, _misaligned((H,)), 1e-5, None), "w must start")
+    _refused(lambda: C.rmsnorm_fwd(x, w, 1e-5, _misaligned((T, H))), "residual must start")
+    _refused(lambda: C.rmsnorm_bwd(_misaligned((T, H)), x, w, rstd, None), "dy must start")
+    _refused(lambda: C.rmsnorm_bwd(x, _misaligned((T, H)), w, rstd, None), "h must start")
+    _refused(lambda: C.rmsnorm_bwd(x, x, _misaligned((H,)), rstd, None), "w must start")
+    _refused(lambda: C.rmsnorm_bwd(x, x, w, rstd, _misaligned((T, H))), "dres must start")
+    cos, sin = f32(T, 64), f32(T, 64)
+    _refused(lambda: C.rope_inplace(_misaligned((1, T, 4, 128)), cos, sin, 2, False), "qkv must start")
+    _refused(lambda: C.rope_inplace(bf(1, T, 4, 128), _misaligned((T, 64), torch.float32), sin, 2, False),
+             "cos must start")
+    _refused(lambda: C.rope_inplace(bf(1, T, 4, 128), cos, _misaligned((T, 64), torch.float32), 2, False),
+             "sin must start")
+    _refused(lambda: C.swiglu_fwd(_misaligned((T, 2 * H))), "gu must start")
+    _refused(lambda: C.swiglu_bwd(_misaligned((T, H)), bf(T, 2 * H)), "dh must start")
+    _refused(lambda: C.swiglu_bwd(bf(T, H), _misaligned((T, 2 * H))), "gu must start")
+    tgt = torch.zeros(T, device="cuda", dtype=torch.long)
+    _refused(lambda: C.cross_entropy_fwd_bwd(_misaligned((T, V)), tgt), "logits must start")
+    _refused(lambda: C.scale_inplace(_misaligned((T * H,)), torch.ones(1, device="cuda")), "x must start")
+    ids = torch.zeros(T, device="cuda", dtype=torch.long)
+    _refused(lambda: C.embedding_fwd(ids, _misaligned((V, H))), "w must start")
+    _refused(lambda: C.embedding_bwd(_misaligned((T, H)), ids, bf(V, H), False), "dout must start")
+    _refused(lambda: C.embedding_bwd(bf(T, H), ids, _misaligned((V, H)), True), "dw must start")
+    _refused(lambda: C.embedding_bwd_sorted(_misaligned((T, H)), ids, ids, bf(V, H), True), "dout must start")
+    _refused(lambda: C.embedding_bwd_sorted(bf(T, H), ids, ids, _misaligned((V, H)), True), "dw must start")
+    n = 8 * 1000
+    p, g, m, v = bf(n), bf(n), f32(n), f32(n)
+    _refused(lambda: C.adamw_flat(_misaligned((n,)), g, m, v, 1e-3, 0.9, 0.999, 1e-8, 0.0, 1, 1.0), "p must start")
+    _refused(lambda: C.adamw_flat(p, _misaligned((n,)), m, v, 1e-3, 0.9, 0.999, 1e-8, 0.0, 1, 1.0), "g must start")
+    _refused(lambda: C.adamw_flat(p, g, _misaligned((n,), torch.float32), v, 1e-3, 0.9, 0.999, 1e-8, 0.0, 1, 1.0),
+             "exp_avg must start")
+    _refused(lambda: C.adamw_flat(p, g, m, _misaligned((n,), torch.float32), 1e-3, 0.9, 0.999, 1e-8, 0.0, 1, 1.0),
+             "exp_avg_sq must start")
