@@ -19,6 +19,19 @@ void check_qkv(const Tensor& qkv, int64_t nh, int64_t nkv) {
               "qkv must be [B, S, nh+2*nkv, 128]");
 }
 
+// doc_start (document masking): int32 [B, S] on the device of qkv, contiguous; None = plain causal attention.
+// Any content is safe to pass: the kernels clamp every block index they derive from it.
+const int* doc_start_ptr(const c10::optional<Tensor>& doc_start, const Tensor& qkv) {
+  if (!doc_start.has_value() || !doc_start->defined()) return nullptr;
+  const Tensor& d = *doc_start;
+  TORCH_CHECK(d.scalar_type() == at::kInt, "doc_start must be int32");
+  TORCH_CHECK(d.dim() == 2 && d.size(0) == qkv.size(0) && d.size(1) == qkv.size(1), "doc_start must be [B, S] = [",
+              qkv.size(0), ", ", qkv.size(1), "], got ", d.sizes());
+  TORCH_CHECK(d.is_contiguous(), "doc_start must be contiguous");
+  TORCH_CHECK(d.device() == qkv.device(), "doc_start must be on the device of qkv");
+  return d.data_ptr<int>();
+}
+
 // version: 0 = default (DTG_ATTN_FWD env, else 2), 1 = P through shared memory, 2 = P kept in registers
 // (both in attention_fwd.cu)
 int default_fwd_version() {
@@ -31,8 +44,10 @@ int default_fwd_version() {
   return v;
 }
 
-std::tuple<Tensor, Tensor> py_attn_fwd(const Tensor& qkv, int64_t nh, int64_t nkv, double scale, int64_t version) {
+std::tuple<Tensor, Tensor> py_attn_fwd(const Tensor& qkv, int64_t nh, int64_t nkv, double scale, int64_t version,
+                                       const c10::optional<Tensor>& doc_start) {
   check_qkv(qkv, nh, nkv);
+  const int* ds = doc_start_ptr(doc_start, qkv);
   const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1);
   Tensor o = torch::empty({B, S, nh, 128}, qkv.options());
@@ -40,13 +55,15 @@ std::tuple<Tensor, Tensor> py_attn_fwd(const Tensor& qkv, int64_t nh, int64_t nk
   if (version == 0) version = default_fwd_version();
   auto fn = version == 1 ? dtg::attn_fwd : dtg::attn_fwd2;
   fn(qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), (int)B, (int)S, (int)nh, (int)nkv, (float)scale,
-     at::cuda::getCurrentCUDAStream().stream());
+     at::cuda::getCurrentCUDAStream().stream(), ds);
   return {o, lse};
 }
 
 Tensor py_attn_bwd(const Tensor& d_o, const Tensor& qkv, const Tensor& o, const Tensor& lse, int64_t nh, int64_t nkv,
-                   double scale, const c10::optional<Tensor>& trace, int64_t mode) {
+                   double scale, const c10::optional<Tensor>& trace, int64_t mode,
+                   const c10::optional<Tensor>& doc_start) {
   check_qkv(qkv, nh, nkv);
+  const int* ds = doc_start_ptr(doc_start, qkv);
   TORCH_CHECK(d_o.is_contiguous() && o.is_contiguous() && d_o.scalar_type() == at::kBFloat16, "dO/O must be contiguous bf16");
   const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1);
@@ -59,16 +76,17 @@ Tensor py_attn_bwd(const Tensor& d_o, const Tensor& qkv, const Tensor& o, const 
   }
   dtg::attn_bwd(qkv.data_ptr(), o.data_ptr(), d_o.data_ptr(), lse.data_ptr<float>(), delta.data_ptr<float>(), tr,
                 dqkv.data_ptr(), (int)B, (int)S, (int)nh, (int)nkv, (float)scale, (int)mode,
-                at::cuda::getCurrentCUDAStream().stream());
+                at::cuda::getCurrentCUDAStream().stream(), ds);
   return dqkv;
 }
 }  // namespace
 
 void bind_attention(pybind11::module_& m) {
   m.def("attn_fwd", &py_attn_fwd, pybind11::arg("qkv"), pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("scale"),
-        pybind11::arg("version") = 0);
+        pybind11::arg("version") = 0, pybind11::arg("doc_start") = pybind11::none());
   m.def("attn_bwd", &py_attn_bwd, pybind11::arg("d_o"), pybind11::arg("qkv"), pybind11::arg("o"), pybind11::arg("lse"),
         pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("scale"), pybind11::arg("trace") = pybind11::none(),
-        pybind11::arg("mode") = 0);   // 0 = default (DTG_ATTN_BWD), 1 = P/dS through shared memory, 2 = P/dS in registers
+        pybind11::arg("mode") = 0,   // 0 = default (DTG_ATTN_BWD), 1 = P/dS through shared memory, 2 = P/dS in registers
+        pybind11::arg("doc_start") = pybind11::none());
 }
 }  // namespace dtg

@@ -13,7 +13,10 @@
 // 256 threads = two math warpgroups that own 64 rows of R each and keep their gradient accumulators in
 // registers for the whole pass (up to 255 registers a thread: two warps per SM sub-partition); thread 0 also
 // issues the TMA loads (resident R tiles once, C tiles into a 3-stage ring two blocks ahead).  delta = rowsum(dO o O) is produced by a small preprocess
-// kernel.  Gradients are written into a dqkv buffer with the same fused layout as qkv, so the
+// kernel.  DOC (document masking, key k visible to query q iff doc_start[q] <= k <= q): the KV pass stops at the first
+// query block whose first query starts its document after the 128 keys, the Q pass starts at the block holding the
+// document start of its first query, and the element mask also runs where a document begins inside a block.
+// Gradients are written into a dqkv buffer with the same fused layout as qkv, so the
 // RoPE-backward kernel and the fused qkv dgrad/wgrad GEMMs consume it directly.
 #include <cuda.h>
 
@@ -72,12 +75,13 @@ __global__ void attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ d_o, con
 // registers they were computed in and feed the gradient MMAs as their A operand (RS form).  Per 128x64 block that
 // removes 32 KB of shared-memory stores and 32 KB of A-operand reads.  TS = false stages them through
 // 128B-swizzled shared memory (SS form).
-template <bool KV_MODE, bool TS>
+template <bool KV_MODE, bool TS, bool DOC>
 __global__ void __launch_bounds__(bwd::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_constant__ CUtensorMap tm_qkv_c,
                 const __grid_constant__ CUtensorMap tm_do_r, const __grid_constant__ CUtensorMap tm_do_c,
                 const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv,
-                int S, int nh, int nkv, float scale, int num_r_blocks, long long* __restrict__ trace) {
+                int S, int nh, int nkv, float scale, int num_r_blocks, long long* __restrict__ trace,
+                const int* __restrict__ doc_start) {
   using namespace bwd;
   // optional in-kernel timeline (attn_bwd(..., trace=int64[1024])): CTA (0,0) records clock64() per column block:
   // [iter][0] scores ready, [1] P / dS computed, [3] gradient MMAs retired (thread 0)
@@ -101,8 +105,41 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
   const int R0 = r_block * 128;
   const int kv_head = KV_MODE ? head_r : head_r / group;
   // column-block range
-  const int c_start = KV_MODE ? R0 / 64 : 0;
-  const int n_c = KV_MODE ? (S / 64 - c_start) : (R0 + 128) / 64;
+  int c_start = KV_MODE ? R0 / 64 : 0;
+  int n_c = KV_MODE ? (S / 64 - c_start) : (R0 + 128) / 64;
+  [[maybe_unused]] const int* ds_row = nullptr;   // DOC: this batch row's document starts
+  // DOC: where the document mask starts to matter.  KV pass: the first column block holding a query whose document
+  // starts after R0; Q pass: the document start of the last query of R.  Kept in a register so that no iteration waits
+  // on a load before it can decide whether to mask.
+  [[maybe_unused]] int doc_bound = 0;
+  if constexpr (DOC) {
+    // Every thread derives the same range from the same words (issue_y splits t by n_c), and every index stays
+    // inside the plain causal range whatever doc_start holds.
+    ds_row = doc_start + (long long)batch * S;
+    if (KV_MODE) {
+      // last query block whose first query (the smallest start) can see one of the keys R0..R0+127
+      int lo = c_start, hi = S / 64 - 1;
+      while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (__ldg(ds_row + mid * 64) <= R0 + 127) lo = mid;
+        else hi = mid - 1;
+      }
+      n_c = lo - c_start + 1;
+      hi = c_start + n_c;
+      lo = c_start;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (__ldg(ds_row + mid * 64 + 63) > R0) hi = mid;
+        else lo = mid + 1;
+      }
+      doc_bound = lo;
+    } else {
+      // first key block: the one holding the document start of the first query
+      c_start = min(max(__ldg(ds_row + R0) / 64, 0), n_c - 1);
+      n_c -= c_start;
+      doc_bound = __ldg(ds_row + R0 + 127);
+    }
+  }
   const int n_iter = KV_MODE ? n_c * group : n_c;
 
   if (threadIdx.x == 0) {
@@ -166,12 +203,30 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
     const bool tr_thread = tracing && threadIdx.x == 0;
     const float sl2 = scale * LOG2E;
     float lse_r[2] = {0.f, 0.f}, delta_r[2] = {0.f, 0.f};
+    // DOC, Q pass: my rows' document starts.  KV pass: for each of my two keys, the first query that starts its
+    // document after the key (the next document's first token, S if none): with starts non-decreasing along a row,
+    // key k is visible to query q >= k iff q < that bound, so the mask needs no per-column load.
+    [[maybe_unused]] int ds_r[2] = {0, 0};
+    if constexpr (DOC && KV_MODE) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int k = R0 + rl0 + 8 * h;
+        int lo = k + 1, hi = S;
+        while (lo < hi) {
+          const int mid = (lo + hi) >> 1;
+          if (__ldg(ds_row + mid) > k) hi = mid;
+          else lo = mid + 1;
+        }
+        ds_r[h] = lo;
+      }
+    }
     if (!KV_MODE) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const long long idx = ((long long)batch * nh + head_r) * S + R0 + rl0 + 8 * h;
         lse_r[h] = lse[idx] * LOG2E;
         delta_r[h] = delta[idx];
+        if constexpr (DOC) ds_r[h] = __ldg(ds_row + R0 + rl0 + 8 * h);
       }
     }
     [[maybe_unused]] float acc_a[KV_MODE ? 64 : 1];   // dV (KV pass)
@@ -226,7 +281,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
       fence_regs(dp);
       if (tr_thread && t < 64) trace[t * 8 + 0] = clock64();
       // causal: query index >= key index.  Only blocks that touch the diagonal need the compare.
-      const bool need_mask = KV_MODE ? (C0 < R0 + 127) : (C0 + 63 > R0);
+      bool need_mask = KV_MODE ? (C0 < R0 + 127) : (C0 + 63 > R0);
+      // DOC: and key index >= the query's document start, where a document begins inside the block
+      if constexpr (DOC) need_mask = need_mask || (KV_MODE ? c >= doc_bound : C0 < doc_bound);
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         const int col = 8 * (i >> 2) + 2 * tq + (i & 1);
@@ -242,7 +299,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
         }
         float p = fast_exp2(fmaf(sc[i], sl2, -l2));
         if (need_mask) {
-          const bool ok = KV_MODE ? (C0 + col >= R0 + row) : (R0 + row >= C0 + col);
+          bool ok = KV_MODE ? (C0 + col >= R0 + row) : (R0 + row >= C0 + col);
+          if constexpr (DOC) ok = ok && (KV_MODE ? C0 + col < ds_r[h] : C0 + col >= ds_r[h]);
           p = ok ? p : 0.f;
         }
         sc[i] = p;
@@ -318,8 +376,29 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
   }
 }
 
+template <bool TS, bool DOC>
+static void launch_attn_bwd(const CUtensorMap& tq_r, const CUtensorMap& tq_c, const CUtensorMap& td_r,
+                            const CUtensorMap& td_c, const float* lse, const float* delta, void* dqkv, int B, int S,
+                            int nh, int nkv, float scale, long long* trace, const int* doc_start, cudaStream_t s) {
+  static bool attr = false;
+  if (!attr) {
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<true, TS, DOC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        bwd::SMEM_BYTES));
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false, TS, DOC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        bwd::SMEM_BYTES));
+    attr = true;
+  }
+  const int nblk = S / 128;
+  attn_bwd_kernel<true, TS, DOC><<<dim3(B * nkv, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
+      tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace, doc_start);
+  attn_bwd_kernel<false, TS, DOC><<<dim3(B * nh, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
+      tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace ? trace + 512 : nullptr,
+      doc_start);
+}
+
 void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* trace_buf,
-              void* dqkv, int B, int S, int nh, int nkv, float scale, int mode, cudaStream_t s) {
+              void* dqkv, int B, int S, int nh, int nkv, float scale, int mode, cudaStream_t s,
+              const int* doc_start) {
   long long* trace = reinterpret_cast<long long*>(trace_buf);  // [2][64][8] int64 or nullptr
   if (S % 128 != 0) throw std::runtime_error("attn_bwd: sequence length must be a multiple of 128");
   const long long rows = (long long)B * S * nh;
@@ -329,30 +408,17 @@ void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse,
   const CUtensorMap tq_c = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 64);
   const CUtensorMap td_r = make_tmap_heads(d_o, B, S, nh, 128);
   const CUtensorMap td_c = make_tmap_heads(d_o, B, S, nh, 64);
-  static bool attr = false;
-  if (!attr) {
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
-    attr = true;
-  }
   static const bool ts_default = []() {   // DTG_ATTN_BWD=rs (default: P / dS stay in registers) | ss
     const char* e = getenv("DTG_ATTN_BWD");
     return e ? e[0] != 's' : true;
   }();
   const bool ts = mode == 0 ? ts_default : mode == 2;   // mode: 0 default, 1 = ss, 2 = rs
-  const int nblk = S / 128;
   if (ts) {
-    attn_bwd_kernel<true, true><<<dim3(B * nkv, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
-        tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace);
-    attn_bwd_kernel<false, true><<<dim3(B * nh, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
-        tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace ? trace + 512 : nullptr);
+    if (doc_start) launch_attn_bwd<true, true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, s);
+    else launch_attn_bwd<true, false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, s);
   } else {
-    attn_bwd_kernel<true, false><<<dim3(B * nkv, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
-        tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace);
-    attn_bwd_kernel<false, false><<<dim3(B * nh, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
-        tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace ? trace + 512 : nullptr);
+    if (doc_start) launch_attn_bwd<false, true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, s);
+    else launch_attn_bwd<false, false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, s);
   }
   note_launch(3);
   DTG_LAUNCH_CHECK();

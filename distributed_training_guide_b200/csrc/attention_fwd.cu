@@ -12,6 +12,11 @@
 // A operand (RS form) — the accumulator fragment of two n8 column blocks is exactly the A fragment of one
 // k16 step.  Version 1 stages P through 128B-swizzled shared memory (SS form).
 //
+// DOC (document masking): doc_start[b, q] is the first token of query q's document and key k is visible to q iff
+// doc_start[q] <= k <= q.  The first query of the tile has the smallest start, so the CTA visits key blocks from
+// doc_start[q0] / 128 to the diagonal and skips the rest; the element mask runs on the diagonal block and on the
+// blocks where some row's document begins.  DOC = false compiles to the plain causal kernel.
+//
 // Replaces torch SDPA / flash-attn-2 (mma.sync) that the reference uses (SURVEY.md K2/K3).
 #include <cuda.h>
 
@@ -37,10 +42,10 @@ struct Layout {
 };
 }  // namespace fwd
 
-template <bool P_REGS>
+template <bool P_REGS, bool DOC>
 __global__ void __launch_bounds__(fwd::THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __restrict__ o, float* __restrict__ lse,
-                int S, int nh, int nkv, float scale_log2, int num_m_blocks) {
+                int S, int nh, int nkv, float scale_log2, int num_m_blocks, const int* __restrict__ doc_start) {
   using namespace fwd;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -60,6 +65,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
   const int kv_head = head / (nh / nkv);
   const int n_blocks = m_block + 1;  // causal, BM == BN
   const int q0 = m_block * BM;
+  // first key block: the block holding the start of the tile's first query, clamped into [0, m_block]
+  int j_lo = 0;
+  if constexpr (DOC) j_lo = min(max(__ldg(doc_start + (long long)batch * S + q0) / BN, 0), m_block);
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tm_qkv);
@@ -81,9 +89,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
       tma_load_4d(&tm_qkv, q_full, smem + OFF_Q, 0, head, q0, batch);
       tma_load_4d(&tm_qkv, q_full, smem + OFF_Q + HALF_BYTES, 64, head, q0, batch);
       const int kh = nh + kv_head, vh = nh + nkv + kv_head;
-      for (int j = 0; j < n_blocks; ++j) {
-        const int st = j & 1;
-        const uint32_t ph = (uint32_t)((j >> 1) & 1);
+      for (int j = j_lo; j < n_blocks; ++j) {
+        const int st = (j - j_lo) & 1;
+        const uint32_t ph = (uint32_t)(((j - j_lo) >> 1) & 1);
         mbar_wait_mma(&k_empty[st], ph ^ 1);
         mbar_arrive_expect_tx(&k_full[st], TILE_BYTES);
         tma_load_4d(&tm_qkv, &k_full[st], smem + OFF_K + st * TILE_BYTES, 0, kh, j * BN, batch);
@@ -105,10 +113,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // l_run: this thread's partial row sums
+    [[maybe_unused]] int ds_r[2] = {0, 0};   // DOC: my rows' document starts
+    if constexpr (DOC && P_REGS) {
+      const int* ds = doc_start + (long long)batch * S + q0;
+      ds_r[0] = __ldg(ds + rl0);
+      ds_r[1] = __ldg(ds + rl0 + 8);
+    }
     mbar_wait_mma(q_full, 0);
-    for (int j = 0; j < n_blocks; ++j) {
-      const int st = j & 1;
-      const uint32_t ph = (uint32_t)((j >> 1) & 1);
+    for (int j = j_lo; j < n_blocks; ++j) {
+      const int st = (j - j_lo) & 1;
+      const uint32_t ph = (uint32_t)(((j - j_lo) >> 1) & 1);
       float s[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) s[i] = 0.f;
@@ -127,7 +141,24 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
         fence_regs(s);
       }
       if (signal) mbar_arrive(&k_empty[st]);
-      if (j == n_blocks - 1) {   // diagonal block: mask keys after the query
+      if constexpr (DOC) {
+        // mask keys after the query (diagonal block) and keys before the query's document start (blocks where
+        // one of my rows' documents begins)
+        if constexpr (!P_REGS) {
+          // version 1 runs at the 168-register cap: re-read the two starts (L1 hits) rather than keep them live
+          const int* ds = doc_start + (long long)batch * S + q0;
+          ds_r[0] = __ldg(ds + rl0);
+          ds_r[1] = __ldg(ds + rl0 + 8);
+        }
+        if (j == n_blocks - 1 || j * BN < max(ds_r[0], ds_r[1])) {
+#pragma unroll
+          for (int i = 0; i < 64; ++i) {
+            const int key = j * BN + 8 * (i >> 2) + 2 * tq + (i & 1);
+            const int h = (i >> 1) & 1;
+            if (key > q0 + rl0 + 8 * h || key < ds_r[h]) s[i] = -INFINITY;
+          }
+        }
+      } else if (j == n_blocks - 1) {   // diagonal block: mask keys after the query
 #pragma unroll
         for (int i = 0; i < 64; ++i) {
           const int col = 8 * (i >> 2) + 2 * tq + (i & 1);
@@ -146,6 +177,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
         mx = fmaxf(m_run[h], mx);
         alpha[h] = fast_exp2((m_run[h] - mx) * scale_log2);  // 0 on the first block (m_run = -inf)
         mb[h] = mx * scale_log2;
+        if constexpr (DOC) {
+          // a row whose document starts after every key seen so far: keep it empty (p = 0) instead of
+          // exp2(-inf - -inf) = NaN
+          if (mx == -INFINITY) {
+            alpha[h] = 1.f;
+            mb[h] = 0.f;
+          }
+        }
         m_run[h] = mx;
       }
       float sum[2] = {0.f, 0.f};
@@ -233,32 +272,36 @@ CUtensorMap make_tmap_heads(const void* base, int B, int S, int heads, int box_r
   return make_tmap_bf16(base, 4, dims, strides, box, true);
 }
 
-template <bool P_REGS>
+template <bool P_REGS, bool DOC>
 static void launch_attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale,
-                            cudaStream_t s) {
+                            cudaStream_t s, const int* doc_start) {
   if (S % 128 != 0) throw std::runtime_error("attn_fwd: sequence length must be a multiple of 128");
   if (nh % nkv != 0) throw std::runtime_error("attn_fwd: nh must be a multiple of nkv");
   const CUtensorMap tm = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 128);
   constexpr int smem = fwd::Layout<P_REGS>::SMEM_BYTES;
   static bool attr = false;
   if (!attr) {
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<P_REGS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<P_REGS, DOC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr = true;
   }
   const int num_m = S / 128;
-  attn_fwd_kernel<P_REGS><<<dim3(B * nh, num_m, 1), fwd::THREADS, smem, s>>>(tm, (__nv_bfloat16*)o, lse, S, nh, nkv,
-                                                                            scale * 1.4426950408889634f, num_m);
+  attn_fwd_kernel<P_REGS, DOC><<<dim3(B * nh, num_m, 1), fwd::THREADS, smem, s>>>(
+      tm, (__nv_bfloat16*)o, lse, S, nh, nkv, scale * 1.4426950408889634f, num_m, doc_start);
   note_launch();
   DTG_LAUNCH_CHECK();
 }
 
 // version 1: P through shared memory
-void attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s) {
-  launch_attn_fwd<false>(qkv, o, lse, B, S, nh, nkv, scale, s);
+void attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s,
+              const int* doc_start) {
+  if (doc_start) launch_attn_fwd<false, true>(qkv, o, lse, B, S, nh, nkv, scale, s, doc_start);
+  else launch_attn_fwd<false, false>(qkv, o, lse, B, S, nh, nkv, scale, s, nullptr);
 }
 // version 2: P stays in registers (RS-form PV MMA)
-void attn_fwd2(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s) {
-  launch_attn_fwd<true>(qkv, o, lse, B, S, nh, nkv, scale, s);
+void attn_fwd2(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s,
+               const int* doc_start) {
+  if (doc_start) launch_attn_fwd<true, true>(qkv, o, lse, B, S, nh, nkv, scale, s, doc_start);
+  else launch_attn_fwd<true, false>(qkv, o, lse, B, S, nh, nkv, scale, s, nullptr);
 }
 
 }  // namespace dtg

@@ -50,8 +50,11 @@ class TrainEngine:
     def create(cls, model_name: str, parallelism: str = "auto", batch_size: int = 1, seq_length: int = 1024,
                lr: float = 3e-5, seed: int = 0, device: Optional[str] = None, tensor_parallel: Optional[int] = None,
                cpu_offload: bool = False, checkpoint_activations: bool = False, prefetch_layers: bool = False,
-               num_layers: Optional[int] = None, lr_scaling: str = "none", fp8: bool = False, **extra):
-        """``fp8=True`` runs the decoder-layer projections in fp8 (``ops.fp8_linear``); single and ddp engines only."""
+               num_layers: Optional[int] = None, lr_scaling: str = "none", fp8: bool = False,
+               document_masking: bool = False, **extra):
+        """``fp8=True`` runs the decoder-layer projections in fp8 (``ops.fp8_linear``); single and ddp engines only.
+        ``document_masking=True``: batches that carry ``position_ids`` are packed documents, each starting where its
+        position id is 0; attention and targets stay inside each document (single, ddp and fsdp engines, Llama)."""
         import os
 
         world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -61,11 +64,15 @@ class TrainEngine:
             from .parallel.strategies import check_fp8_supported
 
             check_fp8_supported(parallelism)
+        if document_masking:
+            from .parallel.strategies import check_document_masking_supported
+
+            check_document_masking_supported(parallelism)
         args = SimpleNamespace(
             model_name=model_name, batch_size=batch_size, seq_length=seq_length, lr=lr, seed=seed, device=device,
             tensor_parallel=tensor_parallel or world, cpu_offload=cpu_offload,
             checkpoint_activations=checkpoint_activations, prefetch_layers=prefetch_layers, lr_scaling=lr_scaling,
-            fp8=fp8,
+            fp8=fp8, document_masking=document_masking,
             experiment_name=None, save_dir="../outputs", deterministic=False, local_rank=None, **extra,
         )
         strategy = make_strategy(parallelism, args)

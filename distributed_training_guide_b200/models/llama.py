@@ -203,9 +203,10 @@ class LlamaDecoderLayer(nn.Module):
         return torch.cat([self.mlp.gate_proj.weight, self.mlp.up_proj.weight], dim=0), None
 
     # forward ---------------------------------------------------------------------------
-    def forward(self, x, residual, cos, sin):
+    def forward(self, x, residual, cos, sin, doc_start=None):
         """x: [B,S,H] branch output of the previous layer (or the embeddings);
-        residual: running residual stream *before* adding x (None for the first layer).
+        residual: running residual stream *before* adding x (None for the first layer);
+        doc_start: None or int32 [B,S] from ``ops.document_starts`` (attention stays inside each document).
         Returns (mlp_out, residual) with the final add again deferred to the consumer."""
         att = self.self_attn
         B, S, _ = x.shape
@@ -214,7 +215,8 @@ class LlamaDecoderLayer(nn.Module):
         w, owner = self._qkv_weight()
         qkv = fused_linear(y, w, owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
         qkv = ops.rope_qkv_(qkv, cos, sin, att.num_heads + att.num_kv_heads)
-        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads).reshape(B, S, att.num_heads * att.head_dim)
+        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start)
+        a = a.reshape(B, S, att.num_heads * att.head_dim)
         a = ops.fp8_linear(a, att.o_proj.weight) if self.fp8 else att.o_proj(a)
         y, h = self.post_attention_layernorm(a, h)
         w, owner = self._gate_up_weight()
@@ -256,6 +258,10 @@ class LlamaForCausalLM(nn.Module):
         self.activation_checkpointing = False
         self.tp = None
         self.fp8 = False
+        #: packed documents (``--document-masking``): with ``position_ids`` given, a document starts at every token
+        #: whose position id is 0 (``ops.document_starts``); attention stays inside each document and the last token
+        #: of a document is not trained to predict the first token of the next.  Off: ``position_ids`` only feeds RoPE.
+        self.document_masking = False
 
     @property
     def fp8(self) -> bool:
@@ -295,7 +301,8 @@ class LlamaForCausalLM(nn.Module):
     def forward(self, input_ids, attention_mask=None, labels=None, position_ids=None, return_logits=None):
         """``attention_mask`` is accepted for API parity; the data pipeline only produces full
         (unpadded) chunks so only the causal mask is applied (the reference's all-ones mask
-        collapses to the same thing inside transformers, SURVEY.md K3)."""
+        collapses to the same thing inside transformers, SURVEY.md K3).  With ``document_masking``
+        and ``position_ids``, attention and targets stay inside each packed document."""
         if self.tp is not None:
             return self.tp.model_forward(self, input_ids, labels, position_ids)
         B, S = input_ids.shape
@@ -304,6 +311,9 @@ class LlamaForCausalLM(nn.Module):
             cos, sin = m.rotary_emb.tables(S, input_ids.device)
         else:
             cos, sin = m.rotary_emb(position_ids)
+        doc_start = None
+        if self.document_masking and position_ids is not None:
+            doc_start = ops.document_starts(position_ids)
         eng = self.engine
         if eng is not None:
             eng.pre_forward(self)
@@ -315,9 +325,9 @@ class LlamaForCausalLM(nn.Module):
             if self.activation_checkpointing and torch.is_grad_enabled():
                 from ..parallel.act_ckpt import checkpoint_layer
 
-                x, residual = checkpoint_layer(layer, x, residual, cos, sin)
+                x, residual = checkpoint_layer(layer, x, residual, cos, sin, doc_start)
             else:
-                x, residual = layer(x, residual, cos, sin)
+                x, residual = layer(x, residual, cos, sin, doc_start)
             if eng is not None:
                 x, residual = eng.post_layer(i, layer, x, residual)
         if eng is not None:
@@ -326,7 +336,10 @@ class LlamaForCausalLM(nn.Module):
         logits = self.lm_head(y.reshape(B * S, -1))  # [T, V], a fresh tensor the loss may consume
         loss = None
         if labels is not None:
-            tgt = ref.shift_labels(labels).reshape(-1)
+            tgt = ref.shift_labels(labels)
+            if doc_start is not None:
+                tgt = ref.drop_cross_document_targets(tgt, doc_start)
+            tgt = tgt.reshape(-1)
             if return_logits:
                 loss = ops.cross_entropy(logits.clone(), tgt)
             else:

@@ -27,7 +27,7 @@ from .. import _ext
 from . import reference as ref
 
 __all__ = [
-    "linear", "fused_linear", "rms_norm", "add_rms_norm", "rope_qkv_", "attention_qkv", "swiglu", "cross_entropy",
+    "linear", "fused_linear", "rms_norm", "add_rms_norm", "rope_qkv_", "attention_qkv", "document_starts", "swiglu", "cross_entropy",
     "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "ref",
 ]
 
@@ -367,38 +367,60 @@ def rope_qkv_(qkv, cos, sin, n_rot_heads):
 # --------------------------------------------------------------------------------------
 class _AttentionQKV(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, nh, nkv, scale):
+    def forward(ctx, qkv, nh, nkv, scale, doc_start=None):
         C = _ext.load()
-        o, lse = C.attn_fwd(qkv, nh, nkv, float(scale))
-        ctx.save_for_backward(qkv, o, lse)
+        o, lse = C.attn_fwd(qkv, nh, nkv, float(scale), doc_start=doc_start)
+        ctx.save_for_backward(qkv, o, lse, doc_start)
         ctx.meta = (nh, nkv, scale)
         return o
 
     @staticmethod
     def backward(ctx, do):
         C = _ext.load()
-        qkv, o, lse = ctx.saved_tensors
+        qkv, o, lse, doc_start = ctx.saved_tensors
         nh, nkv, scale = ctx.meta
-        dqkv = C.attn_bwd(do.contiguous(), qkv, o, lse, nh, nkv, float(scale))
-        return dqkv, None, None, None
+        dqkv = C.attn_bwd(do.contiguous(), qkv, o, lse, nh, nkv, float(scale), doc_start=doc_start)
+        return dqkv, None, None, None, None
 
 
-def attention_qkv(qkv, nh, nkv, scale=None):
-    """Causal self-attention. qkv: [B,S,nh+2*nkv,d] (q heads | k heads | v heads) -> [B,S,nh,d]."""
+def document_starts(position_ids):
+    """Document masking convention: a document starts at every token whose position id is 0, and at the first
+    token of every row.  ``position_ids`` [B, S] -> int32 [B, S]: for each token, the index within its row of the
+    first token of its document.  Non-decreasing along a row and never above the token's own index.  One cummax on
+    the device, no host synchronisation.  The attention kernels let query q see key k iff start[q] <= k <= q."""
+    B, S = position_ids.shape
+    idx = torch.arange(S, device=position_ids.device, dtype=torch.int32).expand(B, S)
+    is_start = position_ids == 0
+    is_start[:, 0] = True
+    return torch.where(is_start, idx, torch.zeros_like(idx)).cummax(dim=1).values.to(torch.int32).contiguous()
+
+
+def attention_qkv(qkv, nh, nkv, scale=None, doc_start=None):
+    """Causal self-attention. qkv: [B,S,nh+2*nkv,d] (q heads | k heads | v heads) -> [B,S,nh,d].
+    ``doc_start`` (int32 [B,S] from ``document_starts``, or None): document masking, query q sees key k iff
+    ``doc_start[q] <= k <= q``."""
     d = qkv.shape[-1]
     scale = scale if scale is not None else 1.0 / math.sqrt(d)
     if _ext.use_cuda_kernel("attention", qkv) and qkv.dtype == torch.bfloat16 and d == 128 and qkv.shape[1] % 128 == 0:
+        if doc_start is not None:
+            return _AttentionQKV.apply(qkv, nh, nkv, scale, doc_start.to(torch.int32).contiguous())
         return _AttentionQKV.apply(qkv, nh, nkv, scale)
     q, k, v = qkv[:, :, :nh], qkv[:, :, nh:nh + nkv], qkv[:, :, nh + nkv:]
     if qkv.is_cuda:
         # head dims other than 128 (GPT-2 style / toy configs) and sequence lengths that are not a multiple of
         # the 128-row tile are outside the sm_90a kernel's scope; use the library kernel rather than the
         # O(S^2)-memory reference
-        o = torch.nn.functional.scaled_dot_product_attention(
-            q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=True, scale=scale,
-            enable_gqa=(nh != nkv))
+        if doc_start is not None:
+            mask = ref.document_mask(doc_start, qkv.shape[1])[:, None]  # [B, 1, S, S]
+            o = torch.nn.functional.scaled_dot_product_attention(
+                q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), attn_mask=mask, scale=scale,
+                enable_gqa=(nh != nkv))
+        else:
+            o = torch.nn.functional.scaled_dot_product_attention(
+                q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=True, scale=scale,
+                enable_gqa=(nh != nkv))
         return o.transpose(1, 2)
-    return ref.attention(q, k, v, causal=True, scale=scale)
+    return ref.attention(q, k, v, causal=True, scale=scale, doc_start=doc_start)
 
 
 # --------------------------------------------------------------------------------------

@@ -67,8 +67,17 @@ def rope_apply(x, cos, sin, inverse=False):
     return out.to(x.dtype)
 
 
-def attention(q, k, v, causal=True, scale=None):
-    """q: [B, S, nh, d]; k, v: [B, S, nkv, d] -> [B, S, nh, d]. fp32 softmax."""
+def document_mask(doc_start, S):
+    """bool [B, S, S]: query q may see key k iff ``doc_start[b, q] <= k <= q`` (causal attention inside each
+    document; ``doc_start`` as ``ops.document_starts`` returns it)."""
+    k = torch.arange(S, device=doc_start.device)
+    causal = k[None, :] <= k[:, None]
+    return causal[None] & (k[None, None, :] >= doc_start.long()[:, :, None])
+
+
+def attention(q, k, v, causal=True, scale=None, doc_start=None):
+    """q: [B, S, nh, d]; k, v: [B, S, nkv, d] -> [B, S, nh, d]. fp32 softmax.  ``doc_start`` (int [B, S]):
+    document masking on top of the causal mask (see ``document_mask``)."""
     B, S, nh, d = q.shape
     nkv = k.shape[2]
     scale = scale if scale is not None else 1.0 / math.sqrt(d)
@@ -80,7 +89,9 @@ def attention(q, k, v, causal=True, scale=None):
         kf = kf.repeat_interleave(rep, dim=1)
         vf = vf.repeat_interleave(rep, dim=1)
     s = torch.matmul(qf, kf.transpose(-1, -2)) * scale
-    if causal:
+    if doc_start is not None:
+        s = s.masked_fill(~document_mask(doc_start, S)[:, None], float("-inf"))
+    elif causal:
         mask = torch.ones(S, k.shape[1], dtype=torch.bool, device=q.device).tril()
         s = s.masked_fill(~mask, float("-inf"))
     p = torch.softmax(s, dim=-1)
@@ -102,6 +113,17 @@ def shift_labels(labels):
     """HF causal-LM convention: token t predicts label t+1; last position ignored."""
     pad = torch.full_like(labels[..., :1], -100)
     return torch.cat([labels[..., 1:], pad], dim=-1)
+
+
+def drop_cross_document_targets(shifted, doc_start, ignore_index=-100):
+    """``shifted`` [B, S] targets after ``shift_labels``: the target of token t is token t+1.  Where token t+1 starts
+    a document (``doc_start[t+1] == t+1``), the target becomes ``ignore_index``, so the last token of one document
+    is not trained to predict the first token of the next."""
+    S = doc_start.shape[-1]
+    first = doc_start == torch.arange(S, device=doc_start.device, dtype=doc_start.dtype)
+    nxt = torch.zeros_like(first)
+    nxt[..., :-1] = first[..., 1:]
+    return shifted.masked_fill(nxt, ignore_index)
 
 
 def cross_entropy(logits, targets, ignore_index=-100):

@@ -12,14 +12,19 @@ from __future__ import annotations
 import torch
 
 
+def _doc(doc_start):
+    # the tensor-parallel layer adapter takes no doc_start: pass it only when there is one
+    return () if doc_start is None else (doc_start,)
+
+
 class _CheckpointLayer(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, layer, cos, sin, x, residual):
-        ctx.layer, ctx.cos, ctx.sin = layer, cos, sin
+    def forward(ctx, layer, cos, sin, doc_start, x, residual):
+        ctx.layer, ctx.cos, ctx.sin, ctx.doc_start = layer, cos, sin, doc_start
         ctx.has_res = residual is not None
         ctx.save_for_backward(x, *([residual] if residual is not None else []))
         with torch.no_grad():
-            out, res = layer(x, residual, cos, sin)
+            out, res = layer(x, residual, cos, sin, *_doc(doc_start))
         return out, res
 
     @staticmethod
@@ -28,15 +33,16 @@ class _CheckpointLayer(torch.autograd.Function):
         x = saved[0].detach().requires_grad_(True)
         residual = saved[1].detach().requires_grad_(True) if ctx.has_res else None
         with torch.enable_grad():
-            out, res = ctx.layer(x, residual, ctx.cos, ctx.sin)
+            out, res = ctx.layer(x, residual, ctx.cos, ctx.sin, *_doc(ctx.doc_start))
         outs, grads = [], []
         for o, g in ((out, d_out), (res, d_res)):
             if g is not None and o.requires_grad:
                 outs.append(o)
                 grads.append(g)
         torch.autograd.backward(outs, grads)
-        return None, None, None, x.grad, (residual.grad if ctx.has_res else None)
+        return None, None, None, None, x.grad, (residual.grad if ctx.has_res else None)
 
 
-def checkpoint_layer(layer, x, residual, cos, sin):
-    return _CheckpointLayer.apply(layer, cos, sin, x, residual)
+def checkpoint_layer(layer, x, residual, cos, sin, doc_start=None):
+    """``doc_start``: None or the int32 [B,S] document starts the layer's attention masks with."""
+    return _CheckpointLayer.apply(layer, cos, sin, doc_start, x, residual)

@@ -142,6 +142,7 @@ class SingleDevice(Strategy):
         self.groups, self.symm, self.registry = _flat_groups_on(self, model, 1)
         _load_pretrained(args, model=model)
         _apply_fp8(args, model)
+        _apply_document_masking(args, model)
         return model
 
     def build_optimizer(self, args, model, lr):
@@ -181,6 +182,28 @@ def _apply_fp8(args, model):
 def check_fp8_supported(parallelism: str):
     if parallelism not in FP8_PARALLELISMS:
         raise ValueError(f"fp8 is supported by the {', '.join(FP8_PARALLELISMS)} engines, not {parallelism!r}")
+
+
+#: engines that run ``LlamaForCausalLM.forward`` and so support ``--document-masking``; the tensor-parallel and 2-D
+#: engines run their own layer loop (``tp.model_forward``)
+DOCUMENT_MASKING_PARALLELISMS = ("single", "ddp", "ddp_allreduce", "fsdp")
+
+
+def _apply_document_masking(args, model):
+    """``model.document_masking = args.document_masking`` (Llama models only)."""
+    if not getattr(args, "document_masking", False):
+        return
+    from ..models.llama import LlamaForCausalLM
+
+    if not isinstance(model, LlamaForCausalLM):
+        raise ValueError(f"document masking applies to the Llama models, not {type(model).__name__}")
+    model.document_masking = True
+
+
+def check_document_masking_supported(parallelism: str):
+    if parallelism not in DOCUMENT_MASKING_PARALLELISMS:
+        raise ValueError(f"document masking is supported by the {', '.join(DOCUMENT_MASKING_PARALLELISMS)} engines, "
+                         f"not {parallelism!r}")
 
 
 def _load_pretrained(args, model=None, engine=None, default="never"):
@@ -242,6 +265,7 @@ class DataParallelZero1(Strategy):
                 for g in self.groups:
                     dist.broadcast(g.param, src=0)
         _apply_fp8(args, model)
+        _apply_document_masking(args, model)
         self.model = model
         return model
 
@@ -296,6 +320,7 @@ class FullyShardedDataParallel(Strategy):
                                  seed=getattr(args, "seed", 0), cpu_offload=getattr(args, "cpu_offload", False),
                                  prefetch=True, prefetch_depth=2 if getattr(args, "prefetch_layers", False) else 1)
         model.activation_checkpointing = bool(getattr(args, "checkpoint_activations", False))
+        _apply_document_masking(args, model)
         self.groups = self.engine.groups
         self.model = model
         # chapter 05 (reference 05:76-145): rank 0 reads the checkpoint, every rank keeps its slice of each group

@@ -43,6 +43,7 @@ def _record(fn):
 
 def train(args, strategy):
     """Run the chapter.  Returns the final ``state`` dict plus the last log record."""
+    data_utils.check_document_masking_args(args)
     env = strategy.setup(args)
     setup_logging(env.rank if strategy.log_rank_prefix else None)
     LOGGER.debug(args)

@@ -13,10 +13,10 @@ COMMON = ("experiment-name", "dataset-name", "dataset-subset", "model-name", "sa
           "num-epochs", "lr", "batch-size", "log-freq", "ckpt-freq", "seq-length")
 
 CHAPTER_EXTRAS = {
-    "01-single-gpu": ("fp8",),
-    "02-distributed-data-parallel": ("fp8",),
-    "04-fully-sharded-data-parallel": ("cpu-offload",),
-    "05-training-llama-405b": ("cpu-offload", "checkpoint-activations", "prefetch-layers"),
+    "01-single-gpu": ("fp8", "document-masking"),
+    "02-distributed-data-parallel": ("fp8", "document-masking"),
+    "04-fully-sharded-data-parallel": ("cpu-offload", "document-masking"),
+    "05-training-llama-405b": ("cpu-offload", "checkpoint-activations", "prefetch-layers", "document-masking"),
     "06-tensor-parallel": (),
     "07-2d-parallel": ("tensor-parallel",),
     "deepspeed": ("local_rank", "zero_config"),
@@ -61,6 +61,14 @@ def get_parser(chapter: str = "01-single-gpu", require_experiment: bool = False)
         p.add_argument("--fp8", default=False, action="store_true",
                        help="run the decoder-layer projections (q|k|v, o, gate|up, down) as fp8 GEMMs with per-tensor "
                             "current scaling: x and W in e4m3, output gradients in e5m2")
+    if "document-masking" in extras:
+        p.add_argument("--document-masking", default=False, action="store_true",
+                       help="packed documents: every sample carries position_ids that restart at 0 at each document, "
+                            "attention stays inside each document and no token is trained to predict the next "
+                            "document's first token (Llama models)")
+        p.add_argument("--eos-token-id", default=None, type=int,
+                       help="with --document-masking and a .bin dataset: a document starts after each occurrence of "
+                            "this token id")
     if "cpu-offload" in extras:
         p.add_argument("--cpu-offload", default=False, action="store_true")
     if "checkpoint-activations" in extras:

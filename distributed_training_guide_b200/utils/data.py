@@ -12,6 +12,12 @@ sources because the GPU boxes have no network:
                           tokenised with the model's tokenizer if one is on disk, else bytes;
   * ``-d <hf dataset id>`` the reference's path through ``datasets`` + ``AutoTokenizer``.
 
+``--document-masking`` adds ``position_ids`` to every sample: they count up from 0 inside each document, and a
+chunk's first token always has position 0 (a document cut by a chunk boundary continues as a new document in the
+next chunk).  Without the flag the samples keep exactly the three keys above.  Where documents come from: each
+text of a ``.txt`` / ``.jsonl`` file, each example of a hub dataset, the tokens after each ``--eos-token-id`` in a
+``.bin`` file, and seeded random cut points for ``synthetic``.
+
 Differences kept deliberately: pinned host memory + non-blocking H2D (the reference copies
 from pageable memory, SURVEY.md §8 #24), and ``set_epoch`` is called in every chapter
 (the reference forgets it in chapters 06/07, §8 #6).
@@ -32,29 +38,68 @@ from torch.utils.data.distributed import DistributedSampler
 LOGGER = logging.getLogger("dtg_b200")
 
 
-class SyntheticTokens(Dataset):
-    """``num_samples`` chunks of uniformly random token ids (generated once, up front)."""
+def positions_from_starts(starts):
+    """Position ids (int64, same shape) from boolean document-start flags [..., S]: each token's distance from the
+    last start at or before it.  The first token of every row is a start whatever its flag says."""
+    starts = torch.as_tensor(starts, dtype=torch.bool).clone()
+    starts[..., 0] = True
+    idx = torch.arange(starts.shape[-1], device=starts.device).expand(starts.shape)
+    return idx - torch.where(starts, idx, torch.zeros_like(idx)).cummax(dim=-1).values
 
-    def __init__(self, num_samples: int, seq_length: int, vocab_size: int, seed: int = 0):
+
+def positions_after_eos(ids, eos_token_id: int):
+    """Position ids of a [..., S] id tensor in which a document starts after each ``eos_token_id``; runs on the
+    tensor's device without a host synchronisation."""
+    starts = torch.zeros(ids.shape, dtype=torch.bool, device=ids.device)
+    starts[..., 1:] = ids[..., :-1] == eos_token_id
+    return positions_from_starts(starts)
+
+
+class SyntheticTokens(Dataset):
+    """``num_samples`` chunks of uniformly random token ids (generated once, up front).
+
+    ``document_masking=True`` keeps the same tokens and adds ``position_ids`` from seeded random document cut
+    points (a generator of its own, so the tokens do not change): inside each chunk, document lengths are drawn
+    independently and uniformly from 1 .. max(1, seq_length // 2) starting at token 0, and the last document is cut
+    at the chunk end.  Documents therefore average about seq_length / 4 tokens."""
+
+    def __init__(self, num_samples: int, seq_length: int, vocab_size: int, seed: int = 0, document_masking=False):
         g = torch.Generator().manual_seed(seed)
         self.tokens = torch.randint(0, vocab_size, (num_samples, seq_length), generator=g, dtype=torch.int64)
+        self.starts = None
+        if document_masking:
+            gd = torch.Generator().manual_seed(seed + 0x5EED)
+            max_len = max(1, seq_length // 2)
+            self.starts = torch.zeros(num_samples, seq_length, dtype=torch.bool)
+            for i in range(num_samples):
+                pos = 0
+                while pos < seq_length:
+                    self.starts[i, pos] = True
+                    pos += int(torch.randint(1, max_len + 1, (1,), generator=gd))
 
     def __len__(self):
         return self.tokens.shape[0]
 
     def __getitem__(self, i):
         t = self.tokens[i]
-        return {"input_ids": t, "attention_mask": torch.ones_like(t), "labels": t.clone()}
+        out = {"input_ids": t, "attention_mask": torch.ones_like(t), "labels": t.clone()}
+        if self.starts is not None:
+            out["position_ids"] = positions_from_starts(self.starts[i])
+        return out
 
 
 class TokenChunks(Dataset):
-    """A flat token stream cut into ``seq_length`` chunks (remainder dropped)."""
+    """A flat token stream cut into ``seq_length`` chunks (remainder dropped).  For document masking, either
+    ``starts`` (a boolean array over the stream: the token begins a document) or ``eos_token_id`` (a document starts
+    after each occurrence) gives every chunk its ``position_ids``."""
 
-    def __init__(self, tokens, seq_length: int):
+    def __init__(self, tokens, seq_length: int, starts=None, eos_token_id=None):
         n = (len(tokens) // seq_length) * seq_length
         self.tokens = tokens
         self.seq_length = seq_length
         self.n_chunks = n // seq_length
+        self.starts = starts
+        self.eos_token_id = eos_token_id
 
     def __len__(self):
         return self.n_chunks
@@ -62,7 +107,12 @@ class TokenChunks(Dataset):
     def __getitem__(self, i):
         s = self.seq_length
         t = torch.from_numpy(np.asarray(self.tokens[i * s:(i + 1) * s]).astype(np.int64))
-        return {"input_ids": t, "attention_mask": torch.ones_like(t), "labels": t.clone()}
+        out = {"input_ids": t, "attention_mask": torch.ones_like(t), "labels": t.clone()}
+        if self.starts is not None:
+            out["position_ids"] = positions_from_starts(torch.from_numpy(np.asarray(self.starts[i * s:(i + 1) * s])))
+        elif self.eos_token_id is not None:
+            out["position_ids"] = positions_after_eos(t, self.eos_token_id)
+        return out
 
 
 class ByteTokenizer:
@@ -107,32 +157,49 @@ def clamp_seq_length(seq_length, config):
     return seq_length
 
 
+def check_document_masking_args(args):
+    """Refuse, before anything is built, a ``--document-masking`` run whose documents cannot be found."""
+    if not getattr(args, "document_masking", False):
+        return
+    name = getattr(args, "dataset_name", None) or ""
+    if name.endswith(".bin") and getattr(args, "eos_token_id", None) is None:
+        raise ValueError("--document-masking with a .bin dataset needs --eos-token-id: documents start after it")
+
+
 def load_and_preprocess_data(args, config, dp_size: int = 1):
     """Returns the training ``Dataset``.  ``args`` needs dataset_name, dataset_subset,
-    model_name, seq_length, seed, batch_size (+ optional num_samples)."""
+    model_name, seq_length, seed, batch_size (+ optional num_samples, document_masking, eos_token_id)."""
+    check_document_masking_args(args)
+    docs = bool(getattr(args, "document_masking", False))
     seq_length = clamp_seq_length(args.seq_length, config)
     name = args.dataset_name
     if name == "synthetic":
         n = getattr(args, "num_samples", None) or 64 * args.batch_size * dp_size
-        return SyntheticTokens(n, seq_length, config.vocab_size, seed=args.seed)
+        return SyntheticTokens(n, seq_length, config.vocab_size, seed=args.seed, document_masking=docs)
     if os.path.isfile(name) and name.endswith(".bin"):
         dtype = np.uint16 if config.vocab_size <= 65536 else np.uint32
-        ds = TokenChunks(np.memmap(name, dtype=dtype, mode="r"), seq_length)
+        ds = TokenChunks(np.memmap(name, dtype=dtype, mode="r"), seq_length,
+                         eos_token_id=args.eos_token_id if docs else None)
         ds.path, ds.vocab_size = name, config.vocab_size  # lets build_dataloader pick the native C++ loader
         return ds
     if os.path.isfile(name):
         tok = _load_tokenizer(args.model_name)
         if tok is None:
             bt = ByteTokenizer()
-            ids = list(chain.from_iterable(bt.encode(t) for t in _read_texts(name)))
+            texts = [bt.encode(t) for t in _read_texts(name)]
         else:
-            ids = list(chain.from_iterable(tok(t)["input_ids"] for t in _read_texts(name)))
-        ids = np.asarray(ids, dtype=np.int64) % config.vocab_size
-        return TokenChunks(ids, seq_length)
-    return _load_hf(args, config, seq_length)
+            texts = [tok(t)["input_ids"] for t in _read_texts(name)]
+        ids = np.asarray(list(chain.from_iterable(texts)), dtype=np.int64) % config.vocab_size
+        starts = None
+        if docs:  # each text is one document
+            offsets = np.cumsum([0] + [len(t) for t in texts[:-1]])
+            starts = np.zeros(len(ids), dtype=bool)
+            starts[offsets[offsets < len(ids)]] = True
+        return TokenChunks(ids, seq_length, starts=starts)
+    return _load_hf(args, config, seq_length, docs)
 
 
-def _load_hf(args, config, seq_length):
+def _load_hf(args, config, seq_length, document_masking=False):
     """The reference's path (HF hub or ``$HF_HOME`` cache)."""
     import multiprocessing
 
@@ -148,10 +215,14 @@ def _load_hf(args, config, seq_length):
                          num_proc=nproc, desc="tokenizing")
 
     def group(examples):
+        if document_masking:  # each example is one document: its positions count up from 0
+            examples = dict(examples, position_ids=[list(range(len(x))) for x in examples["input_ids"]])
         cat = {k: list(chain(*examples[k])) for k in examples.keys()}
         total = (len(cat["input_ids"]) // seq_length) * seq_length
         out = {k: [v[i:i + seq_length] for i in range(0, total, seq_length)] for k, v in cat.items()}
         out["labels"] = [list(x) for x in out["input_ids"]]
+        if document_masking:  # a document cut by the chunk boundary continues as a new one
+            out["position_ids"] = [positions_from_starts(torch.tensor(p) == 0).tolist() for p in out["position_ids"]]
         return out
 
     lm = tokenized.map(group, batched=True, num_proc=nproc, desc=f"chunking to {seq_length}")
@@ -164,7 +235,8 @@ class NativeTokenLoader:
     producer thread filling a ring of pinned [batch, seq] buffers.  Quacks like a DataLoader as far as
     ``trainer.train`` is concerned (``len``, ``iter``, ``.sampler.set_epoch``)."""
 
-    def __init__(self, path, seq_length, vocab_size, batch_size, dp_size=1, dp_rank=0, seed=0, depth=4):
+    def __init__(self, path, seq_length, vocab_size, batch_size, dp_size=1, dp_rank=0, seed=0, depth=4,
+                 eos_token_id=None):
         from .. import _ext
 
         C = _ext.load(required=True)
@@ -174,6 +246,7 @@ class NativeTokenLoader:
         self.sampler = self
         self._epoch = 0
         self._started = True  # the constructor already started epoch 0
+        self.eos_token_id = eos_token_id  # document masking: to_device derives position_ids on the device
 
     def set_epoch(self, epoch):
         self._epoch = epoch
@@ -189,16 +262,18 @@ class NativeTokenLoader:
         self._started = False
         for _ in range(len(self)):
             ids = self._loader.next()
-            yield RingBatch({"input_ids": ids, "attention_mask": torch.ones_like(ids), "labels": ids}, self._loader)
+            yield RingBatch({"input_ids": ids, "attention_mask": torch.ones_like(ids), "labels": ids}, self._loader,
+                            self.eos_token_id)
 
 
 class RingBatch(dict):
     """A batch whose tensors alias a pinned ring slot of the native loader.  ``to_device`` reports its asynchronous
     H2D copies back (``copied()``) so the producer thread never overwrites a slot whose DMA has not executed yet."""
 
-    def __init__(self, tensors, loader):
+    def __init__(self, tensors, loader, eos_token_id=None):
         super().__init__(tensors)
         self._loader = loader
+        self.eos_token_id = eos_token_id
 
     def copied(self):
         if torch.cuda.is_available():
@@ -226,7 +301,7 @@ def build_dataloader(dataset, batch_size, dp_size=1, dp_rank=0, seed=0, distribu
 
         if _ext.available():
             return NativeTokenLoader(dataset.path, dataset.seq_length, dataset.vocab_size, batch_size, dp_size, dp_rank,
-                                     seed)
+                                     seed, eos_token_id=dataset.eos_token_id)
     if pin_memory is None:
         pin_memory = torch.cuda.is_available()
     gen = torch.Generator().manual_seed(seed)
@@ -248,4 +323,7 @@ def to_device(batch, device):
     out = {k: v.to(device=device, non_blocking=nb) for k, v in batch.items()}
     if nb and isinstance(batch, RingBatch):
         batch.copied()
+    if getattr(batch, "eos_token_id", None) is not None:
+        # native .bin loader with document masking: positions from the ids already on the device
+        out["position_ids"] = positions_after_eos(out["input_ids"], batch.eos_token_id)
     return out
