@@ -43,6 +43,19 @@ void comm_nvls_allreduce_scale(void* mc, const SymmPads& pads, size_t elem_off, 
 void comm_nvls_rs_adamw(const void* grads_mc, void* params_mc, void* params_local, void* m, void* v, bool state_fp32,
                         bool push_params, const SymmPads& pads, size_t elem_off, size_t n, const AdamWHyper& hp, int rank,
                         int nranks, uint32_t epoch, int* err, int blocks, cudaStream_t s);
+// Gradient clipping, grad_clip.cu.  `ranges`: device int64 [nranges][2] of [begin, end) parameter element ranges
+// of the bucket (sorted, disjoint); `partials`: one fp64 sum of squares per CTA.
+void comm_reduce_sumsq(const SymmPtrs& buf, const SymmPads& pads, size_t elem_off, size_t n, float scale,
+                       bool broadcast, const long long* ranges, int nranges, double* partials, int rank, int nranks,
+                       uint32_t epoch, int* err, int blocks, cudaStream_t s);
+void comm_nvls_reduce_sumsq(void* mc, void* local, const SymmPads& pads, size_t elem_off, size_t n, float scale,
+                            bool broadcast, const long long* ranges, int nranges, double* partials, int rank,
+                            int nranks, uint32_t epoch, int* err, int blocks, cudaStream_t s);
+void comm_clip_finalize(const double* partials, int nparts, const SymmPtrs& slots, const SymmPads& pads, int parity,
+                        float norm_scale, float max_norm, float* out, int rank, int nranks, uint32_t epoch, int* err,
+                        cudaStream_t s);
+void adamw_clip(const SymmPtrs& dst, void* dst_mc, const void* p_src, const void* g, void* m, void* v, bool state_fp32,
+                long long n, const AdamWHyper& hp, const float* coef, int ndst, cudaStream_t s);
 
 
 // ---- fused_tp.cu / cross_entropy.cu helpers used by the tensor-parallel path ------------------------

@@ -180,6 +180,74 @@ void barrier(const std::vector<uint64_t>& pads, int64_t rank, int64_t epoch, con
   comm_barrier(pads_of(pads), (int)rank, (int)pads.size(), (uint32_t)epoch, err_ptr(err), stream());
 }
 
+// ---- gradient clipping (grad_clip.cu) ---------------------------------------------------------------------------
+void check_clip_tables(const Tensor& ranges, const Tensor& partials, int64_t blocks) {
+  TORCH_CHECK(ranges.is_cuda() && ranges.scalar_type() == at::kLong && ranges.is_contiguous() && ranges.dim() == 2 &&
+                  ranges.size(1) == 2,
+              "ranges must be a contiguous int64 [R, 2] CUDA tensor");
+  TORCH_CHECK(partials.is_cuda() && partials.scalar_type() == at::kDouble && partials.is_contiguous() &&
+                  partials.numel() >= blocks,
+              "partials must be a contiguous fp64 CUDA tensor of at least `blocks` elements");
+}
+
+void reduce_sumsq(const std::vector<uint64_t>& buf, const std::vector<uint64_t>& pads, int64_t elem_off, int64_t n,
+                  double scale, bool broadcast, const Tensor& ranges, Tensor& partials, int64_t rank, int64_t epoch,
+                  const c10::optional<Tensor>& err, int64_t blocks) {
+  check_clip_tables(ranges, partials, blocks);
+  comm_reduce_sumsq(rotated(buf, (int)rank), pads_of(pads), (size_t)elem_off, (size_t)n, (float)scale, broadcast,
+                    (const long long*)ranges.data_ptr<int64_t>(), (int)ranges.size(0), partials.data_ptr<double>(), (int)rank,
+                    (int)buf.size(), (uint32_t)epoch, err_ptr(err), (int)blocks, stream());
+}
+
+void nvls_reduce_sumsq(uint64_t mc, uint64_t local, const std::vector<uint64_t>& pads, int64_t elem_off, int64_t n,
+                       double scale, bool broadcast, const Tensor& ranges, Tensor& partials, int64_t rank,
+                       int64_t epoch, const c10::optional<Tensor>& err, int64_t blocks) {
+  check_clip_tables(ranges, partials, blocks);
+  comm_nvls_reduce_sumsq((void*)mc, (void*)local, pads_of(pads), (size_t)elem_off, (size_t)n, (float)scale, broadcast,
+                         (const long long*)ranges.data_ptr<int64_t>(), (int)ranges.size(0), partials.data_ptr<double>(), (int)rank,
+                         (int)pads.size(), (uint32_t)epoch, err_ptr(err), (int)blocks, stream());
+}
+
+// slots: every rank's slot buffer in RANK order (not rotated)
+void clip_finalize(const Tensor& partials, const std::vector<uint64_t>& slots, const std::vector<uint64_t>& pads,
+                   int64_t parity, double norm_scale, double max_norm, Tensor& out, int64_t rank, int64_t epoch,
+                   const c10::optional<Tensor>& err) {
+  TORCH_CHECK(partials.is_cuda() && partials.scalar_type() == at::kDouble && partials.is_contiguous(),
+              "partials must be a contiguous fp64 CUDA tensor");
+  TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kFloat && out.is_contiguous() && out.numel() >= 2,
+              "out must be a contiguous fp32 CUDA tensor of 2 elements (norm, coef)");
+  TORCH_CHECK(slots.size() == pads.size() && slots.size() >= 1 && slots.size() <= (size_t)kMaxRanks,
+              "one slot buffer per rank");
+  SymmPtrs sp{};
+  for (size_t k = 0; k < slots.size(); ++k) sp.ptr[k] = (char*)slots[k];
+  comm_clip_finalize(partials.data_ptr<double>(), (int)partials.numel(), sp, pads_of(pads), (int)parity,
+                     (float)norm_scale, (float)max_norm, out.data_ptr<float>(), (int)rank, (int)pads.size(),
+                     (uint32_t)epoch, err_ptr(err), stream());
+}
+
+// AdamW on p_src / g / m / v (one rank's range) with g *= coef[0]; the new parameters go to every address of `dst`
+// (the same range on each replica), or through the multicast address `dst_mc` when it is not 0.
+void adamw_clip_(const std::vector<uint64_t>& dst, uint64_t dst_mc, const Tensor& p_src, const Tensor& g, Tensor& m,
+                 Tensor& v, double lr, double b1, double b2, double eps, double wd, int64_t step, double grad_scale,
+                 const Tensor& coef) {
+  for (const Tensor* t : {&p_src, &g}) {
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kBFloat16 && t->is_contiguous() &&
+                    (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0,
+                "adamw_clip: parameters and gradients must be contiguous, 16-byte aligned bf16 CUDA tensors");
+  }
+  const bool fp32 = m.scalar_type() == at::kFloat;
+  TORCH_CHECK(m.scalar_type() == v.scalar_type() && (fp32 || m.scalar_type() == at::kBFloat16), "bad state dtype");
+  TORCH_CHECK(m.is_contiguous() && v.is_contiguous(), "optimizer state must be contiguous");
+  TORCH_CHECK(p_src.numel() == g.numel() && g.numel() == m.numel() && m.numel() == v.numel(), "size mismatch");
+  TORCH_CHECK(coef.is_cuda() && coef.scalar_type() == at::kFloat && coef.numel() >= 1, "coef must be fp32 on the device");
+  TORCH_CHECK(dst_mc != 0 || (dst.size() >= 1 && dst.size() <= (size_t)kMaxRanks), "1..8 destinations");
+  SymmPtrs sp{};
+  for (size_t k = 0; k < dst.size() && k < (size_t)kMaxRanks; ++k) sp.ptr[k] = (char*)dst[k];
+  AdamWHyper hp = make_adamw_hyper((float)lr, (float)b1, (float)b2, (float)eps, (float)wd, (int)step, (float)grad_scale);
+  adamw_clip(sp, (void*)dst_mc, p_src.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), fp32, p_src.numel(), hp,
+             coef.data_ptr<float>(), (int)dst.size(), stream());
+}
+
 }  // namespace
 
 void bind_comm(pybind11::module_& m) {
@@ -198,5 +266,9 @@ void bind_comm(pybind11::module_& m) {
   m.def("comm_reduce_scatter", &reduce_scatter);
   m.def("comm_gather_range", &gather_range);
   m.def("comm_barrier", &barrier);
+  m.def("comm_reduce_sumsq", &reduce_sumsq);
+  m.def("comm_nvls_reduce_sumsq", &nvls_reduce_sumsq);
+  m.def("comm_clip_finalize", &clip_finalize);
+  m.def("comm_adamw_clip", &adamw_clip_);
 }
 }  // namespace dtg

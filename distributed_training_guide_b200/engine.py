@@ -51,10 +51,12 @@ class TrainEngine:
                lr: float = 3e-5, seed: int = 0, device: Optional[str] = None, tensor_parallel: Optional[int] = None,
                cpu_offload: bool = False, checkpoint_activations: bool = False, prefetch_layers: bool = False,
                num_layers: Optional[int] = None, lr_scaling: str = "none", fp8: bool = False,
-               document_masking: bool = False, **extra):
+               document_masking: bool = False, max_grad_norm: Optional[float] = None, **extra):
         """``fp8=True`` runs the decoder-layer projections in fp8 (``ops.fp8_linear``); single and ddp engines only.
         ``document_masking=True``: batches that carry ``position_ids`` are packed documents, each starting where its
-        position id is 0; attention and targets stay inside each document (single, ddp and fsdp engines, Llama)."""
+        position id is 0; attention and targets stay inside each document (single, ddp and fsdp engines, Llama).
+        ``max_grad_norm``: clip the gradients by their global L2 norm before AdamW
+        (``torch.nn.utils.clip_grad_norm_`` semantics; single and ddp engines); see ``grad_norm()``."""
         import os
 
         world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -68,11 +70,17 @@ class TrainEngine:
             from .parallel.strategies import check_document_masking_supported
 
             check_document_masking_supported(parallelism)
+        if max_grad_norm is not None:
+            from .parallel.strategies import check_max_grad_norm_supported
+
+            check_max_grad_norm_supported(parallelism)
+            if not max_grad_norm > 0:
+                raise ValueError(f"max_grad_norm must be > 0, got {max_grad_norm}")
         args = SimpleNamespace(
             model_name=model_name, batch_size=batch_size, seq_length=seq_length, lr=lr, seed=seed, device=device,
             tensor_parallel=tensor_parallel or world, cpu_offload=cpu_offload,
             checkpoint_activations=checkpoint_activations, prefetch_layers=prefetch_layers, lr_scaling=lr_scaling,
-            fp8=fp8, document_masking=document_masking,
+            fp8=fp8, document_masking=document_masking, max_grad_norm=max_grad_norm,
             experiment_name=None, save_dir="../outputs", deterministic=False, local_rank=None, **extra,
         )
         strategy = make_strategy(parallelism, args)
@@ -86,6 +94,11 @@ class TrainEngine:
         eng = cls(strategy, model, optimizer, lr_scheduler, config, args)
         eng.parallelism = parallelism
         return eng
+
+    def grad_norm(self) -> Optional[torch.Tensor]:
+        """The last step's global gradient L2 norm before clipping, as a device tensor (reading it synchronises);
+        None while clipping is off."""
+        return getattr(self.optimizer, "last_grad_norm", None)
 
     @property
     def tokens_per_step(self) -> int:

@@ -159,10 +159,20 @@ def fp8_gemm(a8, scale_inv_a, b8, scale_inv_b):
     return (a8.float() * scale_inv_a) @ (b8.float() * scale_inv_b).t()
 
 
-def adamw_step(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step, grad_scale=1.0):
+def clip_coefficient(norm, max_norm):
+    """``torch.nn.utils.clip_grad_norm_``'s factor for a gradient of global L2 norm ``norm`` (an fp32 tensor):
+    ``min(1, max_norm / (norm + 1e-6))`` in fp32.  A NaN norm gives NaN and an Inf norm 0, as in torch: the step
+    goes non-finite rather than being skipped."""
+    norm = torch.as_tensor(norm, dtype=torch.float32)
+    return (torch.tensor(max_norm, dtype=torch.float32, device=norm.device) / (norm + 1e-6)).clamp(max=1.0)
+
+
+def adamw_step(p, g, m, v, lr, beta1, beta2, eps, weight_decay, step, grad_scale=1.0, coef=None):
     """Single-tensor AdamW with fp32 math on (possibly bf16) storage, matching
-    ``torch.optim.AdamW`` (decoupled decay, bias correction)."""
-    pf, gf, mf, vf = p.float(), g.float() * grad_scale, m.float(), v.float()
+    ``torch.optim.AdamW`` (decoupled decay, bias correction).  ``coef`` (gradient clipping, ``clip_coefficient``)
+    multiplies the gradient first, as the clipping kernels do."""
+    gf = g.float() if coef is None else g.float() * torch.as_tensor(coef, dtype=torch.float32).to(g.device)
+    pf, gf, mf, vf = p.float(), gf * grad_scale, m.float(), v.float()
     pf = pf * (1 - lr * weight_decay)
     mf = beta1 * mf + (1 - beta1) * gf
     vf = beta2 * vf + (1 - beta2) * gf * gf

@@ -21,6 +21,13 @@ overlapped with the rest of backward, ONE kernel per bucket:
 ``no_sync()`` (gradient accumulation, reference related-topics/gradient-accumulation) skips the
 bucket kernels on non-boundary micro-batches; the wgrad GEMMs keep accumulating in place.
 On CPU (gloo tests) the same engine falls back to ``torch.distributed`` collectives.
+
+Gradient clipping (``optimizer.max_grad_norm``, ``csrc/grad_clip.cu``) needs the norm of every bucket before any
+update, so the step is split: in backward each bucket kernel only reduces its slice, stores it (ZeRO-1: in this
+rank's own slice of its gradient buffer; all-reduce: in every replica) and sums the squares of what it stored; in
+``optimizer.step()`` one finalize kernel turns those partial sums into the global norm and the clip factor on the
+device, and an AdamW kernel per bucket applies it (ZeRO-1: then pushes the new parameters to every replica).  With
+clipping off nothing of this runs.
 """
 from __future__ import annotations
 
@@ -89,6 +96,31 @@ class DataParallelEngine:
         # DTG_DEBUG_MARKERS=1: keep, per bucket of the current step, the event recorded on the compute stream when
         # the bucket became ready and the one behind its kernel on the communication stream (stall post-mortems)
         self.markers = {} if (self.use_kernels and os.environ.get("DTG_DEBUG_MARKERS")) else None
+        self.clip = getattr(optimizer, "max_grad_norm", None) is not None
+        if self.clip and self.use_kernels:
+            self._setup_clip()
+
+    def _setup_clip(self):
+        """Device buffers of the clipped step: per bucket, its parameter element ranges and one fp64 partial sum of
+        squares per CTA; a symmetric slot per rank for the cross-rank sum; (norm, coef) in fp32."""
+        dev, blocks = self.symm.device, self.symm.comm_blocks
+        self._bucket_index = {g.name: i for i, g in enumerate(self.groups)}
+        self._ranges = {}
+        for g in self.groups:
+            merged = []
+            for o, shape in zip(g.offsets, g.shapes):
+                n = 1
+                for d in shape:
+                    n *= d
+                if merged and merged[-1][1] == o:
+                    merged[-1][1] = o + n   # adjacent parameters: one range
+                elif n:
+                    merged.append([o, o + n])
+            self._ranges[g.name] = torch.tensor(merged or [[0, 0]], dtype=torch.int64, device=dev)
+        self._partials = torch.zeros(len(self.groups) * blocks, dtype=torch.float64, device=dev)
+        self._slots = self.symm.alloc(2, torch.float64)   # one sum per step parity (collective allocation)
+        self._clip_out = torch.zeros(2, dtype=torch.float32, device=dev)
+        self._clip_steps = 0
 
     # -- hooks called by the model ---------------------------------------------------------------
     def pre_forward(self, model):
@@ -221,6 +253,14 @@ class DataParallelEngine:
 
     def _run_bucket_impl(self, g, gbuf):
         opt = self.optimizer
+        if self.clip:
+            # reduce + sum of squares only; the update waits for the global norm (_clipped_step)
+            blocks = self.symm.comm_blocks
+            i = self._bucket_index[g.name]
+            scale = (opt.grad_scale if self.zero1 else 1.0) / self.world
+            self.symm.reduce_sumsq_(gbuf, 0, g.padded_numel, scale, not self.zero1, self._ranges[g.name],
+                                    self._partials[i * blocks:(i + 1) * blocks], blocks)
+            return
         if self.zero1:
             st = opt.state[g.param]
             st["step"] += 1
@@ -239,16 +279,53 @@ class DataParallelEngine:
         self._pending.append(g)
 
     # -- optimizer step ---------------------------------------------------------------------------------
+    def _clipped_step(self):
+        """On the communication stream, behind the bucket kernels of backward: the global norm and clip factor
+        (one finalize kernel), then AdamW with ``g *= coef`` per bucket; ZeRO-1 pushes the new parameters of its
+        shard into every replica and ends with one device barrier, so no rank starts its next forward before every
+        push has landed."""
+        opt, sg, C = self.optimizer, self.symm, self.symm.C
+        lr, b1, b2, eps, wd = opt.hyper()
+        with torch.cuda.stream(self.comm_stream), nvtx_range("clip:step"):
+            # ZeRO-1 folded grad_scale into the stored gradient; plain DDP stored g / N and AdamW applies grad_scale
+            norm_scale = 1.0 if self.zero1 else opt.grad_scale
+            sg.clip_finalize_(self._partials, self._slots, self._clip_steps & 1, norm_scale, opt.max_grad_norm,
+                              self._clip_out)
+            self._clip_steps += 1
+            coef = self._clip_out[1:]
+            for g in self.groups:
+                st = opt.state[g.param]
+                st["step"] += 1
+                if self.zero1:
+                    lo, hi = g.shard_range(self.rank, self.world)
+                    pbuf = self.registry[g.param.data_ptr()]
+                    mc = (pbuf.mc_ptr + 2 * lo) if (sg.nvls and pbuf.mc_ptr and self.world > 1) else 0
+                    dst = [] if mc else [pbuf.ptrs[(self.rank + k) % self.world] + 2 * lo for k in range(self.world)]
+                    C.comm_adamw_clip(dst, mc, g.param[lo:hi], g.grad[lo:hi], st["exp_avg"], st["exp_avg_sq"],
+                                      lr, b1, b2, eps, wd, st["step"], 1.0, coef)
+                else:
+                    C.comm_adamw_clip([g.param.data_ptr()], 0, g.param, g.grad, st["exp_avg"], st["exp_avg_sq"],
+                                      lr, b1, b2, eps, wd, st["step"], opt.grad_scale, coef)
+            if self.zero1 and self.world > 1:
+                sg.barrier_()
+            self._done.record(self.comm_stream)
+        torch.cuda.current_stream().wait_event(self._done)
+        opt.last_grad_norm = self._clip_out[0].clone()
+
     def _optimizer_step(self):
         opt = self.optimizer
         if self.use_kernels:
+            if self.clip:
+                self._clipped_step()
+                return
             torch.cuda.current_stream().wait_event(self._done)  # join the communication stream
             if not self.zero1:
                 for g in self.groups:
                     opt.step_group(g)
             return
+        coef = opt.clip_coefficient()  # over the all-reduced full gradients: the same on every rank
         for g in self.groups:
-            opt.step_group(g)  # on its shard when ZeRO-1 (optimizer built with shard=(rank, world))
+            opt.step_group(g, coef)  # on its shard when ZeRO-1 (optimizer built with shard=(rank, world))
             if self.zero1 and self.world > 1:
                 lo, hi = g.shard_range(self.rank, self.world)
                 shards = [torch.empty(hi - lo, dtype=torch.float32) for _ in range(self.world)]

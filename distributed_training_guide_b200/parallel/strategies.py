@@ -146,7 +146,7 @@ class SingleDevice(Strategy):
         return model
 
     def build_optimizer(self, args, model, lr):
-        opt = FlatAdamW(self.groups, lr=lr)
+        opt = FlatAdamW(self.groups, lr=lr, max_grad_norm=getattr(args, "max_grad_norm", None))
         if self.symm is not None and hasattr(model, "engine"):
             # one rank, same engine: AdamW of each bucket runs inside backward on a side stream as soon
             # as that bucket's gradients are final (the N=1 case of the fused reduce-scatter+AdamW kernel)
@@ -204,6 +204,18 @@ def check_document_masking_supported(parallelism: str):
     if parallelism not in DOCUMENT_MASKING_PARALLELISMS:
         raise ValueError(f"document masking is supported by the {', '.join(DOCUMENT_MASKING_PARALLELISMS)} engines, "
                          f"not {parallelism!r}")
+
+
+#: engines that can clip gradients by their global norm (``--max-grad-norm``): the data-parallel bucket engine keeps
+#: every reduced gradient until ``optimizer.step()``; FSDP fuses its reduce-scatter with AdamW per layer and keeps no
+#: reduced gradient shard, and tensor parallelism would need its replicated norm gains counted once
+MAX_GRAD_NORM_PARALLELISMS = ("single", "ddp", "ddp_allreduce")
+
+
+def check_max_grad_norm_supported(parallelism: str):
+    if parallelism not in MAX_GRAD_NORM_PARALLELISMS:
+        raise ValueError(f"gradient clipping (max_grad_norm) is supported by the "
+                         f"{', '.join(MAX_GRAD_NORM_PARALLELISMS)} engines, not {parallelism!r}")
 
 
 def _load_pretrained(args, model=None, engine=None, default="never"):
@@ -274,7 +286,7 @@ class DataParallelZero1(Strategy):
 
         env = self.env
         shard = (env.rank, env.world_size) if (self.zero1 and env.world_size > 1) else None
-        opt = FlatAdamW(self.groups, lr=lr, shard=shard)
+        opt = FlatAdamW(self.groups, lr=lr, shard=shard, max_grad_norm=getattr(args, "max_grad_norm", None))
         self.engine = DataParallelEngine(model, self.groups, opt, symm=self.symm, registry=self.registry,
                                          zero1=self.zero1, world_size=env.world_size, rank=env.rank)
         return opt

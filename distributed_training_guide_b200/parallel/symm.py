@@ -350,6 +350,28 @@ class SymmGroup:
         self.C.comm_reduce_scatter(grads.ptrs, out, self.pad_ptrs, elem_off, n, scale, self.rank, self._epochs(2),
                                    self.err, blocks or self.comm_blocks)
 
+    # -- gradient clipping (csrc/grad_clip.cu) -------------------------------------------------------------------
+    def reduce_sumsq_(self, buf: SymmBuffer, elem_off: int, n: int, scale: float, broadcast: bool,
+                      ranges: torch.Tensor, partials: torch.Tensor, blocks: Optional[int] = None):
+        """Reduce this rank's 1/N slice of ``buf`` (times ``scale``) and store it as bf16: into this rank's own buffer
+        (``broadcast=False``, the reduce-scatter of ZeRO-1) or into every replica (``broadcast=True``, all-reduce).
+        ``partials[b]`` = the sum of squares of the stored values CTA ``b`` wrote, over the element ``ranges``
+        (int64 [R, 2] of [begin, end) relative to ``elem_off``) only."""
+        blocks = blocks or self.comm_blocks
+        if self.nvls and buf.mc_ptr:
+            self.C.comm_nvls_reduce_sumsq(buf.mc_ptr, buf.ptrs[self.rank], self.pad_ptrs, elem_off, n, scale, broadcast,
+                                          ranges, partials, self.rank, self._epochs(2), self.err, blocks)
+            return
+        self.C.comm_reduce_sumsq(buf.ptrs, self.pad_ptrs, elem_off, n, scale, broadcast, ranges, partials, self.rank,
+                                 self._epochs(2), self.err, blocks)
+
+    def clip_finalize_(self, partials: torch.Tensor, slots: SymmBuffer, parity: int, norm_scale: float,
+                       max_norm: float, out: torch.Tensor):
+        """``out[0]`` = sqrt(sum of every rank's ``partials``) * norm_scale, ``out[1]`` = the clip coefficient: the
+        same bits on every rank (fixed-order fp64 sums, one device barrier)."""
+        self.C.comm_clip_finalize(partials, slots.ptrs, self.pad_ptrs, parity, norm_scale, max_norm, out, self.rank,
+                                  self._epochs(1), self.err)
+
     def barrier_(self):
         self.C.comm_barrier(self.pad_ptrs, self.rank, self._epochs(1), self.err)
 

@@ -158,6 +158,8 @@ def train(args, strategy):
                     "time/total": ms_per_step,
                     **{f"time/{k}": t.avg_elapsed_ms() for k, t in timers.items()},
                 }
+                if getattr(args, "max_grad_norm", None) is not None:
+                    info["grad_norm"] = float(optimizer.last_grad_norm)  # pre-clip norm of this step
                 LOGGER.info(info)
                 strategy.check_health()
                 if tracker is not None:

@@ -13,14 +13,21 @@ COMMON = ("experiment-name", "dataset-name", "dataset-subset", "model-name", "sa
           "num-epochs", "lr", "batch-size", "log-freq", "ckpt-freq", "seq-length")
 
 CHAPTER_EXTRAS = {
-    "01-single-gpu": ("fp8", "document-masking"),
-    "02-distributed-data-parallel": ("fp8", "document-masking"),
+    "01-single-gpu": ("fp8", "document-masking", "max-grad-norm"),
+    "02-distributed-data-parallel": ("fp8", "document-masking", "max-grad-norm"),
     "04-fully-sharded-data-parallel": ("cpu-offload", "document-masking"),
     "05-training-llama-405b": ("cpu-offload", "checkpoint-activations", "prefetch-layers", "document-masking"),
     "06-tensor-parallel": (),
     "07-2d-parallel": ("tensor-parallel",),
     "deepspeed": ("local_rank", "zero_config"),
 }
+
+
+def positive_float(text: str) -> float:
+    v = float(text)
+    if not v > 0:
+        raise argparse.ArgumentTypeError(f"must be > 0, got {text}")
+    return v
 
 
 def get_parser(chapter: str = "01-single-gpu", require_experiment: bool = False) -> argparse.ArgumentParser:
@@ -69,6 +76,11 @@ def get_parser(chapter: str = "01-single-gpu", require_experiment: bool = False)
         p.add_argument("--eos-token-id", default=None, type=int,
                        help="with --document-masking and a .bin dataset: a document starts after each occurrence of "
                             "this token id")
+    if "max-grad-norm" in extras:
+        p.add_argument("--max-grad-norm", default=None, type=positive_float,
+                       help="clip the gradients by their global L2 norm before AdamW, as "
+                            "torch.nn.utils.clip_grad_norm_(params, max_norm) does; the log record then carries the "
+                            "pre-clip grad_norm (default: off)")
     if "cpu-offload" in extras:
         p.add_argument("--cpu-offload", default=False, action="store_true")
     if "checkpoint-activations" in extras:
