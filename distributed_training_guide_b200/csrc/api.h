@@ -76,12 +76,14 @@ void fp8_cast_transpose(const void* x, long long ld, int R, int C, bool e5m2, co
 // attn_fwd: P through shared memory; attn_fwd2: P kept in registers
 // doc_start: null (plain causal) or int32 [B,S], the first token of each token's document (document masking:
 // key k is visible to query q iff doc_start[q] <= k <= q)
+// window: 0 (none) or W >= 1, sliding-window attention: key k is also visible only if k > q - W.  W >= S masks
+// nothing and runs the kernels without a window.
 void attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s,
-              const int* doc_start = nullptr);
+              const int* doc_start = nullptr, int window = 0);
 void attn_fwd2(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s,
-               const int* doc_start = nullptr);
+               const int* doc_start = nullptr, int window = 0);
 void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* dq_acc,
               void* dqkv, int B, int S, int nh, int nkv, float scale, int mode, cudaStream_t s,
-              const int* doc_start = nullptr);
+              const int* doc_start = nullptr, int window = 0);
 
 }  // namespace dtg

@@ -3,7 +3,9 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/extension.h>
 
+#include <algorithm>
 #include <cstdlib>
+#include <limits>
 
 #include "api.h"
 #include "comm_api.h"
@@ -32,6 +34,14 @@ const int* doc_start_ptr(const c10::optional<Tensor>& doc_start, const Tensor& q
   return d.data_ptr<int>();
 }
 
+// window (sliding-window attention): None = no window, else an int >= 1; refused before any launch otherwise.
+// The kernels take 0 for no window.
+int window_arg(const c10::optional<int64_t>& window) {
+  if (!window.has_value()) return 0;
+  TORCH_CHECK(*window >= 1, "window must be an int >= 1 or None, got ", *window);
+  return (int)std::min<int64_t>(*window, std::numeric_limits<int>::max());
+}
+
 // version: 0 = default (DTG_ATTN_FWD env, else 2), 1 = P through shared memory, 2 = P kept in registers
 // (both in attention_fwd.cu)
 int default_fwd_version() {
@@ -45,9 +55,10 @@ int default_fwd_version() {
 }
 
 std::tuple<Tensor, Tensor> py_attn_fwd(const Tensor& qkv, int64_t nh, int64_t nkv, double scale, int64_t version,
-                                       const c10::optional<Tensor>& doc_start) {
+                                       const c10::optional<Tensor>& doc_start, const c10::optional<int64_t>& window) {
   check_qkv(qkv, nh, nkv);
   const int* ds = doc_start_ptr(doc_start, qkv);
+  const int win = window_arg(window);
   const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1);
   Tensor o = torch::empty({B, S, nh, 128}, qkv.options());
@@ -55,15 +66,16 @@ std::tuple<Tensor, Tensor> py_attn_fwd(const Tensor& qkv, int64_t nh, int64_t nk
   if (version == 0) version = default_fwd_version();
   auto fn = version == 1 ? dtg::attn_fwd : dtg::attn_fwd2;
   fn(qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), (int)B, (int)S, (int)nh, (int)nkv, (float)scale,
-     at::cuda::getCurrentCUDAStream().stream(), ds);
+     at::cuda::getCurrentCUDAStream().stream(), ds, win);
   return {o, lse};
 }
 
 Tensor py_attn_bwd(const Tensor& d_o, const Tensor& qkv, const Tensor& o, const Tensor& lse, int64_t nh, int64_t nkv,
                    double scale, const c10::optional<Tensor>& trace, int64_t mode,
-                   const c10::optional<Tensor>& doc_start) {
+                   const c10::optional<Tensor>& doc_start, const c10::optional<int64_t>& window) {
   check_qkv(qkv, nh, nkv);
   const int* ds = doc_start_ptr(doc_start, qkv);
+  const int win = window_arg(window);
   TORCH_CHECK(d_o.is_contiguous() && o.is_contiguous() && d_o.scalar_type() == at::kBFloat16, "dO/O must be contiguous bf16");
   const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1);
@@ -76,17 +88,18 @@ Tensor py_attn_bwd(const Tensor& d_o, const Tensor& qkv, const Tensor& o, const 
   }
   dtg::attn_bwd(qkv.data_ptr(), o.data_ptr(), d_o.data_ptr(), lse.data_ptr<float>(), delta.data_ptr<float>(), tr,
                 dqkv.data_ptr(), (int)B, (int)S, (int)nh, (int)nkv, (float)scale, (int)mode,
-                at::cuda::getCurrentCUDAStream().stream(), ds);
+                at::cuda::getCurrentCUDAStream().stream(), ds, win);
   return dqkv;
 }
 }  // namespace
 
 void bind_attention(pybind11::module_& m) {
   m.def("attn_fwd", &py_attn_fwd, pybind11::arg("qkv"), pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("scale"),
-        pybind11::arg("version") = 0, pybind11::arg("doc_start") = pybind11::none());
+        pybind11::arg("version") = 0, pybind11::arg("doc_start") = pybind11::none(),
+        pybind11::arg("window") = pybind11::none());
   m.def("attn_bwd", &py_attn_bwd, pybind11::arg("d_o"), pybind11::arg("qkv"), pybind11::arg("o"), pybind11::arg("lse"),
         pybind11::arg("nh"), pybind11::arg("nkv"), pybind11::arg("scale"), pybind11::arg("trace") = pybind11::none(),
         pybind11::arg("mode") = 0,   // 0 = default (DTG_ATTN_BWD), 1 = P/dS through shared memory, 2 = P/dS in registers
-        pybind11::arg("doc_start") = pybind11::none());
+        pybind11::arg("doc_start") = pybind11::none(), pybind11::arg("window") = pybind11::none());
 }
 }  // namespace dtg

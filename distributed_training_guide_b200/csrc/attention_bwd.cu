@@ -16,6 +16,9 @@
 // kernel.  DOC (document masking, key k visible to query q iff doc_start[q] <= k <= q): the KV pass stops at the first
 // query block whose first query starts its document after the 128 keys, the Q pass starts at the block holding the
 // document start of its first query, and the element mask also runs where a document begins inside a block.
+// WIN (sliding window W, key k visible to query q only if q - W < k): the KV pass also stops after the query block
+// holding R0 + 127 + W - 1 and bounds each key's queries by key + W; the Q pass also starts at the key block holding
+// R0 - W + 1 and bounds each row's keys by row - W + 1.  Both bounds are arithmetic: no loads.
 // Gradients are written into a dqkv buffer with the same fused layout as qkv, so the
 // RoPE-backward kernel and the fused qkv dgrad/wgrad GEMMs consume it directly.
 #include <cuda.h>
@@ -75,13 +78,13 @@ __global__ void attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ d_o, con
 // registers they were computed in and feed the gradient MMAs as their A operand (RS form).  Per 128x64 block that
 // removes 32 KB of shared-memory stores and 32 KB of A-operand reads.  TS = false stages them through
 // 128B-swizzled shared memory (SS form).
-template <bool KV_MODE, bool TS, bool DOC>
+template <bool KV_MODE, bool TS, bool DOC, bool WIN>
 __global__ void __launch_bounds__(bwd::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_constant__ CUtensorMap tm_qkv_c,
                 const __grid_constant__ CUtensorMap tm_do_r, const __grid_constant__ CUtensorMap tm_do_c,
                 const float* __restrict__ lse, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv,
                 int S, int nh, int nkv, float scale, int num_r_blocks, long long* __restrict__ trace,
-                const int* __restrict__ doc_start) {
+                const int* __restrict__ doc_start, int window) {
   using namespace bwd;
   // optional in-kernel timeline (attn_bwd(..., trace=int64[1024])): CTA (0,0) records clock64() per column block:
   // [iter][0] scores ready, [1] P / dS computed, [3] gradient MMAs retired (thread 0)
@@ -138,6 +141,20 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
       c_start = min(max(__ldg(ds_row + R0) / 64, 0), n_c - 1);
       n_c -= c_start;
       doc_bound = __ldg(ds_row + R0 + 127);
+    }
+  }
+  if constexpr (WIN) {
+    // window >= 1, so both ranges keep at least one block
+    if (KV_MODE) {
+      // the last query that can see key R0 + 127 is R0 + 127 + W - 1
+      n_c = min(n_c, min((R0 + 127 + window - 1) / 64, S / 64 - 1) - c_start + 1);
+    } else {
+      // the first key that query R0 can see is R0 - W + 1
+      const int c_win = max(R0 - window + 1, 0) / 64;
+      if (c_win > c_start) {
+        n_c -= c_win - c_start;
+        c_start = c_win;
+      }
     }
   }
   const int n_iter = KV_MODE ? n_c * group : n_c;
@@ -206,6 +223,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
     // DOC, Q pass: my rows' document starts.  KV pass: for each of my two keys, the first query that starts its
     // document after the key (the next document's first token, S if none): with starts non-decreasing along a row,
     // key k is visible to query q >= k iff q < that bound, so the mask needs no per-column load.
+    // WIN tightens both: Q pass max(start, row - W + 1), KV pass min(bound, key + W).
     [[maybe_unused]] int ds_r[2] = {0, 0};
     if constexpr (DOC && KV_MODE) {
 #pragma unroll
@@ -227,6 +245,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
         lse_r[h] = lse[idx] * LOG2E;
         delta_r[h] = delta[idx];
         if constexpr (DOC) ds_r[h] = __ldg(ds_row + R0 + rl0 + 8 * h);
+      }
+    }
+    if constexpr (WIN) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int idx = R0 + rl0 + 8 * h;   // my key (KV pass) or my query (Q pass)
+        if constexpr (KV_MODE) ds_r[h] = DOC ? min(ds_r[h], idx + window) : idx + window;
+        else ds_r[h] = max(ds_r[h], idx - window + 1);
       }
     }
     [[maybe_unused]] float acc_a[KV_MODE ? 64 : 1];   // dV (KV pass)
@@ -284,6 +310,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
       bool need_mask = KV_MODE ? (C0 < R0 + 127) : (C0 + 63 > R0);
       // DOC: and key index >= the query's document start, where a document begins inside the block
       if constexpr (DOC) need_mask = need_mask || (KV_MODE ? c >= doc_bound : C0 < doc_bound);
+      // WIN: and key index > query index - W, where the window edge of some row of R lies inside the block
+      if constexpr (WIN) need_mask = need_mask || (KV_MODE ? C0 + 63 >= R0 + window : C0 < R0 + 128 - window);
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         const int col = 8 * (i >> 2) + 2 * tq + (i & 1);
@@ -300,7 +328,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
         float p = fast_exp2(fmaf(sc[i], sl2, -l2));
         if (need_mask) {
           bool ok = KV_MODE ? (C0 + col >= R0 + row) : (R0 + row >= C0 + col);
-          if constexpr (DOC) ok = ok && (KV_MODE ? C0 + col < ds_r[h] : C0 + col >= ds_r[h]);
+          if constexpr (DOC || WIN) ok = ok && (KV_MODE ? C0 + col < ds_r[h] : C0 + col >= ds_r[h]);
           p = ok ? p : 0.f;
         }
         sc[i] = p;
@@ -376,31 +404,48 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
   }
 }
 
-template <bool TS, bool DOC>
+template <bool TS, bool DOC, bool WIN>
 static void launch_attn_bwd(const CUtensorMap& tq_r, const CUtensorMap& tq_c, const CUtensorMap& td_r,
                             const CUtensorMap& td_c, const float* lse, const float* delta, void* dqkv, int B, int S,
-                            int nh, int nkv, float scale, long long* trace, const int* doc_start, cudaStream_t s) {
+                            int nh, int nkv, float scale, long long* trace, const int* doc_start, int window,
+                            cudaStream_t s) {
   static bool attr = false;
   if (!attr) {
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<true, TS, DOC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        bwd::SMEM_BYTES));
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false, TS, DOC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        bwd::SMEM_BYTES));
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<true, TS, DOC, WIN>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false, TS, DOC, WIN>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
     attr = true;
   }
   const int nblk = S / 128;
-  attn_bwd_kernel<true, TS, DOC><<<dim3(B * nkv, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
-      tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace, doc_start);
-  attn_bwd_kernel<false, TS, DOC><<<dim3(B * nh, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
+  attn_bwd_kernel<true, TS, DOC, WIN><<<dim3(B * nkv, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
+      tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace, doc_start, window);
+  attn_bwd_kernel<false, TS, DOC, WIN><<<dim3(B * nh, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
       tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace ? trace + 512 : nullptr,
-      doc_start);
+      doc_start, window);
+}
+
+template <bool TS>
+static void dispatch_attn_bwd(const CUtensorMap& tq_r, const CUtensorMap& tq_c, const CUtensorMap& td_r,
+                              const CUtensorMap& td_c, const float* lse, const float* delta, void* dqkv, int B, int S,
+                              int nh, int nkv, float scale, long long* trace, const int* doc_start, int window,
+                              cudaStream_t s) {
+  // a window that covers the whole sequence masks nothing: run the kernels without it
+  if (window > 0 && window < S) {
+    if (doc_start) launch_attn_bwd<TS, true, true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
+    else launch_attn_bwd<TS, false, true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, window, s);
+  } else {
+    if (doc_start) launch_attn_bwd<TS, true, false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, 0, s);
+    else launch_attn_bwd<TS, false, false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, 0, s);
+  }
 }
 
 void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* trace_buf,
               void* dqkv, int B, int S, int nh, int nkv, float scale, int mode, cudaStream_t s,
-              const int* doc_start) {
+              const int* doc_start, int window) {
   long long* trace = reinterpret_cast<long long*>(trace_buf);  // [2][64][8] int64 or nullptr
   if (S % 128 != 0) throw std::runtime_error("attn_bwd: sequence length must be a multiple of 128");
+  if (window < 0) throw std::runtime_error("attn_bwd: window must be >= 1 (0 = no window)");
   const long long rows = (long long)B * S * nh;
   attn_bwd_delta_kernel<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
       (const __nv_bfloat16*)d_o, (const __nv_bfloat16*)o, delta, rows, S, nh);
@@ -413,13 +458,8 @@ void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse,
     return e ? e[0] != 's' : true;
   }();
   const bool ts = mode == 0 ? ts_default : mode == 2;   // mode: 0 default, 1 = ss, 2 = rs
-  if (ts) {
-    if (doc_start) launch_attn_bwd<true, true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, s);
-    else launch_attn_bwd<true, false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, s);
-  } else {
-    if (doc_start) launch_attn_bwd<false, true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, s);
-    else launch_attn_bwd<false, false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, s);
-  }
+  if (ts) dispatch_attn_bwd<true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
+  else dispatch_attn_bwd<false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
   note_launch(3);
   DTG_LAUNCH_CHECK();
 }

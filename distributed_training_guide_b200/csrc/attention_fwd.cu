@@ -17,6 +17,10 @@
 // doc_start[q0] / 128 to the diagonal and skips the rest; the element mask runs on the diagonal block and on the
 // blocks where some row's document begins.  DOC = false compiles to the plain causal kernel.
 //
+// WIN (sliding window, runtime `window` = W >= 1): query q sees key k only if k > q - W, a second lower bound that
+// also never decreases along a row.  The CTA starts at the key block holding max(doc start, q0 - W + 1) and masks the
+// (at most two) blocks that straddle some row's window edge.  WIN = false compiles to the kernel without it.
+//
 // Replaces torch SDPA / flash-attn-2 (mma.sync) that the reference uses (SURVEY.md K2/K3).
 #include <cuda.h>
 
@@ -42,10 +46,11 @@ struct Layout {
 };
 }  // namespace fwd
 
-template <bool P_REGS, bool DOC>
+template <bool P_REGS, bool DOC, bool WIN>
 __global__ void __launch_bounds__(fwd::THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __restrict__ o, float* __restrict__ lse,
-                int S, int nh, int nkv, float scale_log2, int num_m_blocks, const int* __restrict__ doc_start) {
+                int S, int nh, int nkv, float scale_log2, int num_m_blocks, const int* __restrict__ doc_start,
+                int window) {
   using namespace fwd;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -68,6 +73,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
   // first key block: the block holding the start of the tile's first query, clamped into [0, m_block]
   int j_lo = 0;
   if constexpr (DOC) j_lo = min(max(__ldg(doc_start + (long long)batch * S + q0) / BN, 0), m_block);
+  // WIN: and the block holding the first query's window start (window >= 1, so never past the diagonal)
+  if constexpr (WIN) j_lo = max(j_lo, max(q0 - window + 1, 0) / BN);
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tm_qkv);
@@ -113,11 +120,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};  // l_run: this thread's partial row sums
-    [[maybe_unused]] int ds_r[2] = {0, 0};   // DOC: my rows' document starts
+    // DOC / WIN: my rows' first visible key, max(document start, row - W + 1)
+    [[maybe_unused]] int ds_r[2] = {0, 0};
     if constexpr (DOC && P_REGS) {
       const int* ds = doc_start + (long long)batch * S + q0;
       ds_r[0] = __ldg(ds + rl0);
       ds_r[1] = __ldg(ds + rl0 + 8);
+    }
+    if constexpr (WIN && P_REGS) {
+      ds_r[0] = max(ds_r[0], q0 + rl0 - window + 1);
+      ds_r[1] = max(ds_r[1], q0 + rl0 + 8 - window + 1);
     }
     mbar_wait_mma(q_full, 0);
     for (int j = j_lo; j < n_blocks; ++j) {
@@ -141,14 +153,18 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
         fence_regs(s);
       }
       if (signal) mbar_arrive(&k_empty[st]);
-      if constexpr (DOC) {
-        // mask keys after the query (diagonal block) and keys before the query's document start (blocks where
-        // one of my rows' documents begins)
-        if constexpr (!P_REGS) {
+      if constexpr (DOC || WIN) {
+        // mask keys after the query (diagonal block) and keys before the query's document start or window (blocks
+        // where one of my rows' first visible key lies)
+        if constexpr (DOC && !P_REGS) {
           // version 1 runs at the 168-register cap: re-read the two starts (L1 hits) rather than keep them live
           const int* ds = doc_start + (long long)batch * S + q0;
           ds_r[0] = __ldg(ds + rl0);
           ds_r[1] = __ldg(ds + rl0 + 8);
+        }
+        if constexpr (WIN && !P_REGS) {
+          ds_r[0] = max(ds_r[0], q0 + rl0 - window + 1);
+          ds_r[1] = max(ds_r[1], q0 + rl0 + 8 - window + 1);
         }
         if (j == n_blocks - 1 || j * BN < max(ds_r[0], ds_r[1])) {
 #pragma unroll
@@ -177,8 +193,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, __nv_bfloat16* __res
         mx = fmaxf(m_run[h], mx);
         alpha[h] = fast_exp2((m_run[h] - mx) * scale_log2);  // 0 on the first block (m_run = -inf)
         mb[h] = mx * scale_log2;
-        if constexpr (DOC) {
-          // a row whose document starts after every key seen so far: keep it empty (p = 0) instead of
+        if constexpr (DOC || WIN) {
+          // a row whose first visible key comes after every key seen so far: keep it empty (p = 0) instead of
           // exp2(-inf - -inf) = NaN
           if (mx == -INFINITY) {
             alpha[h] = 1.f;
@@ -272,36 +288,49 @@ CUtensorMap make_tmap_heads(const void* base, int B, int S, int heads, int box_r
   return make_tmap_bf16(base, 4, dims, strides, box, true);
 }
 
-template <bool P_REGS, bool DOC>
+template <bool P_REGS, bool DOC, bool WIN>
 static void launch_attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale,
-                            cudaStream_t s, const int* doc_start) {
+                            cudaStream_t s, const int* doc_start, int window) {
   if (S % 128 != 0) throw std::runtime_error("attn_fwd: sequence length must be a multiple of 128");
   if (nh % nkv != 0) throw std::runtime_error("attn_fwd: nh must be a multiple of nkv");
   const CUtensorMap tm = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 128);
   constexpr int smem = fwd::Layout<P_REGS>::SMEM_BYTES;
   static bool attr = false;
   if (!attr) {
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<P_REGS, DOC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel<P_REGS, DOC, WIN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        smem));
     attr = true;
   }
   const int num_m = S / 128;
-  attn_fwd_kernel<P_REGS, DOC><<<dim3(B * nh, num_m, 1), fwd::THREADS, smem, s>>>(
-      tm, (__nv_bfloat16*)o, lse, S, nh, nkv, scale * 1.4426950408889634f, num_m, doc_start);
+  attn_fwd_kernel<P_REGS, DOC, WIN><<<dim3(B * nh, num_m, 1), fwd::THREADS, smem, s>>>(
+      tm, (__nv_bfloat16*)o, lse, S, nh, nkv, scale * 1.4426950408889634f, num_m, doc_start, window);
   note_launch();
   DTG_LAUNCH_CHECK();
 }
 
+template <bool P_REGS>
+static void dispatch_attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale,
+                              cudaStream_t s, const int* doc_start, int window) {
+  if (window < 0) throw std::runtime_error("attn_fwd: window must be >= 1 (0 = no window)");
+  // a window that covers the whole sequence masks nothing: run the kernel without it
+  if (window > 0 && window < S) {
+    if (doc_start) launch_attn_fwd<P_REGS, true, true>(qkv, o, lse, B, S, nh, nkv, scale, s, doc_start, window);
+    else launch_attn_fwd<P_REGS, false, true>(qkv, o, lse, B, S, nh, nkv, scale, s, nullptr, window);
+  } else {
+    if (doc_start) launch_attn_fwd<P_REGS, true, false>(qkv, o, lse, B, S, nh, nkv, scale, s, doc_start, 0);
+    else launch_attn_fwd<P_REGS, false, false>(qkv, o, lse, B, S, nh, nkv, scale, s, nullptr, 0);
+  }
+}
+
 // version 1: P through shared memory
 void attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s,
-              const int* doc_start) {
-  if (doc_start) launch_attn_fwd<false, true>(qkv, o, lse, B, S, nh, nkv, scale, s, doc_start);
-  else launch_attn_fwd<false, false>(qkv, o, lse, B, S, nh, nkv, scale, s, nullptr);
+              const int* doc_start, int window) {
+  dispatch_attn_fwd<false>(qkv, o, lse, B, S, nh, nkv, scale, s, doc_start, window);
 }
 // version 2: P stays in registers (RS-form PV MMA)
 void attn_fwd2(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s,
-               const int* doc_start) {
-  if (doc_start) launch_attn_fwd<true, true>(qkv, o, lse, B, S, nh, nkv, scale, s, doc_start);
-  else launch_attn_fwd<true, false>(qkv, o, lse, B, S, nh, nkv, scale, s, nullptr);
+               const int* doc_start, int window) {
+  dispatch_attn_fwd<true>(qkv, o, lse, B, S, nh, nkv, scale, s, doc_start, window);
 }
 
 }  // namespace dtg

@@ -16,7 +16,7 @@ from typing import Optional
 
 @dataclasses.dataclass
 class ModelConfig:
-    arch: str  # "llama" | "gpt2"
+    arch: str  # "llama" | "mistral" | "gpt2"; mistral is llama with a sliding attention window
     vocab_size: int
     hidden_size: int
     intermediate_size: int
@@ -28,6 +28,8 @@ class ModelConfig:
     rope_theta: float = 10000.0
     rope_scaling: Optional[dict] = None
     tie_word_embeddings: bool = False
+    #: sliding-window attention (Mistral): query q sees only the ``sliding_window`` most recent keys, k > q - W
+    sliding_window: Optional[int] = None
     # gpt2 only
     layer_norm_epsilon: float = 1e-5
     dropout: float = 0.0
@@ -70,6 +72,10 @@ def _llama(name, v, h, i, l, nh, nkv, maxpos, theta, scaling=None):
     )
 
 
+def _mistral(name, v, h, i, l, nh, nkv, maxpos, theta, window):
+    return dataclasses.replace(_llama(name, v, h, i, l, nh, nkv, maxpos, theta), arch="mistral", sliding_window=window)
+
+
 _GPT2 = ModelConfig(
     arch="gpt2", vocab_size=50257, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
     num_attention_heads=12, num_key_value_heads=12, max_position_embeddings=1024,
@@ -87,10 +93,13 @@ REGISTRY = {
     "meta-llama/Llama-3.1-70B": _llama("meta-llama/Llama-3.1-70B", 128256, 8192, 28672, 80, 64, 8, 131072, 5e5, _LLAMA3_SCALING),
     "meta-llama/Llama-3.1-405B": _llama("meta-llama/Llama-3.1-405B", 128256, 16384, 53248, 126, 128, 8, 131072, 5e5, _LLAMA3_SCALING),
     "meta-llama/Meta-Llama-3.1-405B": _llama("meta-llama/Meta-Llama-3.1-405B", 128256, 16384, 53248, 126, 128, 8, 131072, 5e5, _LLAMA3_SCALING),
+    "mistralai/Mistral-7B-v0.1": _mistral("mistralai/Mistral-7B-v0.1", 32000, 4096, 14336, 32, 32, 8, 32768, 1e4, 4096),
     # tiny configs for tests / smoke runs (head_dim 128 so the sm_90a attention kernel applies)
     "debug-llama": _llama("debug-llama", 1024, 256, 512, 2, 2, 2, 2048, 1e4),
     "debug-llama-gqa": _llama("debug-llama-gqa", 1024, 512, 1024, 2, 4, 2, 2048, 5e5),
     "debug-llama-tp": _llama("debug-llama-tp", 2048, 1024, 2048, 2, 8, 8, 2048, 1e4),
+    # a window that is not a multiple of the kernels' 128-row tiles
+    "debug-mistral": _mistral("debug-mistral", 1024, 512, 1024, 2, 4, 2, 2048, 1e4, 192),
     "debug-gpt2": dataclasses.replace(_GPT2, vocab_size=512, hidden_size=64, intermediate_size=256,
                                       num_hidden_layers=2, num_attention_heads=2, num_key_value_heads=2,
                                       max_position_embeddings=128, name="debug-gpt2"),
@@ -108,8 +117,14 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
             max_position_embeddings=d.get("n_positions", 1024), tie_word_embeddings=True,
             layer_norm_epsilon=d.get("layer_norm_epsilon", 1e-5), dropout=d.get("resid_pdrop", 0.1), name=name,
         )
-    if mt != "llama":
+    if mt not in ("llama", "mistral"):
         raise ValueError(f"unsupported model_type {mt!r} in {name}")
+    window = None
+    if mt == "mistral":
+        if d.get("head_dim") is not None and d["head_dim"] != d["hidden_size"] // d["num_attention_heads"]:
+            raise ValueError(f"{name}: head_dim {d['head_dim']} differs from hidden_size / num_attention_heads = "
+                             f"{d['hidden_size'] // d['num_attention_heads']}; only head_dim = hidden / heads is supported")
+        window = d.get("sliding_window", 4096)   # MistralConfig's default; null means no window
     scaling = d.get("rope_scaling")
     theta = d.get("rope_theta", 1e4)
     if isinstance(d.get("rope_parameters"), dict):  # transformers>=5 layout
@@ -118,13 +133,14 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
         if rp.get("rope_type", "default") != "default":
             scaling = rp
     return ModelConfig(
-        arch="llama", vocab_size=d["vocab_size"], hidden_size=d["hidden_size"],
+        vocab_size=d["vocab_size"], hidden_size=d["hidden_size"],
         intermediate_size=d["intermediate_size"], num_hidden_layers=d["num_hidden_layers"],
         num_attention_heads=d["num_attention_heads"],
         num_key_value_heads=d.get("num_key_value_heads", d["num_attention_heads"]),
         max_position_embeddings=d.get("max_position_embeddings", 4096),
         rms_norm_eps=d.get("rms_norm_eps", 1e-5), rope_theta=theta, rope_scaling=scaling,
-        tie_word_embeddings=d.get("tie_word_embeddings", False), name=name,
+        tie_word_embeddings=d.get("tie_word_embeddings", False), sliding_window=window, name=name,
+        arch=mt,
     )
 
 
@@ -167,6 +183,17 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
         "tie_word_embeddings": cfg.tie_word_embeddings, "attention_bias": False, "mlp_bias": False,
         "bos_token_id": 1, "eos_token_id": 2, "torch_dtype": "bfloat16",
     }
+    if cfg.arch == "mistral":
+        return {
+            "model_type": "mistral", "architectures": ["MistralForCausalLM"], "vocab_size": cfg.vocab_size,
+            "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size,
+            "num_hidden_layers": cfg.num_hidden_layers, "num_attention_heads": cfg.num_attention_heads,
+            "num_key_value_heads": cfg.num_key_value_heads, "head_dim": cfg.head_dim,
+            "max_position_embeddings": cfg.max_position_embeddings, "rms_norm_eps": cfg.rms_norm_eps,
+            "rope_theta": cfg.rope_theta, "sliding_window": cfg.sliding_window, "hidden_act": "silu",
+            "tie_word_embeddings": cfg.tie_word_embeddings, "bos_token_id": 1, "eos_token_id": 2,
+            "torch_dtype": "bfloat16",
+        }
     if cfg.rope_scaling:
         d["rope_scaling"] = cfg.rope_scaling
     return d

@@ -1,4 +1,4 @@
-"""Llama-family causal LM built on the sm_90a op layer.
+"""Llama-family causal LM built on the sm_90a op layer (Llama, and Mistral: Llama plus a sliding attention window).
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
 the reference instantiates at e.g. ``02-distributed-data-parallel/train_llm.py:57-58``)
@@ -141,6 +141,8 @@ class LlamaAttention(nn.Module):
         self.num_heads = config.num_attention_heads // tp_size
         self.num_kv_heads = config.num_key_value_heads // tp_size
         self.head_dim = d
+        #: sliding-window attention (Mistral): None, or W >= 1 with query q seeing keys k > q - W only
+        self.sliding_window = config.sliding_window
         self.q_proj = Linear(h, self.num_heads * d, dtype, device)
         self.k_proj = Linear(h, self.num_kv_heads * d, dtype, device)
         self.v_proj = Linear(h, self.num_kv_heads * d, dtype, device)
@@ -215,7 +217,7 @@ class LlamaDecoderLayer(nn.Module):
         w, owner = self._qkv_weight()
         qkv = fused_linear(y, w, owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
         qkv = ops.rope_qkv_(qkv, cos, sin, att.num_heads + att.num_kv_heads)
-        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start)
+        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
         a = a.reshape(B, S, att.num_heads * att.head_dim)
         a = ops.fp8_linear(a, att.o_proj.weight) if self.fp8 else att.o_proj(a)
         y, h = self.post_attention_layernorm(a, h)

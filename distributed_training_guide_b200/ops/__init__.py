@@ -367,20 +367,20 @@ def rope_qkv_(qkv, cos, sin, n_rot_heads):
 # --------------------------------------------------------------------------------------
 class _AttentionQKV(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, nh, nkv, scale, doc_start=None):
+    def forward(ctx, qkv, nh, nkv, scale, doc_start=None, window=None):
         C = _ext.load()
-        o, lse = C.attn_fwd(qkv, nh, nkv, float(scale), doc_start=doc_start)
+        o, lse = C.attn_fwd(qkv, nh, nkv, float(scale), doc_start=doc_start, window=window)
         ctx.save_for_backward(qkv, o, lse, doc_start)
-        ctx.meta = (nh, nkv, scale)
+        ctx.meta = (nh, nkv, scale, window)
         return o
 
     @staticmethod
     def backward(ctx, do):
         C = _ext.load()
         qkv, o, lse, doc_start = ctx.saved_tensors
-        nh, nkv, scale = ctx.meta
-        dqkv = C.attn_bwd(do.contiguous(), qkv, o, lse, nh, nkv, float(scale), doc_start=doc_start)
-        return dqkv, None, None, None, None
+        nh, nkv, scale, window = ctx.meta
+        dqkv = C.attn_bwd(do.contiguous(), qkv, o, lse, nh, nkv, float(scale), doc_start=doc_start, window=window)
+        return dqkv, None, None, None, None, None
 
 
 def document_starts(position_ids):
@@ -395,23 +395,30 @@ def document_starts(position_ids):
     return torch.where(is_start, idx, torch.zeros_like(idx)).cummax(dim=1).values.to(torch.int32).contiguous()
 
 
-def attention_qkv(qkv, nh, nkv, scale=None, doc_start=None):
+def attention_qkv(qkv, nh, nkv, scale=None, doc_start=None, window=None):
     """Causal self-attention. qkv: [B,S,nh+2*nkv,d] (q heads | k heads | v heads) -> [B,S,nh,d].
     ``doc_start`` (int32 [B,S] from ``document_starts``, or None): document masking, query q sees key k iff
-    ``doc_start[q] <= k <= q``."""
+    ``doc_start[q] <= k <= q``.  ``window`` (an int >= 1, or None): sliding-window attention (Mistral), query q also
+    sees only the ``window`` most recent keys, ``k > q - window``; a window of S or more changes nothing."""
     d = qkv.shape[-1]
     scale = scale if scale is not None else 1.0 / math.sqrt(d)
+    if window is not None:
+        if isinstance(window, bool) or int(window) != window or window < 1:
+            raise ValueError(f"window must be an int >= 1 or None, got {window!r}")
+        window = None if window >= qkv.shape[1] else int(window)
     if _ext.use_cuda_kernel("attention", qkv) and qkv.dtype == torch.bfloat16 and d == 128 and qkv.shape[1] % 128 == 0:
         if doc_start is not None:
-            return _AttentionQKV.apply(qkv, nh, nkv, scale, doc_start.to(torch.int32).contiguous())
+            return _AttentionQKV.apply(qkv, nh, nkv, scale, doc_start.to(torch.int32).contiguous(), window)
+        if window is not None:
+            return _AttentionQKV.apply(qkv, nh, nkv, scale, None, window)
         return _AttentionQKV.apply(qkv, nh, nkv, scale)
     q, k, v = qkv[:, :, :nh], qkv[:, :, nh:nh + nkv], qkv[:, :, nh + nkv:]
     if qkv.is_cuda:
         # head dims other than 128 (GPT-2 style / toy configs) and sequence lengths that are not a multiple of
         # the 128-row tile are outside the sm_90a kernel's scope; use the library kernel rather than the
         # O(S^2)-memory reference
-        if doc_start is not None:
-            mask = ref.document_mask(doc_start, qkv.shape[1])[:, None]  # [B, 1, S, S]
+        if doc_start is not None or window is not None:
+            mask = ref.document_mask(doc_start, qkv.shape[1], window, device=qkv.device)[:, None]  # [B|1, 1, S, S]
             o = torch.nn.functional.scaled_dot_product_attention(
                 q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), attn_mask=mask, scale=scale,
                 enable_gqa=(nh != nkv))
@@ -420,7 +427,7 @@ def attention_qkv(qkv, nh, nkv, scale=None, doc_start=None):
                 q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=True, scale=scale,
                 enable_gqa=(nh != nkv))
         return o.transpose(1, 2)
-    return ref.attention(q, k, v, causal=True, scale=scale, doc_start=doc_start)
+    return ref.attention(q, k, v, causal=True, scale=scale, doc_start=doc_start, window=window)
 
 
 # --------------------------------------------------------------------------------------

@@ -8,7 +8,7 @@ These serve two roles and are never a second GPU backend:
 
 Semantics follow what the reference guide gets from ``transformers`` (SURVEY.md §3.2 /
 K1-K9): RMSNorm with fp32 statistics, half-rotation RoPE, causal softmax attention
-with GQA, SwiGLU, shifted-label mean cross-entropy with ``ignore_index=-100``.  The fp8 functions define the
+with GQA (optionally document-masked and / or sliding-window), SwiGLU, shifted-label mean cross-entropy with ``ignore_index=-100``.  The fp8 functions define the
 quantisation of ``ops.fp8_linear`` (per-tensor current scaling) exactly, so the cast kernels are tested bit for bit.
 """
 from __future__ import annotations
@@ -67,17 +67,23 @@ def rope_apply(x, cos, sin, inverse=False):
     return out.to(x.dtype)
 
 
-def document_mask(doc_start, S):
-    """bool [B, S, S]: query q may see key k iff ``doc_start[b, q] <= k <= q`` (causal attention inside each
-    document; ``doc_start`` as ``ops.document_starts`` returns it)."""
-    k = torch.arange(S, device=doc_start.device)
-    causal = k[None, :] <= k[:, None]
-    return causal[None] & (k[None, None, :] >= doc_start.long()[:, :, None])
+def document_mask(doc_start, S, window=None, device=None):
+    """bool [B, S, S]: query q may see key k iff ``max(doc_start[b, q], q - window + 1) <= k <= q`` (causal attention
+    inside each document and inside the sliding window; ``doc_start`` as ``ops.document_starts`` returns it).
+    ``doc_start`` None means one document per row and gives a [1, S, S] mask on ``device``; ``window`` None means no
+    window."""
+    k = torch.arange(S, device=doc_start.device if doc_start is not None else device)
+    mask = (k[None, :] <= k[:, None])[None]
+    if doc_start is not None:
+        mask = mask & (k[None, None, :] >= doc_start.long()[:, :, None])
+    if window is not None:
+        mask = mask & (k[None, :] > k[:, None] - window)[None]
+    return mask
 
 
-def attention(q, k, v, causal=True, scale=None, doc_start=None):
-    """q: [B, S, nh, d]; k, v: [B, S, nkv, d] -> [B, S, nh, d]. fp32 softmax.  ``doc_start`` (int [B, S]):
-    document masking on top of the causal mask (see ``document_mask``)."""
+def attention(q, k, v, causal=True, scale=None, doc_start=None, window=None):
+    """q: [B, S, nh, d]; k, v: [B, S, nkv, d] -> [B, S, nh, d]. fp32 softmax.  ``doc_start`` (int [B, S]) and
+    ``window`` (int >= 1): document masking and a sliding window on top of the causal mask (see ``document_mask``)."""
     B, S, nh, d = q.shape
     nkv = k.shape[2]
     scale = scale if scale is not None else 1.0 / math.sqrt(d)
@@ -89,8 +95,8 @@ def attention(q, k, v, causal=True, scale=None, doc_start=None):
         kf = kf.repeat_interleave(rep, dim=1)
         vf = vf.repeat_interleave(rep, dim=1)
     s = torch.matmul(qf, kf.transpose(-1, -2)) * scale
-    if doc_start is not None:
-        s = s.masked_fill(~document_mask(doc_start, S)[:, None], float("-inf"))
+    if doc_start is not None or window is not None:
+        s = s.masked_fill(~document_mask(doc_start, S, window, device=q.device)[:, None], float("-inf"))
     elif causal:
         mask = torch.ones(S, k.shape[1], dtype=torch.bool, device=q.device).tril()
         s = s.masked_fill(~mask, float("-inf"))

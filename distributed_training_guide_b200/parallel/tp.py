@@ -375,7 +375,8 @@ class TensorParallelRuntime:
         qkv = _ColumnParallelLinear.apply(y, w, owner, tp, 2 * layer.layer_idx)
         qkv = qkv.view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
         qkv = ops.rope_qkv_(qkv, cos, sin, att.num_heads + att.num_kv_heads)
-        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads).reshape(B * S, att.num_heads * att.head_dim)
+        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, window=att.sliding_window)
+        a = a.reshape(B * S, att.num_heads * att.head_dim)
         h2 = _RowParallelLinear.apply(a, att.o_proj.weight, att.o_proj.weight, tp, h)   # residual add fused
         y2, _ = layer.post_attention_layernorm(h2, None)
         w, owner = self.fused(layer, "gate_up", (mlp.gate_proj, mlp.up_proj))
