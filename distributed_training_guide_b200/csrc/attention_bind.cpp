@@ -4,6 +4,8 @@
 #include <torch/extension.h>
 
 #include <algorithm>
+#include <cmath>
+#include <cstdint>
 #include <cstdlib>
 #include <limits>
 
@@ -14,11 +16,45 @@ namespace dtg {
 namespace {
 using torch::Tensor;
 
-void check_qkv(const Tensor& qkv, int64_t nh, int64_t nkv) {
+// Every argument is checked here, before the first launch: a bad head count divides by zero (host and device) or
+// reads the wrong heads, and a bad scale turns every output into NaN.
+void check_heads_scale(int64_t nh, int64_t nkv, double scale) {
+  TORCH_CHECK(nh >= 1 && nkv >= 1, "nh and nkv must be >= 1, got nh ", nh, ", nkv ", nkv);
+  TORCH_CHECK(nh % nkv == 0, "nh must be a multiple of nkv, got nh ", nh, ", nkv ", nkv);
+  // the kernels take the scale as fp32: it must stay finite and > 0 after that conversion
+  const float s = (float)scale;
+  TORCH_CHECK(std::isfinite(s) && s > 0.f, "scale must be finite and > 0, got ", scale);
+}
+
+bool aligned16(const Tensor& t) { return reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0; }
+
+void check_qkv(const Tensor& qkv, int64_t nh, int64_t nkv, double scale) {
+  check_heads_scale(nh, nkv, scale);
   TORCH_CHECK(qkv.is_cuda() && qkv.is_contiguous() && qkv.scalar_type() == at::kBFloat16,
               "qkv must be a contiguous bf16 CUDA tensor");
   TORCH_CHECK(qkv.dim() == 4 && qkv.size(2) == nh + 2 * nkv && qkv.size(3) == 128,
               "qkv must be [B, S, nh+2*nkv, 128]");
+  TORCH_CHECK(qkv.size(0) >= 1 && qkv.size(1) >= 128 && qkv.size(1) % 128 == 0,
+              "qkv must have B >= 1 and a sequence length S that is a positive multiple of 128, got ", qkv.sizes());
+  TORCH_CHECK(aligned16(qkv), "qkv must start on a 16-byte boundary");
+}
+
+// o and d_o of the backward: bf16, contiguous, [B, S, nh, 128] on the device of qkv, 16-byte aligned
+void check_rows(const Tensor& t, const char* name, const Tensor& qkv, int64_t nh) {
+  TORCH_CHECK(t.scalar_type() == at::kBFloat16 && t.is_contiguous(), name, " must be a contiguous bf16 tensor");
+  TORCH_CHECK(t.dim() == 4 && t.size(0) == qkv.size(0) && t.size(1) == qkv.size(1) && t.size(2) == nh &&
+                  t.size(3) == 128,
+              name, " must be [B, S, nh, 128] = [", qkv.size(0), ", ", qkv.size(1), ", ", nh, ", 128], got ",
+              t.sizes());
+  TORCH_CHECK(t.device() == qkv.device(), name, " must be on the device of qkv");
+  TORCH_CHECK(aligned16(t), name, " must start on a 16-byte boundary");
+}
+
+void check_lse(const Tensor& lse, const Tensor& qkv, int64_t nh) {
+  TORCH_CHECK(lse.scalar_type() == at::kFloat && lse.is_contiguous(), "lse must be a contiguous fp32 tensor");
+  TORCH_CHECK(lse.dim() == 3 && lse.size(0) == qkv.size(0) && lse.size(1) == nh && lse.size(2) == qkv.size(1),
+              "lse must be [B, nh, S] = [", qkv.size(0), ", ", nh, ", ", qkv.size(1), "], got ", lse.sizes());
+  TORCH_CHECK(lse.device() == qkv.device(), "lse must be on the device of qkv");
 }
 
 // doc_start (document masking): int32 [B, S] on the device of qkv, contiguous; None = plain causal attention.
@@ -56,7 +92,8 @@ int default_fwd_version() {
 
 std::tuple<Tensor, Tensor> py_attn_fwd(const Tensor& qkv, int64_t nh, int64_t nkv, double scale, int64_t version,
                                        const c10::optional<Tensor>& doc_start, const c10::optional<int64_t>& window) {
-  check_qkv(qkv, nh, nkv);
+  check_qkv(qkv, nh, nkv, scale);
+  TORCH_CHECK(version >= 0 && version <= 2, "version must be 0 (default), 1 or 2, got ", version);
   const int* ds = doc_start_ptr(doc_start, qkv);
   const int win = window_arg(window);
   const c10::cuda::CUDAGuard guard(qkv.device());
@@ -73,19 +110,24 @@ std::tuple<Tensor, Tensor> py_attn_fwd(const Tensor& qkv, int64_t nh, int64_t nk
 Tensor py_attn_bwd(const Tensor& d_o, const Tensor& qkv, const Tensor& o, const Tensor& lse, int64_t nh, int64_t nkv,
                    double scale, const c10::optional<Tensor>& trace, int64_t mode,
                    const c10::optional<Tensor>& doc_start, const c10::optional<int64_t>& window) {
-  check_qkv(qkv, nh, nkv);
+  check_qkv(qkv, nh, nkv, scale);
+  TORCH_CHECK(mode >= 0 && mode <= 2, "mode must be 0 (default), 1 or 2, got ", mode);
   const int* ds = doc_start_ptr(doc_start, qkv);
   const int win = window_arg(window);
-  TORCH_CHECK(d_o.is_contiguous() && o.is_contiguous() && d_o.scalar_type() == at::kBFloat16, "dO/O must be contiguous bf16");
+  check_rows(o, "o", qkv, nh);
+  check_rows(d_o, "d_o", qkv, nh);
+  check_lse(lse, qkv, nh);
+  float* tr = nullptr;
+  if (trace.has_value() && trace->defined()) {
+    TORCH_CHECK(trace->scalar_type() == at::kLong && trace->numel() >= 1024 && trace->is_contiguous() &&
+                    trace->device() == qkv.device(),
+                "trace must be a contiguous int64[1024] on the device of qkv");
+    tr = reinterpret_cast<float*>(trace->data_ptr<int64_t>());
+  }
   const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1);
   Tensor dqkv = torch::empty_like(qkv);
   Tensor delta = torch::empty({B, nh, S}, qkv.options().dtype(at::kFloat));
-  float* tr = nullptr;
-  if (trace.has_value()) {
-    TORCH_CHECK(trace->scalar_type() == at::kLong && trace->numel() >= 1024, "trace must be int64[1024]");
-    tr = reinterpret_cast<float*>(trace->data_ptr<int64_t>());
-  }
   dtg::attn_bwd(qkv.data_ptr(), o.data_ptr(), d_o.data_ptr(), lse.data_ptr<float>(), delta.data_ptr<float>(), tr,
                 dqkv.data_ptr(), (int)B, (int)S, (int)nh, (int)nkv, (float)scale, (int)mode,
                 at::cuda::getCurrentCUDAStream().stream(), ds, win);

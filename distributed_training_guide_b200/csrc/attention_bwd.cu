@@ -446,13 +446,15 @@ void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse,
   long long* trace = reinterpret_cast<long long*>(trace_buf);  // [2][64][8] int64 or nullptr
   if (S % 128 != 0) throw std::runtime_error("attn_bwd: sequence length must be a multiple of 128");
   if (window < 0) throw std::runtime_error("attn_bwd: window must be >= 1 (0 = no window)");
-  const long long rows = (long long)B * S * nh;
-  attn_bwd_delta_kernel<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
-      (const __nv_bfloat16*)d_o, (const __nv_bfloat16*)o, delta, rows, S, nh);
+  if (nh < 1 || nkv < 1 || nh % nkv != 0) throw std::runtime_error("attn_bwd: nh must be a positive multiple of nkv");
+  // every tensor map is encoded (and can refuse its pointer) before the first launch
   const CUtensorMap tq_r = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 128);
   const CUtensorMap tq_c = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 64);
   const CUtensorMap td_r = make_tmap_heads(d_o, B, S, nh, 128);
   const CUtensorMap td_c = make_tmap_heads(d_o, B, S, nh, 64);
+  const long long rows = (long long)B * S * nh;
+  attn_bwd_delta_kernel<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
+      (const __nv_bfloat16*)d_o, (const __nv_bfloat16*)o, delta, rows, S, nh);
   static const bool ts_default = []() {   // DTG_ATTN_BWD=rs (default: P / dS stay in registers) | ss
     const char* e = getenv("DTG_ATTN_BWD");
     return e ? e[0] != 's' : true;

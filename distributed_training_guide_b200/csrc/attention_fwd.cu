@@ -292,7 +292,7 @@ template <bool P_REGS, bool DOC, bool WIN>
 static void launch_attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale,
                             cudaStream_t s, const int* doc_start, int window) {
   if (S % 128 != 0) throw std::runtime_error("attn_fwd: sequence length must be a multiple of 128");
-  if (nh % nkv != 0) throw std::runtime_error("attn_fwd: nh must be a multiple of nkv");
+  if (nh < 1 || nkv < 1 || nh % nkv != 0) throw std::runtime_error("attn_fwd: nh must be a positive multiple of nkv");
   const CUtensorMap tm = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 128);
   constexpr int smem = fwd::Layout<P_REGS>::SMEM_BYTES;
   static bool attr = false;

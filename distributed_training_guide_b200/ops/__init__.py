@@ -399,9 +399,12 @@ def attention_qkv(qkv, nh, nkv, scale=None, doc_start=None, window=None):
     """Causal self-attention. qkv: [B,S,nh+2*nkv,d] (q heads | k heads | v heads) -> [B,S,nh,d].
     ``doc_start`` (int32 [B,S] from ``document_starts``, or None): document masking, query q sees key k iff
     ``doc_start[q] <= k <= q``.  ``window`` (an int >= 1, or None): sliding-window attention (Mistral), query q also
-    sees only the ``window`` most recent keys, ``k > q - window``; a window of S or more changes nothing."""
+    sees only the ``window`` most recent keys, ``k > q - window``; a window of S or more changes nothing.  ``scale``
+    (None = 1/sqrt(d)) must be finite and > 0 on every path."""
     d = qkv.shape[-1]
     scale = scale if scale is not None else 1.0 / math.sqrt(d)
+    if isinstance(scale, bool) or not math.isfinite(scale) or scale <= 0:
+        raise ValueError(f"scale must be finite and > 0 or None, got {scale!r}")
     if window is not None:
         if isinstance(window, bool) or int(window) != window or window < 1:
             raise ValueError(f"window must be an int >= 1 or None, got {window!r}")
