@@ -31,7 +31,16 @@ struct GemmCfg {
   // B_MODE 3 (operand B gathered from the ranks' FSDP shards by warp 1 of every CTA): a 2-slot bounce ring
   static constexpr int GATHER_PIECE = 16384;
   static constexpr int GATHER_BYTES = 2 * GATHER_PIECE;
-  static_assert(2 * STAGES + (COMM_SLOTS > 2 ? COMM_SLOTS : 2) <= BAR_BYTES / 8, "barrier area");
+  // TMA-store epilogue (every mode but B_MODE 3 and C_MODE 1): each consumer warpgroup stages half of its 64 x 256
+  // output rows at a time, as two 64 x 64 boxes of 128B-swizzled bf16, behind the barrier area rounded up to 1 KB
+  static constexpr int EPI_BOX_BYTES = 64 * 64 * 2;
+  static constexpr int EPI_WG_BYTES = 2 * EPI_BOX_BYTES;
+  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES + 1024;
+  static constexpr int SMEM_BYTES_EPI = EPI_OFFSET + 2 * EPI_WG_BYTES + 1024;
+  static constexpr int EPI_BAR = 2 * STAGES + 8;   // [2]: one C-load barrier per consumer warpgroup (accumulate mode)
+  static_assert(2 * STAGES + (COMM_SLOTS > 2 ? COMM_SLOTS : 2) <= EPI_BAR && EPI_BAR + 2 <= BAR_BYTES / 8,
+                "barrier area");
+  static_assert(SMEM_BYTES_EPI <= 232448, "staging buffer exceeds the 227 KB of shared memory a CTA may have");
 };
 
 template <int N>

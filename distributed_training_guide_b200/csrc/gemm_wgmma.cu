@@ -4,7 +4,8 @@
 //   warpgroup 0   warp 0  TMA producer     (one elected lane)   smem ring: full/empty mbarriers
 //                 warp 1  B_MODE 3 gather  (one elected lane)   FSDP unshard inside the GEMM
 //   warpgroups 1-2        consumers        64 rows of the 128 x 256 tile each: wgmma m64n256k16 from shared
-//                                          memory, then registers -> bf16 -> global (optionally C += ...)
+//                                          memory, then registers -> bf16 -> shared -> TMA store (optionally
+//                                          C += ..., with C TMA-loaded into the same staging area)
 //
 // CG = 2 runs a cluster of two CTAs on a 256-row tile: each CTA stages its own 128 rows of A and loads half of
 // the 256-row B tile, multicast into both CTAs, so every B byte leaves L2 once per pair.
@@ -43,6 +44,15 @@ using namespace ptx;
 //                    exactly once (peer memory bypasses the local L2, so mode 1 re-fetches it per N tile).
 //   C_MODE           0 = local C;  1 = each `rows_per_peer` row chunk of C is stored into its owner's
 //                    staging buffer (GEMM -> reduce-scatter push).
+//
+// Epilogue.  A local C (C_MODE 0) leaves through shared memory: each consumer warpgroup converts half of its 64 x 256
+// accumulator block at a time into a 32 KB staging area and one thread stores it with two TMA boxes, which clip at M
+// and N, so no element needs a bounds test and the writes are whole 128-byte lines.  Accumulate mode TMA-loads the C
+// boxes into the same staging area first and adds them there.  B_MODE 3 keeps the register epilogue (its gather
+// bounce ring already fills shared memory to within 2 KB of the limit), and so does C_MODE 1 (its rows go to the
+// peers' staging buffers, one base pointer per owner, which one tensor map cannot describe).
+template <int B_MODE, int C_MODE>
+constexpr bool kTmaEpilogue = (B_MODE != 3 && C_MODE == 0);
 // B_MODE 3 helpers.  Chunks are waited for in the order the gather warps fetch them: the chunks behind my own slice
 // of [bg_begin, bg_end) first, then the ones in front of it; my own chunks are local and never waited for.
 __device__ __forceinline__ long long bg_clamp(const GemmDist& d, long long x) {
@@ -61,11 +71,13 @@ template <bool A_K, bool B_K, int CG, int A_MODE = 0, int B_MODE = 0, int C_MODE
 __global__ void __launch_bounds__(GemmCfg<CG>::THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
                  const __grid_constant__ TmapSet<(B_MODE ? kMaxRanks : 1)> tmBs, const __grid_constant__ GemmDist dist,
-                 __nv_bfloat16* __restrict__ C, int M, int N, int K, long long ldc, int accumulate, int num_m_tiles,
-                 int num_tiles, const float* __restrict__ scale_a, const float* __restrict__ scale_b) {
+                 const __grid_constant__ CUtensorMap tmC, __nv_bfloat16* __restrict__ C, int M, int N, int K,
+                 long long ldc, int accumulate, int num_m_tiles, int num_tiles, const float* __restrict__ scale_a,
+                 const float* __restrict__ scale_b) {
   static_assert(ET == 0 || (A_K && B_K && A_MODE == 0 && B_MODE == 0 && C_MODE == 0),
                 "the fp8 GEMM takes K-major operands from one tensor map each");
   using Cfg = GemmCfg<CG>;
+  constexpr bool TMA_EPI = kTmaEpilogue<B_MODE, C_MODE>;
   constexpr int BK = ET ? 2 * Cfg::BK : Cfg::BK;   // elements of K per stage: one 128-byte span either way
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -87,6 +99,10 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmAs.m[0]);
     prefetch_tensormap(&tmBs.m[0]);
+    if constexpr (TMA_EPI) {
+      prefetch_tensormap(&tmC);
+      for (int i = 0; i < 2; ++i) mbar_init(&bars[Cfg::EPI_BAR + i], 1);
+    }
     for (int i = 0; i < Cfg::STAGES; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 2 * CG);  // both consumer warpgroups of every CTA that reads the stage's B
@@ -340,11 +356,30 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
     };
     int stage = 0;
     uint32_t phase = 0;
+    // TMA epilogue: this warpgroup's staging area (two 64 x 64 boxes), its C-load barrier, and this thread's 4-byte
+    // slot for accumulator pair (h = 0, chunk 0) of a box: row 16*wq + lane/4, byte 4*(lane%4) of a 16-byte chunk.
+    // 128B swizzle puts chunk c of row r at chunk c ^ (r % 8), and r % 8 = lane / 4 for every row this thread holds.
+    [[maybe_unused]] uint8_t* const stg = smem + Cfg::EPI_OFFSET + half * Cfg::EPI_WG_BYTES;
+    [[maybe_unused]] uint64_t* const c_bar = bars + Cfg::EPI_BAR + half;
+    [[maybe_unused]] uint32_t c_phase = 0;
+    [[maybe_unused]] const uint32_t stg_s = smem_u32(stg) + (uint32_t)((wq * 16 + (lane >> 2)) * 128 + 4 * (lane & 3));
+    [[maybe_unused]] const int bar_id = 1 + half;   // named barrier of this warpgroup (0 is __syncthreads)
     for (int t = cluster_id; t < num_tiles; t += num_clusters) {
       int tm_, tn_;
       tile_mn(t, num_m_tiles, dist, local_m_tiles, tm_, tn_);
       const int m0 = tm_ * (Cfg::BM * CG) + (int)cta_rank * Cfg::BM + half * 64;
       const int n0 = tn_ * Cfg::BN;
+      // accumulate mode: fetch the first 128 columns of C under the mainloop.  The stores of the previous tile must
+      // have read the staging area; every thread finished writing it before they were issued.
+      // Boxes entirely outside C (rows >= M, columns >= N) are never loaded or stored.
+      if constexpr (TMA_EPI) {
+        if (accumulate && signal && m0 < M) {
+          const int nbox = n0 + 64 < N ? 2 : 1;
+          tma_store_wait_read<0>();
+          mbar_arrive_expect_tx(c_bar, nbox * Cfg::EPI_BOX_BYTES);
+          for (int b = 0; b < nbox; ++b) tma_load_2d(&tmC, c_bar, stg + b * Cfg::EPI_BOX_BYTES, n0 + 64 * b, m0);
+        }
+      }
       float acc[128];
 #pragma unroll
       for (int i = 0; i < 128; ++i) acc[i] = 0.f;
@@ -377,9 +412,65 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
       wgmma_wait<0>();
       fence_regs(acc);
       if (prev >= 0) release(prev);
-      // epilogue: accumulator fragment (x dequantisation scale, fp8) -> bf16 pairs -> global
+      // epilogue: accumulator fragment (x dequantisation scale, fp8) -> bf16 pairs -> staging area -> TMA store
+      // (B_MODE 3 and C_MODE 1: -> global from registers)
       [[maybe_unused]] float deq = 1.f;
       if constexpr (ET != 0) deq = scale_a[0] * scale_b[0];
+      if constexpr (TMA_EPI) {
+        if (m0 >= M) continue;
+#pragma unroll
+        for (int p = 0; p < 2; ++p) {   // columns [n0 + 128p, n0 + 128p + 128): accumulator blocks j = 16p .. 16p+15
+          const int c0 = n0 + 128 * p;
+          if (c0 >= N) break;
+          const int nbox = c0 + 64 < N ? 2 : 1;
+          if (accumulate) {
+            if (p == 1 && signal) {
+              tma_store_wait_read<0>();   // the first half's stores have read the staging area
+              mbar_arrive_expect_tx(c_bar, nbox * Cfg::EPI_BOX_BYTES);
+              for (int b = 0; b < nbox; ++b) tma_load_2d(&tmC, c_bar, stg + b * Cfg::EPI_BOX_BYTES, c0 + 64 * b, m0);
+            }
+            mbar_wait_mma(c_bar, c_phase);
+            c_phase ^= 1;
+          } else {
+            if (signal) tma_store_wait_read<0>();
+            named_bar_sync(bar_id, 128);
+          }
+#pragma unroll
+          for (int b = 0; b < 2; ++b) {
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 16 * p + 8 * b + jj;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {   // rows +8h: 8 rows of 128 B further, same swizzle phase
+                float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
+                const uint32_t q = stg_s + (uint32_t)(b * Cfg::EPI_BOX_BYTES + h * 1024 + ((jj ^ (lane >> 2)) << 4));
+                if (accumulate) {
+                  const uint32_t old = ld_shared_u32(q);
+                  const float2 g = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old));
+                  if constexpr (ET != 0) {   // one rounding for the scale and the add: acc * deq + C
+                    x = __fmaf_rn(x, deq, g.x);
+                    y = __fmaf_rn(y, deq, g.y);
+                  } else {
+                    x += g.x;
+                    y += g.y;
+                  }
+                } else if constexpr (ET != 0) {
+                  x = __fmul_rn(x, deq);
+                  y = __fmul_rn(y, deq);
+                }
+                st_shared_u32(q, pack_bf16x2(x, y));
+              }
+            }
+          }
+          fence_proxy_async();            // the generic-proxy writes are visible to the TMA store
+          named_bar_sync(bar_id, 128);
+          if (signal) {
+            for (int b = 0; b < nbox; ++b) tma_store_2d(&tmC, stg + b * Cfg::EPI_BOX_BYTES, c0 + 64 * b, m0);
+            tma_store_commit();
+          }
+        }
+        continue;
+      }
       const int r0 = m0 + wq * 16 + (lane >> 2);
       const int c0 = n0 + 2 * (lane & 3);
 #pragma unroll
@@ -411,6 +502,8 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
         }
       }
     }
+    if constexpr (TMA_EPI)
+      if (signal) tma_store_wait<0>();   // the staging area must outlive the last stores' reads and writes
   }
 
   if (CG == 2) cluster_sync();  // no CTA may exit while its peer can still multicast into it or arrive on it
@@ -526,8 +619,12 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
   const int num_m_tiles = (M + Cfg::BM * CG - 1) / (Cfg::BM * CG);
   const int num_n_tiles = (N + Cfg::BN - 1) / Cfg::BN;
   const int num_tiles = num_m_tiles * num_n_tiles;
+  // C in 64 x 64 boxes (the staging layout of the epilogue); the other modes store from registers
+  CUtensorMap tmC{};
+  if constexpr (kTmaEpilogue<B_MODE, C_MODE>) tmC = make_tmap_2d(C, N, M, ldc * 2, 64, 64);
   auto kern = gemm_bf16_kernel<A_K, B_K, CG, A_MODE, B_MODE, C_MODE, ET>;
-  constexpr int kSmem = Cfg::SMEM_BYTES + (B_MODE == 3 ? Cfg::GATHER_BYTES : 0);
+  constexpr int kSmem = kTmaEpilogue<B_MODE, C_MODE> ? Cfg::SMEM_BYTES_EPI
+                                                     : Cfg::SMEM_BYTES + (B_MODE == 3 ? Cfg::GATHER_BYTES : 0);
   static bool attr_set = false;
   if (!attr_set) {
     DTG_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
@@ -568,8 +665,8 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
   attrs[0].val.clusterDim.z = 1;
   cfg.attrs = attrs;
   cfg.numAttrs = 1;
-  DTG_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, dist, (__nv_bfloat16*)C, M, N, K, ldc, accumulate ? 1 : 0,
-                                    num_m_tiles, num_tiles, scale_a, scale_b));
+  DTG_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, dist, tmC, (__nv_bfloat16*)C, M, N, K, ldc,
+                                    accumulate ? 1 : 0, num_m_tiles, num_tiles, scale_a, scale_b));
   note_launch();
 }
 
@@ -588,21 +685,21 @@ int gemm_max_active_clusters(int cg) {
   if (cg == 2) {
     auto kern = gemm_bf16_kernel<true, true, 2, 0, 0, 0>;
     cfg.gridDim = dim3(sm_count());
-    cfg.dynamicSmemBytes = GemmCfg<2>::SMEM_BYTES;
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<2>::SMEM_BYTES);
+    cfg.dynamicSmemBytes = GemmCfg<2>::SMEM_BYTES_EPI;
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<2>::SMEM_BYTES_EPI);
     cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
   } else {
     auto kern = gemm_bf16_kernel<true, true, 1, 0, 0, 0>;
     cfg.gridDim = dim3(sm_count());
-    cfg.dynamicSmemBytes = GemmCfg<1>::SMEM_BYTES;
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<1>::SMEM_BYTES);
+    cfg.dynamicSmemBytes = GemmCfg<1>::SMEM_BYTES_EPI;
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<1>::SMEM_BYTES_EPI);
     cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
   }
   return n;
 }
 
-// TMA operands need 16-byte aligned bases (the tensor-map encoder refuses others); the epilogue stores C in
-// bf16 pairs, and 16 bytes keeps every row of C on a vector boundary as ldc % 8 == 0 does for the rows after it.
+// TMA operands need 16-byte aligned bases (the tensor-map encoder refuses others); C is stored by TMA too, and with
+// ldc % 8 == 0 every row of it starts on a 16-byte boundary as well.
 static void check_gemm_bases(const char* who, const void* A, const void* B, const void* C) {
   const struct { const void* p; const char* name; } ops[3] = {{A, "A"}, {B, "B"}, {C, "C"}};
   for (const auto& o : ops)

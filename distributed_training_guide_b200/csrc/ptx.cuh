@@ -127,6 +127,16 @@ __device__ __forceinline__ void mbar_wait_mma(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// 32-bit shared-memory accesses by shared-window address (a generic pointer would compile to generic ST / LD)
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+
 // sub-CTA barrier over `nthreads` threads (ids 1..15; 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
