@@ -16,6 +16,8 @@ void rmsnorm_bwd(const void* dy, const void* h, const void* w, const float* rstd
                  float* dw_partial, float* dw, int T, int H, cudaStream_t s);
 void rope_inplace(void* qkv, const float* cos, const float* sin, long long T, int S, int n_heads, int n_rot, int d,
                   bool per_token, bool inverse, cudaStream_t s);
+// out[c] = sum over rows r of partial[r][c] (fp32 [rows, H]), in a fixed order
+void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s);
 void swiglu_fwd(const void* gu, void* h, long long T, int I, cudaStream_t s);
 void swiglu_bwd(const void* dh, const void* gu, void* dgu, long long T, int I, cudaStream_t s);
 void embedding_fwd(const long long* ids, const void* w, void* out, long long T, int H, cudaStream_t s);
@@ -26,6 +28,21 @@ void embedding_bwd(const void* dout, const long long* ids, void* dw, unsigned in
 void embedding_bwd_sorted(const void* dout, const long long* ids_sorted, const long long* perm, void* dw, long long T, int H,
                           bool accumulate, cudaStream_t s);
 void scale_inplace(void* x, const float* scale, long long n, cudaStream_t s);
+
+// ---- qk_norm_rope.cu -----------------------------------------------------------------------
+// QK-norm + RoPE (Qwen3) in place on heads [0, nh + nkv) of qkv [T, n_heads, 128] bf16 (n_heads = nh + 2*nkv):
+// per head y = bf16(bf16(x * rstd) * w) with w = q_w (heads < nh) or k_w, then the RoPE of rope_inplace.  cos/sin:
+// fp32 [S, 64] (pos = t % S) or per-token [T, 64].  Writes x_save [T, nh + nkv, 128] bf16 (the pre-norm q|k heads)
+// and rstd [T, nh + nkv] fp32 for the backward.
+void qk_norm_rope_fwd(void* qkv, const void* q_w, const void* k_w, const float* cos, const float* sin, void* x_save,
+                      float* rstd, long long T, int S, int n_heads, int nh, int nkv, bool per_token, float eps,
+                      cudaStream_t s);
+int qk_norm_rope_bwd_grid(long long T, int nqk);
+// In place on the q|k heads of dqkv: inverse rotation, then the RMSNorm backward.  dw [2, 128] fp32 = the q and
+// k gain gradients; dw_partial: [qk_norm_rope_bwd_grid(T, nh + nkv), 256] fp32 scratch.
+void qk_norm_rope_bwd(void* dqkv, const void* x_save, const float* rstd, const void* q_w, const void* k_w,
+                      const float* cos, const float* sin, float* dw_partial, float* dw, long long T, int S, int n_heads,
+                      int nh, int nkv, bool per_token, cudaStream_t s);
 
 // ---- cross_entropy.cu ----------------------------------------------------------------------
 // logits [T,V] bf16 are overwritten with dlogits = (softmax - onehot) / n_valid; loss = mean CE.

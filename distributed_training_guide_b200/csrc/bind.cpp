@@ -166,6 +166,67 @@ void rope_inplace(Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t n_r
                     (int)d, per_token, inverse, stream());
 }
 
+// Shared checks of qk_norm_rope_fwd / _bwd; returns per_token.  Every refusal happens before any launch.
+bool check_qk_norm_rope(const Tensor& qkv, const Tensor& q_w, const Tensor& k_w, const Tensor& cos, const Tensor& sin,
+                        int64_t nh, int64_t nkv) {
+  check_vec(qkv, "qkv", at::kBFloat16);
+  TORCH_CHECK(qkv.dim() == 4, "qk_norm_rope: qkv must be [B, S, heads, d]");
+  const int64_t B = qkv.size(0), S = qkv.size(1), NH = qkv.size(2), d = qkv.size(3);
+  TORCH_CHECK(d == 128, "qk_norm_rope: head_dim must be 128, got ", d);
+  TORCH_CHECK(nh >= 1 && nkv >= 1 && NH == nh + 2 * nkv, "qk_norm_rope: qkv has ", NH,
+              " heads, expected nh + 2 * nkv with nh, nkv >= 1 (nh = ", nh, ", nkv = ", nkv, ")");
+  check_vec(q_w, "q_w", at::kBFloat16);
+  check_vec(k_w, "k_w", at::kBFloat16);
+  TORCH_CHECK(q_w.dim() == 1 && q_w.size(0) == d, "qk_norm_rope: q_w must be [", d, "]");
+  TORCH_CHECK(k_w.dim() == 1 && k_w.size(0) == d, "qk_norm_rope: k_w must be [", d, "]");
+  check_vec(cos, "cos", at::kFloat);
+  check_vec(sin, "sin", at::kFloat);
+  TORCH_CHECK(sin.sizes() == cos.sizes(), "qk_norm_rope: cos and sin differ in shape");
+  TORCH_CHECK((cos.dim() == 2 || cos.dim() == 3) && cos.size(-1) == d / 2,
+              "qk_norm_rope: cos/sin must be [S, ", d / 2, "], [T, ", d / 2, "] or [B, S, ", d / 2, "]");
+  const int64_t rows = cos.dim() == 2 ? cos.size(0) : cos.size(0) * cos.size(1);
+  TORCH_CHECK(cos.dim() == 2 || (cos.size(0) == B && cos.size(1) == S),
+              "qk_norm_rope: a 3-D cos/sin table must be [B, S, d/2] = [", B, ", ", S, ", ", d / 2, "]");
+  TORCH_CHECK(rows == S || rows == B * S, "qk_norm_rope: cos/sin have ", rows, " rows, which matches neither S = ", S,
+              " nor T = ", B * S);
+  for (const Tensor* t : {&q_w, &k_w, &cos, &sin})
+    TORCH_CHECK(t->device() == qkv.device(), "qk_norm_rope: every operand must be on the device of qkv");
+  return rows != S;
+}
+
+std::tuple<Tensor, Tensor> qk_norm_rope_fwd(Tensor& qkv, const Tensor& q_w, const Tensor& k_w, const Tensor& cos,
+                                            const Tensor& sin, int64_t nh, int64_t nkv, double eps) {
+  const bool per_token = check_qk_norm_rope(qkv, q_w, k_w, cos, sin, nh, nkv);
+  TORCH_CHECK(std::isfinite(eps) && eps >= 0, "qk_norm_rope: eps must be finite and >= 0");
+  const c10::cuda::CUDAGuard guard(qkv.device());
+  const int64_t B = qkv.size(0), S = qkv.size(1);
+  Tensor x_save = torch::empty({B, S, nh + nkv, 128}, qkv.options());
+  Tensor rstd = torch::empty({B, S, nh + nkv}, qkv.options().dtype(at::kFloat));
+  dtg::qk_norm_rope_fwd(qkv.data_ptr(), q_w.data_ptr(), k_w.data_ptr(), cos.data_ptr<float>(), sin.data_ptr<float>(),
+                        x_save.data_ptr(), rstd.data_ptr<float>(), B * S, (int)S, (int)qkv.size(2), (int)nh, (int)nkv,
+                        per_token, (float)eps, stream());
+  return {x_save, rstd};
+}
+
+Tensor qk_norm_rope_bwd(Tensor& dqkv, const Tensor& x_save, const Tensor& rstd, const Tensor& q_w, const Tensor& k_w,
+                        const Tensor& cos, const Tensor& sin, int64_t nh, int64_t nkv) {
+  const bool per_token = check_qk_norm_rope(dqkv, q_w, k_w, cos, sin, nh, nkv);
+  const int64_t B = dqkv.size(0), S = dqkv.size(1), T = B * S;
+  check_vec(x_save, "x_save", at::kBFloat16);
+  check_contig(rstd, "rstd", at::kFloat);
+  TORCH_CHECK(x_save.sizes() == at::IntArrayRef({B, S, nh + nkv, 128}) && x_save.device() == dqkv.device(),
+              "qk_norm_rope_bwd: x_save must be [B, S, nh + nkv, 128] on the device of dqkv");
+  TORCH_CHECK(rstd.sizes() == at::IntArrayRef({B, S, nh + nkv}) && rstd.device() == dqkv.device(),
+              "qk_norm_rope_bwd: rstd must be [B, S, nh + nkv] on the device of dqkv");
+  const c10::cuda::CUDAGuard guard(dqkv.device());
+  Tensor dw = torch::empty({2, 128}, dqkv.options().dtype(at::kFloat));
+  Tensor partial = torch::empty({dtg::qk_norm_rope_bwd_grid(T, (int)(nh + nkv)), 256}, dqkv.options().dtype(at::kFloat));
+  dtg::qk_norm_rope_bwd(dqkv.data_ptr(), x_save.data_ptr(), rstd.data_ptr<float>(), q_w.data_ptr(), k_w.data_ptr(),
+                        cos.data_ptr<float>(), sin.data_ptr<float>(), partial.data_ptr<float>(), dw.data_ptr<float>(), T,
+                        (int)S, (int)dqkv.size(2), (int)nh, (int)nkv, per_token, stream());
+  return dw;
+}
+
 Tensor swiglu_fwd(const Tensor& gu) {
   check_vec(gu, "gu", at::kBFloat16);
   const c10::cuda::CUDAGuard guard(gu.device());
@@ -272,6 +333,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("rmsnorm_fwd", &rmsnorm_fwd);
   m.def("rmsnorm_bwd", &rmsnorm_bwd);
   m.def("rope_inplace", &rope_inplace);
+  m.def("qk_norm_rope_fwd", &qk_norm_rope_fwd);
+  m.def("qk_norm_rope_bwd", &qk_norm_rope_bwd);
   m.def("swiglu_fwd", &swiglu_fwd);
   m.def("swiglu_bwd", &swiglu_bwd);
   m.def("cross_entropy_fwd_bwd", &cross_entropy_fwd_bwd);

@@ -192,6 +192,12 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ p
 // grid*H*4 bytes of extra traffic, 19 MB at H=4096)
 int rmsnorm_bwd_grid(int T) { return T < 8 * sm_count() ? T : 8 * sm_count(); }
 
+void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s) {
+  colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(partial, out, rows, H);
+  note_launch();
+  DTG_LAUNCH_CHECK();
+}
+
 void rmsnorm_bwd(const void* dy, const void* h, const void* w, const float* rstd, const void* dres, void* dx,
                  float* dw_partial, float* dw, int T, int H, cudaStream_t s) {
   if (H % 8 != 0) throw std::runtime_error("rmsnorm: hidden size must be a multiple of 8");

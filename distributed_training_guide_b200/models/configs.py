@@ -16,7 +16,8 @@ from typing import Optional
 
 @dataclasses.dataclass
 class ModelConfig:
-    arch: str  # "llama" | "mistral" | "gpt2"; mistral is llama with a sliding attention window
+    arch: str  # "llama" | "mistral" | "qwen3" | "gpt2"; mistral is llama with a sliding attention window, qwen3 llama
+    # with QK-norm and a head_dim of its own
     vocab_size: int
     hidden_size: int
     intermediate_size: int
@@ -30,6 +31,11 @@ class ModelConfig:
     tie_word_embeddings: bool = False
     #: sliding-window attention (Mistral): query q sees only the ``sliding_window`` most recent keys, k > q - W
     sliding_window: Optional[int] = None
+    #: per-head dimension when it is not hidden_size // num_attention_heads (Qwen3: 128 at every size); None derives
+    #: it from the hidden size.  Read it through ``head_dim``.
+    explicit_head_dim: Optional[int] = None
+    #: QK-norm (Qwen3): every q and k head is RMS-normalised and scaled by a [head_dim] gain before RoPE
+    qk_norm: bool = False
     # gpt2 only
     layer_norm_epsilon: float = 1e-5
     dropout: float = 0.0
@@ -37,6 +43,8 @@ class ModelConfig:
 
     @property
     def head_dim(self) -> int:
+        if self.explicit_head_dim is not None:
+            return self.explicit_head_dim
         return self.hidden_size // self.num_attention_heads
 
     def num_parameters(self) -> int:
@@ -44,8 +52,11 @@ class ModelConfig:
         if self.arch == "gpt2":
             per_layer = (3 * h * h + 3 * h) + (h * h + h) + (h * i + i) + (i * h + h) + 4 * h
             return v * h + self.max_position_embeddings * h + l * per_layer + 2 * h
+        q = self.num_attention_heads * self.head_dim
         kv = self.num_key_value_heads * self.head_dim
-        per_layer = h * h + 2 * kv * h + h * h + 3 * h * i + 2 * h
+        per_layer = h * q + 2 * kv * h + q * h + 3 * h * i + 2 * h
+        if self.qk_norm:
+            per_layer += 2 * self.head_dim
         n = v * h + l * per_layer + h
         if not self.tie_word_embeddings:
             n += v * h
@@ -76,6 +87,14 @@ def _mistral(name, v, h, i, l, nh, nkv, maxpos, theta, window):
     return dataclasses.replace(_llama(name, v, h, i, l, nh, nkv, maxpos, theta), arch="mistral", sliding_window=window)
 
 
+def _qwen3(name, h, i, l, nh, nkv, tied, v=151936, maxpos=40960):
+    return ModelConfig(
+        arch="qwen3", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
+        num_attention_heads=nh, num_key_value_heads=nkv, max_position_embeddings=maxpos,
+        rms_norm_eps=1e-6, rope_theta=1e6, tie_word_embeddings=tied, explicit_head_dim=128, qk_norm=True, name=name,
+    )
+
+
 _GPT2 = ModelConfig(
     arch="gpt2", vocab_size=50257, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
     num_attention_heads=12, num_key_value_heads=12, max_position_embeddings=1024,
@@ -94,12 +113,19 @@ REGISTRY = {
     "meta-llama/Llama-3.1-405B": _llama("meta-llama/Llama-3.1-405B", 128256, 16384, 53248, 126, 128, 8, 131072, 5e5, _LLAMA3_SCALING),
     "meta-llama/Meta-Llama-3.1-405B": _llama("meta-llama/Meta-Llama-3.1-405B", 128256, 16384, 53248, 126, 128, 8, 131072, 5e5, _LLAMA3_SCALING),
     "mistralai/Mistral-7B-v0.1": _mistral("mistralai/Mistral-7B-v0.1", 32000, 4096, 14336, 32, 32, 8, 32768, 1e4, 4096),
+    "Qwen/Qwen3-0.6B": _qwen3("Qwen/Qwen3-0.6B", 1024, 3072, 28, 16, 8, True),
+    "Qwen/Qwen3-1.7B": _qwen3("Qwen/Qwen3-1.7B", 2048, 6144, 28, 16, 8, True),
+    "Qwen/Qwen3-4B": _qwen3("Qwen/Qwen3-4B", 2560, 9728, 36, 32, 8, True),
+    "Qwen/Qwen3-8B": _qwen3("Qwen/Qwen3-8B", 4096, 12288, 36, 32, 8, False),
+    "Qwen/Qwen3-32B": _qwen3("Qwen/Qwen3-32B", 5120, 25600, 64, 64, 8, False),
     # tiny configs for tests / smoke runs (head_dim 128 so the sm_90a attention kernel applies)
     "debug-llama": _llama("debug-llama", 1024, 256, 512, 2, 2, 2, 2048, 1e4),
     "debug-llama-gqa": _llama("debug-llama-gqa", 1024, 512, 1024, 2, 4, 2, 2048, 5e5),
     "debug-llama-tp": _llama("debug-llama-tp", 2048, 1024, 2048, 2, 8, 8, 2048, 1e4),
     # a window that is not a multiple of the kernels' 128-row tiles
     "debug-mistral": _mistral("debug-mistral", 1024, 512, 1024, 2, 4, 2, 2048, 1e4, 192),
+    # 4 heads x 128 = 512 over a hidden size of 256: head_dim apart from the hidden size, as in Qwen3-0.6B / 4B / 32B
+    "debug-qwen3": _qwen3("debug-qwen3", 256, 512, 2, 4, 2, False, v=1024, maxpos=2048),
     "debug-gpt2": dataclasses.replace(_GPT2, vocab_size=512, hidden_size=64, intermediate_size=256,
                                       num_hidden_layers=2, num_attention_heads=2, num_key_value_heads=2,
                                       max_position_embeddings=128, name="debug-gpt2"),
@@ -117,9 +143,19 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
             max_position_embeddings=d.get("n_positions", 1024), tie_word_embeddings=True,
             layer_norm_epsilon=d.get("layer_norm_epsilon", 1e-5), dropout=d.get("resid_pdrop", 0.1), name=name,
         )
-    if mt not in ("llama", "mistral"):
+    if mt not in ("llama", "mistral", "qwen3"):
         raise ValueError(f"unsupported model_type {mt!r} in {name}")
     window = None
+    head_dim = None
+    if mt == "qwen3":
+        if d.get("use_sliding_window"):
+            raise ValueError(f"{name}: use_sliding_window is true; Qwen3 sliding-window layers are not supported")
+        if "sliding_attention" in (d.get("layer_types") or ()):
+            raise ValueError(f"{name}: layer_types contains 'sliding_attention'; Qwen3 sliding-window layers are "
+                             "not supported")
+        if d.get("attention_bias"):
+            raise ValueError(f"{name}: attention_bias is true; q/k/v/o projections with a bias are not supported")
+        head_dim = d.get("head_dim") or d["hidden_size"] // d["num_attention_heads"]
     if mt == "mistral":
         if d.get("head_dim") is not None and d["head_dim"] != d["hidden_size"] // d["num_attention_heads"]:
             raise ValueError(f"{name}: head_dim {d['head_dim']} differs from hidden_size / num_attention_heads = "
@@ -140,7 +176,7 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
         max_position_embeddings=d.get("max_position_embeddings", 4096),
         rms_norm_eps=d.get("rms_norm_eps", 1e-5), rope_theta=theta, rope_scaling=scaling,
         tie_word_embeddings=d.get("tie_word_embeddings", False), sliding_window=window, name=name,
-        arch=mt,
+        arch=mt, explicit_head_dim=head_dim, qk_norm=mt == "qwen3",
     )
 
 
@@ -192,6 +228,17 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
             "max_position_embeddings": cfg.max_position_embeddings, "rms_norm_eps": cfg.rms_norm_eps,
             "rope_theta": cfg.rope_theta, "sliding_window": cfg.sliding_window, "hidden_act": "silu",
             "tie_word_embeddings": cfg.tie_word_embeddings, "bos_token_id": 1, "eos_token_id": 2,
+            "torch_dtype": "bfloat16",
+        }
+    if cfg.arch == "qwen3":
+        d = {
+            "model_type": "qwen3", "architectures": ["Qwen3ForCausalLM"], "vocab_size": cfg.vocab_size,
+            "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size,
+            "num_hidden_layers": cfg.num_hidden_layers, "num_attention_heads": cfg.num_attention_heads,
+            "num_key_value_heads": cfg.num_key_value_heads, "head_dim": cfg.head_dim,
+            "max_position_embeddings": cfg.max_position_embeddings, "rms_norm_eps": cfg.rms_norm_eps,
+            "rope_theta": cfg.rope_theta, "hidden_act": "silu", "tie_word_embeddings": cfg.tie_word_embeddings,
+            "attention_bias": False, "use_sliding_window": False, "bos_token_id": 151643, "eos_token_id": 151645,
             "torch_dtype": "bfloat16",
         }
     if cfg.rope_scaling:

@@ -1,11 +1,12 @@
-"""Llama-family causal LM built on the sm_90a op layer (Llama, and Mistral: Llama plus a sliding attention window).
+"""Llama-family causal LM built on the sm_90a op layer (Llama; Mistral: Llama plus a sliding attention window; Qwen3:
+Llama plus QK-norm, with a head_dim of its own).
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
 the reference instantiates at e.g. ``02-distributed-data-parallel/train_llm.py:57-58``)
 so checkpoints keep meaningful keys: ``model.embed_tokens.weight``,
 ``model.layers.{i}.self_attn.{q,k,v,o}_proj.weight``, ``model.layers.{i}.mlp.
 {gate,up,down}_proj.weight``, ``...{input,post_attention}_layernorm.weight``,
-``model.norm.weight``, ``lm_head.weight``.
+``model.norm.weight``, ``lm_head.weight``; Qwen3 adds ``...self_attn.{q,k}_norm.weight``.
 
 What is *different* from the HF module code (SURVEY.md §3.2) is the execution plan:
   * q/k/v (and gate/up) projections run as ONE wgmma GEMM over a fused weight that is
@@ -147,6 +148,17 @@ class LlamaAttention(nn.Module):
         self.k_proj = Linear(h, self.num_kv_heads * d, dtype, device)
         self.v_proj = Linear(h, self.num_kv_heads * d, dtype, device)
         self.o_proj = Linear(self.num_heads * d, h, dtype, device)
+        #: QK-norm (Qwen3): [head_dim] gains, replicated under tensor parallelism (every rank normalises its heads)
+        self.q_norm = RMSNorm(d, config.rms_norm_eps, dtype, device) if config.qk_norm else None
+        self.k_norm = RMSNorm(d, config.rms_norm_eps, dtype, device) if config.qk_norm else None
+
+    def position_qk_(self, qkv, cos, sin):
+        """RoPE (after QK-norm, when the layer has it) on the q and k heads of ``qkv`` [B,S,heads,d], in place on
+        the kernel path."""
+        if self.q_norm is None:
+            return ops.rope_qkv_(qkv, cos, sin, self.num_heads + self.num_kv_heads)
+        return ops.qk_norm_rope_(qkv, self.q_norm.weight, self.k_norm.weight, cos, sin, self.num_heads,
+                                 self.num_kv_heads, self.q_norm.eps)
 
 
 class LlamaMLP(nn.Module):
@@ -171,12 +183,15 @@ class FusedWeight:
 
 
 class LlamaDecoderLayer(nn.Module):
-    #: parameter order inside a layer's flat buffer; adjacency is what makes fusion free
+    #: parameter order inside a Llama / Mistral layer's flat buffer; adjacency is what makes fusion free
     FLAT_ORDER = (
         "self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight",
         "self_attn.o_proj.weight", "mlp.gate_proj.weight", "mlp.up_proj.weight",
         "mlp.down_proj.weight", "input_layernorm.weight", "post_attention_layernorm.weight",
     )
+    #: appended with QK-norm: after the layer norms, so the matrices stay first (FSDP's chunked layout) and every
+    #: replicated gain sits in one run at the end (TP sums their gradients over the group in one launch)
+    QK_NORM_ORDER = ("self_attn.q_norm.weight", "self_attn.k_norm.weight")
     FUSED = {"qkv": FLAT_ORDER[0:3], "gate_up": FLAT_ORDER[4:6]}
 
     def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
@@ -186,6 +201,9 @@ class LlamaDecoderLayer(nn.Module):
         self.mlp = LlamaMLP(config, dtype, device, tp_size)
         self.input_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
         self.post_attention_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
+        #: this layer's parameter order in its flat buffer (parallel/flat.py, parallel/fsdp.py); a parameter missing
+        #: here would get no gradient buffer and no optimizer update
+        self.flat_order = self.FLAT_ORDER + (self.QK_NORM_ORDER if config.qk_norm else ())
         self._fused = {}  # name -> FusedWeight, installed by parallel.flat.FlatParamGroup
         self.tp = None  # installed by parallel.tp.apply_tensor_parallel
         self.fp8 = False  # set through LlamaForCausalLM.fp8: the four projections run ops.fp8_linear
@@ -216,7 +234,7 @@ class LlamaDecoderLayer(nn.Module):
         y, h = self.input_layernorm(x, residual)
         w, owner = self._qkv_weight()
         qkv = fused_linear(y, w, owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
-        qkv = ops.rope_qkv_(qkv, cos, sin, att.num_heads + att.num_kv_heads)
+        qkv = att.position_qk_(qkv, cos, sin)
         a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
         a = a.reshape(B, S, att.num_heads * att.head_dim)
         a = ops.fp8_linear(a, att.o_proj.weight) if self.fp8 else att.o_proj(a)

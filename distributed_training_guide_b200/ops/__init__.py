@@ -3,9 +3,9 @@
 On CUDA tensors each op calls a hand-written sm_90a kernel from the in-tree
 extension (``csrc/``): wgmma/TMA GEMM (fwd / dgrad / wgrad) in bf16 and, for
 ``fp8_linear``, in fp8 with its amax and cast-transpose kernels, wgmma
-flash-attention, fused residual-add+RMSNorm, in-place RoPE on the fused qkv buffer,
-SwiGLU, in-place softmax-cross-entropy, embedding gather / scatter-add and flat
-AdamW.  On CPU tensors the same Functions run the reference math in
+flash-attention, fused residual-add+RMSNorm, in-place RoPE on the fused qkv buffer
+(after Qwen3's per-head QK-norm in the same kernel), SwiGLU, in-place
+softmax-cross-entropy, embedding gather / scatter-add and flat AdamW.  On CPU tensors the same Functions run the reference math in
 ``ops/reference.py`` (chapter 01's CPU config and the gloo tests).
 
 Replaces what the reference obtains implicitly from cuBLAS / SDPA / flash-attn /
@@ -27,7 +27,7 @@ from .. import _ext
 from . import reference as ref
 
 __all__ = [
-    "linear", "fused_linear", "rms_norm", "add_rms_norm", "rope_qkv_", "attention_qkv", "document_starts", "swiglu", "cross_entropy",
+    "linear", "fused_linear", "rms_norm", "add_rms_norm", "rope_qkv_", "qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy",
     "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "ref",
 ]
 
@@ -360,6 +360,47 @@ def rope_qkv_(qkv, cos, sin, n_rot_heads):
         return _RopeQKV.apply(qkv, cos.contiguous(), sin.contiguous(), n_rot_heads)
     rot = ref.rope_apply(qkv[:, :, :n_rot_heads], cos, sin)
     return torch.cat([rot, qkv[:, :, n_rot_heads:]], dim=2)
+
+
+class _QKNormRope(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, qkv, q_w, k_w, cos, sin, nh, nkv, eps):
+        C = _ext.load()
+        x_save, rstd = C.qk_norm_rope_fwd(qkv, q_w, k_w, cos, sin, nh, nkv, float(eps))
+        ctx.save_for_backward(x_save, rstd, q_w, k_w, cos, sin)
+        ctx.heads = (nh, nkv)
+        ctx.w_params = (q_w, k_w)
+        return qkv.detach()   # in place, handed to autograd as a fresh tensor (see _RopeQKV)
+
+    @staticmethod
+    def backward(ctx, dqkv):
+        C = _ext.load()
+        x_save, rstd, q_w, k_w, cos, sin = ctx.saved_tensors
+        if not dqkv.is_contiguous():
+            dqkv = dqkv.contiguous()
+        dw32 = C.qk_norm_rope_bwd(dqkv, x_save, rstd, q_w, k_w, cos, sin, *ctx.heads)   # in place on dqkv's q|k
+        dq = _emit_weight_grad(ctx.w_params[0], _norm_dw_into(dw32[0]), q_w)
+        dk = _emit_weight_grad(ctx.w_params[1], _norm_dw_into(dw32[1]), k_w)
+        return dqkv, dq, dk, None, None, None, None, None
+
+
+def qk_norm_rope_(qkv, q_w, k_w, cos, sin, nh, nkv, eps):
+    """Qwen3's QK-norm then RoPE on ``qkv`` [B,S,nh+2*nkv,d]: every q head is RMS-normalised over its d elements
+    and scaled by ``q_w`` [d], every k head likewise with ``k_w``, with ``ref.rms_norm``'s rounding points; then
+    heads [0, nh+nkv) are rotated as ``rope_qkv_`` does, with cos/sin [S,d/2] or [B,S,d/2] (fp32).  V is untouched.
+
+    bf16 CUDA tensors with d = 128 run the sm_90a kernels in place on ``qkv``; anything else composes
+    ``ref.rms_norm`` and ``ref.rope_apply``.  The kernel path keeps the pre-norm q|k heads (bf16) and one fp32 rstd
+    per head for the backward: (nh + nkv) * 128 * 2 bytes per token, 42 MB per layer for Qwen3-8B (32 + 8 heads)
+    at 4096 tokens.  The gain gradients go through ``_emit_weight_grad``, so flat-buffer parameters are overwritten
+    on their first use in a step and accumulated on later ones."""
+    if (_ext.use_cuda_kernel("qk_norm_rope", qkv, q_w, k_w) and qkv.dtype == torch.bfloat16
+            and qkv.shape[-1] == 128):
+        return _QKNormRope.apply(qkv, q_w, k_w, cos.contiguous(), sin.contiguous(), nh, nkv, eps)
+    q = ref.rms_norm(qkv[:, :, :nh], q_w, eps)
+    k = ref.rms_norm(qkv[:, :, nh:nh + nkv], k_w, eps)
+    rot = ref.rope_apply(torch.cat([q, k], dim=2), cos, sin)
+    return torch.cat([rot, qkv[:, :, nh + nkv:]], dim=2)
 
 
 # --------------------------------------------------------------------------------------

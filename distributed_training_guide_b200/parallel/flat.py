@@ -148,7 +148,8 @@ def build_groups(model: nn.Module, device, dtype, world_size: int = 1, alloc=Non
     for i, layer in enumerate(layers):
         named = dict(layer.named_parameters())
         if isinstance(layer, LlamaDecoderLayer):
-            ordered = [(f"model.layers.{i}.{n}", named[n]) for n in LlamaDecoderLayer.FLAT_ORDER]
+            assert set(named) == set(layer.flat_order), f"layer {i}: parameters outside flat_order"
+            ordered = [(f"model.layers.{i}.{n}", named[n]) for n in layer.flat_order]
         else:
             prefix = "transformer.h" if hasattr(core, "h") else "model.layers"
             ordered = [(f"{prefix}.{i}.{n}", p) for n, p in named.items()]

@@ -149,7 +149,8 @@ class FSDPEngine:
         if self.is_llama:
             for i, layer in enumerate(self.layers):
                 named = dict(layer.named_parameters())
-                layer_named.append([(f"model.layers.{i}.{n}", named[n]) for n in LlamaDecoderLayer.FLAT_ORDER])
+                assert set(named) == set(layer.flat_order), f"layer {i}: parameters outside flat_order"
+                layer_named.append([(f"model.layers.{i}.{n}", named[n]) for n in layer.flat_order])
             embed_named = [("model.embed_tokens.weight", core.embed_tokens.weight)]
             head_named = [("model.norm.weight", core.norm.weight)]
             if not self.tied:  # a tied lm_head IS the embedding parameter (it lives in the embed group)

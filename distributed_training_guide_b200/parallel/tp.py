@@ -374,7 +374,7 @@ class TensorParallelRuntime:
         w, owner = self.fused(layer, "qkv", (att.q_proj, att.k_proj, att.v_proj))
         qkv = _ColumnParallelLinear.apply(y, w, owner, tp, 2 * layer.layer_idx)
         qkv = qkv.view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
-        qkv = ops.rope_qkv_(qkv, cos, sin, att.num_heads + att.num_kv_heads)
+        qkv = att.position_qk_(qkv, cos, sin)
         a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, window=att.sliding_window)
         a = a.reshape(B * S, att.num_heads * att.head_dim)
         h2 = _RowParallelLinear.apply(a, att.o_proj.weight, att.o_proj.weight, tp, h)   # residual add fused
