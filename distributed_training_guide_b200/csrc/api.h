@@ -89,18 +89,18 @@ void fp8_cast_transpose(const void* x, long long ld, int R, int C, bool e5m2, co
                         float* scale_inv, cudaStream_t s);
 
 // ---- attention_fwd.cu / attention_bwd.cu ---------------------------------------------------
-// qkv: [B,S,nh+2*nkv,128] bf16 (q heads | k heads | v heads); o: [B,S,nh,128]; lse: [B,nh,S] fp32
+// qkv: [B,S,nh+2*nkv,D] bf16 (q heads | k heads | v heads); o: [B,S,nh,D]; lse: [B,nh,S] fp32; head_dim D = 64 or 128
 // attn_fwd: P through shared memory; attn_fwd2: P kept in registers
 // doc_start: null (plain causal) or int32 [B,S], the first token of each token's document (document masking:
 // key k is visible to query q iff doc_start[q] <= k <= q)
 // window: 0 (none) or W >= 1, sliding-window attention: key k is also visible only if k > q - W.  W >= S masks
 // nothing and runs the kernels without a window.
 void attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s,
-              const int* doc_start = nullptr, int window = 0);
+              const int* doc_start = nullptr, int window = 0, int head_dim = 128);
 void attn_fwd2(const void* qkv, void* o, float* lse, int B, int S, int nh, int nkv, float scale, cudaStream_t s,
-               const int* doc_start = nullptr, int window = 0);
+               const int* doc_start = nullptr, int window = 0, int head_dim = 128);
 void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* dq_acc,
               void* dqkv, int B, int S, int nh, int nkv, float scale, int mode, cudaStream_t s,
-              const int* doc_start = nullptr, int window = 0);
+              const int* doc_start = nullptr, int window = 0, int head_dim = 128);
 
 }  // namespace dtg

@@ -1,4 +1,4 @@
-// Causal flash-attention backward on wgmma (head_dim 128, GQA).
+// Causal flash-attention backward on wgmma (head_dim D = 64 or 128, GQA).
 //
 // Two passes of ONE kernel template, each owning a 128-row block R and streaming 64-wide column
 // blocks C of the opposite kind (no atomics, deterministic):
@@ -6,7 +6,7 @@
 //   KV pass  R = 128 keys of a kv head, C = 64-query blocks of every q head in its GQA group
 //            S^T = K_R Q_C^T,  dP^T = V_R dO_C^T          (wgmma m64n64k16 per warpgroup, fp32 in registers)
 //            P^T = exp2(S^T*c - lse_q),  dS^T = P^T o (dP^T - delta_q) * scale
-//            dV_R += P^T dO_C,   dK_R += dS^T Q_C         (wgmma m64n128k16, B = the C tile, MN-major)
+//            dV_R += P^T dO_C,   dK_R += dS^T Q_C         (wgmma m64nDk16, B = the C tile, MN-major)
 //   Q pass   R = 128 queries of a q head, C = 64-key blocks
 //            S = Q_R K_C^T,  dP = dO_R V_C^T,  dS = P o (dP - delta_q) * scale,   dQ_R += dS K_C
 //
@@ -21,6 +21,8 @@
 // R0 - W + 1 and bounds each row's keys by row - W + 1.  Both bounds are arithmetic: no loads.
 // Gradients are written into a dqkv buffer with the same fused layout as qkv, so the
 // RoPE-backward kernel and the fused qkv dgrad/wgrad GEMMs consume it directly.
+// D: every tile is D / 64 TMA boxes of 128-byte rows; S^T / dP^T take D / 16 k16 steps and each gradient
+// accumulator is D / 2 fp32 registers.  Ranges, masks and block skipping do not depend on D.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -35,33 +37,36 @@ namespace dtg {
 using namespace ptx;
 
 namespace bwd {
-constexpr int D = 128;
-constexpr int R_TILE = 128 * 128 * 2;  // 32 KB resident tile (two 16 KB halves)
-constexpr int R_HALF = R_TILE / 2;
-constexpr int C_TILE = 64 * 128 * 2;   // 16 KB streamed tile (two 8 KB halves)
-constexpr int C_HALF = C_TILE / 2;
-constexpr int OFF_R1 = 0, OFF_R2 = R_TILE;
+constexpr int R_HALF = 128 * 128;      // 16 KB: one resident TMA box, [128 rows x 128 B]
+constexpr int C_HALF = 64 * 128;       // 8 KB: one streamed TMA box, [64 rows x 128 B]
 constexpr int Y_STAGES = 3;                   // TMA ring depth for the streamed tiles
-constexpr int OFF_Y = 2 * R_TILE;             // [stage][Y1 | Y2]
-constexpr int OFF_P = OFF_Y + Y_STAGES * 2 * C_TILE;  // 16 KB: [128 rows x 64] bf16, K-major (SS form only)
-constexpr int OFF_DS = OFF_P + 128 * 128;     // 16 KB
-constexpr int OFF_BAR = OFF_DS + 128 * 128;
-constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
 constexpr float LOG2E = 1.4426950408889634f;
 constexpr int THREADS = 256;
+template <int D>
+struct Layout {
+  static constexpr int R_TILE = 128 * D * 2;   // resident tile: D / 64 boxes (32 KB at D = 128)
+  static constexpr int C_TILE = 64 * D * 2;    // streamed tile: D / 64 boxes (16 KB at D = 128)
+  static constexpr int OFF_R1 = 0, OFF_R2 = R_TILE;
+  static constexpr int OFF_Y = 2 * R_TILE;                         // [stage][Y1 | Y2]
+  static constexpr int OFF_P = OFF_Y + Y_STAGES * 2 * C_TILE;      // 16 KB: [128 rows x 64] bf16, K-major (SS form only)
+  static constexpr int OFF_DS = OFF_P + 128 * 128;                 // 16 KB
+  static constexpr int OFF_BAR = OFF_DS + 128 * 128;
+  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+};
 }  // namespace bwd
 
-// delta[b, h, s] = sum_d dO * O   (one warp per (token, head) row)
+// delta[b, h, s] = sum_d dO * O   (one warp per (token, head) row of D elements, D / 32 per lane)
+template <int D>
 __global__ void attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ d_o, const __nv_bfloat16* __restrict__ o,
                                       float* __restrict__ delta, long long rows, int S, int nh) {
   const long long row = (blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
-  const __nv_bfloat162* a = reinterpret_cast<const __nv_bfloat162*>(d_o + row * 128) + lane * 2;
-  const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(o + row * 128) + lane * 2;
+  const __nv_bfloat162* a = reinterpret_cast<const __nv_bfloat162*>(d_o + row * D) + lane * (D / 64);
+  const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(o + row * D) + lane * (D / 64);
   float acc = 0.f;
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
+  for (int i = 0; i < D / 64; ++i) {
     const float2 x = __bfloat1622float2(a[i]), y = __bfloat1622float2(b[i]);
     acc += x.x * y.x + x.y * y.y;
   }
@@ -78,7 +83,7 @@ __global__ void attn_bwd_delta_kernel(const __nv_bfloat16* __restrict__ d_o, con
 // registers they were computed in and feed the gradient MMAs as their A operand (RS form).  Per 128x64 block that
 // removes 32 KB of shared-memory stores and 32 KB of A-operand reads.  TS = false stages them through
 // 128B-swizzled shared memory (SS form).
-template <bool KV_MODE, bool TS, bool DOC, bool WIN>
+template <bool KV_MODE, bool TS, bool DOC, bool WIN, int D>
 __global__ void __launch_bounds__(bwd::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_constant__ CUtensorMap tm_qkv_c,
                 const __grid_constant__ CUtensorMap tm_do_r, const __grid_constant__ CUtensorMap tm_do_c,
@@ -86,6 +91,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
                 int S, int nh, int nkv, float scale, int num_r_blocks, long long* __restrict__ trace,
                 const int* __restrict__ doc_start, int window) {
   using namespace bwd;
+  using L = Layout<D>;
+  constexpr int R_TILE = L::R_TILE, C_TILE = L::C_TILE, OFF_R1 = L::OFF_R1, OFF_R2 = L::OFF_R2, OFF_Y = L::OFF_Y,
+                OFF_P = L::OFF_P, OFF_DS = L::OFF_DS, OFF_BAR = L::OFF_BAR;
   // optional in-kernel timeline (attn_bwd(..., trace=int64[1024])): CTA (0,0) records clock64() per column block:
   // [iter][0] scores ready, [1] P / dS computed, [3] gradient MMAs retired (thread 0)
   const bool tracing = trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0;
@@ -185,30 +193,34 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
     mbar_arrive_expect_tx(&y_full[st], 2 * C_TILE);
     if (KV_MODE) {
       const int qh = kv_head * group + t / n_c;
-      tma_load_4d(&tm_qkv_c, &y_full[st], y1, 0, qh, C0, batch);
-      tma_load_4d(&tm_qkv_c, &y_full[st], y1 + C_HALF, 64, qh, C0, batch);
-      tma_load_4d(&tm_do_c, &y_full[st], y2, 0, qh, C0, batch);
-      tma_load_4d(&tm_do_c, &y_full[st], y2 + C_HALF, 64, qh, C0, batch);
+#pragma unroll
+      for (int b = 0; b < D / 64; ++b) tma_load_4d(&tm_qkv_c, &y_full[st], y1 + b * C_HALF, 64 * b, qh, C0, batch);
+#pragma unroll
+      for (int b = 0; b < D / 64; ++b) tma_load_4d(&tm_do_c, &y_full[st], y2 + b * C_HALF, 64 * b, qh, C0, batch);
     } else {
-      tma_load_4d(&tm_qkv_c, &y_full[st], y1, 0, nh + kv_head, C0, batch);
-      tma_load_4d(&tm_qkv_c, &y_full[st], y1 + C_HALF, 64, nh + kv_head, C0, batch);
-      tma_load_4d(&tm_qkv_c, &y_full[st], y2, 0, nh + nkv + kv_head, C0, batch);
-      tma_load_4d(&tm_qkv_c, &y_full[st], y2 + C_HALF, 64, nh + nkv + kv_head, C0, batch);
+#pragma unroll
+      for (int b = 0; b < D / 64; ++b)
+        tma_load_4d(&tm_qkv_c, &y_full[st], y1 + b * C_HALF, 64 * b, nh + kv_head, C0, batch);
+#pragma unroll
+      for (int b = 0; b < D / 64; ++b)
+        tma_load_4d(&tm_qkv_c, &y_full[st], y2 + b * C_HALF, 64 * b, nh + nkv + kv_head, C0, batch);
     }
   };
   if (threadIdx.x == 0) {
     // resident tiles: KV pass -> K_R, V_R ; Q pass -> Q_R, dO_R
     mbar_arrive_expect_tx(res_full, 2 * R_TILE);
     if (KV_MODE) {
-      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1, 0, nh + kv_head, R0, batch);
-      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1 + R_HALF, 64, nh + kv_head, R0, batch);
-      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R2, 0, nh + nkv + kv_head, R0, batch);
-      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R2 + R_HALF, 64, nh + nkv + kv_head, R0, batch);
+#pragma unroll
+      for (int b = 0; b < D / 64; ++b)
+        tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1 + b * R_HALF, 64 * b, nh + kv_head, R0, batch);
+#pragma unroll
+      for (int b = 0; b < D / 64; ++b)
+        tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R2 + b * R_HALF, 64 * b, nh + nkv + kv_head, R0, batch);
     } else {
-      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1, 0, head_r, R0, batch);
-      tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1 + R_HALF, 64, head_r, R0, batch);
-      tma_load_4d(&tm_do_r, res_full, smem + OFF_R2, 0, head_r, R0, batch);
-      tma_load_4d(&tm_do_r, res_full, smem + OFF_R2 + R_HALF, 64, head_r, R0, batch);
+#pragma unroll
+      for (int b = 0; b < D / 64; ++b) tma_load_4d(&tm_qkv_r, res_full, smem + OFF_R1 + b * R_HALF, 64 * b, head_r, R0, batch);
+#pragma unroll
+      for (int b = 0; b < D / 64; ++b) tma_load_4d(&tm_do_r, res_full, smem + OFF_R2 + b * R_HALF, 64 * b, head_r, R0, batch);
     }
     for (int t = 0; t < Y_STAGES - 1 && t < n_iter; ++t) issue_y(t);
   }
@@ -255,10 +267,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
         else ds_r[h] = max(ds_r[h], idx - window + 1);
       }
     }
-    [[maybe_unused]] float acc_a[KV_MODE ? 64 : 1];   // dV (KV pass)
-    float acc_b[64];                                  // dK (KV pass) / dQ (Q pass)
+    [[maybe_unused]] float acc_a[KV_MODE ? D / 2 : 1];   // dV (KV pass)
+    float acc_b[D / 2];                                  // dK (KV pass) / dQ (Q pass)
 #pragma unroll
-    for (int i = 0; i < 64; ++i) {
+    for (int i = 0; i < D / 2; ++i) {
       if constexpr (KV_MODE) acc_a[i] = 0.f;
       acc_b[i] = 0.f;
     }
@@ -290,13 +302,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
       fence_regs(sc);
       fence_regs(dp);
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
+      for (int kk = 0; kk < D / 16; ++kk) {
         const uint32_t ra = (uint32_t)((kk >> 2) * R_HALF + (kk & 3) * 32);
         const uint32_t cb = (uint32_t)((kk >> 2) * C_HALF + (kk & 3) * 32);
         wgmma_m64n64k16_ss<0, 0>(sc, desc_kmajor_sw128(r1 + ra), desc_kmajor_sw128(y1 + cb), 1u);
       }
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk) {
+      for (int kk = 0; kk < D / 16; ++kk) {
         const uint32_t ra = (uint32_t)((kk >> 2) * R_HALF + (kk & 3) * 32);
         const uint32_t cb = (uint32_t)((kk >> 2) * C_HALF + (kk & 3) * 32);
         wgmma_m64n64k16_ss<0, 0>(dp, desc_kmajor_sw128(r2 + ra), desc_kmajor_sw128(y2 + cb), 1u);
@@ -365,15 +377,15 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {  // dV += P^T dO_C
           const uint64_t db = desc_mnmajor_sw128(y2 + kk * 2048, C_HALF);
-          if constexpr (TS) wgmma_m64n128k16_rs<1>(acc_a, pp[kk], db, 1u);
-          else wgmma_m64n128k16_ss<0, 1>(acc_a, desc_kmajor_sw128(sp + kk * 32), db, 1u);
+          if constexpr (TS) wgmma_bf16_rs<1>(acc_a, pp[kk], db, 1u);
+          else wgmma_bf16_ss<0, 1>(acc_a, desc_kmajor_sw128(sp + kk * 32), db, 1u);
         }
       }
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {    // dK += dS^T Q_C   /   dQ += dS K_C
         const uint64_t db = desc_mnmajor_sw128(y1 + kk * 2048, C_HALF);
-        if constexpr (TS) wgmma_m64n128k16_rs<1>(acc_b, pd[kk], db, 1u);
-        else wgmma_m64n128k16_ss<0, 1>(acc_b, desc_kmajor_sw128(sds + kk * 32), db, 1u);
+        if constexpr (TS) wgmma_bf16_rs<1>(acc_b, pd[kk], db, 1u);
+        else wgmma_bf16_ss<0, 1>(acc_b, desc_kmajor_sw128(sds + kk * 32), db, 1u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -387,10 +399,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const long long tok = (long long)batch * S + R0 + rl0 + 8 * h;
-      auto write_row = [&](const float (&acc)[64], int out_head) {
+      auto write_row = [&](const float (&acc)[D / 2], int out_head) {
         __nv_bfloat16* dst = dqkv + (tok * nht + out_head) * (long long)D;
 #pragma unroll
-        for (int nb = 0; nb < 16; ++nb)
+        for (int nb = 0; nb < D / 8; ++nb)
           *reinterpret_cast<__nv_bfloat162*>(dst + 8 * nb + 2 * tq) =
               __floats2bfloat162_rn(acc[4 * nb + 2 * h], acc[4 * nb + 2 * h + 1]);
       };
@@ -404,64 +416,76 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv_r, const __grid_const
   }
 }
 
-template <bool TS, bool DOC, bool WIN>
+template <bool TS, bool DOC, bool WIN, int D>
 static void launch_attn_bwd(const CUtensorMap& tq_r, const CUtensorMap& tq_c, const CUtensorMap& td_r,
                             const CUtensorMap& td_c, const float* lse, const float* delta, void* dqkv, int B, int S,
                             int nh, int nkv, float scale, long long* trace, const int* doc_start, int window,
                             cudaStream_t s) {
+  constexpr int smem = bwd::Layout<D>::SMEM_BYTES;
   static bool attr = false;
   if (!attr) {
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<true, TS, DOC, WIN>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
-    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false, TS, DOC, WIN>,
-                                        cudaFuncAttributeMaxDynamicSharedMemorySize, bwd::SMEM_BYTES));
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<true, TS, DOC, WIN, D>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    DTG_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kernel<false, TS, DOC, WIN, D>,
+                                        cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr = true;
   }
   const int nblk = S / 128;
-  attn_bwd_kernel<true, TS, DOC, WIN><<<dim3(B * nkv, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
+  attn_bwd_kernel<true, TS, DOC, WIN, D><<<dim3(B * nkv, nblk, 1), bwd::THREADS, smem, s>>>(
       tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace, doc_start, window);
-  attn_bwd_kernel<false, TS, DOC, WIN><<<dim3(B * nh, nblk, 1), bwd::THREADS, bwd::SMEM_BYTES, s>>>(
+  attn_bwd_kernel<false, TS, DOC, WIN, D><<<dim3(B * nh, nblk, 1), bwd::THREADS, smem, s>>>(
       tq_r, tq_c, td_r, td_c, lse, delta, (__nv_bfloat16*)dqkv, S, nh, nkv, scale, nblk, trace ? trace + 512 : nullptr,
       doc_start, window);
 }
 
-template <bool TS>
+template <bool TS, int D>
 static void dispatch_attn_bwd(const CUtensorMap& tq_r, const CUtensorMap& tq_c, const CUtensorMap& td_r,
                               const CUtensorMap& td_c, const float* lse, const float* delta, void* dqkv, int B, int S,
                               int nh, int nkv, float scale, long long* trace, const int* doc_start, int window,
                               cudaStream_t s) {
   // a window that covers the whole sequence masks nothing: run the kernels without it
   if (window > 0 && window < S) {
-    if (doc_start) launch_attn_bwd<TS, true, true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
-    else launch_attn_bwd<TS, false, true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, window, s);
+    if (doc_start) launch_attn_bwd<TS, true, true, D>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
+    else launch_attn_bwd<TS, false, true, D>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, window, s);
   } else {
-    if (doc_start) launch_attn_bwd<TS, true, false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, 0, s);
-    else launch_attn_bwd<TS, false, false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, 0, s);
+    if (doc_start) launch_attn_bwd<TS, true, false, D>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, 0, s);
+    else launch_attn_bwd<TS, false, false, D>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, nullptr, 0, s);
   }
 }
 
 void attn_bwd(const void* qkv, const void* o, const void* d_o, const float* lse, float* delta, float* trace_buf,
               void* dqkv, int B, int S, int nh, int nkv, float scale, int mode, cudaStream_t s,
-              const int* doc_start, int window) {
+              const int* doc_start, int window, int head_dim) {
   long long* trace = reinterpret_cast<long long*>(trace_buf);  // [2][64][8] int64 or nullptr
   if (S % 128 != 0) throw std::runtime_error("attn_bwd: sequence length must be a multiple of 128");
   if (window < 0) throw std::runtime_error("attn_bwd: window must be >= 1 (0 = no window)");
   if (nh < 1 || nkv < 1 || nh % nkv != 0) throw std::runtime_error("attn_bwd: nh must be a positive multiple of nkv");
+  if (head_dim != 64 && head_dim != 128) throw std::runtime_error("attn_bwd: head_dim must be 64 or 128");
   // every tensor map is encoded (and can refuse its pointer) before the first launch
-  const CUtensorMap tq_r = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 128);
-  const CUtensorMap tq_c = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 64);
-  const CUtensorMap td_r = make_tmap_heads(d_o, B, S, nh, 128);
-  const CUtensorMap td_c = make_tmap_heads(d_o, B, S, nh, 64);
+  const CUtensorMap tq_r = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 128, head_dim);
+  const CUtensorMap tq_c = make_tmap_heads(qkv, B, S, nh + 2 * nkv, 64, head_dim);
+  const CUtensorMap td_r = make_tmap_heads(d_o, B, S, nh, 128, head_dim);
+  const CUtensorMap td_c = make_tmap_heads(d_o, B, S, nh, 64, head_dim);
   const long long rows = (long long)B * S * nh;
-  attn_bwd_delta_kernel<<<(unsigned)((rows * 32 + 255) / 256), 256, 0, s>>>(
-      (const __nv_bfloat16*)d_o, (const __nv_bfloat16*)o, delta, rows, S, nh);
+  const unsigned delta_blocks = (unsigned)((rows * 32 + 255) / 256);
+  if (head_dim == 128)
+    attn_bwd_delta_kernel<128><<<delta_blocks, 256, 0, s>>>((const __nv_bfloat16*)d_o, (const __nv_bfloat16*)o, delta,
+                                                            rows, S, nh);
+  else
+    attn_bwd_delta_kernel<64><<<delta_blocks, 256, 0, s>>>((const __nv_bfloat16*)d_o, (const __nv_bfloat16*)o, delta,
+                                                           rows, S, nh);
   static const bool ts_default = []() {   // DTG_ATTN_BWD=rs (default: P / dS stay in registers) | ss
     const char* e = getenv("DTG_ATTN_BWD");
     return e ? e[0] != 's' : true;
   }();
   const bool ts = mode == 0 ? ts_default : mode == 2;   // mode: 0 default, 1 = ss, 2 = rs
-  if (ts) dispatch_attn_bwd<true>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
-  else dispatch_attn_bwd<false>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
+  if (head_dim == 128) {
+    if (ts) dispatch_attn_bwd<true, 128>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
+    else dispatch_attn_bwd<false, 128>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
+  } else {
+    if (ts) dispatch_attn_bwd<true, 64>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
+    else dispatch_attn_bwd<false, 64>(tq_r, tq_c, td_r, td_c, lse, delta, dqkv, B, S, nh, nkv, scale, trace, doc_start, window, s);
+  }
   note_launch(3);
   DTG_LAUNCH_CHECK();
 }

@@ -338,6 +338,35 @@ __device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], const uint32
       : "memory");
 }
 
+template <int TB>
+__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d), "n"(TB)
+      : "memory");
+}
+
+// The same bf16 MMAs chosen by the accumulator's size: N = 2 * (registers), i.e. m64n128k16 for float[64] and
+// m64n64k16 for float[32].  Lets one kernel template cover head_dim 64 and 128.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  wgmma_m64n128k16_ss<TA, TB>(d, da, db, scale_d);
+}
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_bf16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  wgmma_m64n64k16_ss<TA, TB>(d, da, db, scale_d);
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_bf16_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  wgmma_m64n128k16_rs<TB>(d, a, db, scale_d);
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_bf16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  wgmma_m64n64k16_rs<TB>(d, a, db, scale_d);
+}
+
 // ---- wgmma m64n256k32 fp8 -> fp32, both operands K-major in shared memory (the fp8 forms of the instruction have no
 // transpose immediates).  AE: element type of A, 1 = e4m3, 2 = e5m2; B is always e4m3.  One k32 step reads 32 bytes
 // of a 128-byte swizzle span, like the k16 step of the bf16 form.

@@ -75,11 +75,15 @@ _LLAMA3_SCALING = {
 }
 
 
-def _llama(name, v, h, i, l, nh, nkv, maxpos, theta, scaling=None):
+# Llama 3.2 (1B / 3B): the llama3 rule with a factor of 32
+_LLAMA32_SCALING = {**_LLAMA3_SCALING, "factor": 32.0}
+
+
+def _llama(name, v, h, i, l, nh, nkv, maxpos, theta, scaling=None, tied=False):
     return ModelConfig(
         arch="llama", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
         num_attention_heads=nh, num_key_value_heads=nkv, max_position_embeddings=maxpos,
-        rms_norm_eps=1e-5, rope_theta=theta, rope_scaling=scaling, name=name,
+        rms_norm_eps=1e-5, rope_theta=theta, rope_scaling=scaling, tie_word_embeddings=tied, name=name,
     )
 
 
@@ -112,6 +116,9 @@ REGISTRY = {
     "meta-llama/Llama-3.1-70B": _llama("meta-llama/Llama-3.1-70B", 128256, 8192, 28672, 80, 64, 8, 131072, 5e5, _LLAMA3_SCALING),
     "meta-llama/Llama-3.1-405B": _llama("meta-llama/Llama-3.1-405B", 128256, 16384, 53248, 126, 128, 8, 131072, 5e5, _LLAMA3_SCALING),
     "meta-llama/Meta-Llama-3.1-405B": _llama("meta-llama/Meta-Llama-3.1-405B", 128256, 16384, 53248, 126, 128, 8, 131072, 5e5, _LLAMA3_SCALING),
+    # head_dim 64 (2048 / 32) and 128 (3072 / 24), tied embeddings
+    "meta-llama/Llama-3.2-1B": _llama("meta-llama/Llama-3.2-1B", 128256, 2048, 8192, 16, 32, 8, 131072, 5e5, _LLAMA32_SCALING, tied=True),
+    "meta-llama/Llama-3.2-3B": _llama("meta-llama/Llama-3.2-3B", 128256, 3072, 8192, 28, 24, 8, 131072, 5e5, _LLAMA32_SCALING, tied=True),
     "mistralai/Mistral-7B-v0.1": _mistral("mistralai/Mistral-7B-v0.1", 32000, 4096, 14336, 32, 32, 8, 32768, 1e4, 4096),
     "Qwen/Qwen3-0.6B": _qwen3("Qwen/Qwen3-0.6B", 1024, 3072, 28, 16, 8, True),
     "Qwen/Qwen3-1.7B": _qwen3("Qwen/Qwen3-1.7B", 2048, 6144, 28, 16, 8, True),
@@ -122,6 +129,8 @@ REGISTRY = {
     "debug-llama": _llama("debug-llama", 1024, 256, 512, 2, 2, 2, 2048, 1e4),
     "debug-llama-gqa": _llama("debug-llama-gqa", 1024, 512, 1024, 2, 4, 2, 2048, 5e5),
     "debug-llama-tp": _llama("debug-llama-tp", 2048, 1024, 2048, 2, 8, 8, 2048, 1e4),
+    # 4 heads x 64 over a hidden size of 256: head_dim 64, as in Llama-3.2-1B
+    "debug-llama-d64": _llama("debug-llama-d64", 1024, 256, 512, 2, 4, 2, 2048, 5e5),
     # a window that is not a multiple of the kernels' 128-row tiles
     "debug-mistral": _mistral("debug-mistral", 1024, 512, 1024, 2, 4, 2, 2048, 1e4, 192),
     # 4 heads x 128 = 512 over a hidden size of 256: head_dim apart from the hidden size, as in Qwen3-0.6B / 4B / 32B
@@ -156,6 +165,9 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
         if d.get("attention_bias"):
             raise ValueError(f"{name}: attention_bias is true; q/k/v/o projections with a bias are not supported")
         head_dim = d.get("head_dim") or d["hidden_size"] // d["num_attention_heads"]
+    if mt == "llama" and d.get("head_dim") is not None and d["head_dim"] != d["hidden_size"] // d["num_attention_heads"]:
+        # a head_dim of its own (as transformers' LlamaConfig allows); equal or absent derives it from the hidden size
+        head_dim = d["head_dim"]
     if mt == "mistral":
         if d.get("head_dim") is not None and d["head_dim"] != d["hidden_size"] // d["num_attention_heads"]:
             raise ValueError(f"{name}: head_dim {d['head_dim']} differs from hidden_size / num_attention_heads = "
@@ -241,6 +253,8 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
             "attention_bias": False, "use_sliding_window": False, "bos_token_id": 151643, "eos_token_id": 151645,
             "torch_dtype": "bfloat16",
         }
+    if cfg.arch == "llama" and cfg.explicit_head_dim is not None:
+        d["head_dim"] = cfg.explicit_head_dim
     if cfg.rope_scaling:
         d["rope_scaling"] = cfg.rope_scaling
     return d

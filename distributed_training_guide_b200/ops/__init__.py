@@ -410,17 +410,19 @@ class _AttentionQKV(torch.autograd.Function):
     @staticmethod
     def forward(ctx, qkv, nh, nkv, scale, doc_start=None, window=None):
         C = _ext.load()
-        o, lse = C.attn_fwd(qkv, nh, nkv, float(scale), doc_start=doc_start, window=window)
+        head_dim = qkv.shape[-1]
+        o, lse = C.attn_fwd(qkv, nh, nkv, float(scale), doc_start=doc_start, window=window, head_dim=head_dim)
         ctx.save_for_backward(qkv, o, lse, doc_start)
-        ctx.meta = (nh, nkv, scale, window)
+        ctx.meta = (nh, nkv, scale, window, head_dim)
         return o
 
     @staticmethod
     def backward(ctx, do):
         C = _ext.load()
         qkv, o, lse, doc_start = ctx.saved_tensors
-        nh, nkv, scale, window = ctx.meta
-        dqkv = C.attn_bwd(do.contiguous(), qkv, o, lse, nh, nkv, float(scale), doc_start=doc_start, window=window)
+        nh, nkv, scale, window, head_dim = ctx.meta
+        dqkv = C.attn_bwd(do.contiguous(), qkv, o, lse, nh, nkv, float(scale), doc_start=doc_start, window=window,
+                          head_dim=head_dim)
         return dqkv, None, None, None, None, None
 
 
@@ -441,7 +443,8 @@ def attention_qkv(qkv, nh, nkv, scale=None, doc_start=None, window=None):
     ``doc_start`` (int32 [B,S] from ``document_starts``, or None): document masking, query q sees key k iff
     ``doc_start[q] <= k <= q``.  ``window`` (an int >= 1, or None): sliding-window attention (Mistral), query q also
     sees only the ``window`` most recent keys, ``k > q - window``; a window of S or more changes nothing.  ``scale``
-    (None = 1/sqrt(d)) must be finite and > 0 on every path."""
+    (None = 1/sqrt(d)) must be finite and > 0 on every path.  bf16 CUDA tensors with d = 64 or 128 and S a multiple
+    of 128 run the sm_90a kernels."""
     d = qkv.shape[-1]
     scale = scale if scale is not None else 1.0 / math.sqrt(d)
     if isinstance(scale, bool) or not math.isfinite(scale) or scale <= 0:
@@ -450,7 +453,8 @@ def attention_qkv(qkv, nh, nkv, scale=None, doc_start=None, window=None):
         if isinstance(window, bool) or int(window) != window or window < 1:
             raise ValueError(f"window must be an int >= 1 or None, got {window!r}")
         window = None if window >= qkv.shape[1] else int(window)
-    if _ext.use_cuda_kernel("attention", qkv) and qkv.dtype == torch.bfloat16 and d == 128 and qkv.shape[1] % 128 == 0:
+    if (_ext.use_cuda_kernel("attention", qkv) and qkv.dtype == torch.bfloat16 and d in (64, 128)
+            and qkv.shape[1] % 128 == 0):
         if doc_start is not None:
             return _AttentionQKV.apply(qkv, nh, nkv, scale, doc_start.to(torch.int32).contiguous(), window)
         if window is not None:
@@ -458,8 +462,8 @@ def attention_qkv(qkv, nh, nkv, scale=None, doc_start=None, window=None):
         return _AttentionQKV.apply(qkv, nh, nkv, scale)
     q, k, v = qkv[:, :, :nh], qkv[:, :, nh:nh + nkv], qkv[:, :, nh + nkv:]
     if qkv.is_cuda:
-        # head dims other than 128 (GPT-2 style / toy configs) and sequence lengths that are not a multiple of
-        # the 128-row tile are outside the sm_90a kernel's scope; use the library kernel rather than the
+        # head dims other than 64 and 128 (toy configs) and sequence lengths that are not a multiple of the
+        # 128-row tile are outside the sm_90a kernels' scope; use the library kernel rather than the
         # O(S^2)-memory reference
         if doc_start is not None or window is not None:
             mask = ref.document_mask(doc_start, qkv.shape[1], window, device=qkv.device)[:, None]  # [B|1, 1, S, S]
