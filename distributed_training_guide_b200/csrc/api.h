@@ -18,6 +18,11 @@ void rope_inplace(void* qkv, const float* cos, const float* sin, long long T, in
                   bool per_token, bool inverse, cudaStream_t s);
 // out[c] = sum over rows r of partial[r][c] (fp32 [rows, H]), in a fixed order
 void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s);
+// bias gradient: db[n] = sum over t of dy[t, n], dy bf16 [T, N] with row stride ld (elements); N, ld multiples of 8.
+// Each CTA sums a fixed range of rows in fp32 into one row of `partial` (fp32 [bias_grad_chunks(T, N), N]), which
+// colsum then adds in a fixed order: no atomics, bit-identical from run to run.
+int bias_grad_chunks(long long T, int N);
+void bias_grad(const void* dy, long long T, int N, long long ld, float* partial, float* db, cudaStream_t s);
 void swiglu_fwd(const void* gu, void* h, long long T, int I, cudaStream_t s);
 void swiglu_bwd(const void* dh, const void* gu, void* dgu, long long T, int I, cudaStream_t s);
 void embedding_fwd(const long long* ids, const void* w, void* out, long long T, int H, cudaStream_t s);
@@ -58,13 +63,16 @@ void adamw_flat(void* p, const void* g, void* m, void* v, long long n, float lr,
 // out[M,N] (+)= op(A) @ op(B), bf16 in / fp32 register accumulate / bf16 out, row-major storage:
 //   a_kmajor: A stored [M,K] (else [K,M]);  b_kmajor: B stored [N,K] (else [K,N]).
 // lda/ldb/ldc are row strides in elements.  variant: 0 = auto, 1 = 1-CTA 128x256, 2 = 2-CTA cluster 256x256
+// bias: null, or bf16 [N] added to every row before the rounding to bf16 (forward layout, a_kmajor and b_kmajor,
+// overwrite mode only; 16-byte aligned).  The same holds for the bias of gemm_fp8 (e4m3 A), _ag and _bgather.
 void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
-               bool a_kmajor, bool b_kmajor, bool accumulate, int variant, cudaStream_t s);
+               bool a_kmajor, bool b_kmajor, bool accumulate, int variant, cudaStream_t s, const void* bias = nullptr);
 
 // C[M,N] (+)= scale_a[0] * scale_b[0] * A8[M,K] . B8[N,K]^T with fp8 operands (A e4m3, or e5m2 when a_e5m2; B e4m3),
 // both K-major; scale_a / scale_b are device pointers.  N, lda, ldb and ldc must be multiples of 16.
 void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
-              bool a_e5m2, const float* scale_a, const float* scale_b, bool accumulate, int variant, cudaStream_t s);
+              bool a_e5m2, const float* scale_a, const float* scale_b, bool accumulate, int variant, cudaStream_t s,
+              const void* bias = nullptr);
 
 int gemm_max_active_clusters(int cg);
 // tensor-parallel variants over symmetric buffers (see gemm_wgmma.cu)
@@ -75,10 +83,10 @@ void gemm_bf16_dist(int mode, const void* const* a_srcs, const void* const* b_sr
 void gemm_bf16_bgather(const void* A, void* full_base, void* C, int M, int N, int K, long long lda, long long ldb,
                        long long ldc, bool b_kmajor, const void* const* shards, long long per_bytes, long long w_off,
                        long long w_bytes, uint32_t* counters, uint32_t target, int chunk_shift, uint32_t* const* pads,
-                       int nranks, int rank, uint32_t bar_epoch, cudaStream_t s);
+                       int nranks, int rank, uint32_t bar_epoch, cudaStream_t s, const void* bias = nullptr);
 void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int N, int K, long long ldb, long long ldc,
                   bool b_kmajor, int nranks, int rank, int rows_per_peer, uint32_t* flags, uint32_t ag_epoch,
-                  uint32_t* const* pads, uint32_t bar_epoch, int n_comm, cudaStream_t s);
+                  uint32_t* const* pads, uint32_t bar_epoch, int n_comm, cudaStream_t s, const void* bias = nullptr);
 
 // ---- fp8.cu --------------------------------------------------------------------------------
 // amax[0] = max |x| of a bf16 [R, C] matrix with row stride ld (elements), on the device.

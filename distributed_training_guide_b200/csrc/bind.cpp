@@ -29,7 +29,24 @@ void check_vec(const Tensor& t, const char* name, at::ScalarType dt) {
               " must start at a 16-byte aligned address (the kernel accesses it in 16-byte vectors)");
 }
 
-void gemm(const Tensor& a, const Tensor& b, Tensor& out, bool trans_a, bool trans_b, bool accumulate, int variant) {
+// A bias [N] for the bias epilogue of the forward GEMMs: every refusal names the argument and happens before a launch.
+const void* check_gemm_bias(const c10::optional<Tensor>& bias, const Tensor& out, int64_t N, bool accumulate,
+                            bool forward_layout, const char* who) {
+  if (!bias.has_value()) return nullptr;
+  const Tensor& b = *bias;
+  TORCH_CHECK(b.is_cuda() && b.device() == out.device(), who, ": bias must be on the device of out");
+  TORCH_CHECK(b.scalar_type() == at::kBFloat16, who, ": bias must be bfloat16");
+  TORCH_CHECK(b.dim() == 1 && b.size(0) == N, who, ": bias must be [N] = [", N, "]");
+  TORCH_CHECK(b.is_contiguous(), who, ": bias must be contiguous");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(b.data_ptr()) % 16 == 0, who,
+              ": bias must start at a 16-byte aligned address");
+  TORCH_CHECK(!accumulate, who, ": bias cannot be combined with accumulate=True");
+  TORCH_CHECK(forward_layout, who, ": bias needs the forward layout (trans_a unset, trans_b set)");
+  return b.data_ptr();
+}
+
+void gemm(const Tensor& a, const Tensor& b, Tensor& out, bool trans_a, bool trans_b, bool accumulate, int variant,
+          const c10::optional<Tensor>& bias) {
   check_bf16_2d(a, "a");
   check_bf16_2d(b, "b");
   check_bf16_2d(out, "out");
@@ -40,8 +57,10 @@ void gemm(const Tensor& a, const Tensor& b, Tensor& out, bool trans_a, bool tran
   const int Kb = (int)(trans_b ? b.size(1) : b.size(0));
   TORCH_CHECK(K == Kb, "gemm: inner dimensions differ (", K, " vs ", Kb, ")");
   TORCH_CHECK(out.size(0) == M && out.size(1) == N, "gemm: out has the wrong shape");
+  const void* bp = check_gemm_bias(bias, out, N, accumulate, !trans_a && trans_b, "gemm");
+  TORCH_CHECK(!bp || K > 0, "gemm: bias needs K >= 1");
   dtg::gemm_bf16(a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0), out.stride(0),
-                 /*a_kmajor=*/!trans_a, /*b_kmajor=*/trans_b, accumulate, variant, stream());
+                 /*a_kmajor=*/!trans_a, /*b_kmajor=*/trans_b, accumulate, variant, stream(), bp);
 }
 
 void check_fp8_2d(const Tensor& t, const char* name) {
@@ -58,7 +77,7 @@ void check_scalar_f32(const Tensor& t, const char* name) {
 
 // out[M,N] (+)= scale_a * scale_b * a[M,K] @ b[N,K]^T; a e4m3 or e5m2, b e4m3; the scales stay on the device
 void gemm_fp8(const Tensor& a, const Tensor& b, Tensor& out, const Tensor& scale_a, const Tensor& scale_b,
-              bool accumulate, int variant) {
+              bool accumulate, int variant, const c10::optional<Tensor>& bias) {
   check_fp8_2d(a, "a");
   check_fp8_2d(b, "b");
   check_bf16_2d(out, "out");
@@ -69,9 +88,12 @@ void gemm_fp8(const Tensor& a, const Tensor& b, Tensor& out, const Tensor& scale
   const int M = (int)a.size(0), K = (int)a.size(1), N = (int)b.size(0);
   TORCH_CHECK(b.size(1) == K, "gemm_fp8: inner dimensions differ (", K, " vs ", b.size(1), ")");
   TORCH_CHECK(out.size(0) == M && out.size(1) == N, "gemm_fp8: out has the wrong shape");
+  const void* bp = check_gemm_bias(bias, out, N, accumulate, true, "gemm_fp8");
+  TORCH_CHECK(!bp || a.scalar_type() == at::kFloat8_e4m3fn, "gemm_fp8: bias needs a float8_e4m3fn a (the forward GEMM)");
+  TORCH_CHECK(!bp || K > 0, "gemm_fp8: bias needs K >= 1");
   dtg::gemm_fp8(a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0), out.stride(0),
                 a.scalar_type() == at::kFloat8_e5m2, scale_a.data_ptr<float>(), scale_b.data_ptr<float>(), accumulate,
-                variant, stream());
+                variant, stream(), bp);
 }
 
 Tensor fp8_amax(const Tensor& x) {
@@ -227,6 +249,24 @@ Tensor qk_norm_rope_bwd(Tensor& dqkv, const Tensor& x_save, const Tensor& rstd, 
   return dw;
 }
 
+// db[N] fp32 = the column sums of dy [T, N] (bf16, contiguous last dimension), in a fixed order (no atomics)
+Tensor bias_grad(const Tensor& dy) {
+  TORCH_CHECK(dy.is_cuda(), "bias_grad: dy must be a CUDA tensor");
+  TORCH_CHECK(dy.scalar_type() == at::kBFloat16, "bias_grad: dy must be bfloat16");
+  TORCH_CHECK(dy.dim() == 2, "bias_grad: dy must be 2-D [T, N]");
+  TORCH_CHECK(dy.stride(1) == 1, "bias_grad: dy must have a contiguous last dimension");
+  const int64_t T = dy.size(0), N = dy.size(1);
+  TORCH_CHECK(N % 8 == 0 && N > 0, "bias_grad: N must be a positive multiple of 8, got ", N);
+  TORCH_CHECK(T >= 1, "bias_grad: dy must have at least one row");
+  TORCH_CHECK(dy.stride(0) % 8 == 0 && reinterpret_cast<uintptr_t>(dy.data_ptr()) % 16 == 0,
+              "bias_grad: dy must start at a 16-byte aligned address with a row stride that is a multiple of 8");
+  const c10::cuda::CUDAGuard guard(dy.device());
+  Tensor db = torch::empty({N}, dy.options().dtype(at::kFloat));
+  Tensor partial = torch::empty({dtg::bias_grad_chunks(T, (int)N), N}, dy.options().dtype(at::kFloat));
+  dtg::bias_grad(dy.data_ptr(), T, (int)N, dy.stride(0), partial.data_ptr<float>(), db.data_ptr<float>(), stream());
+  return db;
+}
+
 Tensor swiglu_fwd(const Tensor& gu) {
   check_vec(gu, "gu", at::kBFloat16);
   const c10::cuda::CUDAGuard guard(gu.device());
@@ -323,9 +363,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "distributed_training_guide_b200 sm_90a kernels";
   m.def("launch_count", []() { return (uint64_t)dtg::launch_count(); });
   m.def("gemm", &gemm, py::arg("a"), py::arg("b"), py::arg("out"), py::arg("trans_a") = false,
-        py::arg("trans_b") = false, py::arg("accumulate") = false, py::arg("variant") = 0);
+        py::arg("trans_b") = false, py::arg("accumulate") = false, py::arg("variant") = 0,
+        py::arg("bias") = py::none());
   m.def("gemm_fp8", &gemm_fp8, py::arg("a"), py::arg("b"), py::arg("out"), py::arg("scale_a"), py::arg("scale_b"),
-        py::arg("accumulate") = false, py::arg("variant") = 0);
+        py::arg("accumulate") = false, py::arg("variant") = 0, py::arg("bias") = py::none());
+  m.def("bias_grad", &bias_grad, py::arg("dy"));
   m.def("fp8_amax", &fp8_amax);
   m.def("fp8_cast_transpose", &fp8_cast_transpose, py::arg("x"), py::arg("amax"), py::arg("e5m2"),
         py::arg("rowwise") = true, py::arg("transposed") = true);

@@ -1,6 +1,6 @@
 // Memory-bound ops of the Llama step, hand-written for sm_90a:
 //   fused (residual add +) RMSNorm fwd / bwd, in-place RoPE on the fused qkv activation,
-//   SwiGLU fwd / bwd, embedding gather / scatter-add, scalar scale.
+//   SwiGLU fwd / bwd, embedding gather / scatter-add, scalar scale, the bias gradient (column sums).
 // All are pure-bandwidth kernels: 16-byte vector accesses, fp32 math in registers, one pass
 // over the activations (the row is cached in registers between the statistic and the
 // normalisation).  Replaces the ~6 ATen kernels per RMSNorm / ~10 per RoPE the reference runs
@@ -195,6 +195,75 @@ int rmsnorm_bwd_grid(int T) { return T < 8 * sm_count() ? T : 8 * sm_count(); }
 void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s) {
   colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(partial, out, rows, H);
   note_launch();
+  DTG_LAUNCH_CHECK();
+}
+
+// ------------------------------------------------------------------------------------------
+// Bias gradient: db[n] = sum_t dy[t, n].  CTA (x, y) owns 256 columns and the y-th range of rows; its 32 x 8
+// threads each sum every 8th row of the range over one 16-byte vector (8 columns) in fp32, the 8 row lanes are
+// added in a fixed order through shared memory, and the CTA writes one fp32 partial row.  colsum_kernel adds the
+// partial rows, again in a fixed order.  The split depends on T and N only, so every run (and every GPU) sums in
+// the same order.
+// ------------------------------------------------------------------------------------------
+constexpr int kBiasGradCols = 256;       // columns per CTA: 32 vectors of 8
+constexpr int kBiasGradMinRows = 64;     // rows per CTA at least (8 per thread)
+constexpr int kBiasGradTargetCtas = 1024;
+
+__global__ void __launch_bounds__(256) bias_grad_kernel(const __nv_bfloat16* __restrict__ dy, long long T, int N,
+                                                        long long ld, long long rows_per_chunk,
+                                                        float* __restrict__ partial) {
+  __shared__ float sm[8][kBiasGradCols + 4];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int c0 = blockIdx.x * kBiasGradCols;
+  const int col = c0 + 8 * tx;
+  const long long r0 = (long long)blockIdx.y * rows_per_chunk;
+  const long long r1 = r0 + rows_per_chunk < T ? r0 + rows_per_chunk : T;
+  float s[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) s[k] = 0.f;
+  if (col < N) {
+#pragma unroll 4
+    for (long long r = r0 + ty; r < r1; r += 8) {
+      const uint4 v = *reinterpret_cast<const uint4*>(dy + r * ld + col);
+      const __nv_bfloat162* p = reinterpret_cast<const __nv_bfloat162*>(&v);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float2 f = __bfloat1622float2(p[k]);
+        s[2 * k] += f.x;
+        s[2 * k + 1] += f.y;
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) sm[ty][8 * tx + k] = s[k];
+  __syncthreads();
+  const int c = c0 + (int)threadIdx.x;   // one column per thread for the fixed-order sum of the 8 row lanes
+  if (c < N) {
+    float t = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) t += sm[i][threadIdx.x];
+    partial[(size_t)blockIdx.y * N + c] = t;
+  }
+}
+
+int bias_grad_chunks(long long T, int N) {
+  const int col_blocks = (N + kBiasGradCols - 1) / kBiasGradCols;
+  long long by_rows = (T + kBiasGradMinRows - 1) / kBiasGradMinRows;
+  long long by_ctas = kBiasGradTargetCtas / (col_blocks > 0 ? col_blocks : 1);
+  long long c = by_rows < by_ctas ? by_rows : by_ctas;
+  return (int)(c < 1 ? 1 : c);
+}
+
+void bias_grad(const void* dy, long long T, int N, long long ld, float* partial, float* db, cudaStream_t s) {
+  if (N % 8 || ld % 8 || reinterpret_cast<uintptr_t>(dy) % 16)
+    throw std::runtime_error("bias_grad: N and the row stride must be multiples of 8, dy 16-byte aligned");
+  if (T <= 0 || N <= 0) throw std::runtime_error("bias_grad: dy must have at least one row and one column");
+  const int chunks = bias_grad_chunks(T, N);
+  const long long rpc = (T + chunks - 1) / chunks;
+  bias_grad_kernel<<<dim3((N + kBiasGradCols - 1) / kBiasGradCols, chunks), 256, 0, s>>>(
+      (const __nv_bfloat16*)dy, T, N, ld, rpc, partial);
+  colsum_kernel<<<(N + 31) / 32, 256, 0, s>>>(partial, db, chunks, N);
+  note_launch(2);
   DTG_LAUNCH_CHECK();
 }
 

@@ -67,15 +67,23 @@ __device__ __forceinline__ int bg_rotation_chunks(const GemmDist& d) {   // firs
 // the caller passes transposed copies.  A stage then holds a K block of 128 fp8 elements, which is the same 128-byte
 // swizzle span, stage size and descriptor stepping as 64 bf16 elements, and the epilogue multiplies the fp32
 // accumulators by the two per-tensor dequantisation scales `scale_a[0] * scale_b[0]`, read from device memory.
-template <bool A_K, bool B_K, int CG, int A_MODE = 0, int B_MODE = 0, int C_MODE = 0, int ET = 0>
+//
+// BIAS adds a bf16 bias [N] to every row of the forward product before the one rounding to bf16: bf16(acc + b), fp8
+// bf16(acc * deq + b), with the operation order of the C += path (so the result is bit-identical to accumulating
+// over a C prefilled with the broadcast bias).  Every thread holds columns 8j + 2 (lane % 4) + {0, 1} of its
+// accumulator fragment, so it reads one bf16 pair per block j of 8 columns, straight from global memory (L1 / L2
+// serve the 2 N bytes to all CTAs); N is a multiple of 8, so a block is wholly inside or outside [0, N).  Forward
+// layout only (A and B K-major), never together with accumulate.
+template <bool A_K, bool B_K, int CG, int A_MODE = 0, int B_MODE = 0, int C_MODE = 0, int ET = 0, bool BIAS = false>
 __global__ void __launch_bounds__(GemmCfg<CG>::THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
                  const __grid_constant__ TmapSet<(B_MODE ? kMaxRanks : 1)> tmBs, const __grid_constant__ GemmDist dist,
                  const __grid_constant__ CUtensorMap tmC, __nv_bfloat16* __restrict__ C, int M, int N, int K,
                  long long ldc, int accumulate, int num_m_tiles, int num_tiles, const float* __restrict__ scale_a,
-                 const float* __restrict__ scale_b) {
+                 const float* __restrict__ scale_b, const __nv_bfloat16* __restrict__ bias) {
   static_assert(ET == 0 || (A_K && B_K && A_MODE == 0 && B_MODE == 0 && C_MODE == 0),
                 "the fp8 GEMM takes K-major operands from one tensor map each");
+  static_assert(!BIAS || (A_K && B_K && C_MODE == 0), "the bias epilogue serves the forward layout with a local C");
   using Cfg = GemmCfg<CG>;
   constexpr bool TMA_EPI = kTmaEpilogue<B_MODE, C_MODE>;
   constexpr int BK = ET ? 2 * Cfg::BK : Cfg::BK;   // elements of K per stage: one 128-byte span either way
@@ -440,11 +448,25 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj) {
               const int j = 16 * p + 8 * b + jj;
+              [[maybe_unused]] float2 bj;
+              if constexpr (BIAS) {
+                const int col = n0 + 8 * j + 2 * (lane & 3);
+                bj = col < N ? __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + col))
+                             : make_float2(0.f, 0.f);
+              }
 #pragma unroll
               for (int h = 0; h < 2; ++h) {   // rows +8h: 8 rows of 128 B further, same swizzle phase
                 float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
                 const uint32_t q = stg_s + (uint32_t)(b * Cfg::EPI_BOX_BYTES + h * 1024 + ((jj ^ (lane >> 2)) << 4));
-                if (accumulate) {
+                if constexpr (BIAS) {     // as the C += path below, with the bias in place of C
+                  if constexpr (ET != 0) {
+                    x = __fmaf_rn(x, deq, bj.x);
+                    y = __fmaf_rn(y, deq, bj.y);
+                  } else {
+                    x += bj.x;
+                    y += bj.y;
+                  }
+                } else if (accumulate) {
                   const uint32_t old = ld_shared_u32(q);
                   const float2 g = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&old));
                   if constexpr (ET != 0) {   // one rounding for the scale and the add: acc * deq + C
@@ -492,7 +514,11 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
               y *= deq;
             }
             __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(crow + col);
-            if (accumulate) {
+            if constexpr (BIAS) {
+              const float2 g = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + col));
+              x += g.x;
+              y += g.y;
+            } else if (accumulate) {
               const float2 g = __bfloat1622float2(*p);
               x += g.x;
               y += g.y;
@@ -594,10 +620,11 @@ int default_gemm_variant() {
 
 // One launcher for the plain and the tensor-parallel GEMMs.  `a_srcs` / `b_srcs`: base pointer of the
 // operand on every rank (only [0] is used in mode 0); `dist.c_ptr` set by the caller for C_MODE 1.
-template <bool A_K, bool B_K, int CG, int A_MODE, int B_MODE, int C_MODE, int ET = 0>
+template <bool A_K, bool B_K, int CG, int A_MODE, int B_MODE, int C_MODE, int ET = 0, bool BIAS = false>
 static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, void* C, int M, int N, int K,
                         long long lda, long long ldb, long long ldc, bool accumulate, GemmDist dist, int nranks,
-                        cudaStream_t s, const float* scale_a = nullptr, const float* scale_b = nullptr) {
+                        cudaStream_t s, const float* scale_a = nullptr, const float* scale_b = nullptr,
+                        const void* bias = nullptr) {
   using Cfg = GemmCfg<CG>;
   constexpr int ESIZE = ET ? 1 : 2;   // bytes per operand element
   TmapSet<(A_MODE ? kMaxRanks : 1)> tmA;
@@ -622,7 +649,7 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
   // C in 64 x 64 boxes (the staging layout of the epilogue); the other modes store from registers
   CUtensorMap tmC{};
   if constexpr (kTmaEpilogue<B_MODE, C_MODE>) tmC = make_tmap_2d(C, N, M, ldc * 2, 64, 64);
-  auto kern = gemm_bf16_kernel<A_K, B_K, CG, A_MODE, B_MODE, C_MODE, ET>;
+  auto kern = gemm_bf16_kernel<A_K, B_K, CG, A_MODE, B_MODE, C_MODE, ET, BIAS>;
   constexpr int kSmem = kTmaEpilogue<B_MODE, C_MODE> ? Cfg::SMEM_BYTES_EPI
                                                      : Cfg::SMEM_BYTES + (B_MODE == 3 ? Cfg::GATHER_BYTES : 0);
   static bool attr_set = false;
@@ -666,7 +693,8 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
   cfg.attrs = attrs;
   cfg.numAttrs = 1;
   DTG_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, dist, tmC, (__nv_bfloat16*)C, M, N, K, ldc,
-                                    accumulate ? 1 : 0, num_m_tiles, num_tiles, scale_a, scale_b));
+                                    accumulate ? 1 : 0, num_m_tiles, num_tiles, scale_a, scale_b,
+                                    (const __nv_bfloat16*)bias));
   note_launch();
 }
 
@@ -713,12 +741,25 @@ static void gemm_empty_k(void* C, int M, int N, long long ldc, bool accumulate, 
     DTG_CUDA_CHECK(cudaMemset2DAsync(C, (size_t)ldc * 2, 0, (size_t)N * 2, (size_t)M, s));
 }
 
+// The bias epilogue's preconditions, checked before any launch: forward layout, overwrite mode, K >= 1 (with K = 0 the
+// output would be the broadcast bias, which no kernel here writes), and a 16-byte aligned [N] vector.
+static void check_bias(const char* who, const void* bias, bool a_kmajor, bool b_kmajor, bool accumulate, int K) {
+  if (!bias) return;
+  if (!a_kmajor || !b_kmajor)
+    throw std::runtime_error(std::string(who) + ": a bias needs the forward layout (A [M,K] and B [N,K], K-major)");
+  if (accumulate) throw std::runtime_error(std::string(who) + ": a bias cannot be combined with accumulate");
+  if (K <= 0) throw std::runtime_error(std::string(who) + ": a bias needs K >= 1");
+  if (reinterpret_cast<uintptr_t>(bias) % 16)
+    throw std::runtime_error(std::string(who) + ": bias must start at a 16-byte aligned address");
+}
+
 void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
-               bool a_kmajor, bool b_kmajor, bool accumulate, int variant, cudaStream_t s) {
+               bool a_kmajor, bool b_kmajor, bool accumulate, int variant, cudaStream_t s, const void* bias) {
   if (M <= 0 || N <= 0) return;
   if ((N % 8) || (ldc % 8) || (lda % 8) || (ldb % 8))
     throw std::runtime_error("gemm_bf16: N and the leading dimensions must be multiples of 8 elements");
   check_gemm_bases("gemm_bf16", A, B, C);
+  check_bias("gemm_bf16", bias, a_kmajor, b_kmajor, accumulate, K);
   if (K <= 0) return gemm_empty_k(C, M, N, ldc, accumulate, s);
   if (variant == 0) variant = default_gemm_variant();
   if (variant == 3) variant = (M > 128) ? 2 : 1;  // auto: the CTA-pair tile is 256 rows tall
@@ -726,6 +767,13 @@ void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long 
   const void* as[1] = {A};
   const void* bs[1] = {B};
   GemmDist dist{};
+  if (bias) {
+    if (cg == 2) launch_gemm<true, true, 2, 0, 0, 0, 0, true>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, 1, s,
+                                                             nullptr, nullptr, bias);
+    else launch_gemm<true, true, 1, 0, 0, 0, 0, true>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, 1, s, nullptr,
+                                                      nullptr, bias);
+    return;
+  }
 #define DTG_GEMM_CASE(AK, BK)                                                                                    \
   if (a_kmajor == AK && b_kmajor == BK) {                                                                        \
     if (cg == 2) launch_gemm<AK, BK, 2, 0, 0, 0>(as, bs, C, M, N, K, lda, ldb, ldc, accumulate, dist, 1, s);      \
@@ -744,12 +792,15 @@ void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long 
 // e5m2 when `a_e5m2` (an output gradient); B is e4m3.  The scales are device pointers, so nothing here waits on the
 // kernels that computed them.
 void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
-              bool a_e5m2, const float* scale_a, const float* scale_b, bool accumulate, int variant, cudaStream_t s) {
+              bool a_e5m2, const float* scale_a, const float* scale_b, bool accumulate, int variant, cudaStream_t s,
+              const void* bias) {
   if (M <= 0 || N <= 0) return;
   if ((N % 16) || (lda % 16) || (ldb % 16) || (ldc % 16))
     throw std::runtime_error("gemm_fp8: N and the leading dimensions must be multiples of 16 elements (TMA needs "
                              "16-byte row strides of the fp8 operands)");
   check_gemm_bases("gemm_fp8", A, B, C);
+  check_bias("gemm_fp8", bias, true, true, accumulate, K);
+  if (bias && a_e5m2) throw std::runtime_error("gemm_fp8: a bias needs an e4m3 A (the forward GEMM)");
   if (K <= 0) return gemm_empty_k(C, M, N, ldc, accumulate, s);
   if (variant == 0) variant = default_gemm_variant();
   if (variant == 3) variant = (M > 128) ? 2 : 1;
@@ -757,6 +808,13 @@ void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long l
   const void* as[1] = {A};
   const void* bs[1] = {B};
   GemmDist dist{};
+  if (bias) {
+    if (cg == 2) launch_gemm<true, true, 2, 0, 0, 0, 1, true>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, 1, s,
+                                                             scale_a, scale_b, bias);
+    else launch_gemm<true, true, 1, 0, 0, 0, 1, true>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, 1, s, scale_a,
+                                                      scale_b, bias);
+    return;
+  }
 #define DTG_GEMM_FP8_CASE(ET)                                                                                     \
   if (cg == 2) launch_gemm<true, true, 2, 0, 0, 0, ET>(as, bs, C, M, N, K, lda, ldb, ldc, accumulate, dist, 1, s,  \
                                                        scale_a, scale_b);                                        \
@@ -821,11 +879,12 @@ void gemm_bf16_dist(int mode, const void* const* a_srcs, const void* const* b_sr
 //   destination of the gather.  flags: local uint32 [M / 256].  pads: the group's signal pads.
 void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int N, int K, long long ldb, long long ldc,
                   bool b_kmajor, int nranks, int rank, int rows_per_peer, uint32_t* flags, uint32_t ag_epoch,
-                  uint32_t* const* pads, uint32_t bar_epoch, int n_comm, cudaStream_t s) {
+                  uint32_t* const* pads, uint32_t bar_epoch, int n_comm, cudaStream_t s, const void* bias) {
   constexpr int TM = GemmCfg<2>::BM * 2;
   if (rows_per_peer % TM != 0 || rows_per_peer * nranks != M) throw std::runtime_error("gemm_bf16_ag: bad row split");
   if ((K * 2LL * TM) % GemmCfg<2>::COMM_PIECE != 0) throw std::runtime_error("gemm_bf16_ag: K must be a multiple of 64");
   if ((N % 8) || (ldc % 8) || (ldb % 8)) throw std::runtime_error("gemm_bf16_ag: N / leading dims must be multiples of 8");
+  check_bias("gemm_bf16_ag", bias, true, b_kmajor, false, K);
   GemmDist dist{};
   dist.rows_per_peer = rows_per_peer;
   dist.m_tile_shift = rank * (rows_per_peer / TM);
@@ -840,7 +899,9 @@ void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int 
   dist.tile_bytes = (long long)TM * K * 2;
   const void* as[1] = {a_bufs[rank]};
   const void* bs[1] = {B};
-  if (b_kmajor) launch_gemm<true, true, 2, 3, 0, 0>(as, bs, C, M, N, K, K, ldb, ldc, false, dist, nranks, s);
+  if (bias) launch_gemm<true, true, 2, 3, 0, 0, 0, true>(as, bs, C, M, N, K, K, ldb, ldc, false, dist, nranks, s,
+                                                          nullptr, nullptr, bias);
+  else if (b_kmajor) launch_gemm<true, true, 2, 3, 0, 0>(as, bs, C, M, N, K, K, ldb, ldc, false, dist, nranks, s);
   else launch_gemm<true, false, 2, 3, 0, 0>(as, bs, C, M, N, K, K, ldb, ldc, false, dist, nranks, s);
 }
 
@@ -853,10 +914,11 @@ void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int 
 void gemm_bf16_bgather(const void* A, void* full_base, void* C, int M, int N, int K, long long lda, long long ldb,
                        long long ldc, bool b_kmajor, const void* const* shards, long long per_bytes, long long w_off,
                        long long w_bytes, uint32_t* counters, uint32_t target, int chunk_shift, uint32_t* const* pads,
-                       int nranks, int rank, uint32_t bar_epoch, cudaStream_t s) {
+                       int nranks, int rank, uint32_t bar_epoch, cudaStream_t s, const void* bias) {
   using Cfg = GemmCfg<2>;
   if ((N % 8) || (ldc % 8) || (lda % 8) || (ldb % 8))
     throw std::runtime_error("gemm_bf16_bgather: N and the leading dimensions must be multiples of 8 elements");
+  check_bias("gemm_bf16_bgather", bias, true, b_kmajor, false, K);
   if (nranks < 1 || nranks > kMaxRanks) throw std::runtime_error("gemm_bf16_bgather: 1..8 ranks");
   const long long chunk = 1LL << chunk_shift;
   if (chunk < Cfg::GATHER_PIECE || (w_off % chunk) || (w_bytes % chunk) || (per_bytes % chunk))
@@ -890,7 +952,9 @@ void gemm_bf16_bgather(const void* A, void* full_base, void* C, int M, int N, in
   else dist.k_shift = (int)(my_row / Cfg::BK);
   const void* as[1] = {A};
   const void* bs[1] = {(const char*)full_base + w_off};
-  if (b_kmajor) launch_gemm<true, true, 2, 0, 3, 0>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s);
+  if (bias) launch_gemm<true, true, 2, 0, 3, 0, 0, true>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s,
+                                                          nullptr, nullptr, bias);
+  else if (b_kmajor) launch_gemm<true, true, 2, 0, 3, 0>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s);
   else launch_gemm<true, false, 2, 0, 3, 0>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s);
 }
 

@@ -14,6 +14,21 @@ namespace {
 using torch::Tensor;
 inline cudaStream_t stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
+// bias [N] of the all-gather / gather GEMMs' forward (b_kmajor) form: each refusal names the argument
+const void* check_bias(const c10::optional<Tensor>& bias, const Tensor& out, bool b_kmajor, const char* who) {
+  if (!bias.has_value()) return nullptr;
+  const Tensor& b = *bias;
+  const int64_t N = out.size(1);
+  TORCH_CHECK(b.is_cuda() && b.device() == out.device(), who, ": bias must be on the device of out");
+  TORCH_CHECK(b.scalar_type() == at::kBFloat16, who, ": bias must be bfloat16");
+  TORCH_CHECK(b.dim() == 1 && b.size(0) == N, who, ": bias must be [N] = [", N, "]");
+  TORCH_CHECK(b.is_contiguous(), who, ": bias must be contiguous");
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(b.data_ptr()) % 16 == 0, who,
+              ": bias must start at a 16-byte aligned address");
+  TORCH_CHECK(b_kmajor, who, ": bias needs the forward layout (b_kmajor set)");
+  return b.data_ptr();
+}
+
 SymmPtrs plain(const std::vector<uint64_t>& ptrs) {
   SymmPtrs s{};
   TORCH_CHECK(ptrs.size() >= 1 && ptrs.size() <= (size_t)kMaxRanks, "1..8 ranks supported");
@@ -39,10 +54,11 @@ void py_gemm_dist(int64_t mode, const std::vector<uint64_t>& a_ptrs, const std::
 
 void py_gemm_ag(const std::vector<uint64_t>& a_bufs, const Tensor& b, Tensor& out, bool b_kmajor, int64_t rank,
                 int64_t rows_per_peer, Tensor& flags, int64_t ag_epoch, const std::vector<uint64_t>& pads,
-                int64_t bar_epoch, int64_t n_comm) {
+                int64_t bar_epoch, int64_t n_comm, const c10::optional<Tensor>& bias) {
   TORCH_CHECK(b.is_cuda() && b.scalar_type() == at::kBFloat16 && b.dim() == 2 && b.stride(1) == 1, "bad B");
   TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kBFloat16 && out.dim() == 2 && out.stride(1) == 1, "bad out");
   TORCH_CHECK(flags.scalar_type() == at::kInt && flags.is_cuda(), "flags must be an int32 CUDA tensor");
+  const void* bp = check_bias(bias, out, b_kmajor, "gemm_ag");
   const c10::cuda::CUDAGuard guard(out.device());
   const int nr = (int)a_bufs.size();
   const int M = (int)out.size(0), N = (int)out.size(1);
@@ -57,7 +73,7 @@ void py_gemm_ag(const std::vector<uint64_t>& a_bufs, const Tensor& b, Tensor& ou
   }
   dtg::gemm_bf16_ag(as, b.data_ptr(), out.data_ptr(), M, N, K, b.stride(0), out.stride(0), b_kmajor, nr, (int)rank,
                     (int)rows_per_peer, (uint32_t*)flags.data_ptr<int>(), (uint32_t)ag_epoch, pd, (uint32_t)bar_epoch,
-                    (int)n_comm, stream());
+                    (int)n_comm, stream(), bp);
 }
 
 // C = a @ op(B) with B = a weight inside the flat buffer `full` (element offset w_off, w_numel elements), gathered
@@ -65,9 +81,10 @@ void py_gemm_ag(const std::vector<uint64_t>& a_bufs, const Tensor& b, Tensor& ou
 void py_gemm_bgather(const Tensor& a, Tensor& full, Tensor& out, bool b_kmajor, int64_t b_rows, int64_t b_cols,
                      const std::vector<uint64_t>& shards, int64_t per_numel, int64_t w_off, int64_t w_numel,
                      Tensor& counters, int64_t target, int64_t chunk_shift, const std::vector<uint64_t>& pads,
-                     int64_t rank, int64_t bar_epoch) {
+                     int64_t rank, int64_t bar_epoch, const c10::optional<Tensor>& bias) {
   TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.stride(1) == 1, "bad A");
   TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kBFloat16 && out.dim() == 2 && out.stride(1) == 1, "bad out");
+  const void* bp = check_bias(bias, out, b_kmajor, "gemm_bgather");
   TORCH_CHECK(full.is_contiguous() && full.scalar_type() == at::kBFloat16, "full must be the flat bf16 buffer");
   TORCH_CHECK(counters.scalar_type() == at::kInt && counters.is_cuda(), "counters must be an int32 CUDA tensor");
   TORCH_CHECK(w_off + w_numel <= full.numel() && b_rows * b_cols <= w_numel, "weight outside the flat buffer");
@@ -87,7 +104,7 @@ void py_gemm_bgather(const Tensor& a, Tensor& full, Tensor& out, bool b_kmajor, 
   }
   dtg::gemm_bf16_bgather(a.data_ptr(), full.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b_cols, out.stride(0),
                          b_kmajor, sh, per_numel * 2, w_off * 2, w_numel * 2, (uint32_t*)counters.data_ptr<int>(),
-                         (uint32_t)target, (int)chunk_shift, pd, nr, (int)rank, (uint32_t)bar_epoch, stream());
+                         (uint32_t)target, (int)chunk_shift, pd, nr, (int)rank, (uint32_t)bar_epoch, stream(), bp);
 }
 
 void py_reduce_parts(const Tensor& parts, const c10::optional<Tensor>& residual, Tensor& out) {
@@ -148,8 +165,13 @@ void py_embed_bwd(const Tensor& ids, const std::vector<uint64_t>& dx_ptrs, Tenso
 
 void bind_tp(pybind11::module_& m) {
   m.def("gemm_dist", &py_gemm_dist);
-  m.def("gemm_ag", &py_gemm_ag);
-  m.def("gemm_bgather", &py_gemm_bgather);
+  m.def("gemm_ag", &py_gemm_ag, py::arg("a_bufs"), py::arg("b"), py::arg("out"), py::arg("b_kmajor"), py::arg("rank"),
+        py::arg("rows_per_peer"), py::arg("flags"), py::arg("ag_epoch"), py::arg("pads"), py::arg("bar_epoch"),
+        py::arg("n_comm"), py::arg("bias") = py::none());
+  m.def("gemm_bgather", &py_gemm_bgather, py::arg("a"), py::arg("full"), py::arg("out"), py::arg("b_kmajor"),
+        py::arg("b_rows"), py::arg("b_cols"), py::arg("shards"), py::arg("per_numel"), py::arg("w_off"),
+        py::arg("w_numel"), py::arg("counters"), py::arg("target"), py::arg("chunk_shift"), py::arg("pads"),
+        py::arg("rank"), py::arg("bar_epoch"), py::arg("bias") = py::none());
   m.def("tp_reduce_parts", &py_reduce_parts);
   m.def("tp_reduce_mc", &py_reduce_mc);
   m.def("vp_ce_stats", &py_vp_ce_stats);

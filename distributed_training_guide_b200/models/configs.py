@@ -16,8 +16,8 @@ from typing import Optional
 
 @dataclasses.dataclass
 class ModelConfig:
-    arch: str  # "llama" | "mistral" | "qwen3" | "gpt2"; mistral is llama with a sliding attention window, qwen3 llama
-    # with QK-norm and a head_dim of its own
+    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "gpt2"; mistral is llama with a sliding attention window,
+    # qwen3 llama with QK-norm and a head_dim of its own, qwen2 llama with q/k/v biases
     vocab_size: int
     hidden_size: int
     intermediate_size: int
@@ -36,6 +36,8 @@ class ModelConfig:
     explicit_head_dim: Optional[int] = None
     #: QK-norm (Qwen3): every q and k head is RMS-normalised and scaled by a [head_dim] gain before RoPE
     qk_norm: bool = False
+    #: q/k/v projection biases (Qwen2); o_proj and the MLP stay bias-free
+    qkv_bias: bool = False
     # gpt2 only
     layer_norm_epsilon: float = 1e-5
     dropout: float = 0.0
@@ -57,6 +59,8 @@ class ModelConfig:
         per_layer = h * q + 2 * kv * h + q * h + 3 * h * i + 2 * h
         if self.qk_norm:
             per_layer += 2 * self.head_dim
+        if self.qkv_bias:
+            per_layer += q + 2 * kv
         n = v * h + l * per_layer + h
         if not self.tie_word_embeddings:
             n += v * h
@@ -99,6 +103,14 @@ def _qwen3(name, h, i, l, nh, nkv, tied, v=151936, maxpos=40960):
     )
 
 
+def _qwen2(name, h, i, l, nh, nkv, tied, v, maxpos):
+    return ModelConfig(
+        arch="qwen2", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
+        num_attention_heads=nh, num_key_value_heads=nkv, max_position_embeddings=maxpos,
+        rms_norm_eps=1e-6, rope_theta=1e6, tie_word_embeddings=tied, qkv_bias=True, name=name,
+    )
+
+
 _GPT2 = ModelConfig(
     arch="gpt2", vocab_size=50257, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
     num_attention_heads=12, num_key_value_heads=12, max_position_embeddings=1024,
@@ -125,6 +137,14 @@ REGISTRY = {
     "Qwen/Qwen3-4B": _qwen3("Qwen/Qwen3-4B", 2560, 9728, 36, 32, 8, True),
     "Qwen/Qwen3-8B": _qwen3("Qwen/Qwen3-8B", 4096, 12288, 36, 32, 8, False),
     "Qwen/Qwen3-32B": _qwen3("Qwen/Qwen3-32B", 5120, 25600, 64, 64, 8, False),
+    # Qwen2.5: q/k/v biases; head_dim 64 (0.5B) or 128
+    "Qwen/Qwen2.5-0.5B": _qwen2("Qwen/Qwen2.5-0.5B", 896, 4864, 24, 14, 2, True, 151936, 32768),
+    "Qwen/Qwen2.5-1.5B": _qwen2("Qwen/Qwen2.5-1.5B", 1536, 8960, 28, 12, 2, True, 151936, 131072),
+    "Qwen/Qwen2.5-3B": _qwen2("Qwen/Qwen2.5-3B", 2048, 11008, 36, 16, 2, True, 151936, 32768),
+    "Qwen/Qwen2.5-7B": _qwen2("Qwen/Qwen2.5-7B", 3584, 18944, 28, 28, 4, False, 152064, 131072),
+    "Qwen/Qwen2.5-14B": _qwen2("Qwen/Qwen2.5-14B", 5120, 13824, 48, 40, 8, False, 152064, 131072),
+    "Qwen/Qwen2.5-32B": _qwen2("Qwen/Qwen2.5-32B", 5120, 27648, 64, 40, 8, False, 152064, 131072),
+    "Qwen/Qwen2.5-72B": _qwen2("Qwen/Qwen2.5-72B", 8192, 29568, 80, 64, 8, False, 152064, 131072),
     # tiny configs for tests / smoke runs (head_dim 128 so the sm_90a attention kernel applies)
     "debug-llama": _llama("debug-llama", 1024, 256, 512, 2, 2, 2, 2048, 1e4),
     "debug-llama-gqa": _llama("debug-llama-gqa", 1024, 512, 1024, 2, 4, 2, 2048, 5e5),
@@ -135,6 +155,8 @@ REGISTRY = {
     "debug-mistral": _mistral("debug-mistral", 1024, 512, 1024, 2, 4, 2, 2048, 1e4, 192),
     # 4 heads x 128 = 512 over a hidden size of 256: head_dim apart from the hidden size, as in Qwen3-0.6B / 4B / 32B
     "debug-qwen3": _qwen3("debug-qwen3", 256, 512, 2, 4, 2, False, v=1024, maxpos=2048),
+    # 4 heads x 64 over a hidden size of 256, with q/k/v biases: head_dim 64, as in Qwen2.5-0.5B
+    "debug-qwen2": _qwen2("debug-qwen2", 256, 512, 2, 4, 2, False, 1024, 2048),
     "debug-gpt2": dataclasses.replace(_GPT2, vocab_size=512, hidden_size=64, intermediate_size=256,
                                       num_hidden_layers=2, num_attention_heads=2, num_key_value_heads=2,
                                       max_position_embeddings=128, name="debug-gpt2"),
@@ -152,10 +174,29 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
             max_position_embeddings=d.get("n_positions", 1024), tie_word_embeddings=True,
             layer_norm_epsilon=d.get("layer_norm_epsilon", 1e-5), dropout=d.get("resid_pdrop", 0.1), name=name,
         )
-    if mt not in ("llama", "mistral", "qwen3"):
+    if mt not in ("llama", "mistral", "qwen3", "qwen2"):
         raise ValueError(f"unsupported model_type {mt!r} in {name}")
     window = None
     head_dim = None
+    if mt == "llama":
+        for key in ("attention_bias", "mlp_bias"):
+            if d.get(key):
+                raise ValueError(f"{name}: {key} is true; Llama projections with a bias are not supported (Qwen2's "
+                                 "q/k/v biases are: model_type 'qwen2')")
+    if mt == "qwen2":
+        if d.get("use_sliding_window"):
+            raise ValueError(f"{name}: use_sliding_window is true; Qwen2 sliding-window layers are not supported")
+        if "sliding_attention" in (d.get("layer_types") or ()):
+            raise ValueError(f"{name}: layer_types contains 'sliding_attention'; Qwen2 sliding-window layers are "
+                             "not supported")
+        rope = d.get("rope_parameters") if isinstance(d.get("rope_parameters"), dict) else d.get("rope_scaling")
+        if rope and (rope.get("rope_type") or rope.get("type") or "default") != "default":
+            key = "rope_parameters" if isinstance(d.get("rope_parameters"), dict) else "rope_scaling"
+            raise ValueError(f"{name}: {key} has type {rope.get('rope_type') or rope.get('type')!r}; only the default "
+                             "RoPE is supported for Qwen2")
+        if d.get("head_dim") is not None and d["head_dim"] != d["hidden_size"] // d["num_attention_heads"]:
+            raise ValueError(f"{name}: head_dim {d['head_dim']} differs from hidden_size / num_attention_heads = "
+                             f"{d['hidden_size'] // d['num_attention_heads']}; only head_dim = hidden / heads is supported")
     if mt == "qwen3":
         if d.get("use_sliding_window"):
             raise ValueError(f"{name}: use_sliding_window is true; Qwen3 sliding-window layers are not supported")
@@ -188,7 +229,7 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
         max_position_embeddings=d.get("max_position_embeddings", 4096),
         rms_norm_eps=d.get("rms_norm_eps", 1e-5), rope_theta=theta, rope_scaling=scaling,
         tie_word_embeddings=d.get("tie_word_embeddings", False), sliding_window=window, name=name,
-        arch=mt, explicit_head_dim=head_dim, qk_norm=mt == "qwen3",
+        arch=mt, explicit_head_dim=head_dim, qk_norm=mt == "qwen3", qkv_bias=mt == "qwen2",
     )
 
 
@@ -252,6 +293,16 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
             "rope_theta": cfg.rope_theta, "hidden_act": "silu", "tie_word_embeddings": cfg.tie_word_embeddings,
             "attention_bias": False, "use_sliding_window": False, "bos_token_id": 151643, "eos_token_id": 151645,
             "torch_dtype": "bfloat16",
+        }
+    if cfg.arch == "qwen2":
+        d = {
+            "model_type": "qwen2", "architectures": ["Qwen2ForCausalLM"], "vocab_size": cfg.vocab_size,
+            "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size,
+            "num_hidden_layers": cfg.num_hidden_layers, "num_attention_heads": cfg.num_attention_heads,
+            "num_key_value_heads": cfg.num_key_value_heads, "max_position_embeddings": cfg.max_position_embeddings,
+            "rms_norm_eps": cfg.rms_norm_eps, "rope_theta": cfg.rope_theta, "hidden_act": "silu",
+            "tie_word_embeddings": cfg.tie_word_embeddings, "use_sliding_window": False, "bos_token_id": 151643,
+            "eos_token_id": 151643, "torch_dtype": "bfloat16",
         }
     if cfg.arch == "llama" and cfg.explicit_head_dim is not None:
         d["head_dim"] = cfg.explicit_head_dim

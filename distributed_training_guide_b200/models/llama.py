@@ -1,12 +1,13 @@
 """Llama-family causal LM built on the sm_90a op layer (Llama; Mistral: Llama plus a sliding attention window; Qwen3:
-Llama plus QK-norm, with a head_dim of its own).
+Llama plus QK-norm, with a head_dim of its own; Qwen2: Llama plus q/k/v biases).
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
 the reference instantiates at e.g. ``02-distributed-data-parallel/train_llm.py:57-58``)
 so checkpoints keep meaningful keys: ``model.embed_tokens.weight``,
 ``model.layers.{i}.self_attn.{q,k,v,o}_proj.weight``, ``model.layers.{i}.mlp.
 {gate,up,down}_proj.weight``, ``...{input,post_attention}_layernorm.weight``,
-``model.norm.weight``, ``lm_head.weight``; Qwen3 adds ``...self_attn.{q,k}_norm.weight``.
+``model.norm.weight``, ``lm_head.weight``; Qwen3 adds ``...self_attn.{q,k}_norm.weight``, Qwen2
+``...self_attn.{q,k,v}_proj.bias``.
 
 What is *different* from the HF module code (SURVEY.md §3.2) is the execution plan:
   * q/k/v (and gate/up) projections run as ONE wgmma GEMM over a fused weight that is
@@ -43,6 +44,9 @@ def init_parameter_(p, name: str, seed: int, std: float = 0.02, full_shape=None,
     if name.endswith("norm.weight") or name.endswith("layernorm.weight"):
         p.fill_(1.0)
         return
+    if name.endswith(".bias"):   # projection biases start at zero, as in transformers
+        p.zero_()
+        return
     gen = torch.Generator(device=p.device)
     gen.manual_seed(_name_seed(seed, name))
     shape = tuple(full_shape) if full_shape is not None else tuple(p.shape)
@@ -52,7 +56,8 @@ def init_parameter_(p, name: str, seed: int, std: float = 0.02, full_shape=None,
     p.copy_(full.to(p.dtype))
 
 
-#: which dimension of each parameter tensor parallelism splits (None = replicated)
+#: which dimension of each parameter tensor parallelism splits (None = replicated); a projection's bias (q/k/v, Qwen2)
+#: is split with its output features, dimension 0
 TP_SHARD_DIM = {"q_proj": 0, "k_proj": 0, "v_proj": 0, "gate_proj": 0, "up_proj": 0, "o_proj": 1, "down_proj": 1,
                 "embed_tokens": 1, "lm_head": 0}
 
@@ -62,7 +67,7 @@ def tp_shard_spec(name: str, p, tp_size: int, tp_rank: int) -> dict:
     if tp_size == 1:
         return {}
     for key, dim in TP_SHARD_DIM.items():
-        if f"{key}.weight" in name:
+        if f"{key}.weight" in name or (f"{key}.bias" in name and dim == 0):
             full = list(p.shape)
             full[dim] *= tp_size
             return dict(full_shape=full, shard_dim=dim, shard_index=tp_rank, shard_count=tp_size)
@@ -70,18 +75,21 @@ def tp_shard_spec(name: str, p, tp_size: int, tp_rank: int) -> dict:
 
 
 class Linear(nn.Module):
-    """Bias-free projection holding ``weight`` [out, in] (HF naming)."""
+    """Projection holding ``weight`` [out, in] and, with ``bias=True``, ``bias`` [out] (HF naming)."""
 
-    def __init__(self, in_features, out_features, dtype=None, device=None):
+    def __init__(self, in_features, out_features, dtype=None, device=None, bias=False):
         super().__init__()
         self.in_features, self.out_features = in_features, out_features
         self.weight = nn.Parameter(torch.empty(out_features, in_features, dtype=dtype, device=device))
+        self.bias = nn.Parameter(torch.zeros(out_features, dtype=dtype, device=device)) if bias else None
 
     def forward(self, x):
-        return ops.linear(x, self.weight)
+        return ops.linear(x, self.weight, self.bias)
 
     def reset_parameters(self, std=0.02):
         nn.init.normal_(self.weight, mean=0.0, std=std)
+        if self.bias is not None:
+            nn.init.zeros_(self.bias)
 
 
 class RMSNorm(nn.Module):
@@ -144,9 +152,10 @@ class LlamaAttention(nn.Module):
         self.head_dim = d
         #: sliding-window attention (Mistral): None, or W >= 1 with query q seeing keys k > q - W only
         self.sliding_window = config.sliding_window
-        self.q_proj = Linear(h, self.num_heads * d, dtype, device)
-        self.k_proj = Linear(h, self.num_kv_heads * d, dtype, device)
-        self.v_proj = Linear(h, self.num_kv_heads * d, dtype, device)
+        #: q/k/v biases (Qwen2), split with their heads under tensor parallelism
+        self.q_proj = Linear(h, self.num_heads * d, dtype, device, bias=config.qkv_bias)
+        self.k_proj = Linear(h, self.num_kv_heads * d, dtype, device, bias=config.qkv_bias)
+        self.v_proj = Linear(h, self.num_kv_heads * d, dtype, device, bias=config.qkv_bias)
         self.o_proj = Linear(self.num_heads * d, h, dtype, device)
         #: QK-norm (Qwen3): [head_dim] gains, replicated under tensor parallelism (every rank normalises its heads)
         self.q_norm = RMSNorm(d, config.rms_norm_eps, dtype, device) if config.qk_norm else None
@@ -192,6 +201,9 @@ class LlamaDecoderLayer(nn.Module):
     #: appended with QK-norm: after the layer norms, so the matrices stay first (FSDP's chunked layout) and every
     #: replicated gain sits in one run at the end (TP sums their gradients over the group in one launch)
     QK_NORM_ORDER = ("self_attn.q_norm.weight", "self_attn.k_norm.weight")
+    #: appended with q/k/v biases (Qwen2), also after the layer norms: adjacent, and each a multiple of 8 elements, so
+    #: they form one [(nh + 2 nkv) d] q|k|v bias (``fused_view_1d``) next to the fused q|k|v weight
+    QKV_BIAS_ORDER = ("self_attn.q_proj.bias", "self_attn.k_proj.bias", "self_attn.v_proj.bias")
     FUSED = {"qkv": FLAT_ORDER[0:3], "gate_up": FLAT_ORDER[4:6]}
 
     def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
@@ -203,7 +215,8 @@ class LlamaDecoderLayer(nn.Module):
         self.post_attention_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
         #: this layer's parameter order in its flat buffer (parallel/flat.py, parallel/fsdp.py); a parameter missing
         #: here would get no gradient buffer and no optimizer update
-        self.flat_order = self.FLAT_ORDER + (self.QK_NORM_ORDER if config.qk_norm else ())
+        self.flat_order = (self.FLAT_ORDER + (self.QK_NORM_ORDER if config.qk_norm else ())
+                           + (self.QKV_BIAS_ORDER if config.qkv_bias else ()))
         self._fused = {}  # name -> FusedWeight, installed by parallel.flat.FlatParamGroup
         self.tp = None  # installed by parallel.tp.apply_tensor_parallel
         self.fp8 = False  # set through LlamaForCausalLM.fp8: the four projections run ops.fp8_linear
@@ -215,6 +228,16 @@ class LlamaDecoderLayer(nn.Module):
             return f.data, f
         a = self.self_attn
         return torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], dim=0), None
+
+    def _qkv_bias(self):
+        """(fused q|k|v bias, its flat-gradient owner) or (None, None) without biases."""
+        a = self.self_attn
+        if a.q_proj.bias is None:
+            return None, None
+        f = self._fused.get("qkv_bias")
+        if f is not None and _ext.use_cuda_kernel("gemm", f.data):
+            return f.data, f
+        return torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias]), None
 
     def _gate_up_weight(self):
         f = self._fused.get("gate_up")
@@ -233,7 +256,8 @@ class LlamaDecoderLayer(nn.Module):
         fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
         y, h = self.input_layernorm(x, residual)
         w, owner = self._qkv_weight()
-        qkv = fused_linear(y, w, owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
+        b, b_owner = self._qkv_bias()
+        qkv = fused_linear(y, w, owner, b, b_owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
         qkv = att.position_qk_(qkv, cos, sin)
         a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
         a = a.reshape(B, S, att.num_heads * att.head_dim)

@@ -28,7 +28,7 @@ from . import reference as ref
 
 __all__ = [
     "linear", "fused_linear", "rms_norm", "add_rms_norm", "rope_qkv_", "qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy",
-    "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "ref",
+    "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "bias_grad", "ref",
 ]
 
 
@@ -78,11 +78,13 @@ def _emit_weight_grad(param, compute_into, shape_like):
     return out
 
 
-def gemm(a, b, out=None, trans_a=False, trans_b=False, accumulate=False):
-    """out[M,N] (+)= op(a) @ op(b) on the wgmma GEMM (bf16 in, fp32 accumulate in registers).
+def gemm(a, b, out=None, trans_a=False, trans_b=False, accumulate=False, bias=None):
+    """out[M,N] (+)= op(a) @ op(b) (+ bias) on the wgmma GEMM (bf16 in, fp32 accumulate in registers).
 
     ``op(a)`` is ``a`` ([M,K]) or ``a.T`` when ``trans_a`` (a given as [K,M]);
     ``op(b)`` is ``b`` ([K,N]) or ``b.T`` when ``trans_b`` (b given as [N,K]).
+    ``bias`` ([N] bf16, forward layout and overwrite mode only) is added to the fp32 accumulators before the one
+    rounding to bf16, in the kernel's epilogue.
     """
     M = a.shape[1] if trans_a else a.shape[0]
     N = b.shape[0] if trans_b else b.shape[1]
@@ -90,11 +92,16 @@ def gemm(a, b, out=None, trans_a=False, trans_b=False, accumulate=False):
         out = torch.empty(M, N, dtype=a.dtype, device=a.device)
         accumulate = False
     if _ext.use_cuda_kernel("gemm", a, b, out):
-        _ext.load().gemm(a, b, out, trans_a, trans_b, accumulate)
+        if bias is None:
+            _ext.load().gemm(a, b, out, trans_a, trans_b, accumulate)
+        else:
+            _ext.load().gemm(a, b, out, trans_a, trans_b, accumulate, bias=bias)
     else:
         A = a.t() if trans_a else a
         Bm = b.t() if trans_b else b
         r = (A.float() @ Bm.float())
+        if bias is not None:
+            r = r + bias.float()
         if accumulate:
             out.add_(r.to(out.dtype))
         else:
@@ -102,22 +109,41 @@ def gemm(a, b, out=None, trans_a=False, trans_b=False, accumulate=False):
     return out
 
 
+def bias_grad(dy):
+    """fp32 [N] column sums of ``dy`` [T, N] (the gradient of a bias added to every row).  bf16 CUDA tensors run the
+    sm_90a kernel: per-CTA fp32 partial rows summed in a fixed order, no atomics, so two runs are bit-identical."""
+    if _ext.use_cuda_kernel("gemm", dy) and dy.dtype == torch.bfloat16:
+        return _ext.load().bias_grad(dy)
+    return dy.float().sum(0)
+
+
+def _emit_bias_grad(bias_param, dy2, bias):
+    """The bias gradient of a linear op from its 2-D output gradient, routed like a norm gain's (overwrite on the
+    first write of a step, accumulate after it)."""
+    if bias_param is None:
+        return None
+    return _emit_weight_grad(bias_param, _norm_dw_into(bias_grad(dy2)), bias)
+
+
 # --------------------------------------------------------------------------------------
 # linear
 # --------------------------------------------------------------------------------------
 class _Linear(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w, w_param):
-        # x: [..., K], w: [N, K]; w_param is the nn.Parameter that owns the grad-buffer hooks
+    def forward(ctx, x, w, w_param, bias=None, bias_param=None):
+        # x: [..., K], w: [N, K]; w_param is the nn.Parameter that owns the grad-buffer hooks; bias: None or [N],
+        # added in the GEMM's epilogue, with bias_param (or the bias itself) owning its gradient routing
         x2 = x.reshape(-1, x.shape[-1])
         ctx.save_for_backward(x2, w)
         ctx.w_param = w_param if w_param is not None else w
+        ctx.bias = bias
+        ctx.bias_param = (bias_param if bias_param is not None else bias) if bias is not None else None
         ctx.x_shape = x.shape
         gs = getattr(ctx.w_param, "_dtg_gather", None)   # FSDP: the weight may still have to be gathered
         if gs is not None and x2.is_cuda and gs.pending():
-            y = gs.gemm(x2 if x2.is_contiguous() else x2.contiguous(), True)   # unshard fused into this GEMM
+            y = gs.gemm(x2 if x2.is_contiguous() else x2.contiguous(), True, bias)   # unshard fused into this GEMM
         else:
-            y = gemm(x2, w, trans_b=True)
+            y = gemm(x2, w, trans_b=True, bias=bias)
         return y.view(*x.shape[:-1], w.shape[0])
 
     @staticmethod
@@ -151,23 +177,29 @@ class _Linear(torch.autograd.Function):
                     lambda out, acc: gemm(dy2, x2, out=out, trans_a=True, accumulate=acc),  # dy^T @ x
                     w,
                 )
-        return dx, dw, None
+        db = _emit_bias_grad(ctx.bias_param, dy2, ctx.bias)
+        return dx, dw, None, db, None
 
 
 def linear(x, w, bias=None):
-    """y = x @ w.T (+ bias).  bf16 CUDA tensors run the wgmma GEMM."""
-    if bias is None and _ext.use_cuda_kernel("gemm", x, w) and x.dtype == torch.bfloat16:
-        return _Linear.apply(x, w, w)
+    """y = x @ w.T (+ bias).  bf16 CUDA tensors run the wgmma GEMM, the bias in its epilogue."""
+    if _ext.use_cuda_kernel("gemm", x, w) and x.dtype == torch.bfloat16:
+        if bias is None:
+            return _Linear.apply(x, w, w)
+        return _Linear.apply(x, w, w, bias, bias)
     return ref.linear(x, w, bias)
 
 
-def fused_linear(x, w, owner=None):
+def fused_linear(x, w, owner=None, bias=None, bias_owner=None):
     """``linear`` over a fused weight (q|k|v or gate|up).  ``owner`` is the
     ``models.llama.FusedWeight`` carrying the flat-gradient view, or None when ``w`` is an
-    ordinary autograd tensor (e.g. a ``torch.cat`` of the individual parameters)."""
+    ordinary autograd tensor (e.g. a ``torch.cat`` of the individual parameters).  ``bias`` /
+    ``bias_owner``: the fused bias (q|k|v, Qwen2) and what carries its flat-gradient view, likewise."""
     if _ext.use_cuda_kernel("gemm", x, w) and x.dtype == torch.bfloat16:
-        return _Linear.apply(x, w, owner if owner is not None else w)
-    return ref.linear(x, w)
+        if bias is None:
+            return _Linear.apply(x, w, owner if owner is not None else w)
+        return _Linear.apply(x, w, owner if owner is not None else w, bias, bias_owner)
+    return ref.linear(x, w, bias)
 
 
 # --------------------------------------------------------------------------------------
@@ -193,16 +225,22 @@ def fp8_cast(t, dtype, rowwise=True, transposed=True, amax=None):
     return (t8 if rowwise else None), (t8.t().contiguous() if transposed else None), scale_inv
 
 
-def gemm_fp8(a8, scale_inv_a, b8, scale_inv_b, out=None, accumulate=False, out_dtype=torch.bfloat16):
-    """out[M,N] (+)= scale_inv_a * scale_inv_b * a8[M,K] @ b8[N,K].T with fp32 accumulation.  a8 is e4m3 or e5m2,
-    b8 e4m3, both with K contiguous; ``out`` may be a strided view (of a flat gradient)."""
+def gemm_fp8(a8, scale_inv_a, b8, scale_inv_b, out=None, accumulate=False, out_dtype=torch.bfloat16, bias=None):
+    """out[M,N] (+)= scale_inv_a * scale_inv_b * a8[M,K] @ b8[N,K].T (+ bias) with fp32 accumulation.  a8 is e4m3 or
+    e5m2, b8 e4m3, both with K contiguous; ``out`` may be a strided view (of a flat gradient).  ``bias`` ([N] bf16,
+    e4m3 a8, overwrite mode) is added in the epilogue: bf16(acc * scale + bias) with one rounding."""
     if out is None:
         out = torch.empty(a8.shape[0], b8.shape[0], dtype=out_dtype, device=a8.device)
         accumulate = False
     if _ext.use_cuda_kernel("fp8", a8, b8, out):
-        _ext.load().gemm_fp8(a8, b8, out, scale_inv_a, scale_inv_b, accumulate)
+        if bias is None:
+            _ext.load().gemm_fp8(a8, b8, out, scale_inv_a, scale_inv_b, accumulate)
+        else:
+            _ext.load().gemm_fp8(a8, b8, out, scale_inv_a, scale_inv_b, accumulate, bias=bias)
     else:
         r = ref.fp8_gemm(a8, scale_inv_a, b8, scale_inv_b)
+        if bias is not None:
+            r = r + bias.float()
         out.copy_((out.float() + r) if accumulate else r)
     return out
 
@@ -216,14 +254,19 @@ class _FP8Linear(torch.autograd.Function):
     parameter through the step (6.5 GB for Llama-2-7B, more than an 80 GB H100 has left at S 4096)."""
 
     @staticmethod
-    def forward(ctx, x, w, w_param):
+    def forward(ctx, x, w, w_param, bias=None, bias_param=None):
         x2 = x.reshape(-1, x.shape[-1])
         x8, x8t, sx = fp8_cast(x2, torch.float8_e4m3fn)
         amax_w = fp8_amax(w)
         w8, _, sw = fp8_cast(w, torch.float8_e4m3fn, transposed=False, amax=amax_w)
-        y = gemm_fp8(x8, sx, w8, sw, out_dtype=x.dtype)
+        if bias is None:
+            y = gemm_fp8(x8, sx, w8, sw, out_dtype=x.dtype)
+        else:
+            y = gemm_fp8(x8, sx, w8, sw, out_dtype=x.dtype, bias=bias)
         ctx.save_for_backward(x8t, sx, w, amax_w)
         ctx.w_param = w_param
+        ctx.bias = bias
+        ctx.bias_param = (bias_param if bias_param is not None else bias) if bias is not None else None
         ctx.x_shape = x.shape
         return y.view(*x.shape[:-1], w.shape[0])
 
@@ -245,14 +288,18 @@ class _FP8Linear(torch.autograd.Function):
                 lambda out, acc: gemm_fp8(dy8t, sdy, x8t, sx, out=out, accumulate=acc),  # [N,T] . [K,T]^T
                 ctx.w_param,
             )
-        return dx, dw, None
+        db = _emit_bias_grad(ctx.bias_param, dy2, ctx.bias)   # from the bf16 dy, not its fp8 copy
+        return dx, dw, None, db, None
 
 
-def fp8_linear(x, w, owner=None):
+def fp8_linear(x, w, owner=None, bias=None, bias_owner=None):
     """``linear`` with fp8 GEMMs (forward, dgrad and wgrad).  ``owner`` is what carries the flat-gradient view: the
     ``models.llama.FusedWeight`` of a fused weight, or the parameter itself; None when ``w`` is an ordinary autograd
-    tensor.  CPU tensors run the same quantisation through ``ops/reference.py``."""
-    return _FP8Linear.apply(x, w, owner if owner is not None else w)
+    tensor.  ``bias`` / ``bias_owner`` likewise for a bias added in the forward GEMM's epilogue; its gradient is
+    summed from the bf16 output gradient.  CPU tensors run the same quantisation through ``ops/reference.py``."""
+    if bias is None:
+        return _FP8Linear.apply(x, w, owner if owner is not None else w)
+    return _FP8Linear.apply(x, w, owner if owner is not None else w, bias, bias_owner)
 
 
 # --------------------------------------------------------------------------------------

@@ -86,6 +86,18 @@ class FlatGroup:
         grad = self.grad[o:o + rows * cols].view(rows, cols) if self.grad is not None else None
         return data, grad
 
+    def fused_view_1d(self, names: Sequence[str]):
+        """(data, grad) 1-D views spanning adjacent 1-D parameters with no padding between them (the q|k|v bias)."""
+        idx = [self.index_of(n) for n in names]
+        assert idx == list(range(idx[0], idx[0] + len(idx))), "fused parameters must be adjacent"
+        n = 0
+        for i in idx:
+            assert len(self.shapes[i]) == 1
+            assert self.offsets[i] == self.offsets[idx[0]] + n, "padding between fused parameters"
+            n += self.shapes[i][0]
+        o = self.offsets[idx[0]]
+        return self.param[o:o + n], (self.grad[o:o + n] if self.grad is not None else None)
+
     # -- gradient bookkeeping -----------------------------------------------------------------
     def zero_grad(self):
         """Start a new accumulation window.  With ``direct_write`` (every parameter's gradient
@@ -106,6 +118,19 @@ class FlatGroup:
         return rank * n, (rank + 1) * n
 
 
+def install_fused_views(layer, g: FlatGroup, i: int):
+    """Give decoder layer ``i`` its fused weights (q|k|v, gate|up) and, with q/k/v biases, the fused q|k|v bias, as
+    views of its flat group ``g``."""
+    from ..models.llama import FusedWeight, LlamaDecoderLayer
+
+    for fname, members in LlamaDecoderLayer.FUSED.items():
+        data, grad = g.fused_view([f"model.layers.{i}.{m}" for m in members])
+        layer._fused[fname] = g.fused[fname] = FusedWeight(data, grad)
+    if layer.self_attn.q_proj.bias is not None:
+        data, grad = g.fused_view_1d([f"model.layers.{i}.{m}" for m in LlamaDecoderLayer.QKV_BIAS_ORDER])
+        layer._fused["qkv_bias"] = g.fused["qkv_bias"] = FusedWeight(data, grad)
+
+
 def build_groups(model: nn.Module, device, dtype, world_size: int = 1, alloc=None, direct_write=None,
                  with_grad: bool = True) -> List[FlatGroup]:
     """Partition ``model`` into flat groups: ``embed``, one per decoder layer, ``head``.
@@ -114,7 +139,7 @@ def build_groups(model: nn.Module, device, dtype, world_size: int = 1, alloc=Non
     the embedding last.  Tied embeddings collapse embed+head into the ``embed`` group.
     ``pad_multiple`` makes every group divisible into ``world_size`` 16-byte aligned shards.
     """
-    from ..models.llama import FusedWeight, LlamaDecoderLayer, LlamaForCausalLM
+    from ..models.llama import LlamaDecoderLayer, LlamaForCausalLM
 
     pad = ALIGN * world_size * 16  # shards stay 256-byte aligned
     is_llama = isinstance(model, LlamaForCausalLM)
@@ -156,11 +181,7 @@ def build_groups(model: nn.Module, device, dtype, world_size: int = 1, alloc=Non
         g = mk(f"layer{i}", ordered)
         layer._flat_group = g
         if isinstance(layer, LlamaDecoderLayer) and g is not None:
-            for fname, members in LlamaDecoderLayer.FUSED.items():
-                data, grad = g.fused_view([f"model.layers.{i}.{m}" for m in members])
-                fw = FusedWeight(data, grad)
-                layer._fused[fname] = fw
-                g.fused[fname] = fw
+            install_fused_views(layer, g, i)
     mk("head", post)
     model._flat_groups = groups
     return groups

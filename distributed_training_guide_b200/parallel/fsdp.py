@@ -36,12 +36,12 @@ import torch
 import torch.distributed as dist
 from torch.autograd import Variable
 
-from ..models.llama import FusedWeight, LlamaDecoderLayer, LlamaForCausalLM, init_parameter_
+from ..models.llama import LlamaDecoderLayer, LlamaForCausalLM, init_parameter_
 from ..ops import reference as ref
 from ..ops import join_wgrad_stream
 from ..utils.timers import nvtx_range
 from .ddp import boundary
-from .flat import ALIGN, FlatGroup, _round_up
+from .flat import ALIGN, FlatGroup, _round_up, install_fused_views
 from .optim import FlatAdamW
 
 
@@ -78,9 +78,10 @@ class _GatherSpec:
     def pending(self) -> bool:
         return self.eng.gather_pending(self)
 
-    def gemm(self, a, b_kmajor: bool):
-        """a @ W^T (``b_kmajor``: forward) or a @ W (dgrad) with W gathered from the ranks' shards by the GEMM itself."""
-        return self.eng._gather_gemm(self, a, b_kmajor)
+    def gemm(self, a, b_kmajor: bool, bias=None):
+        """a @ W^T (+ bias) (``b_kmajor``: forward) or a @ W (dgrad) with W gathered from the ranks' shards by the GEMM
+        itself.  The bias is a 1-D parameter of the group's prefetched tail, already local."""
+        return self.eng._gather_gemm(self, a, b_kmajor, bias)
 
 
 class FSDPEngine:
@@ -219,11 +220,7 @@ class FSDPEngine:
             layer._flat_group = g
             if not self.is_llama:
                 continue
-            for fname, members in LlamaDecoderLayer.FUSED.items():
-                data, grad = g.fused_view([f"model.layers.{i}.{m}" for m in members])
-                fw = FusedWeight(data, grad)
-                layer._fused[fname] = fw
-                g.fused[fname] = fw
+            install_fused_views(layer, g, i)
         self.head = make_group("head", head_named, local(layout(head_named)), symmetric(layout(head_named)))
         self.layer_groups = self.groups[1:1 + L]
         self.shard_of = {s.name: s for s in self.shards}
@@ -290,6 +287,8 @@ class FSDPEngine:
             by_name = dict(zip(g.names, zip(g.params, g.offsets, g.shapes)))
             covered = set()
             for fname, fw in g.fused.items():
+                if fw.data.dim() != 2:   # the fused q|k|v bias (Qwen2): 1-D, it lives in the prefetched tail
+                    continue
                 members = [n for n in g.names if any(n.endswith(m) for m in LlamaDecoderLayer.FUSED[fname])]
                 off = by_name[members[0]][1]
                 rows = sum(by_name[n][2][0] for n in members)
@@ -306,7 +305,7 @@ class FSDPEngine:
             # what is left after the matrices (norm gains): a prefetched copy-engine gather of that flat range
             g.tail = (end_of_matrices, g.numel) if g.numel > end_of_matrices else None
 
-    def _gather_gemm(self, sp, a, b_kmajor):
+    def _gather_gemm(self, sp, a, b_kmajor, bias=None):
         g = sp.g
         C = self.symm.C
         full = g.param
@@ -321,7 +320,7 @@ class FSDPEngine:
         with nvtx_range(f"gather_gemm:{g.name}"):
             C.gemm_bgather(a, full, out, b_kmajor, sp.rows, sp.cols, self._symm_of[sh.param.data_ptr()].ptrs,
                            sh.padded_numel, sp.off, sp.numel, self._counters[full.data_ptr()], n * ppc, shift,
-                           self.gather_pads.ptrs, self.rank, 0)   # epoch 0: no entry barrier (see the kernel)
+                           self.gather_pads.ptrs, self.rank, 0, bias)   # epoch 0: no entry barrier (see the kernel)
         g._gathered.add(sp.off)
         return out
 

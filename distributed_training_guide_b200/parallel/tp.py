@@ -91,11 +91,12 @@ class TPContext:
         mine = full[self.rank * self.rpp:(self.rank + 1) * self.rpp]
         return full, mine, [p + idx * n * 2 for p in self.act.ptrs]
 
-    def gather_gemm(self, bufs, b, out, b_kmajor):
-        """out = all_gather_rows(symmetric buffer) @ op(b): ONE kernel, the gather runs on communication CTAs."""
+    def gather_gemm(self, bufs, b, out, b_kmajor, bias=None):
+        """out = all_gather_rows(symmetric buffer) @ op(b) (+ bias): ONE kernel, the gather runs on communication
+        CTAs, the bias is added in the epilogue (forward form only)."""
         self.ag_epoch += 1
         self.symm.C.gemm_ag(bufs, b, out, b_kmajor, self.rank, self.rpp, self.flags, self.ag_epoch, self.symm.pad_ptrs,
-                            self.symm._epochs(1), self.n_comm)
+                            self.symm._epochs(1), self.n_comm, bias)
 
     def row_parallel_gemm(self, a, w, trans_b, residual):
         """reduce_scatter_rows(a @ op(w)) (+ residual) -> [T/t, H] for this rank (GPU kernels).
@@ -164,20 +165,24 @@ class TPContext:
 
 
 class _ColumnParallelLinear(torch.autograd.Function):
-    """y_full[T, n_local] = all_gather_rows(x_local)[T, H] @ W_local[n_local, H]^T"""
+    """y_full[T, n_local] = all_gather_rows(x_local)[T, H] @ W_local[n_local, H]^T (+ b_local[n_local])
+
+    A bias is split with the output features.  Every rank's output gradient covers all T tokens, so the gradient of
+    its bias slice is complete without any reduction over the group."""
 
     @staticmethod
-    def forward(ctx, x_local, w, owner, tp: TPContext, slot):
+    def forward(ctx, x_local, w, owner, tp: TPContext, slot, bias=None, bias_owner=None):
         ctx.tp, ctx.owner, ctx.slot = tp, owner, slot
+        ctx.bias, ctx.bias_owner = bias, bias_owner
         T, H, n = tp.rpp * tp.t, x_local.shape[1], w.shape[0]
         if not tp.use_kernels:
             xf = tp.all_gather_rows(x_local)
             ctx.save_for_backward(x_local, w)
-            return xf @ w.t()
+            return xf @ w.t() if bias is None else xf @ w.t() + bias
         full, mine, ptrs = tp.act_slot(slot)
         mine.copy_(x_local)          # my sequence shard, where the peers' copy engines can reach it
         out = torch.empty(T, n, dtype=x_local.dtype, device=x_local.device)
-        tp.gather_gemm(ptrs, w, out, True)   # barrier + all-gather + GEMM in one kernel; `full` is now complete
+        tp.gather_gemm(ptrs, w, out, True, bias)   # barrier + all-gather + GEMM in one kernel; `full` is now complete
         ctx.save_for_backward(w)
         return out
 
@@ -186,12 +191,19 @@ class _ColumnParallelLinear(torch.autograd.Function):
         tp, owner = ctx.tp, ctx.owner
         dy = dy.contiguous()
         T, n = dy.shape
+        db = None
+        if ctx.bias is not None:
+            bo = ctx.bias_owner if ctx.bias_owner is not None else ctx.bias
+            if tp.use_kernels:
+                db = ops._emit_bias_grad(bo, dy, ctx.bias)
+            else:
+                db = _route_dw(bo, dy.float().sum(0).to(ctx.bias.dtype))
         if not tp.use_kernels:
             x_local, w = ctx.saved_tensors
             xf = tp.all_gather_rows(x_local)
             dw = dy.t() @ xf
             dx = tp.reduce_scatter_rows(dy @ w)
-            return dx, dw if owner is None else _route_dw(owner, dw), None, None, None
+            return dx, dw if owner is None else _route_dw(owner, dw), None, None, None, db, None
         C = _ext.load()
         (w,) = ctx.saved_tensors
         H = w.shape[1]
@@ -203,7 +215,7 @@ class _ColumnParallelLinear(torch.autograd.Function):
         ops.gemm(dy, full, out=gbuf, trans_a=True, accumulate=acc)
         # dgrad: dx[T/t, H] = reduce_scatter_rows(dy[T, n] @ W[n, H])
         dx = tp.row_parallel_gemm(dy, w, False, None)
-        return dx, None, None, None, None
+        return dx, None, None, None, None, db, None
 
 
 def _route_dw(owner, dw):
@@ -366,13 +378,24 @@ class TensorParallelRuntime:
             return f.data, f
         return torch.cat([m.weight for m in members], dim=0), None
 
+    def fused_bias(self, layer):
+        """(q|k|v bias slice, its flat-gradient owner); (None, None) without biases."""
+        att = layer.self_attn
+        if att.q_proj.bias is None:
+            return None, None
+        f = layer._fused.get("qkv_bias")
+        if f is not None:
+            return f.data, f
+        return torch.cat([att.q_proj.bias, att.k_proj.bias, att.v_proj.bias]), None
+
     def layer_forward(self, layer, x, residual, cos, sin, B, S):
         """x, residual: sequence shards [T/t, H]; returns (mlp_out_local, residual_local)."""
         tp = self.ctx
         att, mlp = layer.self_attn, layer.mlp
         y, h = layer.input_layernorm(x, residual)
         w, owner = self.fused(layer, "qkv", (att.q_proj, att.k_proj, att.v_proj))
-        qkv = _ColumnParallelLinear.apply(y, w, owner, tp, 2 * layer.layer_idx)
+        b, b_owner = self.fused_bias(layer)
+        qkv = _ColumnParallelLinear.apply(y, w, owner, tp, 2 * layer.layer_idx, b, b_owner)
         qkv = qkv.view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
         qkv = att.position_qk_(qkv, cos, sin)
         a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, window=att.sliding_window)
