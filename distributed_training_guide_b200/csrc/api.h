@@ -11,6 +11,9 @@ unsigned long long launch_count();
 // ---- elementwise.cu ------------------------------------------------------------------------
 void rmsnorm_fwd(const void* x, const void* res, const void* w, void* y, void* h_out, float* rstd, int T, int H,
                  float eps, cudaStream_t s);
+// norm-then-add: h_out = bf16(r + bf16(x * rstd * w)), rstd [T] fp32 (the RMSNorm backward of x takes it as is)
+void rmsnorm_add_fwd(const void* x, const void* res, const void* w, void* h_out, float* rstd, int T, int H, float eps,
+                     cudaStream_t s);
 int rmsnorm_bwd_grid(int T);
 void rmsnorm_bwd(const void* dy, const void* h, const void* w, const float* rstd, const void* dres, void* dx,
                  float* dw_partial, float* dw, int T, int H, cudaStream_t s);
@@ -48,6 +51,20 @@ int qk_norm_rope_bwd_grid(long long T, int nqk);
 void qk_norm_rope_bwd(void* dqkv, const void* x_save, const float* rstd, const void* q_w, const void* k_w,
                       const float* cos, const float* sin, float* dw_partial, float* dw, long long T, int S, int n_heads,
                       int nh, int nkv, bool per_token, cudaStream_t s);
+// Full-width QK-norm + RoPE (OLMo 2) on the same layout: one RMSNorm over a token's whole q region (nh * 128
+// elements, gain q_w [nh * 128]) and one over its k region (k_w [nkv * 128]), y = bf16(x * rstd * w), then the RoPE
+// of rope_inplace.  Writes x_save [T, nh + nkv, 128] bf16 and rstd [T, 2] fp32 (q, k).  nh + nkv <=
+// qk_norm_full_rope_max_heads().
+int qk_norm_full_rope_max_heads();
+void qk_norm_full_rope_fwd(void* qkv, const void* q_w, const void* k_w, const float* cos, const float* sin,
+                           void* x_save, float* rstd, long long T, int S, int n_heads, int nh, int nkv, bool per_token,
+                           float eps, cudaStream_t s);
+int qk_norm_full_rope_bwd_grid(long long T, int nqk);
+// dw [(nh + nkv) * 128] fp32 = the q gain gradient followed by the k gain gradient; dw_partial:
+// [qk_norm_full_rope_bwd_grid(T, nh + nkv), (nh + nkv) * 128] fp32 scratch.
+void qk_norm_full_rope_bwd(void* dqkv, const void* x_save, const float* rstd, const void* q_w, const void* k_w,
+                           const float* cos, const float* sin, float* dw_partial, float* dw, long long T, int S,
+                           int n_heads, int nh, int nkv, bool per_token, cudaStream_t s);
 
 // ---- cross_entropy.cu ----------------------------------------------------------------------
 // logits [T,V] bf16 are overwritten with dlogits = (softmax - onehot) / n_valid; loss = mean CE.

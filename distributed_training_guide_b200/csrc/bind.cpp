@@ -149,6 +149,28 @@ std::tuple<Tensor, Tensor, c10::optional<Tensor>> rmsnorm_fwd(const Tensor& x, c
   return {y, rstd, h};
 }
 
+// (h, rstd) with h = bf16(r + bf16(rmsnorm(x) * w)): the norm-then-add of OLMo 2's post-sublayer norms
+std::tuple<Tensor, Tensor> rmsnorm_add_fwd(const Tensor& x, const Tensor& r, const Tensor& w, double eps) {
+  check_vec(x, "x", at::kBFloat16);
+  check_vec(r, "r", at::kBFloat16);
+  check_vec(w, "w", at::kBFloat16);
+  TORCH_CHECK(x.dim() == 2, "rmsnorm_add: x must be 2-D [T, H]");
+  TORCH_CHECK(r.sizes() == x.sizes(), "rmsnorm_add: r and x differ in shape");
+  const int T = (int)x.size(0), H = (int)x.size(1);
+  TORCH_CHECK(w.dim() == 1 && w.numel() == H, "rmsnorm_add: w must have one entry per column of x");
+  TORCH_CHECK(H % 8 == 0 && H <= 16384, "rmsnorm_add: hidden size must be a multiple of 8 and <= 16384, got ", H);
+  TORCH_CHECK(std::isfinite(eps) && eps >= 0, "rmsnorm_add: eps must be finite and >= 0");
+  for (const Tensor* t : {&r, &w})
+    TORCH_CHECK(t->device() == x.device(), "rmsnorm_add: every operand must be on the device of x");
+  const c10::cuda::CUDAGuard guard(x.device());
+  Tensor h = torch::empty_like(x);
+  Tensor rstd = torch::empty({T}, x.options().dtype(at::kFloat));
+  if (T > 0)
+    dtg::rmsnorm_add_fwd(x.data_ptr(), r.data_ptr(), w.data_ptr(), h.data_ptr(), rstd.data_ptr<float>(), T, H,
+                         (float)eps, stream());
+  return {h, rstd};
+}
+
 std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& h, const Tensor& w, const Tensor& rstd,
                                        const c10::optional<Tensor>& dres) {
   check_vec(dy, "dy", at::kBFloat16);
@@ -188,19 +210,24 @@ void rope_inplace(Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t n_r
                     (int)d, per_token, inverse, stream());
 }
 
-// Shared checks of qk_norm_rope_fwd / _bwd; returns per_token.  Every refusal happens before any launch.
+// Shared checks of qk_norm_rope_fwd / _bwd and, with `full`, of the full-width qk_norm_full_rope_fwd / _bwd (gains
+// [nh * d] and [nkv * d]); returns per_token.  Every refusal happens before any launch.
 bool check_qk_norm_rope(const Tensor& qkv, const Tensor& q_w, const Tensor& k_w, const Tensor& cos, const Tensor& sin,
-                        int64_t nh, int64_t nkv) {
+                        int64_t nh, int64_t nkv, bool full = false) {
   check_vec(qkv, "qkv", at::kBFloat16);
   TORCH_CHECK(qkv.dim() == 4, "qk_norm_rope: qkv must be [B, S, heads, d]");
   const int64_t B = qkv.size(0), S = qkv.size(1), NH = qkv.size(2), d = qkv.size(3);
   TORCH_CHECK(d == 128, "qk_norm_rope: head_dim must be 128, got ", d);
   TORCH_CHECK(nh >= 1 && nkv >= 1 && NH == nh + 2 * nkv, "qk_norm_rope: qkv has ", NH,
               " heads, expected nh + 2 * nkv with nh, nkv >= 1 (nh = ", nh, ", nkv = ", nkv, ")");
+  if (full)
+    TORCH_CHECK(nh + nkv <= dtg::qk_norm_full_rope_max_heads(), "qk_norm_full_rope: nh + nkv = ", nh + nkv,
+                " exceeds the ", dtg::qk_norm_full_rope_max_heads(), " q + k heads per token the kernel holds");
   check_vec(q_w, "q_w", at::kBFloat16);
   check_vec(k_w, "k_w", at::kBFloat16);
-  TORCH_CHECK(q_w.dim() == 1 && q_w.size(0) == d, "qk_norm_rope: q_w must be [", d, "]");
-  TORCH_CHECK(k_w.dim() == 1 && k_w.size(0) == d, "qk_norm_rope: k_w must be [", d, "]");
+  const int64_t qn = full ? nh * d : d, kn = full ? nkv * d : d;
+  TORCH_CHECK(q_w.dim() == 1 && q_w.size(0) == qn, "qk_norm_rope: q_w must be [", qn, "]");
+  TORCH_CHECK(k_w.dim() == 1 && k_w.size(0) == kn, "qk_norm_rope: k_w must be [", kn, "]");
   check_vec(cos, "cos", at::kFloat);
   check_vec(sin, "sin", at::kFloat);
   TORCH_CHECK(sin.sizes() == cos.sizes(), "qk_norm_rope: cos and sin differ in shape");
@@ -246,6 +273,42 @@ Tensor qk_norm_rope_bwd(Tensor& dqkv, const Tensor& x_save, const Tensor& rstd, 
   dtg::qk_norm_rope_bwd(dqkv.data_ptr(), x_save.data_ptr(), rstd.data_ptr<float>(), q_w.data_ptr(), k_w.data_ptr(),
                         cos.data_ptr<float>(), sin.data_ptr<float>(), partial.data_ptr<float>(), dw.data_ptr<float>(), T,
                         (int)S, (int)dqkv.size(2), (int)nh, (int)nkv, per_token, stream());
+  return dw;
+}
+
+std::tuple<Tensor, Tensor> qk_norm_full_rope_fwd(Tensor& qkv, const Tensor& q_w, const Tensor& k_w, const Tensor& cos,
+                                                 const Tensor& sin, int64_t nh, int64_t nkv, double eps) {
+  const bool per_token = check_qk_norm_rope(qkv, q_w, k_w, cos, sin, nh, nkv, true);
+  TORCH_CHECK(std::isfinite(eps) && eps >= 0, "qk_norm_full_rope: eps must be finite and >= 0");
+  const c10::cuda::CUDAGuard guard(qkv.device());
+  const int64_t B = qkv.size(0), S = qkv.size(1);
+  Tensor x_save = torch::empty({B, S, nh + nkv, 128}, qkv.options());
+  Tensor rstd = torch::empty({B, S, 2}, qkv.options().dtype(at::kFloat));
+  dtg::qk_norm_full_rope_fwd(qkv.data_ptr(), q_w.data_ptr(), k_w.data_ptr(), cos.data_ptr<float>(),
+                             sin.data_ptr<float>(), x_save.data_ptr(), rstd.data_ptr<float>(), B * S, (int)S,
+                             (int)qkv.size(2), (int)nh, (int)nkv, per_token, (float)eps, stream());
+  return {x_save, rstd};
+}
+
+Tensor qk_norm_full_rope_bwd(Tensor& dqkv, const Tensor& x_save, const Tensor& rstd, const Tensor& q_w,
+                             const Tensor& k_w, const Tensor& cos, const Tensor& sin, int64_t nh, int64_t nkv) {
+  const bool per_token = check_qk_norm_rope(dqkv, q_w, k_w, cos, sin, nh, nkv, true);
+  const int64_t B = dqkv.size(0), S = dqkv.size(1), T = B * S;
+  check_vec(x_save, "x_save", at::kBFloat16);
+  check_contig(rstd, "rstd", at::kFloat);
+  TORCH_CHECK(x_save.sizes() == at::IntArrayRef({B, S, nh + nkv, 128}) && x_save.device() == dqkv.device(),
+              "qk_norm_full_rope_bwd: x_save must be [B, S, nh + nkv, 128] on the device of dqkv");
+  TORCH_CHECK(rstd.sizes() == at::IntArrayRef({B, S, 2}) && rstd.device() == dqkv.device(),
+              "qk_norm_full_rope_bwd: rstd must be [B, S, 2] on the device of dqkv");
+  const c10::cuda::CUDAGuard guard(dqkv.device());
+  const int64_t W = (nh + nkv) * 128;
+  Tensor dw = torch::empty({W}, dqkv.options().dtype(at::kFloat));
+  Tensor partial = torch::empty({T > 0 ? dtg::qk_norm_full_rope_bwd_grid(T, (int)(nh + nkv)) : 1, W},
+                                dqkv.options().dtype(at::kFloat));
+  dtg::qk_norm_full_rope_bwd(dqkv.data_ptr(), x_save.data_ptr(), rstd.data_ptr<float>(), q_w.data_ptr(),
+                             k_w.data_ptr(), cos.data_ptr<float>(), sin.data_ptr<float>(), partial.data_ptr<float>(),
+                             dw.data_ptr<float>(), T, (int)S, (int)dqkv.size(2), (int)nh, (int)nkv, per_token,
+                             stream());
   return dw;
 }
 
@@ -377,6 +440,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("rope_inplace", &rope_inplace);
   m.def("qk_norm_rope_fwd", &qk_norm_rope_fwd);
   m.def("qk_norm_rope_bwd", &qk_norm_rope_bwd);
+  m.def("rmsnorm_add_fwd", &rmsnorm_add_fwd);
+  m.def("qk_norm_full_rope_fwd", &qk_norm_full_rope_fwd);
+  m.def("qk_norm_full_rope_bwd", &qk_norm_full_rope_bwd);
+  m.def("qk_norm_full_rope_bwd_grid", [](int64_t T, int64_t nqk) {
+    TORCH_CHECK(T > 0 && nqk >= 2 && nqk <= dtg::qk_norm_full_rope_max_heads(), "qk_norm_full_rope_bwd_grid: bad shape");
+    return dtg::qk_norm_full_rope_bwd_grid(T, (int)nqk);
+  });
   m.def("swiglu_fwd", &swiglu_fwd);
   m.def("swiglu_bwd", &swiglu_bwd);
   m.def("cross_entropy_fwd_bwd", &cross_entropy_fwd_bwd);

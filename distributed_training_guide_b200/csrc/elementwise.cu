@@ -95,6 +95,67 @@ void rmsnorm_fwd(const void* x, const void* res, const void* w, void* y, void* h
 }
 
 // ------------------------------------------------------------------------------------------
+// Norm-then-add (OLMo 2's post-sublayer norms):  h = bf16(r + bf16(x * rsqrt(mean(x^2) + eps) * w))
+// The statistic and the normalisation are rmsnorm_fwd_kernel's without a residual, operation for operation, so h is
+// bit-identical to rmsnorm_fwd followed by a bf16 add; y is never written.
+// ------------------------------------------------------------------------------------------
+template <int kMaxVec, int kNormThreads>
+__global__ void __launch_bounds__(kNormThreads) rmsnorm_add_fwd_kernel(
+    const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w,
+    __nv_bfloat16* __restrict__ h_out, float* __restrict__ rstd_out, int H, float eps) {
+  __shared__ float red[32];
+  const int row = blockIdx.x;
+  const int nvec = H >> 3;
+  const __nv_bfloat16* xr = x + (size_t)row * H;
+  bf16x8 cache[kMaxVec];
+  float ss = 0.f;
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    const int i = threadIdx.x + k * kNormThreads;
+    if (i < nvec) {
+      cache[k] = ld8(xr + i * 8);
+      float f[8];
+      unpack8(cache[k], f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) ss += f[j] * f[j];
+    }
+  }
+  ss = block_sum(ss, red);
+  const float rstd = rsqrtf(ss / (float)H + eps);
+  if (threadIdx.x == 0) rstd_out[row] = rstd;
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    const int i = threadIdx.x + k * kNormThreads;
+    if (i < nvec) {
+      float f[8], g[8], fr[8];
+      unpack8(cache[k], f);
+      unpack8(ld8(w + i * 8), g);
+      unpack8(ld8(r + (size_t)row * H + i * 8), fr);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = f[j] * rstd * g[j];
+      unpack8(pack8(f), f);   // the normalised branch is rounded to bf16 before the add
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] += fr[j];
+      st8(h_out + (size_t)row * H + i * 8, pack8(f));
+    }
+  }
+}
+
+void rmsnorm_add_fwd(const void* x, const void* res, const void* w, void* h_out, float* rstd, int T, int H, float eps,
+                     cudaStream_t s) {
+  if (H % 8 != 0) throw std::runtime_error("rmsnorm: hidden size must be a multiple of 8");
+  auto X = (const __nv_bfloat16*)x;
+  auto R = (const __nv_bfloat16*)res;
+  auto W = (const __nv_bfloat16*)w;
+#define CALL_ADD(NV, NT) \
+  rmsnorm_add_fwd_kernel<NV, NT><<<T, NT, 0, s>>>(X, R, W, (__nv_bfloat16*)h_out, rstd, H, eps);
+  DTG_NORM_DISPATCH(H, CALL_ADD);
+#undef CALL_ADD
+  note_launch();
+  DTG_LAUNCH_CHECK();
+}
+
+// ------------------------------------------------------------------------------------------
 // RMSNorm backward.  xhat = h*rstd, g = dy*w:
 //   dx = rstd * (g - xhat * mean(g*xhat)) (+ dres),   dw = sum_rows dy * xhat
 // Persistent CTAs stride over rows and keep their dw partial in registers; partials go to a

@@ -4,7 +4,8 @@ The GPU boxes have no network, so the handful of Hugging Face model ids the
 guide uses (reference: every chapter's ``-m/--model-name`` flag, e.g.
 ``02-distributed-data-parallel/train_llm.py:57``) are resolved from this table
 instead of the hub.  A local directory containing a ``config.json`` is also
-accepted, and tiny ``debug-*`` configs exist for tests.
+accepted, and tiny ``debug-*`` configs exist for tests.  Families: Llama 2 / 3 / 3.1 / 3.2, Mistral, Qwen3, Qwen2.5,
+OLMo 2 (``allenai/OLMo-2-*``, ``model_type: "olmo2"``) and GPT-2.
 """
 from __future__ import annotations
 
@@ -16,8 +17,9 @@ from typing import Optional
 
 @dataclasses.dataclass
 class ModelConfig:
-    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "gpt2"; mistral is llama with a sliding attention window,
-    # qwen3 llama with QK-norm and a head_dim of its own, qwen2 llama with q/k/v biases
+    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "olmo2" | "gpt2"; mistral is llama with a sliding attention
+    # window, qwen3 llama with QK-norm and a head_dim of its own, qwen2 llama with q/k/v biases, olmo2 llama with a
+    # full-width QK-norm and post-sublayer norms instead of the pre-norms (``full_qk_norm``, ``post_norm``)
     vocab_size: int
     hidden_size: int
     intermediate_size: int
@@ -49,6 +51,17 @@ class ModelConfig:
             return self.explicit_head_dim
         return self.hidden_size // self.num_attention_heads
 
+    @property
+    def full_qk_norm(self) -> bool:
+        """OLMo 2's QK-norm: one RMSNorm over each token's whole q (nh * head_dim) and one over its whole k (nkv *
+        head_dim), with gains of those lengths.  Exclusive of Qwen3's per-head ``qk_norm``."""
+        return self.arch == "olmo2"
+
+    @property
+    def post_norm(self) -> bool:
+        """OLMo 2's layer: no input_layernorm; h1 = h + norm(attn(h)), h2 = h1 + norm(mlp(h1))."""
+        return self.arch == "olmo2"
+
     def num_parameters(self) -> int:
         h, i, v, l = self.hidden_size, self.intermediate_size, self.vocab_size, self.num_hidden_layers
         if self.arch == "gpt2":
@@ -61,6 +74,8 @@ class ModelConfig:
             per_layer += 2 * self.head_dim
         if self.qkv_bias:
             per_layer += q + 2 * kv
+        if self.full_qk_norm:
+            per_layer += q + kv
         n = v * h + l * per_layer + h
         if not self.tie_word_embeddings:
             n += v * h
@@ -111,6 +126,14 @@ def _qwen2(name, h, i, l, nh, nkv, tied, v, maxpos):
     )
 
 
+def _olmo2(name, h, i, l, nh, nkv, v=100352, maxpos=4096):
+    return ModelConfig(
+        arch="olmo2", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
+        num_attention_heads=nh, num_key_value_heads=nkv, max_position_embeddings=maxpos,
+        rms_norm_eps=1e-6, rope_theta=5e5, tie_word_embeddings=False, name=name,
+    )
+
+
 _GPT2 = ModelConfig(
     arch="gpt2", vocab_size=50257, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
     num_attention_heads=12, num_key_value_heads=12, max_position_embeddings=1024,
@@ -145,6 +168,11 @@ REGISTRY = {
     "Qwen/Qwen2.5-14B": _qwen2("Qwen/Qwen2.5-14B", 5120, 13824, 48, 40, 8, False, 152064, 131072),
     "Qwen/Qwen2.5-32B": _qwen2("Qwen/Qwen2.5-32B", 5120, 27648, 64, 40, 8, False, 152064, 131072),
     "Qwen/Qwen2.5-72B": _qwen2("Qwen/Qwen2.5-72B", 8192, 29568, 80, 64, 8, False, 152064, 131072),
+    # OLMo 2: full-width QK-norm and post-sublayer norms; head_dim 128 at every size, untied
+    "allenai/OLMo-2-0425-1B": _olmo2("allenai/OLMo-2-0425-1B", 2048, 8192, 16, 16, 16),
+    "allenai/OLMo-2-1124-7B": _olmo2("allenai/OLMo-2-1124-7B", 4096, 11008, 32, 32, 32),
+    "allenai/OLMo-2-1124-13B": _olmo2("allenai/OLMo-2-1124-13B", 5120, 13824, 40, 40, 40),
+    "allenai/OLMo-2-0325-32B": _olmo2("allenai/OLMo-2-0325-32B", 5120, 27648, 64, 40, 8),
     # tiny configs for tests / smoke runs (head_dim 128 so the sm_90a attention kernel applies)
     "debug-llama": _llama("debug-llama", 1024, 256, 512, 2, 2, 2, 2048, 1e4),
     "debug-llama-gqa": _llama("debug-llama-gqa", 1024, 512, 1024, 2, 4, 2, 2048, 5e5),
@@ -157,6 +185,8 @@ REGISTRY = {
     "debug-qwen3": _qwen3("debug-qwen3", 256, 512, 2, 4, 2, False, v=1024, maxpos=2048),
     # 4 heads x 64 over a hidden size of 256, with q/k/v biases: head_dim 64, as in Qwen2.5-0.5B
     "debug-qwen2": _qwen2("debug-qwen2", 256, 512, 2, 4, 2, False, 1024, 2048),
+    # 4 q heads and 2 k heads x 128 over a hidden size of 512: GQA, and a k norm narrower than the q norm
+    "debug-olmo2": _olmo2("debug-olmo2", 512, 1024, 2, 4, 2, v=1024, maxpos=2048),
     "debug-gpt2": dataclasses.replace(_GPT2, vocab_size=512, hidden_size=64, intermediate_size=256,
                                       num_hidden_layers=2, num_attention_heads=2, num_key_value_heads=2,
                                       max_position_embeddings=128, name="debug-gpt2"),
@@ -174,8 +204,19 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
             max_position_embeddings=d.get("n_positions", 1024), tie_word_embeddings=True,
             layer_norm_epsilon=d.get("layer_norm_epsilon", 1e-5), dropout=d.get("resid_pdrop", 0.1), name=name,
         )
-    if mt not in ("llama", "mistral", "qwen3", "qwen2"):
+    if mt not in ("llama", "mistral", "qwen3", "qwen2", "olmo2"):
         raise ValueError(f"unsupported model_type {mt!r} in {name}")
+    if mt == "olmo2":
+        if d.get("attention_bias"):
+            raise ValueError(f"{name}: attention_bias is true; OLMo 2 projections with a bias are not supported")
+        rope = d.get("rope_parameters") if isinstance(d.get("rope_parameters"), dict) else d.get("rope_scaling")
+        if rope and (rope.get("rope_type") or rope.get("type") or "default") != "default":
+            key = "rope_parameters" if isinstance(d.get("rope_parameters"), dict) else "rope_scaling"
+            raise ValueError(f"{name}: {key} has type {rope.get('rope_type') or rope.get('type')!r}; only the default "
+                             "RoPE is supported for OLMo 2")
+        if d.get("head_dim") is not None and d["head_dim"] != d["hidden_size"] // d["num_attention_heads"]:
+            raise ValueError(f"{name}: head_dim {d['head_dim']} differs from hidden_size / num_attention_heads = "
+                             f"{d['hidden_size'] // d['num_attention_heads']}; only head_dim = hidden / heads is supported")
     window = None
     head_dim = None
     if mt == "llama":
@@ -303,6 +344,16 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
             "rms_norm_eps": cfg.rms_norm_eps, "rope_theta": cfg.rope_theta, "hidden_act": "silu",
             "tie_word_embeddings": cfg.tie_word_embeddings, "use_sliding_window": False, "bos_token_id": 151643,
             "eos_token_id": 151643, "torch_dtype": "bfloat16",
+        }
+    if cfg.arch == "olmo2":
+        d = {
+            "model_type": "olmo2", "architectures": ["Olmo2ForCausalLM"], "vocab_size": cfg.vocab_size,
+            "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size,
+            "num_hidden_layers": cfg.num_hidden_layers, "num_attention_heads": cfg.num_attention_heads,
+            "num_key_value_heads": cfg.num_key_value_heads, "max_position_embeddings": cfg.max_position_embeddings,
+            "rms_norm_eps": cfg.rms_norm_eps, "rope_theta": cfg.rope_theta, "hidden_act": "silu",
+            "tie_word_embeddings": cfg.tie_word_embeddings, "attention_bias": False, "pad_token_id": None,
+            "bos_token_id": None, "eos_token_id": 100257, "torch_dtype": "bfloat16",
         }
     if cfg.arch == "llama" and cfg.explicit_head_dim is not None:
         d["head_dim"] = cfg.explicit_head_dim

@@ -1,5 +1,6 @@
 """Llama-family causal LM built on the sm_90a op layer (Llama; Mistral: Llama plus a sliding attention window; Qwen3:
-Llama plus QK-norm, with a head_dim of its own; Qwen2: Llama plus q/k/v biases).
+Llama plus QK-norm, with a head_dim of its own; Qwen2: Llama plus q/k/v biases; OLMo 2: Llama with a full-width
+QK-norm and RMSNorms after each sublayer instead of before it, ``Olmo2DecoderLayer``).
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
 the reference instantiates at e.g. ``02-distributed-data-parallel/train_llm.py:57-58``)
@@ -7,7 +8,8 @@ so checkpoints keep meaningful keys: ``model.embed_tokens.weight``,
 ``model.layers.{i}.self_attn.{q,k,v,o}_proj.weight``, ``model.layers.{i}.mlp.
 {gate,up,down}_proj.weight``, ``...{input,post_attention}_layernorm.weight``,
 ``model.norm.weight``, ``lm_head.weight``; Qwen3 adds ``...self_attn.{q,k}_norm.weight``, Qwen2
-``...self_attn.{q,k,v}_proj.bias``.
+``...self_attn.{q,k,v}_proj.bias``; OLMo 2 has ``...self_attn.{q,k}_norm.weight`` ([nh*d], [nkv*d]) and
+``...post_{attention,feedforward}_layernorm.weight`` and no ``input_layernorm``.
 
 What is *different* from the HF module code (SURVEY.md §3.2) is the execution plan:
   * q/k/v (and gate/up) projections run as ONE wgmma GEMM over a fused weight that is
@@ -160,12 +162,21 @@ class LlamaAttention(nn.Module):
         #: QK-norm (Qwen3): [head_dim] gains, replicated under tensor parallelism (every rank normalises its heads)
         self.q_norm = RMSNorm(d, config.rms_norm_eps, dtype, device) if config.qk_norm else None
         self.k_norm = RMSNorm(d, config.rms_norm_eps, dtype, device) if config.qk_norm else None
+        #: full-width QK-norm (OLMo 2): [nh * head_dim] and [nkv * head_dim] gains, one statistic over all of a
+        #: token's q (k) heads, so tensor parallelism cannot split them (it is refused for OLMo 2)
+        self.full_qk_norm = config.full_qk_norm
+        if self.full_qk_norm:
+            self.q_norm = RMSNorm(self.num_heads * d, config.rms_norm_eps, dtype, device)
+            self.k_norm = RMSNorm(self.num_kv_heads * d, config.rms_norm_eps, dtype, device)
 
     def position_qk_(self, qkv, cos, sin):
         """RoPE (after QK-norm, when the layer has it) on the q and k heads of ``qkv`` [B,S,heads,d], in place on
         the kernel path."""
         if self.q_norm is None:
             return ops.rope_qkv_(qkv, cos, sin, self.num_heads + self.num_kv_heads)
+        if self.full_qk_norm:
+            return ops.olmo_qk_norm_rope_(qkv, self.q_norm.weight, self.k_norm.weight, cos, sin, self.num_heads,
+                                          self.num_kv_heads, self.q_norm.eps)
         return ops.qk_norm_rope_(qkv, self.q_norm.weight, self.k_norm.weight, cos, sin, self.num_heads,
                                  self.num_kv_heads, self.q_norm.eps)
 
@@ -269,6 +280,51 @@ class LlamaDecoderLayer(nn.Module):
         return down, h
 
 
+class Olmo2DecoderLayer(LlamaDecoderLayer):
+    """OLMo 2's layer: the Llama layer with full-width QK-norm and RMSNorms after each sublayer instead of before it:
+    ``h1 = h + norm_pa(o_proj(attn(h)))``, ``h2 = h1 + norm_pf(mlp(h1))``; there is no ``input_layernorm``."""
+
+    #: matrices first in the Llama order (FSDP's chunked layout; ``FUSED``'s q|k|v and gate|up), then the gains
+    FLAT_ORDER = LlamaDecoderLayer.FLAT_ORDER[:7] + (
+        "post_attention_layernorm.weight", "post_feedforward_layernorm.weight", "self_attn.q_norm.weight",
+        "self_attn.k_norm.weight",
+    )
+
+    def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
+        nn.Module.__init__(self)
+        self.layer_idx = layer_idx
+        self.self_attn = LlamaAttention(config, dtype, device, tp_size)
+        self.mlp = LlamaMLP(config, dtype, device, tp_size)
+        self.post_attention_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
+        self.post_feedforward_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
+        self.flat_order = self.FLAT_ORDER
+        self._fused = {}
+        self.tp = None
+        self.fp8 = False
+
+    def forward(self, x, residual, cos, sin, doc_start=None):
+        """x: [B,S,H] the residual stream (the embeddings for the first layer); residual: None.  The pending add
+        needs this layer's post_feedforward_layernorm gain, which FSDP may reshard before the next layer runs, so the
+        layer completes its stream and returns (h2, None): every layer sees ``residual = None``."""
+        assert residual is None, "an OLMo 2 layer takes the complete residual stream"
+        att = self.self_attn
+        B, S, _ = x.shape
+        fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
+        w, owner = self._qkv_weight()
+        qkv = fused_linear(x, w, owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
+        qkv = att.position_qk_(qkv, cos, sin)
+        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
+        a = a.reshape(B, S, att.num_heads * att.head_dim)
+        a = ops.fp8_linear(a, att.o_proj.weight) if self.fp8 else att.o_proj(a)
+        n = self.post_attention_layernorm
+        h1 = ops.rms_norm_add(a, x, n.weight, n.eps)
+        w, owner = self._gate_up_weight()
+        act = ops.swiglu(fused_linear(h1, w, owner))
+        down = ops.fp8_linear(act, self.mlp.down_proj.weight) if self.fp8 else self.mlp.down_proj(act)
+        n = self.post_feedforward_layernorm
+        return ops.rms_norm_add(down, h1, n.weight, n.eps), None
+
+
 class LlamaModel(nn.Module):
     def __init__(self, config: ModelConfig, dtype=None, device=None, tp_size=1):
         super().__init__()
@@ -276,8 +332,9 @@ class LlamaModel(nn.Module):
         # tensor parallel: the table is sharded over the hidden dimension (reference: ColwiseParallel on
         # nn.Embedding, 06-tensor-parallel/train_llm.py:82)
         self.embed_tokens = Embedding(config.vocab_size, config.hidden_size // tp_size, dtype, device)
+        layer_cls = Olmo2DecoderLayer if config.post_norm else LlamaDecoderLayer
         self.layers = nn.ModuleList(
-            [LlamaDecoderLayer(config, i, dtype, device, tp_size) for i in range(config.num_hidden_layers)]
+            [layer_cls(config, i, dtype, device, tp_size) for i in range(config.num_hidden_layers)]
         )
         self.norm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
         self.rotary_emb = RotaryEmbedding(config)

@@ -3,8 +3,8 @@
 On CUDA tensors each op calls a hand-written sm_90a kernel from the in-tree
 extension (``csrc/``): wgmma/TMA GEMM (fwd / dgrad / wgrad) in bf16 and, for
 ``fp8_linear``, in fp8 with its amax and cast-transpose kernels, wgmma
-flash-attention, fused residual-add+RMSNorm, in-place RoPE on the fused qkv buffer
-(after Qwen3's per-head QK-norm in the same kernel), SwiGLU, in-place
+flash-attention, fused residual-add+RMSNorm and norm-then-add (OLMo 2), in-place RoPE on the fused qkv buffer
+(after Qwen3's per-head or OLMo 2's full-width QK-norm in the same kernel), SwiGLU, in-place
 softmax-cross-entropy, embedding gather / scatter-add and flat AdamW.  On CPU tensors the same Functions run the reference math in
 ``ops/reference.py`` (chapter 01's CPU config and the gloo tests).
 
@@ -27,7 +27,8 @@ from .. import _ext
 from . import reference as ref
 
 __all__ = [
-    "linear", "fused_linear", "rms_norm", "add_rms_norm", "rope_qkv_", "qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy",
+    "linear", "fused_linear", "rms_norm", "add_rms_norm", "rms_norm_add", "rope_qkv_", "qk_norm_rope_",
+    "olmo_qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy",
     "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "bias_grad", "ref",
 ]
 
@@ -375,6 +376,39 @@ def add_rms_norm(x, residual, w, eps):
     return ref.add_rms_norm(x, residual, w, eps)
 
 
+class _RMSNormAdd(torch.autograd.Function):
+    """h = r + rmsnorm(x) * w in one pass: the normalised branch is never stored.  Backward: dr = dh, and dx / dw are
+    the RMSNorm backward of x (rmsnorm_bwd with h := x, no residual gradient)."""
+
+    @staticmethod
+    def forward(ctx, x, r, w, eps):
+        C = _ext.load()
+        x2 = x.reshape(-1, x.shape[-1])
+        h, rstd = C.rmsnorm_add_fwd(x2, r.reshape(-1, r.shape[-1]), w, float(eps))
+        ctx.save_for_backward(x2, w, rstd)
+        ctx.shape = x.shape
+        ctx.w_param = w
+        return h.view(x.shape)
+
+    @staticmethod
+    def backward(ctx, dh):
+        C = _ext.load()
+        x2, w, rstd = ctx.saved_tensors
+        dh2 = dh.reshape(-1, dh.shape[-1]).contiguous()
+        dx, dw32 = C.rmsnorm_bwd(dh2, x2, w, rstd, None)
+        dw = _emit_weight_grad(ctx.w_param, _norm_dw_into(dw32), w)
+        return dx.view(ctx.shape), dh, dw, None
+
+
+def rms_norm_add(x, r, w, eps):
+    """Norm-then-add (OLMo 2's post-sublayer norms): ``bf16(r + bf16(rmsnorm(x) * w))``, the gain applied in fp32 with
+    one rounding (``ref.rms_norm_add``).  bf16 CUDA tensors run the sm_90a kernel, whose output is bit-identical to
+    ``rmsnorm_fwd`` followed by a bf16 add; the gain gradient goes through ``_emit_weight_grad``."""
+    if _ext.use_cuda_kernel("rmsnorm", x, r, w) and x.dtype == torch.bfloat16:
+        return _RMSNormAdd.apply(x.contiguous(), r.contiguous(), w, eps)
+    return ref.rms_norm_add(x, r, w, eps)
+
+
 # --------------------------------------------------------------------------------------
 # RoPE, applied in place on the q and k heads of the fused qkv activation
 # --------------------------------------------------------------------------------------
@@ -446,6 +480,49 @@ def qk_norm_rope_(qkv, q_w, k_w, cos, sin, nh, nkv, eps):
         return _QKNormRope.apply(qkv, q_w, k_w, cos.contiguous(), sin.contiguous(), nh, nkv, eps)
     q = ref.rms_norm(qkv[:, :, :nh], q_w, eps)
     k = ref.rms_norm(qkv[:, :, nh:nh + nkv], k_w, eps)
+    rot = ref.rope_apply(torch.cat([q, k], dim=2), cos, sin)
+    return torch.cat([rot, qkv[:, :, nh + nkv:]], dim=2)
+
+
+class _OlmoQKNormRope(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, qkv, q_w, k_w, cos, sin, nh, nkv, eps):
+        C = _ext.load()
+        x_save, rstd = C.qk_norm_full_rope_fwd(qkv, q_w, k_w, cos, sin, nh, nkv, float(eps))
+        ctx.save_for_backward(x_save, rstd, q_w, k_w, cos, sin)
+        ctx.heads = (nh, nkv)
+        ctx.w_params = (q_w, k_w)
+        return qkv.detach()   # in place, handed to autograd as a fresh tensor (see _RopeQKV)
+
+    @staticmethod
+    def backward(ctx, dqkv):
+        C = _ext.load()
+        x_save, rstd, q_w, k_w, cos, sin = ctx.saved_tensors
+        if not dqkv.is_contiguous():
+            dqkv = dqkv.contiguous()
+        dw32 = C.qk_norm_full_rope_bwd(dqkv, x_save, rstd, q_w, k_w, cos, sin, *ctx.heads)   # in place on q|k
+        nq = q_w.numel()
+        dq = _emit_weight_grad(ctx.w_params[0], _norm_dw_into(dw32[:nq]), q_w)
+        dk = _emit_weight_grad(ctx.w_params[1], _norm_dw_into(dw32[nq:]), k_w)
+        return dqkv, dq, dk, None, None, None, None, None
+
+
+def olmo_qk_norm_rope_(qkv, q_w, k_w, cos, sin, nh, nkv, eps):
+    """OLMo 2's full-width QK-norm then RoPE on ``qkv`` [B,S,nh+2*nkv,d]: each token's q heads are RMS-normalised
+    together, over all nh*d elements, and scaled by ``q_w`` [nh*d]; its k heads likewise with ``k_w`` [nkv*d]; the
+    gain is applied in fp32 with one rounding (``ref.rms_norm_one_rounding``).  Then heads [0, nh+nkv) are rotated as
+    ``rope_qkv_`` does, with cos/sin [S,d/2] or [B,S,d/2] (fp32).  V is untouched.
+
+    bf16 CUDA tensors with d = 128 run the sm_90a kernels in place on ``qkv``; anything else composes
+    ``ref.rms_norm_one_rounding`` and ``ref.rope_apply``.  The kernel path keeps the pre-norm q|k heads (bf16) and
+    two fp32 rstd per token for the backward.  The gain gradients go through ``_emit_weight_grad``, so flat-buffer
+    parameters are overwritten on their first use in a step and accumulated on later ones."""
+    if (_ext.use_cuda_kernel("qk_norm_rope", qkv, q_w, k_w) and qkv.dtype == torch.bfloat16
+            and qkv.shape[-1] == 128):
+        return _OlmoQKNormRope.apply(qkv, q_w, k_w, cos.contiguous(), sin.contiguous(), nh, nkv, eps)
+    B, S, _, d = qkv.shape
+    q = ref.rms_norm_one_rounding(qkv[:, :, :nh].reshape(B, S, nh * d), q_w, eps).view(B, S, nh, d)
+    k = ref.rms_norm_one_rounding(qkv[:, :, nh:nh + nkv].reshape(B, S, nkv * d), k_w, eps).view(B, S, nkv, d)
     rot = ref.rope_apply(torch.cat([q, k], dim=2), cos, sin)
     return torch.cat([rot, qkv[:, :, nh + nkv:]], dim=2)
 

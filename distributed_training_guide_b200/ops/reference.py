@@ -29,6 +29,20 @@ def rms_norm(x, w, eps):
     return ((xf * rstd).to(x.dtype) * w).to(x.dtype)
 
 
+def rms_norm_one_rounding(x, w, eps):
+    """RMSNorm with the gain applied in fp32 and one rounding to ``x.dtype`` (transformers' ``Olmo2RMSNorm``, and what
+    the rmsnorm kernels compute): ``(w * (x * rsqrt(mean(x^2) + eps))).to(x.dtype)``."""
+    xf = x.float()
+    rstd = torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps)
+    return (w.float() * (xf * rstd)).to(x.dtype)
+
+
+def rms_norm_add(x, r, w, eps):
+    """Norm-then-add (OLMo 2's post-sublayer norms): ``r + rms_norm_one_rounding(x, w, eps)``, the normalised branch
+    rounded to ``x.dtype`` before the add and the sum rounded again."""
+    return r + rms_norm_one_rounding(x, w, eps)
+
+
 def add_rms_norm(x, residual, w, eps):
     """returns (normed, new_residual) with new_residual = x + residual."""
     h = x + residual

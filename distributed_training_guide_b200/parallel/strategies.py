@@ -425,6 +425,12 @@ class TwoDParallel(Strategy):
         from .tp import TensorParallelRuntime, TPContext
 
         env, mesh = self.env, self.mesh
+        if getattr(config, "full_qk_norm", False):
+            # the layer path below is the tensor-parallel one at every tp size, and it has no full-width norm
+            raise ValueError(
+                f"{config.name or config.arch}: tensor parallelism does not support the full-width q/k norm (OLMo 2): "
+                "its statistic spans the q (k) heads that tensor parallelism splits across ranks; train it with the "
+                "single-GPU, DDP or FSDP engines (chapters 01, 02, 04, 05)")
         cuda = env.device.type == "cuda"
         seed = getattr(args, "seed", 0)
         use_fsdp = mesh.dp_size > 1
