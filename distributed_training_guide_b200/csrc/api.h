@@ -26,6 +26,19 @@ void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s);
 // colsum then adds in a fixed order: no atomics, bit-identical from run to run.
 int bias_grad_chunks(long long T, int N);
 void bias_grad(const void* dy, long long T, int N, long long ld, float* partial, float* db, cudaStream_t s);
+// LayerNorm (StarCoder2): h_out = bf16(x + res) when res is given (else h = x), y = bf16((h - mean) * rstd * w + b);
+// mean, rstd [T] fp32 for the backward.  H % 8 == 0, H <= 16384.
+void layernorm_fwd(const void* x, const void* res, const void* w, const void* b, void* y, void* h_out, float* mean,
+                   float* rstd, int T, int H, float eps, cudaStream_t s);
+int layernorm_bwd_grid(int T, int H);
+// dx = the LayerNorm backward (+ dres); dw, db [H] fp32 summed through dw_partial / db_partial
+// ([layernorm_bwd_grid(T, H), H] fp32 scratch each) in a fixed order
+void layernorm_bwd(const void* dy, const void* h, const void* w, const float* mean, const float* rstd,
+                   const void* dres, void* dx, float* dw_partial, float* db_partial, float* dw, float* db, int T,
+                   int H, cudaStream_t s);
+// GELU with the tanh approximation on n bf16 elements (n % 8 == 0); the backward from the saved pre-activation x
+void gelu_tanh_fwd(const void* x, void* y, long long n, cudaStream_t s);
+void gelu_tanh_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t s);
 void swiglu_fwd(const void* gu, void* h, long long T, int I, cudaStream_t s);
 void swiglu_bwd(const void* dh, const void* gu, void* dgu, long long T, int I, cudaStream_t s);
 void embedding_fwd(const long long* ids, const void* w, void* out, long long T, int H, cudaStream_t s);

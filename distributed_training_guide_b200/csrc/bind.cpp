@@ -194,6 +194,101 @@ std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& h, const 
   return {dx, dw};
 }
 
+// Shared LayerNorm checks: x (or dy) bf16 [T, H] with H % 8 == 0 and H <= 16384, and a [H] gain; returns H.
+int64_t check_layernorm(const Tensor& x, const char* xname, const Tensor& w, const char* who) {
+  check_vec(x, xname, at::kBFloat16);
+  TORCH_CHECK(x.dim() == 2, who, ": ", xname, " must be 2-D [T, H]");
+  const int64_t H = x.size(1);
+  TORCH_CHECK(H % 8 == 0 && H > 0 && H <= 16384, who, ": hidden size must be a positive multiple of 8 and <= 16384, got ",
+              H);
+  check_vec(w, "w", at::kBFloat16);
+  TORCH_CHECK(w.dim() == 1 && w.size(0) == H, who, ": w must be [H] = [", H, "]");
+  TORCH_CHECK(w.device() == x.device(), who, ": w must be on the device of ", xname);
+  return H;
+}
+
+// (y, h or None, mean, rstd): h = bf16(x + residual) when a residual is given, y = LayerNorm(h) * w + b
+std::tuple<Tensor, c10::optional<Tensor>, Tensor, Tensor> layernorm_fwd(const Tensor& x,
+                                                                       const c10::optional<Tensor>& res,
+                                                                       const Tensor& w, const Tensor& b, double eps) {
+  const int64_t H = check_layernorm(x, "x", w, "layernorm_fwd");
+  check_vec(b, "b", at::kBFloat16);
+  TORCH_CHECK(b.dim() == 1 && b.size(0) == H, "layernorm_fwd: b must be [H] = [", H, "]");
+  TORCH_CHECK(b.device() == x.device(), "layernorm_fwd: b must be on the device of x");
+  TORCH_CHECK(std::isfinite(eps) && eps > 0, "layernorm_fwd: eps must be finite and > 0, got ", eps);
+  const void* rp = nullptr;
+  if (res.has_value()) {
+    check_vec(*res, "residual", at::kBFloat16);
+    TORCH_CHECK(res->sizes() == x.sizes(), "layernorm_fwd: residual and x differ in shape");
+    TORCH_CHECK(res->device() == x.device(), "layernorm_fwd: residual must be on the device of x");
+    rp = res->data_ptr();
+  }
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int64_t T = x.size(0);
+  Tensor y = torch::empty_like(x);
+  Tensor mean = torch::empty({T}, x.options().dtype(at::kFloat));
+  Tensor rstd = torch::empty({T}, x.options().dtype(at::kFloat));
+  c10::optional<Tensor> h;
+  if (rp) h = torch::empty_like(x);
+  if (T > 0)
+    dtg::layernorm_fwd(x.data_ptr(), rp, w.data_ptr(), b.data_ptr(), y.data_ptr(), h ? h->data_ptr() : nullptr,
+                       mean.data_ptr<float>(), rstd.data_ptr<float>(), (int)T, (int)H, (float)eps, stream());
+  return {y, h, mean, rstd};
+}
+
+// (dx, dw fp32, db fp32) of y = LayerNorm(h) * w + b, with dx += dres when dres is given
+std::tuple<Tensor, Tensor, Tensor> layernorm_bwd(const Tensor& dy, const Tensor& h, const Tensor& w, const Tensor& mean,
+                                                 const Tensor& rstd, const c10::optional<Tensor>& dres) {
+  const int64_t H = check_layernorm(dy, "dy", w, "layernorm_bwd");
+  check_vec(h, "h", at::kBFloat16);
+  TORCH_CHECK(h.sizes() == dy.sizes() && h.device() == dy.device(),
+              "layernorm_bwd: h and dy differ in shape or device");
+  const int64_t T = dy.size(0);
+  for (const Tensor* t : {&mean, &rstd}) {
+    check_contig(*t, t == &mean ? "mean" : "rstd", at::kFloat);
+    TORCH_CHECK(t->dim() == 1 && t->size(0) == T && t->device() == dy.device(), "layernorm_bwd: ",
+                t == &mean ? "mean" : "rstd", " must be [T] = [", T, "] on the device of dy");
+  }
+  const void* dr = nullptr;
+  if (dres.has_value()) {
+    check_vec(*dres, "dres", at::kBFloat16);
+    TORCH_CHECK(dres->sizes() == dy.sizes() && dres->device() == dy.device(),
+                "layernorm_bwd: dres and dy differ in shape or device");
+    dr = dres->data_ptr();
+  }
+  const c10::cuda::CUDAGuard guard(dy.device());
+  Tensor dx = torch::empty_like(dy);
+  Tensor dw = torch::zeros({H}, dy.options().dtype(at::kFloat));
+  Tensor db = torch::zeros({H}, dy.options().dtype(at::kFloat));
+  if (T > 0) {
+    Tensor partial = torch::empty({2, dtg::layernorm_bwd_grid((int)T, (int)H), H}, dy.options().dtype(at::kFloat));
+    dtg::layernorm_bwd(dy.data_ptr(), h.data_ptr(), w.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), dr,
+                       dx.data_ptr(), partial[0].data_ptr<float>(), partial[1].data_ptr<float>(),
+                       dw.data_ptr<float>(), db.data_ptr<float>(), (int)T, (int)H, stream());
+  }
+  return {dx, dw, db};
+}
+
+Tensor gelu_tanh_fwd(const Tensor& x) {
+  check_vec(x, "x", at::kBFloat16);
+  TORCH_CHECK(x.numel() % 8 == 0, "gelu_tanh_fwd: x must have a multiple of 8 elements, got ", x.numel());
+  const c10::cuda::CUDAGuard guard(x.device());
+  Tensor y = torch::empty_like(x);
+  if (x.numel() > 0) dtg::gelu_tanh_fwd(x.data_ptr(), y.data_ptr(), x.numel(), stream());
+  return y;
+}
+
+Tensor gelu_tanh_bwd(const Tensor& dy, const Tensor& x) {
+  check_vec(dy, "dy", at::kBFloat16);
+  check_vec(x, "x", at::kBFloat16);
+  TORCH_CHECK(dy.sizes() == x.sizes() && dy.device() == x.device(), "gelu_tanh_bwd: dy and x differ in shape or device");
+  TORCH_CHECK(x.numel() % 8 == 0, "gelu_tanh_bwd: x must have a multiple of 8 elements, got ", x.numel());
+  const c10::cuda::CUDAGuard guard(x.device());
+  Tensor dx = torch::empty_like(x);
+  if (x.numel() > 0) dtg::gelu_tanh_bwd(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), x.numel(), stream());
+  return dx;
+}
+
 void rope_inplace(Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t n_rot, bool inverse) {
   // qkv: [B, S, heads, d] contiguous; cos/sin fp32 [S, d/2] or [B, S, d/2]
   check_vec(qkv, "qkv", at::kBFloat16);
@@ -447,6 +542,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     TORCH_CHECK(T > 0 && nqk >= 2 && nqk <= dtg::qk_norm_full_rope_max_heads(), "qk_norm_full_rope_bwd_grid: bad shape");
     return dtg::qk_norm_full_rope_bwd_grid(T, (int)nqk);
   });
+  m.def("layernorm_fwd", &layernorm_fwd, py::arg("x"), py::arg("residual"), py::arg("w"), py::arg("b"),
+        py::arg("eps"));
+  m.def("layernorm_bwd", &layernorm_bwd, py::arg("dy"), py::arg("h"), py::arg("w"), py::arg("mean"),
+        py::arg("rstd"), py::arg("dres") = py::none());
+  m.def("layernorm_bwd_grid", [](int64_t T, int64_t H) {
+    TORCH_CHECK(T > 0 && H > 0 && H % 8 == 0 && H <= 16384, "layernorm_bwd_grid: bad shape");
+    return dtg::layernorm_bwd_grid((int)T, (int)H);
+  });
+  m.def("gelu_tanh_fwd", &gelu_tanh_fwd, py::arg("x"));
+  m.def("gelu_tanh_bwd", &gelu_tanh_bwd, py::arg("dy"), py::arg("x"));
   m.def("swiglu_fwd", &swiglu_fwd);
   m.def("swiglu_bwd", &swiglu_bwd);
   m.def("cross_entropy_fwd_bwd", &cross_entropy_fwd_bwd);

@@ -1,6 +1,7 @@
 // Memory-bound ops of the Llama step, hand-written for sm_90a:
 //   fused (residual add +) RMSNorm fwd / bwd, in-place RoPE on the fused qkv activation,
-//   SwiGLU fwd / bwd, embedding gather / scatter-add, scalar scale, the bias gradient (column sums).
+//   SwiGLU fwd / bwd, embedding gather / scatter-add, scalar scale, the bias gradient (column sums),
+//   fused (residual add +) LayerNorm fwd / bwd and GELU-tanh fwd / bwd (StarCoder2).
 // All are pure-bandwidth kernels: 16-byte vector accesses, fp32 math in registers, one pass
 // over the activations (the row is cached in registers between the statistic and the
 // normalisation).  Replaces the ~6 ATen kernels per RMSNorm / ~10 per RoPE the reference runs
@@ -345,6 +346,328 @@ void rmsnorm_bwd(const void* dy, const void* h, const void* w, const float* rstd
 #undef CALL_BWD
   colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(dw_partial, dw, grid, H);
   note_launch(2);
+  DTG_LAUNCH_CHECK();
+}
+
+// ------------------------------------------------------------------------------------------
+// LayerNorm forward (StarCoder2):  h = bf16(x (+ r));  y = bf16((h - mean) * rstd * w + b)
+//   mean = sum(h) / H,  var = sum((h - mean)^2) / H (a second pass over the cached row),  rstd = rsqrt(var + eps)
+// One CTA per row with the row cached in registers, as rmsnorm_fwd_kernel.  A row whose sums overflow fp32 (elements
+// near the bf16 limit) is redone scaled by 2^-72, which is exact for every element above 2^-77; mean and rstd are
+// saved in the row's own units.
+// ------------------------------------------------------------------------------------------
+constexpr float kLnDown = 0x1p-72f, kLnUp = 0x1p72f;
+
+// this thread's sum of h * scale, and of (h * scale - mean)^2, over its cached vectors
+template <int kMaxVec, int kNormThreads>
+__device__ __forceinline__ float ln_sum(const bf16x8 (&cache)[kMaxVec], int nvec, float scale) {
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    if (threadIdx.x + k * kNormThreads < nvec) {
+      float f[8];
+      unpack8(cache[k], f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s += f[j] * scale;
+    }
+  }
+  return s;
+}
+template <int kMaxVec, int kNormThreads>
+__device__ __forceinline__ float ln_sq_dev(const bf16x8 (&cache)[kMaxVec], int nvec, float mean, float scale) {
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    if (threadIdx.x + k * kNormThreads < nvec) {
+      float f[8];
+      unpack8(cache[k], f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float d = f[j] * scale - mean;
+        s += d * d;
+      }
+    }
+  }
+  return s;
+}
+
+template <int kMaxVec, int kNormThreads, bool HAS_RES>
+__global__ void __launch_bounds__(kNormThreads) layernorm_fwd_kernel(
+    const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w,
+    const __nv_bfloat16* __restrict__ b, __nv_bfloat16* __restrict__ y, __nv_bfloat16* __restrict__ h_out,
+    float* __restrict__ mean_out, float* __restrict__ rstd_out, int H, float eps) {
+  __shared__ float red[32];
+  const int row = blockIdx.x;
+  const int nvec = H >> 3;
+  const __nv_bfloat16* xr = x + (size_t)row * H;
+  const __nv_bfloat16* rr = HAS_RES ? r + (size_t)row * H : nullptr;
+  bf16x8 cache[kMaxVec];
+  float sum = 0.f;
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    const int i = threadIdx.x + k * kNormThreads;
+    if (i < nvec) {
+      bf16x8 v = ld8(xr + i * 8);
+      float f[8];
+      unpack8(v, f);
+      if (HAS_RES) {
+        float g[8];
+        unpack8(ld8(rr + i * 8), g);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f[j] += g[j];
+        v = pack8(f);          // the residual stream is stored (and normalised) in bf16
+        unpack8(v, f);
+        st8(h_out + (size_t)row * H + i * 8, v);
+      }
+      cache[k] = v;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) sum += f[j];
+    }
+  }
+  float scale = 1.f;
+  float mean = block_sum(sum, red) / (float)H;
+  float ss = block_sum(ln_sq_dev<kMaxVec, kNormThreads>(cache, nvec, mean, 1.f), red);
+  if (!(isfinite(mean) && isfinite(ss))) {   // uniform over the CTA: block_sum broadcasts
+    scale = kLnDown;
+    mean = block_sum(ln_sum<kMaxVec, kNormThreads>(cache, nvec, kLnDown), red) / (float)H;
+    ss = block_sum(ln_sq_dev<kMaxVec, kNormThreads>(cache, nvec, mean, kLnDown), red);
+  }
+  const float rstd = rsqrtf(ss / (float)H + eps * scale * scale);
+  if (threadIdx.x == 0) {
+    mean_out[row] = scale == 1.f ? mean : mean * kLnUp;
+    rstd_out[row] = scale == 1.f ? rstd : rstd * kLnDown;
+  }
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    const int i = threadIdx.x + k * kNormThreads;
+    if (i < nvec) {
+      float f[8], g[8], c[8];
+      unpack8(cache[k], f);
+      unpack8(ld8(w + i * 8), g);
+      unpack8(ld8(b + i * 8), c);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) f[j] = (f[j] * scale - mean) * rstd * g[j] + c[j];
+      st8(y + (size_t)row * H + i * 8, pack8(f));
+    }
+  }
+}
+
+void layernorm_fwd(const void* x, const void* res, const void* w, const void* b, void* y, void* h_out, float* mean,
+                   float* rstd, int T, int H, float eps, cudaStream_t s) {
+  if (H % 8 != 0) throw std::runtime_error("layernorm: hidden size must be a multiple of 8");
+  auto X = (const __nv_bfloat16*)x;
+  auto R = (const __nv_bfloat16*)res;
+  auto W = (const __nv_bfloat16*)w;
+  auto B = (const __nv_bfloat16*)b;
+  auto Y = (__nv_bfloat16*)y;
+#define CALL_LN_FWD(NV, NT)                                                                                  \
+  if (res)                                                                                                   \
+    layernorm_fwd_kernel<NV, NT, true><<<T, NT, 0, s>>>(X, R, W, B, Y, (__nv_bfloat16*)h_out, mean, rstd, H, eps); \
+  else                                                                                                       \
+    layernorm_fwd_kernel<NV, NT, false><<<T, NT, 0, s>>>(X, R, W, B, Y, nullptr, mean, rstd, H, eps);
+  DTG_NORM_DISPATCH(H, CALL_LN_FWD);
+#undef CALL_LN_FWD
+  note_launch();
+  DTG_LAUNCH_CHECK();
+}
+
+// ------------------------------------------------------------------------------------------
+// LayerNorm backward.  xhat = (h - mean) * rstd, g = dy * w:
+//   dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dres),   dw = sum_rows dy * xhat,   db = sum_rows dy
+// Persistent CTAs stride over rows as rmsnorm_bwd_kernel does; dw and db partials go to two [grid, H] fp32 scratch
+// rows per CTA, reduced by colsum_kernel in a fixed order (no atomics).  h - mean can only overflow when rstd is below
+// 2^-121, so rows with rstd < 2^-100 recompute xhat from h and mean scaled by 2^-72 (exact powers of two).
+// ------------------------------------------------------------------------------------------
+template <int kMaxVec, int kNormThreads, bool HAS_DRES>
+__global__ void __launch_bounds__(kNormThreads) layernorm_bwd_kernel(
+    const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restrict__ w,
+    const float* __restrict__ mean, const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres,
+    __nv_bfloat16* __restrict__ dx, float* __restrict__ dw_partial, float* __restrict__ db_partial, int T, int H) {
+  __shared__ float red[32];
+  const int nvec = H >> 3;
+  float dw_acc[kMaxVec][8], db_acc[kMaxVec][8];
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) dw_acc[k][j] = db_acc[k][j] = 0.f;
+
+  for (int row = blockIdx.x; row < T; row += gridDim.x) {
+    float rs = rstd[row], mu = mean[row], scale = 1.f;
+    if (rs < 0x1p-100f) {
+      scale = kLnDown;
+      mu *= kLnDown;
+      rs *= kLnUp;
+    }
+    const size_t base = (size_t)row * H;
+    float sg = 0.f, sgx = 0.f;
+    bf16x8 cg[kMaxVec], cx[kMaxVec];
+#pragma unroll
+    for (int k = 0; k < kMaxVec; ++k) {
+      const int i = threadIdx.x + k * kNormThreads;
+      if (i < nvec) {
+        cg[k] = ld8(dy + base + i * 8);
+        cx[k] = ld8(h + base + i * 8);
+        float fdy[8], fx[8], fw[8];
+        unpack8(cg[k], fdy);
+        unpack8(cx[k], fx);
+        unpack8(ld8(w + i * 8), fw);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float xhat = (fx[j] * scale - mu) * rs;
+          const float g = fdy[j] * fw[j];
+          sg += g;
+          sgx += g * xhat;
+          dw_acc[k][j] += fdy[j] * xhat;
+          db_acc[k][j] += fdy[j];
+        }
+      }
+    }
+    sg = block_sum(sg, red) / (float)H;
+    sgx = block_sum(sgx, red) / (float)H;
+    const float rs_out = scale == 1.f ? rs : rs * kLnDown;   // rstd in the row's own units
+#pragma unroll
+    for (int k = 0; k < kMaxVec; ++k) {
+      const int i = threadIdx.x + k * kNormThreads;
+      if (i < nvec) {
+        float fdy[8], fx[8], fw[8], out[8];
+        unpack8(cg[k], fdy);
+        unpack8(cx[k], fx);
+        unpack8(ld8(w + i * 8), fw);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float xhat = (fx[j] * scale - mu) * rs;
+          out[j] = rs_out * (fdy[j] * fw[j] - sg - xhat * sgx);
+        }
+        if (HAS_DRES) {
+          float fr[8];
+          unpack8(ld8(dres + base + i * 8), fr);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) out[j] += fr[j];
+        }
+        st8(dx + base + i * 8, pack8(out));
+      }
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    const int i = threadIdx.x + k * kNormThreads;
+    if (i < nvec) {
+      float4* dst = reinterpret_cast<float4*>(dw_partial + (size_t)blockIdx.x * H + i * 8);
+      dst[0] = make_float4(dw_acc[k][0], dw_acc[k][1], dw_acc[k][2], dw_acc[k][3]);
+      dst[1] = make_float4(dw_acc[k][4], dw_acc[k][5], dw_acc[k][6], dw_acc[k][7]);
+      dst = reinterpret_cast<float4*>(db_partial + (size_t)blockIdx.x * H + i * 8);
+      dst[0] = make_float4(db_acc[k][0], db_acc[k][1], db_acc[k][2], db_acc[k][3]);
+      dst[1] = make_float4(db_acc[k][4], db_acc[k][5], db_acc[k][6], db_acc[k][7]);
+    }
+  }
+}
+
+// The db accumulators double the per-thread partial state of rmsnorm_bwd_kernel, so above H 4096 the row is spread
+// over more threads (at most 4 vectors each) instead of more registers.
+#define DTG_LN_BWD_DISPATCH(H, CALL)                                        \
+  do {                                                                     \
+    const int nvec_ = (H) >> 3;                                            \
+    if (nvec_ <= 128) { CALL(1, 128); }                                    \
+    else if (nvec_ <= 256) { CALL(2, 128); }                               \
+    else if (nvec_ <= 512) { CALL(4, 128); }                               \
+    else if (nvec_ <= 1024) { CALL(4, 256); }                              \
+    else if (nvec_ <= 2048) { CALL(4, 512); }                              \
+    else throw std::runtime_error("layernorm: hidden size > 16384 unsupported"); \
+  } while (0)
+
+// 1024 threads per SM (the CTA size grows with H): enough rows in flight to cover HBM latency while the two [grid, H]
+// fp32 partials stay small (13 MB at H 6144)
+int layernorm_bwd_grid(int T, int H) {
+  const int nvec = H >> 3;
+  const int nt = nvec <= 512 ? 128 : nvec <= 1024 ? 256 : 512;
+  const int g = sm_count() * (1024 / nt);
+  return T < g ? T : g;
+}
+
+void layernorm_bwd(const void* dy, const void* h, const void* w, const float* mean, const float* rstd,
+                   const void* dres, void* dx, float* dw_partial, float* db_partial, float* dw, float* db, int T,
+                   int H, cudaStream_t s) {
+  if (H % 8 != 0) throw std::runtime_error("layernorm: hidden size must be a multiple of 8");
+  const int grid = layernorm_bwd_grid(T, H);
+  auto DY = (const __nv_bfloat16*)dy;
+  auto HH = (const __nv_bfloat16*)h;
+  auto W = (const __nv_bfloat16*)w;
+  auto DR = (const __nv_bfloat16*)dres;
+  auto DX = (__nv_bfloat16*)dx;
+#define CALL_LN_BWD(NV, NT)                                                                                         \
+  if (dres)                                                                                                         \
+    layernorm_bwd_kernel<NV, NT, true><<<grid, NT, 0, s>>>(DY, HH, W, mean, rstd, DR, DX, dw_partial, db_partial, T, H); \
+  else                                                                                                              \
+    layernorm_bwd_kernel<NV, NT, false><<<grid, NT, 0, s>>>(DY, HH, W, mean, rstd, nullptr, DX, dw_partial, db_partial, T, H);
+  DTG_LN_BWD_DISPATCH(H, CALL_LN_BWD);
+#undef CALL_LN_BWD
+  colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(dw_partial, dw, grid, H);
+  colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(db_partial, db, grid, H);
+  note_launch(3);
+  DTG_LAUNCH_CHECK();
+}
+
+// ------------------------------------------------------------------------------------------
+// GELU, tanh approximation (StarCoder2's gelu_pytorch_tanh), elementwise on the c_fc output:
+//   y = 0.5 x (1 + tanh(k (x + 0.044715 x^3))),  k = sqrt(2/pi)
+// fp32 math in ATen's operation order with tanhf (not tanh.approx) and one rounding.  The backward is ATen's too,
+// except that the sech^2 term is taken as 0 where tanh has saturated, where ATen's 0 * (1 + 3 * 0.044715 * x^2)
+// becomes NaN once x^2 overflows.
+// ------------------------------------------------------------------------------------------
+constexpr float kGeluBeta = 0.7978845608028654f, kGeluKappa = 0.044715f;
+
+__global__ void gelu_tanh_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
+                                     long long nvec) {
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < nvec;
+       idx += (long long)gridDim.x * blockDim.x) {
+    float f[8], o[8];
+    unpack8(ld8(x + idx * 8), f);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float cube = f[j] * f[j] * f[j];
+      const float inner = kGeluBeta * (f[j] + kGeluKappa * cube);
+      o[j] = 0.5f * f[j] * (1.f + tanhf(inner));
+    }
+    st8(y + idx * 8, pack8(o));
+  }
+}
+
+__global__ void gelu_tanh_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                                     __nv_bfloat16* __restrict__ dx, long long nvec) {
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < nvec;
+       idx += (long long)gridDim.x * blockDim.x) {
+    float f[8], d[8], o[8];
+    unpack8(ld8(x + idx * 8), f);
+    unpack8(ld8(dy + idx * 8), d);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float sq = f[j] * f[j];
+      const float cube = sq * f[j];
+      const float t = tanhf(kGeluBeta * (f[j] + kGeluKappa * cube));
+      const float left = 0.5f * f[j];
+      const float right = 1.f + t;
+      const float sech2 = 1.f - t * t;
+      const float right_d = sech2 == 0.f ? 0.f : left * sech2 * kGeluBeta * (1.f + 3.f * kGeluKappa * sq);
+      o[j] = d[j] * (0.5f * right + right_d);
+    }
+    st8(dx + idx * 8, pack8(o));
+  }
+}
+
+static int ew_grid(long long total_threads);
+
+void gelu_tanh_fwd(const void* x, void* y, long long n, cudaStream_t s) {
+  if (n % 8 != 0) throw std::runtime_error("gelu_tanh: the element count must be a multiple of 8");
+  gelu_tanh_fwd_kernel<<<ew_grid(n / 8), 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, n / 8);
+  note_launch();
+  DTG_LAUNCH_CHECK();
+}
+
+void gelu_tanh_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t s) {
+  if (n % 8 != 0) throw std::runtime_error("gelu_tanh: the element count must be a multiple of 8");
+  gelu_tanh_bwd_kernel<<<ew_grid(n / 8), 256, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
+                                                      (__nv_bfloat16*)dx, n / 8);
+  note_launch();
   DTG_LAUNCH_CHECK();
 }
 

@@ -5,7 +5,8 @@ guide uses (reference: every chapter's ``-m/--model-name`` flag, e.g.
 ``02-distributed-data-parallel/train_llm.py:57``) are resolved from this table
 instead of the hub.  A local directory containing a ``config.json`` is also
 accepted, and tiny ``debug-*`` configs exist for tests.  Families: Llama 2 / 3 / 3.1 / 3.2, Mistral, Qwen3, Qwen2.5,
-OLMo 2 (``allenai/OLMo-2-*``, ``model_type: "olmo2"``) and GPT-2.
+OLMo 2 (``allenai/OLMo-2-*``, ``model_type: "olmo2"``), StarCoder2 (``bigcode/starcoder2-*``,
+``model_type: "starcoder2"``) and GPT-2.
 """
 from __future__ import annotations
 
@@ -17,9 +18,11 @@ from typing import Optional
 
 @dataclasses.dataclass
 class ModelConfig:
-    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "olmo2" | "gpt2"; mistral is llama with a sliding attention
-    # window, qwen3 llama with QK-norm and a head_dim of its own, qwen2 llama with q/k/v biases, olmo2 llama with a
-    # full-width QK-norm and post-sublayer norms instead of the pre-norms (``full_qk_norm``, ``post_norm``)
+    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "olmo2" | "starcoder2" | "gpt2"; mistral is llama with a
+    # sliding attention window, qwen3 llama with QK-norm and a head_dim of its own, qwen2 llama with q/k/v biases,
+    # olmo2 llama with a full-width QK-norm and post-sublayer norms instead of the pre-norms (``full_qk_norm``,
+    # ``post_norm``), starcoder2 llama with LayerNorms, a GELU MLP and biases on every projection (``layer_norm``,
+    # ``gelu_mlp``, ``all_bias``)
     vocab_size: int
     hidden_size: int
     intermediate_size: int
@@ -40,7 +43,7 @@ class ModelConfig:
     qk_norm: bool = False
     #: q/k/v projection biases (Qwen2); o_proj and the MLP stay bias-free
     qkv_bias: bool = False
-    # gpt2 only
+    # gpt2 and starcoder2 (their LayerNorms' eps)
     layer_norm_epsilon: float = 1e-5
     dropout: float = 0.0
     name: str = ""
@@ -62,6 +65,21 @@ class ModelConfig:
         """OLMo 2's layer: no input_layernorm; h1 = h + norm(attn(h)), h2 = h1 + norm(mlp(h1))."""
         return self.arch == "olmo2"
 
+    @property
+    def layer_norm(self) -> bool:
+        """StarCoder2: LayerNorms with a gain and a bias (eps ``layer_norm_epsilon``) instead of the RMSNorms."""
+        return self.arch == "starcoder2"
+
+    @property
+    def gelu_mlp(self) -> bool:
+        """StarCoder2's MLP: c_fc -> GELU (tanh approximation) -> c_proj instead of SwiGLU's three matrices."""
+        return self.arch == "starcoder2"
+
+    @property
+    def all_bias(self) -> bool:
+        """StarCoder2: every projection (q, k, v, o, c_fc, c_proj) has a bias; the lm_head has none."""
+        return self.arch == "starcoder2"
+
     def num_parameters(self) -> int:
         h, i, v, l = self.hidden_size, self.intermediate_size, self.vocab_size, self.num_hidden_layers
         if self.arch == "gpt2":
@@ -69,6 +87,10 @@ class ModelConfig:
             return v * h + self.max_position_embeddings * h + l * per_layer + 2 * h
         q = self.num_attention_heads * self.head_dim
         kv = self.num_key_value_heads * self.head_dim
+        if self.arch == "starcoder2":
+            per_layer = (h * q + q) + 2 * (kv * h + kv) + (q * h + h) + (h * i + i) + (i * h + h) + 4 * h
+            n = v * h + l * per_layer + 2 * h
+            return n if self.tie_word_embeddings else n + v * h
         per_layer = h * q + 2 * kv * h + q * h + 3 * h * i + 2 * h
         if self.qk_norm:
             per_layer += 2 * self.head_dim
@@ -134,6 +156,14 @@ def _olmo2(name, h, i, l, nh, nkv, v=100352, maxpos=4096):
     )
 
 
+def _starcoder2(name, h, i, l, nh, nkv, theta, tied, v=49152, maxpos=16384, window=4096):
+    return ModelConfig(
+        arch="starcoder2", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
+        num_attention_heads=nh, num_key_value_heads=nkv, max_position_embeddings=maxpos, rope_theta=theta,
+        tie_word_embeddings=tied, sliding_window=window, layer_norm_epsilon=1e-5, name=name,
+    )
+
+
 _GPT2 = ModelConfig(
     arch="gpt2", vocab_size=50257, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
     num_attention_heads=12, num_key_value_heads=12, max_position_embeddings=1024,
@@ -173,6 +203,15 @@ REGISTRY = {
     "allenai/OLMo-2-1124-7B": _olmo2("allenai/OLMo-2-1124-7B", 4096, 11008, 32, 32, 32),
     "allenai/OLMo-2-1124-13B": _olmo2("allenai/OLMo-2-1124-13B", 5120, 13824, 40, 40, 40),
     "allenai/OLMo-2-0325-32B": _olmo2("allenai/OLMo-2-0325-32B", 5120, 27648, 64, 40, 8),
+    # StarCoder2: LayerNorms, a GELU MLP, biases on every projection, sliding window 4096; head_dim 128 at every size.
+    # Shapes, RoPE theta, window, norm eps and max positions are those of the public config.json files as recalled
+    # when this table was written; no copy of those files was at hand to check them against.  transformers'
+    # Starcoder2Config defaults (the 3B shapes: 3072 / 12288 / 30 layers / 24:2 heads, vocab 49152, eps 1e-5, tied)
+    # agree with the 3B row.  The tie flags follow the published parameter counts: 3.03B and 7.17B are the tied
+    # counts of the 3B and 7B shapes, and about 16B (15.96B) the untied count of the 15B shape (tied would be 15.66B).
+    "bigcode/starcoder2-3b": _starcoder2("bigcode/starcoder2-3b", 3072, 12288, 30, 24, 2, 999999.4420358813, True),
+    "bigcode/starcoder2-7b": _starcoder2("bigcode/starcoder2-7b", 4608, 18432, 32, 36, 4, 1e6, True),
+    "bigcode/starcoder2-15b": _starcoder2("bigcode/starcoder2-15b", 6144, 24576, 40, 48, 4, 1e5, False),
     # tiny configs for tests / smoke runs (head_dim 128 so the sm_90a attention kernel applies)
     "debug-llama": _llama("debug-llama", 1024, 256, 512, 2, 2, 2, 2048, 1e4),
     "debug-llama-gqa": _llama("debug-llama-gqa", 1024, 512, 1024, 2, 4, 2, 2048, 5e5),
@@ -187,6 +226,8 @@ REGISTRY = {
     "debug-qwen2": _qwen2("debug-qwen2", 256, 512, 2, 4, 2, False, 1024, 2048),
     # 4 q heads and 2 k heads x 128 over a hidden size of 512: GQA, and a k norm narrower than the q norm
     "debug-olmo2": _olmo2("debug-olmo2", 512, 1024, 2, 4, 2, v=1024, maxpos=2048),
+    # 4 q heads and 2 kv heads x 128 over a hidden size of 512, tied, with StarCoder2's block
+    "debug-starcoder2": _starcoder2("debug-starcoder2", 512, 2048, 2, 4, 2, 1e5, True, v=1024, maxpos=2048),
     "debug-gpt2": dataclasses.replace(_GPT2, vocab_size=512, hidden_size=64, intermediate_size=256,
                                       num_hidden_layers=2, num_attention_heads=2, num_key_value_heads=2,
                                       max_position_embeddings=128, name="debug-gpt2"),
@@ -204,6 +245,8 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
             max_position_embeddings=d.get("n_positions", 1024), tie_word_embeddings=True,
             layer_norm_epsilon=d.get("layer_norm_epsilon", 1e-5), dropout=d.get("resid_pdrop", 0.1), name=name,
         )
+    if mt == "starcoder2":
+        return _starcoder2_from_hf_dict(d, name)
     if mt not in ("llama", "mistral", "qwen3", "qwen2", "olmo2"):
         raise ValueError(f"unsupported model_type {mt!r} in {name}")
     if mt == "olmo2":
@@ -271,6 +314,44 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
         rms_norm_eps=d.get("rms_norm_eps", 1e-5), rope_theta=theta, rope_scaling=scaling,
         tie_word_embeddings=d.get("tie_word_embeddings", False), sliding_window=window, name=name,
         arch=mt, explicit_head_dim=head_dim, qk_norm=mt == "qwen3", qkv_bias=mt == "qwen2",
+    )
+
+
+def _starcoder2_from_hf_dict(d: dict, name: str) -> ModelConfig:
+    """A ``Starcoder2Config`` payload.  Every setting the kernel path does not implement is refused, naming its key,
+    rather than dropped."""
+    if d.get("use_bias", True) is not True:
+        raise ValueError(f"{name}: use_bias is {d['use_bias']!r}; only StarCoder2 with biases on every projection "
+                         "is supported")
+    if d.get("hidden_act", "gelu_pytorch_tanh") != "gelu_pytorch_tanh":
+        raise ValueError(f"{name}: hidden_act is {d['hidden_act']!r}; only 'gelu_pytorch_tanh' is supported")
+    if d.get("norm_type", "layer_norm") != "layer_norm":
+        raise ValueError(f"{name}: norm_type is {d['norm_type']!r}; only 'layer_norm' is supported")
+    if d.get("mlp_type", "default") != "default":
+        raise ValueError(f"{name}: mlp_type is {d['mlp_type']!r}; only 'default' is supported")
+    rope = d.get("rope_parameters") if isinstance(d.get("rope_parameters"), dict) else d.get("rope_scaling")
+    if rope and (rope.get("rope_type") or rope.get("type") or "default") != "default":
+        key = "rope_parameters" if isinstance(d.get("rope_parameters"), dict) else "rope_scaling"
+        raise ValueError(f"{name}: {key} has type {rope.get('rope_type') or rope.get('type')!r}; only the default "
+                         "RoPE is supported for StarCoder2")
+    if d.get("head_dim") is not None and d["head_dim"] != d["hidden_size"] // d["num_attention_heads"]:
+        raise ValueError(f"{name}: head_dim {d['head_dim']} differs from hidden_size / num_attention_heads = "
+                         f"{d['hidden_size'] // d['num_attention_heads']}; only head_dim = hidden / heads is supported")
+    for key in ("attention_dropout", "residual_dropout", "embedding_dropout"):
+        if d.get(key, 0.0):
+            raise ValueError(f"{name}: {key} is {d[key]!r}; the kernel path has no dropout, set {key} to 0.0 to "
+                             "train without it")
+    theta = d.get("rope_theta", 1e4)
+    if isinstance(d.get("rope_parameters"), dict):  # transformers>=5 layout
+        theta = d["rope_parameters"].get("rope_theta", theta)
+    return ModelConfig(
+        arch="starcoder2", vocab_size=d["vocab_size"], hidden_size=d["hidden_size"],
+        intermediate_size=d["intermediate_size"], num_hidden_layers=d["num_hidden_layers"],
+        num_attention_heads=d["num_attention_heads"],
+        num_key_value_heads=d.get("num_key_value_heads", d["num_attention_heads"]),
+        max_position_embeddings=d.get("max_position_embeddings", 4096), rope_theta=theta,
+        tie_word_embeddings=d.get("tie_word_embeddings", True), sliding_window=d.get("sliding_window"),
+        layer_norm_epsilon=d.get("norm_epsilon", 1e-5), name=name,
     )
 
 
@@ -354,6 +435,17 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
             "rms_norm_eps": cfg.rms_norm_eps, "rope_theta": cfg.rope_theta, "hidden_act": "silu",
             "tie_word_embeddings": cfg.tie_word_embeddings, "attention_bias": False, "pad_token_id": None,
             "bos_token_id": None, "eos_token_id": 100257, "torch_dtype": "bfloat16",
+        }
+    if cfg.arch == "starcoder2":
+        d = {
+            "model_type": "starcoder2", "architectures": ["Starcoder2ForCausalLM"], "vocab_size": cfg.vocab_size,
+            "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size,
+            "num_hidden_layers": cfg.num_hidden_layers, "num_attention_heads": cfg.num_attention_heads,
+            "num_key_value_heads": cfg.num_key_value_heads, "max_position_embeddings": cfg.max_position_embeddings,
+            "norm_epsilon": cfg.layer_norm_epsilon, "rope_theta": cfg.rope_theta, "sliding_window": cfg.sliding_window,
+            "hidden_act": "gelu_pytorch_tanh", "use_bias": True, "tie_word_embeddings": cfg.tie_word_embeddings,
+            "attention_dropout": 0.0, "residual_dropout": 0.0, "embedding_dropout": 0.0, "bos_token_id": 0,
+            "eos_token_id": 0, "torch_dtype": "bfloat16",
         }
     if cfg.arch == "llama" and cfg.explicit_head_dim is not None:
         d["head_dim"] = cfg.explicit_head_dim

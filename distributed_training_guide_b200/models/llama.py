@@ -1,6 +1,7 @@
 """Llama-family causal LM built on the sm_90a op layer (Llama; Mistral: Llama plus a sliding attention window; Qwen3:
 Llama plus QK-norm, with a head_dim of its own; Qwen2: Llama plus q/k/v biases; OLMo 2: Llama with a full-width
-QK-norm and RMSNorms after each sublayer instead of before it, ``Olmo2DecoderLayer``).
+QK-norm and RMSNorms after each sublayer instead of before it, ``Olmo2DecoderLayer``; StarCoder2: Llama with
+LayerNorms, a c_fc -> GELU-tanh -> c_proj MLP and a bias on every projection, ``Starcoder2DecoderLayer``).
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
 the reference instantiates at e.g. ``02-distributed-data-parallel/train_llm.py:57-58``)
@@ -9,7 +10,8 @@ so checkpoints keep meaningful keys: ``model.embed_tokens.weight``,
 {gate,up,down}_proj.weight``, ``...{input,post_attention}_layernorm.weight``,
 ``model.norm.weight``, ``lm_head.weight``; Qwen3 adds ``...self_attn.{q,k}_norm.weight``, Qwen2
 ``...self_attn.{q,k,v}_proj.bias``; OLMo 2 has ``...self_attn.{q,k}_norm.weight`` ([nh*d], [nkv*d]) and
-``...post_{attention,feedforward}_layernorm.weight`` and no ``input_layernorm``.
+``...post_{attention,feedforward}_layernorm.weight`` and no ``input_layernorm``; StarCoder2 ``...mlp.{c_fc,c_proj}.{weight,bias}``,
+``...self_attn.{q,k,v,o}_proj.bias`` and a ``.bias`` beside every norm gain.
 
 What is *different* from the HF module code (SURVEY.md §3.2) is the execution plan:
   * q/k/v (and gate/up) projections run as ONE wgmma GEMM over a fused weight that is
@@ -109,6 +111,25 @@ class RMSNorm(nn.Module):
         nn.init.ones_(self.weight)
 
 
+class LayerNorm(nn.Module):
+    """LayerNorm with a gain ``weight`` and a ``bias`` (HF names), StarCoder2's norm."""
+
+    def __init__(self, hidden, eps, dtype=None, device=None):
+        super().__init__()
+        self.eps = eps
+        self.weight = nn.Parameter(torch.ones(hidden, dtype=dtype, device=device))
+        self.bias = nn.Parameter(torch.zeros(hidden, dtype=dtype, device=device))
+
+    def forward(self, x, residual=None):
+        if residual is None:
+            return ops.layer_norm(x, self.weight, self.bias, self.eps), x
+        return ops.add_layer_norm(x, residual, self.weight, self.bias, self.eps)
+
+    def reset_parameters(self):
+        nn.init.ones_(self.weight)
+        nn.init.zeros_(self.bias)
+
+
 class Embedding(nn.Module):
     def __init__(self, n, dim, dtype=None, device=None):
         super().__init__()
@@ -154,11 +175,13 @@ class LlamaAttention(nn.Module):
         self.head_dim = d
         #: sliding-window attention (Mistral): None, or W >= 1 with query q seeing keys k > q - W only
         self.sliding_window = config.sliding_window
-        #: q/k/v biases (Qwen2), split with their heads under tensor parallelism
-        self.q_proj = Linear(h, self.num_heads * d, dtype, device, bias=config.qkv_bias)
-        self.k_proj = Linear(h, self.num_kv_heads * d, dtype, device, bias=config.qkv_bias)
-        self.v_proj = Linear(h, self.num_kv_heads * d, dtype, device, bias=config.qkv_bias)
-        self.o_proj = Linear(self.num_heads * d, h, dtype, device)
+        #: q/k/v biases (Qwen2, StarCoder2), split with their heads under tensor parallelism; an o_proj bias
+        #: (StarCoder2) only without it
+        qkv_bias = config.qkv_bias or config.all_bias
+        self.q_proj = Linear(h, self.num_heads * d, dtype, device, bias=qkv_bias)
+        self.k_proj = Linear(h, self.num_kv_heads * d, dtype, device, bias=qkv_bias)
+        self.v_proj = Linear(h, self.num_kv_heads * d, dtype, device, bias=qkv_bias)
+        self.o_proj = Linear(self.num_heads * d, h, dtype, device, bias=config.all_bias)
         #: QK-norm (Qwen3): [head_dim] gains, replicated under tensor parallelism (every rank normalises its heads)
         self.q_norm = RMSNorm(d, config.rms_norm_eps, dtype, device) if config.qk_norm else None
         self.k_norm = RMSNorm(d, config.rms_norm_eps, dtype, device) if config.qk_norm else None
@@ -189,6 +212,16 @@ class LlamaMLP(nn.Module):
         self.gate_proj = Linear(h, i // tp_size, dtype, device)
         self.up_proj = Linear(h, i // tp_size, dtype, device)
         self.down_proj = Linear(i // tp_size, h, dtype, device)
+
+
+class Starcoder2MLP(nn.Module):
+    """StarCoder2's MLP: ``c_proj(gelu_tanh(c_fc(x)))``, both projections with a bias."""
+
+    def __init__(self, config: ModelConfig, dtype=None, device=None):
+        super().__init__()
+        h, i = config.hidden_size, config.intermediate_size
+        self.c_fc = Linear(h, i, dtype, device, bias=True)
+        self.c_proj = Linear(i, h, dtype, device, bias=True)
 
 
 class FusedWeight:
@@ -325,6 +358,52 @@ class Olmo2DecoderLayer(LlamaDecoderLayer):
         return ops.rms_norm_add(down, h1, n.weight, n.eps), None
 
 
+class Starcoder2DecoderLayer(LlamaDecoderLayer):
+    """StarCoder2's layer: the Llama layer with LayerNorms, a c_fc -> GELU-tanh -> c_proj MLP and a bias on every
+    projection.  The residual add stays deferred: the layer returns ``(c_proj_out, h)``."""
+
+    #: matrices first (FSDP's chunked layout; ``FUSED``'s q|k|v), then the norm gains and biases, then the adjacent
+    #: q|k|v biases (one 1-D view, ``fused_view_1d``), then the o_proj, c_fc and c_proj biases
+    FLAT_ORDER = LlamaDecoderLayer.FLAT_ORDER[:4] + (
+        "mlp.c_fc.weight", "mlp.c_proj.weight", "input_layernorm.weight", "input_layernorm.bias",
+        "post_attention_layernorm.weight", "post_attention_layernorm.bias",
+    ) + LlamaDecoderLayer.QKV_BIAS_ORDER + ("self_attn.o_proj.bias", "mlp.c_fc.bias", "mlp.c_proj.bias")
+    FUSED = {"qkv": FLAT_ORDER[0:3]}
+
+    def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
+        nn.Module.__init__(self)
+        assert tp_size == 1, "StarCoder2 layers are not tensor-parallel"
+        self.layer_idx = layer_idx
+        self.self_attn = LlamaAttention(config, dtype, device)   # q, k, v and o with biases (``all_bias``)
+        h = config.hidden_size
+        self.mlp = Starcoder2MLP(config, dtype, device)
+        self.input_layernorm = LayerNorm(h, config.layer_norm_epsilon, dtype, device)
+        self.post_attention_layernorm = LayerNorm(h, config.layer_norm_epsilon, dtype, device)
+        self.flat_order = self.FLAT_ORDER
+        self._fused = {}
+        self.tp = None
+        self.fp8 = False
+
+    def forward(self, x, residual, cos, sin, doc_start=None):
+        att = self.self_attn
+        B, S, _ = x.shape
+        fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
+        y, h = self.input_layernorm(x, residual)
+        w, owner = self._qkv_weight()
+        b, b_owner = self._qkv_bias()
+        qkv = fused_linear(y, w, owner, b, b_owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
+        qkv = att.position_qk_(qkv, cos, sin)
+        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
+        a = a.reshape(B, S, att.num_heads * att.head_dim)
+        a = ops.fp8_linear(a, att.o_proj.weight, None, att.o_proj.bias) if self.fp8 else att.o_proj(a)
+        y, h = self.post_attention_layernorm(a, h)
+        mlp = self.mlp
+        up = ops.fp8_linear(y, mlp.c_fc.weight, None, mlp.c_fc.bias) if self.fp8 else mlp.c_fc(y)
+        act = ops.gelu_tanh(up)
+        down = ops.fp8_linear(act, mlp.c_proj.weight, None, mlp.c_proj.bias) if self.fp8 else mlp.c_proj(act)
+        return down, h
+
+
 class LlamaModel(nn.Module):
     def __init__(self, config: ModelConfig, dtype=None, device=None, tp_size=1):
         super().__init__()
@@ -332,11 +411,15 @@ class LlamaModel(nn.Module):
         # tensor parallel: the table is sharded over the hidden dimension (reference: ColwiseParallel on
         # nn.Embedding, 06-tensor-parallel/train_llm.py:82)
         self.embed_tokens = Embedding(config.vocab_size, config.hidden_size // tp_size, dtype, device)
-        layer_cls = Olmo2DecoderLayer if config.post_norm else LlamaDecoderLayer
+        layer_cls = (Olmo2DecoderLayer if config.post_norm else
+                     Starcoder2DecoderLayer if config.arch == "starcoder2" else LlamaDecoderLayer)
         self.layers = nn.ModuleList(
             [layer_cls(config, i, dtype, device, tp_size) for i in range(config.num_hidden_layers)]
         )
-        self.norm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
+        if config.layer_norm:
+            self.norm = LayerNorm(config.hidden_size, config.layer_norm_epsilon, dtype, device)
+        else:
+            self.norm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
         self.rotary_emb = RotaryEmbedding(config)
 
 

@@ -4,7 +4,8 @@ On CUDA tensors each op calls a hand-written sm_90a kernel from the in-tree
 extension (``csrc/``): wgmma/TMA GEMM (fwd / dgrad / wgrad) in bf16 and, for
 ``fp8_linear``, in fp8 with its amax and cast-transpose kernels, wgmma
 flash-attention, fused residual-add+RMSNorm and norm-then-add (OLMo 2), in-place RoPE on the fused qkv buffer
-(after Qwen3's per-head or OLMo 2's full-width QK-norm in the same kernel), SwiGLU, in-place
+(after Qwen3's per-head or OLMo 2's full-width QK-norm in the same kernel), SwiGLU, fused residual-add+LayerNorm
+and GELU-tanh (StarCoder2), in-place
 softmax-cross-entropy, embedding gather / scatter-add and flat AdamW.  On CPU tensors the same Functions run the reference math in
 ``ops/reference.py`` (chapter 01's CPU config and the gloo tests).
 
@@ -28,7 +29,8 @@ from . import reference as ref
 
 __all__ = [
     "linear", "fused_linear", "rms_norm", "add_rms_norm", "rms_norm_add", "rope_qkv_", "qk_norm_rope_",
-    "olmo_qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy",
+    "olmo_qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy", "layer_norm",
+    "add_layer_norm", "gelu_tanh",
     "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "bias_grad", "ref",
 ]
 
@@ -407,6 +409,97 @@ def rms_norm_add(x, r, w, eps):
     if _ext.use_cuda_kernel("rmsnorm", x, r, w) and x.dtype == torch.bfloat16:
         return _RMSNormAdd.apply(x.contiguous(), r.contiguous(), w, eps)
     return ref.rms_norm_add(x, r, w, eps)
+
+
+# --------------------------------------------------------------------------------------
+# LayerNorm (+ fused residual add), StarCoder2
+# --------------------------------------------------------------------------------------
+class _LayerNorm(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w, b, eps):
+        C = _ext.load()
+        x2 = x.reshape(-1, x.shape[-1])
+        y, _, mean, rstd = C.layernorm_fwd(x2, None, w, b, float(eps))
+        ctx.save_for_backward(x2, w, mean, rstd)
+        ctx.shape = x.shape
+        ctx.params = (w, b)
+        return y.view(x.shape)
+
+    @staticmethod
+    def backward(ctx, dy):
+        C = _ext.load()
+        x2, w, mean, rstd = ctx.saved_tensors
+        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
+        dx, dw32, db32 = C.layernorm_bwd(dy2, x2, w, mean, rstd, None)
+        dw = _emit_weight_grad(ctx.params[0], _norm_dw_into(dw32), w)
+        db = _emit_weight_grad(ctx.params[1], _norm_dw_into(db32), ctx.params[1])
+        return dx.view(ctx.shape), dw, db, None
+
+
+class _AddLayerNorm(torch.autograd.Function):
+    """(y, h) = (layernorm(x + r) * w + b, x + r) in one pass over the activations."""
+
+    @staticmethod
+    def forward(ctx, x, r, w, b, eps):
+        C = _ext.load()
+        x2 = x.reshape(-1, x.shape[-1])
+        y, h, mean, rstd = C.layernorm_fwd(x2, r.reshape(-1, r.shape[-1]), w, b, float(eps))
+        ctx.save_for_backward(h, w, mean, rstd)
+        ctx.shape = x.shape
+        ctx.params = (w, b)
+        return y.view(x.shape), h.view(x.shape)
+
+    @staticmethod
+    def backward(ctx, dy, dh):
+        C = _ext.load()
+        h, w, mean, rstd = ctx.saved_tensors
+        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
+        dh2 = dh.reshape(-1, dh.shape[-1]).contiguous() if dh is not None else None
+        # dx = layernorm_bwd(dy) + dh : the gradient of both x and r (h = x + r)
+        dx, dw32, db32 = C.layernorm_bwd(dy2, h, w, mean, rstd, dh2)
+        dw = _emit_weight_grad(ctx.params[0], _norm_dw_into(dw32), w)
+        db = _emit_weight_grad(ctx.params[1], _norm_dw_into(db32), ctx.params[1])
+        dx = dx.view(ctx.shape)
+        return dx, dx, dw, db, None
+
+
+def layer_norm(x, w, b, eps):
+    """``y = (x - mean) * rsqrt(var + eps) * w + b`` over the last dimension with fp32 statistics and one rounding
+    (ATen's bf16 ``layer_norm``).  bf16 CUDA tensors run the sm_90a kernels; the gain and bias gradients go through
+    ``_emit_weight_grad`` (overwrite on the first write of a step, accumulate after it)."""
+    if _ext.use_cuda_kernel("layernorm", x, w, b) and x.dtype == torch.bfloat16:
+        return _LayerNorm.apply(x.contiguous(), w, b, eps)
+    return ref.layer_norm(x, w, b, eps)
+
+
+def add_layer_norm(x, residual, w, b, eps):
+    """Fused ``h = x + residual; y = layer_norm(h, w, b)`` -> (y, h), with ``h`` rounded to the input dtype before it
+    is normalised."""
+    if _ext.use_cuda_kernel("layernorm", x, residual, w, b) and x.dtype == torch.bfloat16:
+        return _AddLayerNorm.apply(x.contiguous(), residual.contiguous(), w, b, eps)
+    h = x + residual
+    return ref.layer_norm(h, w, b, eps), h
+
+
+class _GeluTanh(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        ctx.save_for_backward(x)
+        return _ext.load().gelu_tanh_fwd(x)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        return _ext.load().gelu_tanh_bwd(dy.contiguous(), x)
+
+
+def gelu_tanh(x):
+    """GELU with the tanh approximation (``F.gelu(x, approximate="tanh")``, StarCoder2's ``gelu_pytorch_tanh``) in
+    fp32 with one rounding.  bf16 CUDA tensors run the sm_90a kernels, which keep the pre-activation for the
+    backward."""
+    if _ext.use_cuda_kernel("gelu", x) and x.dtype == torch.bfloat16:
+        return _GeluTanh.apply(x.contiguous())
+    return ref.gelu_new(x.float()).to(x.dtype)
 
 
 # --------------------------------------------------------------------------------------

@@ -43,6 +43,12 @@ def rms_norm_add(x, r, w, eps):
     return r + rms_norm_one_rounding(x, w, eps)
 
 
+def layer_norm(x, w, b, eps):
+    """LayerNorm over the last dimension in fp32 with one rounding to ``x.dtype`` (what ATen's bf16 ``layer_norm`` and
+    the layernorm kernels compute): ``((x - mean) * rsqrt(var + eps) * w + b).to(x.dtype)``, biased variance."""
+    return F.layer_norm(x.float(), (x.shape[-1],), w.float(), b.float(), eps).to(x.dtype)
+
+
 def add_rms_norm(x, residual, w, eps):
     """returns (normed, new_residual) with new_residual = x + residual."""
     h = x + residual

@@ -119,11 +119,11 @@ class FlatGroup:
 
 
 def install_fused_views(layer, g: FlatGroup, i: int):
-    """Give decoder layer ``i`` its fused weights (q|k|v, gate|up) and, with q/k/v biases, the fused q|k|v bias, as
-    views of its flat group ``g``."""
+    """Give decoder layer ``i`` its fused weights (its class's ``FUSED``: q|k|v, and gate|up where the layer has
+    one) and, with q/k/v biases, the fused q|k|v bias, as views of its flat group ``g``."""
     from ..models.llama import FusedWeight, LlamaDecoderLayer
 
-    for fname, members in LlamaDecoderLayer.FUSED.items():
+    for fname, members in type(layer).FUSED.items():
         data, grad = g.fused_view([f"model.layers.{i}.{m}" for m in members])
         layer._fused[fname] = g.fused[fname] = FusedWeight(data, grad)
     if layer.self_attn.q_proj.bias is not None:

@@ -153,7 +153,7 @@ class FSDPEngine:
                 assert set(named) == set(layer.flat_order), f"layer {i}: parameters outside flat_order"
                 layer_named.append([(f"model.layers.{i}.{n}", named[n]) for n in layer.flat_order])
             embed_named = [("model.embed_tokens.weight", core.embed_tokens.weight)]
-            head_named = [("model.norm.weight", core.norm.weight)]
+            head_named = [(f"model.norm.{n}", p) for n, p in core.norm.named_parameters()]   # gain (+ bias)
             if not self.tied:  # a tied lm_head IS the embedding parameter (it lives in the embed group)
                 head_named.insert(0, ("lm_head.weight", model.lm_head.weight))  # matrix first: chunk-aligned
             default_init = lambda p, n: init_parameter_(p, n, seed)  # noqa: E731
@@ -278,6 +278,7 @@ class FSDPEngine:
         def spec(g, holder, off, numel, rows, cols):
             holder._dtg_gather = _GatherSpec(self, g, off, numel, rows, cols)
 
+        fused_of = {l._flat_group.name: type(l).FUSED for l in self.layers}   # each layer's own fused weights
         for g in self.groups:
             g._gathered, g._full_now = set(), False
             if not g.chunk_bytes:
@@ -289,7 +290,7 @@ class FSDPEngine:
             for fname, fw in g.fused.items():
                 if fw.data.dim() != 2:   # the fused q|k|v bias (Qwen2): 1-D, it lives in the prefetched tail
                     continue
-                members = [n for n in g.names if any(n.endswith(m) for m in LlamaDecoderLayer.FUSED[fname])]
+                members = [n for n in g.names if any(n.endswith(m) for m in fused_of[g.name][fname])]
                 off = by_name[members[0]][1]
                 rows = sum(by_name[n][2][0] for n in members)
                 cols = by_name[members[0]][2][1]

@@ -431,6 +431,11 @@ class TwoDParallel(Strategy):
                 f"{config.name or config.arch}: tensor parallelism does not support the full-width q/k norm (OLMo 2): "
                 "its statistic spans the q (k) heads that tensor parallelism splits across ranks; train it with the "
                 "single-GPU, DDP or FSDP engines (chapters 01, 02, 04, 05)")
+        if getattr(config, "all_bias", False):
+            raise ValueError(
+                f"{config.name or config.arch}: tensor parallelism does not support biases on the row-parallel "
+                "o_proj / c_proj (StarCoder2): they must be added once after the reduction, which the tensor-parallel "
+                "layer path does not do; train it with the single-GPU, DDP or FSDP engines (chapters 01, 02, 04, 05)")
         cuda = env.device.type == "cuda"
         seed = getattr(args, "seed", 0)
         use_fsdp = mesh.dp_size > 1
