@@ -17,8 +17,10 @@ void rmsnorm_add_fwd(const void* x, const void* res, const void* w, void* h_out,
 int rmsnorm_bwd_grid(int T);
 void rmsnorm_bwd(const void* dy, const void* h, const void* w, const float* rstd, const void* dres, void* dx,
                  float* dw_partial, float* dw, int T, int H, cudaStream_t s);
+// rotates the first rot_dim elements (rot_dim % 16 == 0, <= d; d for the full head) of heads [0, n_rot); cos/sin
+// [S, rot_dim/2] or [T, rot_dim/2]
 void rope_inplace(void* qkv, const float* cos, const float* sin, long long T, int S, int n_heads, int n_rot, int d,
-                  bool per_token, bool inverse, cudaStream_t s);
+                  int rot_dim, bool per_token, bool inverse, cudaStream_t s);
 // out[c] = sum over rows r of partial[r][c] (fp32 [rows, H]), in a fixed order
 void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s);
 // bias gradient: db[n] = sum over t of dy[t, n], dy bf16 [T, N] with row stride ld (elements); N, ld multiples of 8.
@@ -39,6 +41,20 @@ void layernorm_bwd(const void* dy, const void* h, const void* w, const float* me
 // GELU with the tanh approximation on n bf16 elements (n % 8 == 0); the backward from the saved pre-activation x
 void gelu_tanh_fwd(const void* x, void* y, long long n, cudaStream_t s);
 void gelu_tanh_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t s);
+// GELU, exact erf form, likewise
+void gelu_fwd(const void* x, void* y, long long n, cudaStream_t s);
+void gelu_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t s);
+// Two LayerNorms over one residual stream (GPT-NeoX): h_out = bf16(x + res) when res is given (else h = x), one mean
+// and rstd [T] fp32, y1 = bf16(xhat * w1 + b1), y2 = bf16(xhat * w2 + b2).  H % 8 == 0, H <= 8192.
+void layernorm2_fwd(const void* x, const void* res, const void* w1, const void* b1, const void* w2, const void* b2,
+                    void* y1, void* y2, void* h_out, float* mean, float* rstd, int T, int H, float eps,
+                    cudaStream_t s);
+int layernorm2_bwd_grid(int T, int H);
+// dx = the backward of both norms (+ dres); dparams [4, H] fp32 = dw1, db1, dw2, db2, summed through partial
+// ([4, layernorm2_bwd_grid(T, H), H] fp32 scratch) in a fixed order
+void layernorm2_bwd(const void* dy1, const void* dy2, const void* h, const void* w1, const void* w2, const float* mean,
+                    const float* rstd, const void* dres, void* dx, float* partial, float* dparams, int T, int H,
+                    cudaStream_t s);
 void swiglu_fwd(const void* gu, void* h, long long T, int I, cudaStream_t s);
 void swiglu_bwd(const void* dh, const void* gu, void* dgu, long long T, int I, cudaStream_t s);
 void embedding_fwd(const long long* ids, const void* w, void* out, long long T, int H, cudaStream_t s);

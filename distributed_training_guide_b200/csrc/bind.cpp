@@ -289,20 +289,124 @@ Tensor gelu_tanh_bwd(const Tensor& dy, const Tensor& x) {
   return dx;
 }
 
-void rope_inplace(Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t n_rot, bool inverse) {
-  // qkv: [B, S, heads, d] contiguous; cos/sin fp32 [S, d/2] or [B, S, d/2]
+void rope_inplace(Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t n_rot, bool inverse,
+                  const c10::optional<int64_t>& rot_dim_arg) {
+  // qkv: [B, S, heads, d] contiguous; cos/sin fp32 [S, rot_dim/2] or [B, S, rot_dim/2]; rot_dim defaults to d
   check_vec(qkv, "qkv", at::kBFloat16);
   check_vec(cos, "cos", at::kFloat);
   check_vec(sin, "sin", at::kFloat);
   TORCH_CHECK(qkv.dim() == 4, "qkv must be [B,S,heads,d]");
   const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1), NH = qkv.size(2), d = qkv.size(3);
+  const int64_t rot_dim = rot_dim_arg.has_value() ? *rot_dim_arg : d;
+  TORCH_CHECK(rot_dim > 0 && rot_dim <= d && rot_dim % 16 == 0,
+              "rope: rot_dim must be a positive multiple of 16 and <= head_dim ", d, ", got ", rot_dim);
   const bool per_token = cos.dim() == 3;
-  TORCH_CHECK(cos.size(-1) == d / 2 && cos.size(per_token ? 1 : 0) == S, "cos/sin table has the wrong shape");
+  TORCH_CHECK(cos.size(-1) == rot_dim / 2 && cos.size(per_token ? 1 : 0) == S, "cos/sin table has the wrong shape");
   TORCH_CHECK(sin.sizes() == cos.sizes(), "cos and sin differ in shape");
   TORCH_CHECK(n_rot >= 0 && n_rot <= NH, "rope: n_rot must be within [0, heads]");
   dtg::rope_inplace(qkv.data_ptr(), cos.data_ptr<float>(), sin.data_ptr<float>(), B * S, (int)S, (int)NH, (int)n_rot,
-                    (int)d, per_token, inverse, stream());
+                    (int)d, (int)rot_dim, per_token, inverse, stream());
+}
+
+Tensor gelu_fwd(const Tensor& x) {
+  check_vec(x, "x", at::kBFloat16);
+  TORCH_CHECK(x.numel() % 8 == 0, "gelu_fwd: x must have a multiple of 8 elements, got ", x.numel());
+  const c10::cuda::CUDAGuard guard(x.device());
+  Tensor y = torch::empty_like(x);
+  if (x.numel() > 0) dtg::gelu_fwd(x.data_ptr(), y.data_ptr(), x.numel(), stream());
+  return y;
+}
+
+Tensor gelu_bwd(const Tensor& dy, const Tensor& x) {
+  check_vec(dy, "dy", at::kBFloat16);
+  check_vec(x, "x", at::kBFloat16);
+  TORCH_CHECK(dy.sizes() == x.sizes() && dy.device() == x.device(), "gelu_bwd: dy and x differ in shape or device");
+  TORCH_CHECK(x.numel() % 8 == 0, "gelu_bwd: x must have a multiple of 8 elements, got ", x.numel());
+  const c10::cuda::CUDAGuard guard(x.device());
+  Tensor dx = torch::empty_like(x);
+  if (x.numel() > 0) dtg::gelu_bwd(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), x.numel(), stream());
+  return dx;
+}
+
+// Checks of the dual LayerNorm: x (or dy1) bf16 [T, H] with H % 8 == 0 and H <= 8192, and [H] bf16 gains / biases
+// on its device; returns H.
+int64_t check_layernorm2(const Tensor& x, const char* xname, std::initializer_list<std::pair<const Tensor*, const char*>> params,
+                         const char* who) {
+  check_vec(x, xname, at::kBFloat16);
+  TORCH_CHECK(x.dim() == 2, who, ": ", xname, " must be 2-D [T, H]");
+  const int64_t H = x.size(1);
+  TORCH_CHECK(H % 8 == 0 && H > 0 && H <= 8192, who, ": hidden size must be a positive multiple of 8 and <= 8192, got ",
+              H);
+  for (const auto& p : params) {
+    check_vec(*p.first, p.second, at::kBFloat16);
+    TORCH_CHECK(p.first->dim() == 1 && p.first->size(0) == H, who, ": ", p.second, " must be [H] = [", H, "]");
+    TORCH_CHECK(p.first->device() == x.device(), who, ": ", p.second, " must be on the device of ", xname);
+  }
+  return H;
+}
+
+// (y1, y2, h or None, mean, rstd): h = bf16(x + residual) when a residual is given, y_i = LayerNorm(h) * w_i + b_i
+std::tuple<Tensor, Tensor, c10::optional<Tensor>, Tensor, Tensor> layernorm2_fwd(
+    const Tensor& x, const c10::optional<Tensor>& res, const Tensor& w1, const Tensor& b1, const Tensor& w2,
+    const Tensor& b2, double eps) {
+  const int64_t H = check_layernorm2(x, "x", {{&w1, "w1"}, {&b1, "b1"}, {&w2, "w2"}, {&b2, "b2"}}, "layernorm2_fwd");
+  TORCH_CHECK(std::isfinite(eps) && eps > 0, "layernorm2_fwd: eps must be finite and > 0, got ", eps);
+  const void* rp = nullptr;
+  if (res.has_value()) {
+    check_vec(*res, "residual", at::kBFloat16);
+    TORCH_CHECK(res->sizes() == x.sizes(), "layernorm2_fwd: residual and x differ in shape");
+    TORCH_CHECK(res->device() == x.device(), "layernorm2_fwd: residual must be on the device of x");
+    rp = res->data_ptr();
+  }
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int64_t T = x.size(0);
+  Tensor y1 = torch::empty_like(x), y2 = torch::empty_like(x);
+  Tensor mean = torch::empty({T}, x.options().dtype(at::kFloat));
+  Tensor rstd = torch::empty({T}, x.options().dtype(at::kFloat));
+  c10::optional<Tensor> h;
+  if (rp) h = torch::empty_like(x);
+  if (T > 0)
+    dtg::layernorm2_fwd(x.data_ptr(), rp, w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), b2.data_ptr(), y1.data_ptr(),
+                        y2.data_ptr(), h ? h->data_ptr() : nullptr, mean.data_ptr<float>(), rstd.data_ptr<float>(),
+                        (int)T, (int)H, (float)eps, stream());
+  return {y1, y2, h, mean, rstd};
+}
+
+// (dx, dparams fp32 [4, H] = dw1, db1, dw2, db2) of the two LayerNorms, with dx += dres when dres is given
+std::tuple<Tensor, Tensor> layernorm2_bwd(const Tensor& dy1, const Tensor& dy2, const Tensor& h, const Tensor& w1,
+                                          const Tensor& w2, const Tensor& mean, const Tensor& rstd,
+                                          const c10::optional<Tensor>& dres) {
+  const int64_t H = check_layernorm2(dy1, "dy1", {{&w1, "w1"}, {&w2, "w2"}}, "layernorm2_bwd");
+  for (const Tensor* t : {&dy2, &h}) {
+    const char* name = t == &dy2 ? "dy2" : "h";
+    check_vec(*t, name, at::kBFloat16);
+    TORCH_CHECK(t->sizes() == dy1.sizes() && t->device() == dy1.device(), "layernorm2_bwd: ", name,
+                " and dy1 differ in shape or device");
+  }
+  const int64_t T = dy1.size(0);
+  for (const Tensor* t : {&mean, &rstd}) {
+    check_contig(*t, t == &mean ? "mean" : "rstd", at::kFloat);
+    TORCH_CHECK(t->dim() == 1 && t->size(0) == T && t->device() == dy1.device(), "layernorm2_bwd: ",
+                t == &mean ? "mean" : "rstd", " must be [T] = [", T, "] on the device of dy1");
+  }
+  const void* dr = nullptr;
+  if (dres.has_value()) {
+    check_vec(*dres, "dres", at::kBFloat16);
+    TORCH_CHECK(dres->sizes() == dy1.sizes() && dres->device() == dy1.device(),
+                "layernorm2_bwd: dres and dy1 differ in shape or device");
+    dr = dres->data_ptr();
+  }
+  const c10::cuda::CUDAGuard guard(dy1.device());
+  Tensor dx = torch::empty_like(dy1);
+  Tensor dparams = torch::zeros({4, H}, dy1.options().dtype(at::kFloat));
+  if (T > 0) {
+    Tensor partial = torch::empty({4, dtg::layernorm2_bwd_grid((int)T, (int)H), H}, dy1.options().dtype(at::kFloat));
+    dtg::layernorm2_bwd(dy1.data_ptr(), dy2.data_ptr(), h.data_ptr(), w1.data_ptr(), w2.data_ptr(),
+                        mean.data_ptr<float>(), rstd.data_ptr<float>(), dr, dx.data_ptr(), partial.data_ptr<float>(),
+                        dparams.data_ptr<float>(), (int)T, (int)H, stream());
+  }
+  return {dx, dparams};
 }
 
 // Shared checks of qk_norm_rope_fwd / _bwd and, with `full`, of the full-width qk_norm_full_rope_fwd / _bwd (gains
@@ -532,7 +636,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("gemm_max_active_clusters",[](int cg) { return dtg::gemm_max_active_clusters(cg); });
   m.def("rmsnorm_fwd", &rmsnorm_fwd);
   m.def("rmsnorm_bwd", &rmsnorm_bwd);
-  m.def("rope_inplace", &rope_inplace);
+  m.def("rope_inplace", &rope_inplace, py::arg("qkv"), py::arg("cos"), py::arg("sin"), py::arg("n_rot"),
+        py::arg("inverse"), py::arg("rot_dim") = py::none());
   m.def("qk_norm_rope_fwd", &qk_norm_rope_fwd);
   m.def("qk_norm_rope_bwd", &qk_norm_rope_bwd);
   m.def("rmsnorm_add_fwd", &rmsnorm_add_fwd);
@@ -552,6 +657,16 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   });
   m.def("gelu_tanh_fwd", &gelu_tanh_fwd, py::arg("x"));
   m.def("gelu_tanh_bwd", &gelu_tanh_bwd, py::arg("dy"), py::arg("x"));
+  m.def("gelu_fwd", &gelu_fwd, py::arg("x"));
+  m.def("gelu_bwd", &gelu_bwd, py::arg("dy"), py::arg("x"));
+  m.def("layernorm2_fwd", &layernorm2_fwd, py::arg("x"), py::arg("residual"), py::arg("w1"), py::arg("b1"),
+        py::arg("w2"), py::arg("b2"), py::arg("eps"));
+  m.def("layernorm2_bwd", &layernorm2_bwd, py::arg("dy1"), py::arg("dy2"), py::arg("h"), py::arg("w1"),
+        py::arg("w2"), py::arg("mean"), py::arg("rstd"), py::arg("dres") = py::none());
+  m.def("layernorm2_bwd_grid", [](int64_t T, int64_t H) {
+    TORCH_CHECK(T > 0 && H > 0 && H % 8 == 0 && H <= 8192, "layernorm2_bwd_grid: bad shape");
+    return dtg::layernorm2_bwd_grid((int)T, (int)H);
+  });
   m.def("swiglu_fwd", &swiglu_fwd);
   m.def("swiglu_bwd", &swiglu_bwd);
   m.def("cross_entropy_fwd_bwd", &cross_entropy_fwd_bwd);

@@ -608,6 +608,253 @@ void layernorm_bwd(const void* dy, const void* h, const void* w, const float* me
 }
 
 // ------------------------------------------------------------------------------------------
+// Two LayerNorms over one residual stream (GPT-NeoX's parallel residual):
+//   h = bf16(x (+ r));  y1 = bf16(xhat * w1 + b1),  y2 = bf16(xhat * w2 + b2),  xhat = (h - mean) * rstd
+// Both norms read the same h, so they share one mean and one rstd: one read of the row, three writes.  The statistic
+// (and its 2^-72 rescaled redo for rows whose sums overflow) and the normalisation are layernorm_fwd_kernel's,
+// operation for operation, so y1 and y2 are bit-identical to layernorm_fwd run with (w1, b1) and with (w2, b2).
+// ------------------------------------------------------------------------------------------
+template <int kMaxVec, int kNormThreads, bool HAS_RES>
+__global__ void __launch_bounds__(kNormThreads) layernorm2_fwd_kernel(
+    const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w1,
+    const __nv_bfloat16* __restrict__ b1, const __nv_bfloat16* __restrict__ w2, const __nv_bfloat16* __restrict__ b2,
+    __nv_bfloat16* __restrict__ y1, __nv_bfloat16* __restrict__ y2, __nv_bfloat16* __restrict__ h_out,
+    float* __restrict__ mean_out, float* __restrict__ rstd_out, int H, float eps) {
+  __shared__ float red[32];
+  const int row = blockIdx.x;
+  const int nvec = H >> 3;
+  const __nv_bfloat16* xr = x + (size_t)row * H;
+  const __nv_bfloat16* rr = HAS_RES ? r + (size_t)row * H : nullptr;
+  bf16x8 cache[kMaxVec];
+  float sum = 0.f;
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    const int i = threadIdx.x + k * kNormThreads;
+    if (i < nvec) {
+      bf16x8 v = ld8(xr + i * 8);
+      float f[8];
+      unpack8(v, f);
+      if (HAS_RES) {
+        float g[8];
+        unpack8(ld8(rr + i * 8), g);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) f[j] += g[j];
+        v = pack8(f);          // the residual stream is stored (and normalised) in bf16
+        unpack8(v, f);
+        st8(h_out + (size_t)row * H + i * 8, v);
+      }
+      cache[k] = v;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) sum += f[j];
+    }
+  }
+  float scale = 1.f;
+  float mean = block_sum(sum, red) / (float)H;
+  float ss = block_sum(ln_sq_dev<kMaxVec, kNormThreads>(cache, nvec, mean, 1.f), red);
+  if (!(isfinite(mean) && isfinite(ss))) {   // uniform over the CTA: block_sum broadcasts
+    scale = kLnDown;
+    mean = block_sum(ln_sum<kMaxVec, kNormThreads>(cache, nvec, kLnDown), red) / (float)H;
+    ss = block_sum(ln_sq_dev<kMaxVec, kNormThreads>(cache, nvec, mean, kLnDown), red);
+  }
+  const float rstd = rsqrtf(ss / (float)H + eps * scale * scale);
+  if (threadIdx.x == 0) {
+    mean_out[row] = scale == 1.f ? mean : mean * kLnUp;
+    rstd_out[row] = scale == 1.f ? rstd : rstd * kLnDown;
+  }
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    const int i = threadIdx.x + k * kNormThreads;
+    if (i < nvec) {
+      float f[8], g[8], c[8], o[8];
+      unpack8(cache[k], f);
+      unpack8(ld8(w1 + i * 8), g);
+      unpack8(ld8(b1 + i * 8), c);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[j] = (f[j] * scale - mean) * rstd * g[j] + c[j];
+      st8(y1 + (size_t)row * H + i * 8, pack8(o));
+      unpack8(ld8(w2 + i * 8), g);
+      unpack8(ld8(b2 + i * 8), c);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[j] = (f[j] * scale - mean) * rstd * g[j] + c[j];
+      st8(y2 + (size_t)row * H + i * 8, pack8(o));
+    }
+  }
+}
+
+void layernorm2_fwd(const void* x, const void* res, const void* w1, const void* b1, const void* w2, const void* b2,
+                    void* y1, void* y2, void* h_out, float* mean, float* rstd, int T, int H, float eps,
+                    cudaStream_t s) {
+  if (H % 8 != 0 || H > 8192) throw std::runtime_error("layernorm2: hidden size must be a multiple of 8, <= 8192");
+  auto X = (const __nv_bfloat16*)x;
+  auto R = (const __nv_bfloat16*)res;
+  auto W1 = (const __nv_bfloat16*)w1;
+  auto B1 = (const __nv_bfloat16*)b1;
+  auto W2 = (const __nv_bfloat16*)w2;
+  auto B2 = (const __nv_bfloat16*)b2;
+  auto Y1 = (__nv_bfloat16*)y1;
+  auto Y2 = (__nv_bfloat16*)y2;
+#define CALL_LN2_FWD(NV, NT)                                                                                      \
+  if (res)                                                                                                        \
+    layernorm2_fwd_kernel<NV, NT, true><<<T, NT, 0, s>>>(X, R, W1, B1, W2, B2, Y1, Y2, (__nv_bfloat16*)h_out,     \
+                                                         mean, rstd, H, eps);                                     \
+  else                                                                                                            \
+    layernorm2_fwd_kernel<NV, NT, false><<<T, NT, 0, s>>>(X, R, W1, B1, W2, B2, Y1, Y2, nullptr, mean, rstd, H, eps);
+  DTG_NORM_DISPATCH(H, CALL_LN2_FWD);
+#undef CALL_LN2_FWD
+  note_launch();
+  DTG_LAUNCH_CHECK();
+}
+
+__device__ __forceinline__ void st_partial8(float* p, const float (&a)[8]) {
+  float4* dst = reinterpret_cast<float4*>(p);
+  dst[0] = make_float4(a[0], a[1], a[2], a[3]);
+  dst[1] = make_float4(a[4], a[5], a[6], a[7]);
+}
+
+// ------------------------------------------------------------------------------------------
+// Backward of the two LayerNorms.  xhat = (h - mean) * rstd, g = dy1 * w1 + dy2 * w2 (fp32):
+//   dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dres)
+//   dw1 = sum_rows dy1 * xhat,  db1 = sum_rows dy1,  dw2 = sum_rows dy2 * xhat,  db2 = sum_rows dy2
+// Persistent CTAs as layernorm_bwd_kernel, with its scaled xhat for rows with rstd < 2^-100; the four parameter
+// gradients are fp32 partial rows per CTA ([4, grid, H] scratch) reduced by colsum_kernel in a fixed order.
+// ------------------------------------------------------------------------------------------
+template <int kMaxVec, int kNormThreads, bool HAS_DRES>
+__global__ void __launch_bounds__(kNormThreads) layernorm2_bwd_kernel(
+    const __nv_bfloat16* __restrict__ dy1, const __nv_bfloat16* __restrict__ dy2, const __nv_bfloat16* __restrict__ h,
+    const __nv_bfloat16* __restrict__ w1, const __nv_bfloat16* __restrict__ w2, const float* __restrict__ mean,
+    const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres, __nv_bfloat16* __restrict__ dx,
+    float* __restrict__ partial, int T, int H) {
+  __shared__ float red[32];
+  const int nvec = H >> 3;
+  float dw1[kMaxVec][8], db1[kMaxVec][8], dw2[kMaxVec][8], db2[kMaxVec][8];
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) dw1[k][j] = db1[k][j] = dw2[k][j] = db2[k][j] = 0.f;
+
+  for (int row = blockIdx.x; row < T; row += gridDim.x) {
+    float rs = rstd[row], mu = mean[row], scale = 1.f;
+    if (rs < 0x1p-100f) {
+      scale = kLnDown;
+      mu *= kLnDown;
+      rs *= kLnUp;
+    }
+    const size_t base = (size_t)row * H;
+    float sg = 0.f, sgx = 0.f;
+    bf16x8 c1[kMaxVec], c2[kMaxVec];   // h is read again in the second pass: 8 registers fewer, no spill at 512
+#pragma unroll
+    for (int k = 0; k < kMaxVec; ++k) {
+      const int i = threadIdx.x + k * kNormThreads;
+      if (i < nvec) {
+        c1[k] = ld8(dy1 + base + i * 8);
+        c2[k] = ld8(dy2 + base + i * 8);
+        float fd1[8], fd2[8], fx[8], fw1[8], fw2[8];
+        unpack8(c1[k], fd1);
+        unpack8(c2[k], fd2);
+        unpack8(ld8(h + base + i * 8), fx);
+        unpack8(ld8(w1 + i * 8), fw1);
+        unpack8(ld8(w2 + i * 8), fw2);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float xhat = (fx[j] * scale - mu) * rs;
+          const float g = fd1[j] * fw1[j] + fd2[j] * fw2[j];
+          sg += g;
+          sgx += g * xhat;
+          dw1[k][j] += fd1[j] * xhat;
+          db1[k][j] += fd1[j];
+          dw2[k][j] += fd2[j] * xhat;
+          db2[k][j] += fd2[j];
+        }
+      }
+    }
+    sg = block_sum(sg, red) / (float)H;
+    sgx = block_sum(sgx, red) / (float)H;
+    const float rs_out = scale == 1.f ? rs : rs * kLnDown;   // rstd in the row's own units
+#pragma unroll
+    for (int k = 0; k < kMaxVec; ++k) {
+      const int i = threadIdx.x + k * kNormThreads;
+      if (i < nvec) {
+        float fd1[8], fd2[8], fx[8], fw1[8], fw2[8], out[8];
+        unpack8(c1[k], fd1);
+        unpack8(c2[k], fd2);
+        unpack8(ld8(h + base + i * 8), fx);
+        unpack8(ld8(w1 + i * 8), fw1);
+        unpack8(ld8(w2 + i * 8), fw2);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float xhat = (fx[j] * scale - mu) * rs;
+          out[j] = rs_out * (fd1[j] * fw1[j] + fd2[j] * fw2[j] - sg - xhat * sgx);
+        }
+        if (HAS_DRES) {
+          float fr[8];
+          unpack8(ld8(dres + base + i * 8), fr);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) out[j] += fr[j];
+        }
+        st8(dx + base + i * 8, pack8(out));
+      }
+    }
+  }
+  const size_t plane = (size_t)gridDim.x * H;   // partial: [4, grid, H] = dw1, db1, dw2, db2
+#pragma unroll
+  for (int k = 0; k < kMaxVec; ++k) {
+    const int i = threadIdx.x + k * kNormThreads;
+    if (i < nvec) {
+      float* p = partial + (size_t)blockIdx.x * H + i * 8;
+      st_partial8(p, dw1[k]);
+      st_partial8(p + plane, db1[k]);
+      st_partial8(p + 2 * plane, dw2[k]);
+      st_partial8(p + 3 * plane, db2[k]);
+    }
+  }
+}
+
+// Four accumulators per element (dw1, db1, dw2, db2): at most 2 vectors per thread, and the row spread over up to
+// 512 threads, so no variant spills; H <= 8192 (every GPT-NeoX / Pythia width).
+#define DTG_LN2_BWD_DISPATCH(H, CALL)                                       \
+  do {                                                                     \
+    const int nvec_ = (H) >> 3;                                            \
+    if (nvec_ <= 128) { CALL(1, 128); }                                    \
+    else if (nvec_ <= 256) { CALL(2, 128); }                               \
+    else if (nvec_ <= 512) { CALL(2, 256); }                               \
+    else if (nvec_ <= 1024) { CALL(2, 512); }                              \
+    else throw std::runtime_error("layernorm2: hidden size > 8192 unsupported"); \
+  } while (0)
+
+// 1024 threads per SM, as layernorm_bwd_grid
+int layernorm2_bwd_grid(int T, int H) {
+  const int nvec = H >> 3;
+  const int nt = nvec <= 256 ? 128 : nvec <= 512 ? 256 : 512;
+  const int g = sm_count() * (1024 / nt);
+  return T < g ? T : g;
+}
+
+void layernorm2_bwd(const void* dy1, const void* dy2, const void* h, const void* w1, const void* w2, const float* mean,
+                    const float* rstd, const void* dres, void* dx, float* partial, float* dparams, int T, int H,
+                    cudaStream_t s) {
+  if (H % 8 != 0 || H > 8192) throw std::runtime_error("layernorm2: hidden size must be a multiple of 8, <= 8192");
+  const int grid = layernorm2_bwd_grid(T, H);
+  auto D1 = (const __nv_bfloat16*)dy1;
+  auto D2 = (const __nv_bfloat16*)dy2;
+  auto HH = (const __nv_bfloat16*)h;
+  auto W1 = (const __nv_bfloat16*)w1;
+  auto W2 = (const __nv_bfloat16*)w2;
+  auto DR = (const __nv_bfloat16*)dres;
+  auto DX = (__nv_bfloat16*)dx;
+#define CALL_LN2_BWD(NV, NT)                                                                                  \
+  if (dres)                                                                                                   \
+    layernorm2_bwd_kernel<NV, NT, true><<<grid, NT, 0, s>>>(D1, D2, HH, W1, W2, mean, rstd, DR, DX, partial, T, H); \
+  else                                                                                                        \
+    layernorm2_bwd_kernel<NV, NT, false><<<grid, NT, 0, s>>>(D1, D2, HH, W1, W2, mean, rstd, nullptr, DX, partial, T, H);
+  DTG_LN2_BWD_DISPATCH(H, CALL_LN2_BWD);
+#undef CALL_LN2_BWD
+  for (int q = 0; q < 4; ++q)
+    colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(partial + (size_t)q * grid * H, dparams + (size_t)q * H, grid, H);
+  note_launch(5);
+  DTG_LAUNCH_CHECK();
+}
+
+// ------------------------------------------------------------------------------------------
 // GELU, tanh approximation (StarCoder2's gelu_pytorch_tanh), elementwise on the c_fc output:
 //   y = 0.5 x (1 + tanh(k (x + 0.044715 x^3))),  k = sqrt(2/pi)
 // fp32 math in ATen's operation order with tanhf (not tanh.approx) and one rounding.  The backward is ATen's too,
@@ -672,6 +919,57 @@ void gelu_tanh_bwd(const void* dy, const void* x, void* dx, long long n, cudaStr
 }
 
 // ------------------------------------------------------------------------------------------
+// GELU, exact (erf) form (GPT-NeoX's hidden_act "gelu"), elementwise on the c_fc output:
+//   y = x/2 * (1 + erf(x / sqrt(2)))
+// fp32 erff in ATen's operation order, one rounding.  Backward from the saved pre-activation:
+//   dx = dy * (Phi(x) + x * phi(x)),  Phi(x) = (1 + erf(x / sqrt(2))) / 2,  phi(x) = exp(-x^2 / 2) / sqrt(2 pi)
+// ------------------------------------------------------------------------------------------
+constexpr float kSqrtHalf = 0.70710678118654752440f, kInvSqrt2Pi = 0.39894228040143267794f;
+
+__global__ void gelu_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y, long long nvec) {
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < nvec;
+       idx += (long long)gridDim.x * blockDim.x) {
+    float f[8], o[8];
+    unpack8(ld8(x + idx * 8), f);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] = f[j] * 0.5f * (1.f + erff(f[j] * kSqrtHalf));
+    st8(y + idx * 8, pack8(o));
+  }
+}
+
+__global__ void gelu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
+                                __nv_bfloat16* __restrict__ dx, long long nvec) {
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < nvec;
+       idx += (long long)gridDim.x * blockDim.x) {
+    float f[8], d[8], o[8];
+    unpack8(ld8(x + idx * 8), f);
+    unpack8(ld8(dy + idx * 8), d);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float cdf = 0.5f * (1.f + erff(f[j] * kSqrtHalf));
+      const float pdf = expf(-0.5f * f[j] * f[j]) * kInvSqrt2Pi;
+      o[j] = d[j] * (cdf + f[j] * pdf);
+    }
+    st8(dx + idx * 8, pack8(o));
+  }
+}
+
+void gelu_fwd(const void* x, void* y, long long n, cudaStream_t s) {
+  if (n % 8 != 0) throw std::runtime_error("gelu: the element count must be a multiple of 8");
+  gelu_fwd_kernel<<<ew_grid(n / 8), 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, n / 8);
+  note_launch();
+  DTG_LAUNCH_CHECK();
+}
+
+void gelu_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t s) {
+  if (n % 8 != 0) throw std::runtime_error("gelu: the element count must be a multiple of 8");
+  gelu_bwd_kernel<<<ew_grid(n / 8), 256, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,
+                                                 (__nv_bfloat16*)dx, n / 8);
+  note_launch();
+  DTG_LAUNCH_CHECK();
+}
+
+// ------------------------------------------------------------------------------------------
 // RoPE (half-rotation layout) in place on heads [0, n_rot) of qkv [T, n_heads, d].
 // cos/sin: fp32 [S, d/2] (pos = t % S) or per-token [T, d/2].
 // ------------------------------------------------------------------------------------------
@@ -709,16 +1007,60 @@ __global__ void rope_inplace_kernel(__nv_bfloat16* __restrict__ qkv, const float
   }
 }
 
+// Partial rotary (GPT-NeoX): the pairs (j, j + rot_dim/2), j < rot_dim/2, of each head's first rot_dim elements are
+// rotated as rope_inplace_kernel rotates a head of rot_dim; elements [rot_dim, d) are never read or written.
+// cos/sin: [S, rot_dim/2] or [T, rot_dim/2].  A kernel of its own so that the full-width kernel every other family runs
+// is unchanged.
+__global__ void rope_partial_inplace_kernel(__nv_bfloat16* __restrict__ qkv, const float* __restrict__ cs,
+                                            const float* __restrict__ sn, long long T, int S, int n_heads, int n_rot,
+                                            int d, int rot_dim, int per_token, float sign) {
+  const int r2 = rot_dim >> 1;
+  const int vec_per_head = r2 >> 3;
+  const long long total = T * (long long)n_rot * vec_per_head;
+  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
+       idx += (long long)gridDim.x * blockDim.x) {
+    const int v = (int)(idx % vec_per_head);
+    const long long th = idx / vec_per_head;
+    const int head = (int)(th % n_rot);
+    const long long t = th / n_rot;
+    const long long pos = per_token ? t : (t % S);
+    __nv_bfloat16* p = qkv + (t * n_heads + head) * (long long)d + v * 8;
+    float a[8], b[8], c[8], s[8];
+    unpack8(ld8(p), a);
+    unpack8(ld8(p + r2), b);
+    const float4* cp = reinterpret_cast<const float4*>(cs + pos * r2 + v * 8);
+    const float4* sp = reinterpret_cast<const float4*>(sn + pos * r2 + v * 8);
+    float4 c0 = cp[0], c1 = cp[1], s0 = sp[0], s1 = sp[1];
+    c[0] = c0.x; c[1] = c0.y; c[2] = c0.z; c[3] = c0.w; c[4] = c1.x; c[5] = c1.y; c[6] = c1.z; c[7] = c1.w;
+    s[0] = s0.x; s[1] = s0.y; s[2] = s0.z; s[3] = s0.w; s[4] = s1.x; s[5] = s1.y; s[6] = s1.z; s[7] = s1.w;
+    float o1[8], o2[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float sj = s[j] * sign;
+      o1[j] = a[j] * c[j] - b[j] * sj;
+      o2[j] = b[j] * c[j] + a[j] * sj;
+    }
+    st8(p, pack8(o1));
+    st8(p + r2, pack8(o2));
+  }
+}
+
 void rope_inplace(void* qkv, const float* cos, const float* sin, long long T, int S, int n_heads, int n_rot, int d,
-                  bool per_token, bool inverse, cudaStream_t s) {
+                  int rot_dim, bool per_token, bool inverse, cudaStream_t s) {
   if (d % 16 != 0) throw std::runtime_error("rope: head_dim must be a multiple of 16");
-  const long long total = T * (long long)n_rot * (d / 16);
+  if (rot_dim % 16 != 0 || rot_dim <= 0 || rot_dim > d)
+    throw std::runtime_error("rope: rot_dim must be a positive multiple of 16, <= head_dim");
+  const long long total = T * (long long)n_rot * (rot_dim / 16);
   int grid = (int)((total + 255) / 256);
   const int cap = sm_count() * 16;
   if (grid > cap) grid = cap;
   if (grid < 1) grid = 1;
-  rope_inplace_kernel<<<grid, 256, 0, s>>>((__nv_bfloat16*)qkv, cos, sin, T, S, n_heads, n_rot, d, per_token ? 1 : 0,
-                                           inverse ? -1.f : 1.f);
+  if (rot_dim == d)
+    rope_inplace_kernel<<<grid, 256, 0, s>>>((__nv_bfloat16*)qkv, cos, sin, T, S, n_heads, n_rot, d,
+                                             per_token ? 1 : 0, inverse ? -1.f : 1.f);
+  else
+    rope_partial_inplace_kernel<<<grid, 256, 0, s>>>((__nv_bfloat16*)qkv, cos, sin, T, S, n_heads, n_rot, d, rot_dim,
+                                                     per_token ? 1 : 0, inverse ? -1.f : 1.f);
   note_launch();
   DTG_LAUNCH_CHECK();
 }

@@ -6,7 +6,7 @@ guide uses (reference: every chapter's ``-m/--model-name`` flag, e.g.
 instead of the hub.  A local directory containing a ``config.json`` is also
 accepted, and tiny ``debug-*`` configs exist for tests.  Families: Llama 2 / 3 / 3.1 / 3.2, Mistral, Qwen3, Qwen2.5,
 OLMo 2 (``allenai/OLMo-2-*``, ``model_type: "olmo2"``), StarCoder2 (``bigcode/starcoder2-*``,
-``model_type: "starcoder2"``) and GPT-2.
+``model_type: "starcoder2"``), GPT-NeoX / Pythia (``EleutherAI/pythia-*``, ``model_type: "gpt_neox"``) and GPT-2.
 """
 from __future__ import annotations
 
@@ -18,11 +18,12 @@ from typing import Optional
 
 @dataclasses.dataclass
 class ModelConfig:
-    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "olmo2" | "starcoder2" | "gpt2"; mistral is llama with a
-    # sliding attention window, qwen3 llama with QK-norm and a head_dim of its own, qwen2 llama with q/k/v biases,
-    # olmo2 llama with a full-width QK-norm and post-sublayer norms instead of the pre-norms (``full_qk_norm``,
+    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "olmo2" | "starcoder2" | "gpt_neox" | "gpt2"; mistral is
+    # llama with a sliding attention window, qwen3 llama with QK-norm and a head_dim of its own, qwen2 llama with q/k/v
+    # biases, olmo2 llama with a full-width QK-norm and post-sublayer norms instead of the pre-norms (``full_qk_norm``,
     # ``post_norm``), starcoder2 llama with LayerNorms, a GELU MLP and biases on every projection (``layer_norm``,
-    # ``gelu_mlp``, ``all_bias``)
+    # ``gelu_mlp``, ``all_bias``), gpt_neox starcoder2's block with a parallel residual, partial rotary embeddings
+    # and an exact GELU (``parallel_residual``, ``rotary_dim``, ``gelu_exact``)
     vocab_size: int
     hidden_size: int
     intermediate_size: int
@@ -43,8 +44,10 @@ class ModelConfig:
     qk_norm: bool = False
     #: q/k/v projection biases (Qwen2); o_proj and the MLP stay bias-free
     qkv_bias: bool = False
-    # gpt2 and starcoder2 (their LayerNorms' eps)
+    # gpt2, starcoder2 and gpt_neox (their LayerNorms' eps)
     layer_norm_epsilon: float = 1e-5
+    #: share of each q/k head that RoPE rotates (GPT-NeoX's ``rotary_pct``); read it through ``rotary_dim``
+    partial_rotary_factor: float = 1.0
     dropout: float = 0.0
     name: str = ""
 
@@ -53,6 +56,16 @@ class ModelConfig:
         if self.explicit_head_dim is not None:
             return self.explicit_head_dim
         return self.hidden_size // self.num_attention_heads
+
+    @property
+    def rotary_dim(self) -> int:
+        """Leading elements of each q/k head that RoPE rotates (head_dim unless ``partial_rotary_factor`` < 1)."""
+        return int(self.head_dim * self.partial_rotary_factor)
+
+    @property
+    def parallel_residual(self) -> bool:
+        """GPT-NeoX's layer: h' = h + attn(ln1(h)) + mlp(ln2(h)), both norms of the same h."""
+        return self.arch == "gpt_neox"
 
     @property
     def full_qk_norm(self) -> bool:
@@ -67,18 +80,25 @@ class ModelConfig:
 
     @property
     def layer_norm(self) -> bool:
-        """StarCoder2: LayerNorms with a gain and a bias (eps ``layer_norm_epsilon``) instead of the RMSNorms."""
-        return self.arch == "starcoder2"
+        """StarCoder2, GPT-NeoX: LayerNorms with a gain and a bias (eps ``layer_norm_epsilon``) instead of the
+        RMSNorms."""
+        return self.arch in ("starcoder2", "gpt_neox")
 
     @property
     def gelu_mlp(self) -> bool:
-        """StarCoder2's MLP: c_fc -> GELU (tanh approximation) -> c_proj instead of SwiGLU's three matrices."""
-        return self.arch == "starcoder2"
+        """StarCoder2's and GPT-NeoX's MLP: c_fc -> GELU -> c_proj instead of SwiGLU's three matrices; the GELU is
+        the tanh approximation (StarCoder2) or exact (``gelu_exact``, GPT-NeoX)."""
+        return self.arch in ("starcoder2", "gpt_neox")
+
+    @property
+    def gelu_exact(self) -> bool:
+        """GPT-NeoX: the MLP's GELU is the exact erf form (``hidden_act: "gelu"``), not StarCoder2's tanh form."""
+        return self.arch == "gpt_neox"
 
     @property
     def all_bias(self) -> bool:
-        """StarCoder2: every projection (q, k, v, o, c_fc, c_proj) has a bias; the lm_head has none."""
-        return self.arch == "starcoder2"
+        """StarCoder2, GPT-NeoX: every projection (q, k, v, o, c_fc, c_proj) has a bias; the lm_head has none."""
+        return self.arch in ("starcoder2", "gpt_neox")
 
     def num_parameters(self) -> int:
         h, i, v, l = self.hidden_size, self.intermediate_size, self.vocab_size, self.num_hidden_layers
@@ -87,7 +107,7 @@ class ModelConfig:
             return v * h + self.max_position_embeddings * h + l * per_layer + 2 * h
         q = self.num_attention_heads * self.head_dim
         kv = self.num_key_value_heads * self.head_dim
-        if self.arch == "starcoder2":
+        if self.arch in ("starcoder2", "gpt_neox"):   # the same tensors: only the forward differs
             per_layer = (h * q + q) + 2 * (kv * h + kv) + (q * h + h) + (h * i + i) + (i * h + h) + 4 * h
             n = v * h + l * per_layer + 2 * h
             return n if self.tie_word_embeddings else n + v * h
@@ -164,6 +184,20 @@ def _starcoder2(name, h, i, l, nh, nkv, theta, tied, v=49152, maxpos=16384, wind
     )
 
 
+def _gpt_neox(name, h, i, l, nh, v=50304, rotary=0.25, tied=False, maxpos=2048):
+    return ModelConfig(
+        arch="gpt_neox", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
+        num_attention_heads=nh, num_key_value_heads=nh, max_position_embeddings=maxpos, rope_theta=1e4,
+        tie_word_embeddings=tied, layer_norm_epsilon=1e-5, partial_rotary_factor=rotary, name=name,
+    )
+
+
+_PYTHIA = {   # size: (hidden, intermediate, layers, heads, vocab)
+    "70m": (512, 2048, 6, 8, 50304), "160m": (768, 3072, 12, 12, 50304), "410m": (1024, 4096, 24, 16, 50304),
+    "1.4b": (2048, 8192, 24, 16, 50304), "6.9b": (4096, 16384, 32, 32, 50432), "12b": (5120, 20480, 36, 40, 50688),
+}
+
+
 _GPT2 = ModelConfig(
     arch="gpt2", vocab_size=50257, hidden_size=768, intermediate_size=3072, num_hidden_layers=12,
     num_attention_heads=12, num_key_value_heads=12, max_position_embeddings=1024,
@@ -212,6 +246,13 @@ REGISTRY = {
     "bigcode/starcoder2-3b": _starcoder2("bigcode/starcoder2-3b", 3072, 12288, 30, 24, 2, 999999.4420358813, True),
     "bigcode/starcoder2-7b": _starcoder2("bigcode/starcoder2-7b", 4608, 18432, 32, 36, 4, 1e6, True),
     "bigcode/starcoder2-15b": _starcoder2("bigcode/starcoder2-15b", 6144, 24576, 40, 48, 4, 1e5, False),
+    # Pythia (GPT-NeoX): parallel residual, rotary on 25 % of each head, exact GELU, untied, max positions 2048; each
+    # size also under its -deduped name (same shapes, trained on the deduplicated Pile).  Shapes and vocabularies are
+    # those of the public config.json files as recalled when this table was written; no copy of those files was at
+    # hand to check them against.  With them num_parameters() gives the published totals (70,426,624 ... 11,846,072,320
+    # for 70m ... 12b).  Pythia-1b (head_dim 256) and -2.8b (head_dim 80) are outside the attention kernels' head dims.
+    **{f"EleutherAI/pythia-{size}{suffix}": _gpt_neox(f"EleutherAI/pythia-{size}{suffix}", h, i, l, nh, v)
+       for size, (h, i, l, nh, v) in _PYTHIA.items() for suffix in ("", "-deduped")},
     # tiny configs for tests / smoke runs (head_dim 128 so the sm_90a attention kernel applies)
     "debug-llama": _llama("debug-llama", 1024, 256, 512, 2, 2, 2, 2048, 1e4),
     "debug-llama-gqa": _llama("debug-llama-gqa", 1024, 512, 1024, 2, 4, 2, 2048, 5e5),
@@ -228,6 +269,10 @@ REGISTRY = {
     "debug-olmo2": _olmo2("debug-olmo2", 512, 1024, 2, 4, 2, v=1024, maxpos=2048),
     # 4 q heads and 2 kv heads x 128 over a hidden size of 512, tied, with StarCoder2's block
     "debug-starcoder2": _starcoder2("debug-starcoder2", 512, 2048, 2, 4, 2, 1e5, True, v=1024, maxpos=2048),
+    # 4 heads x 128 over a hidden size of 512 with rotary on 32 of them, and 4 heads x 64 over 256 with rotary on 16,
+    # with GPT-NeoX's block
+    "debug-gpt-neox": _gpt_neox("debug-gpt-neox", 512, 2048, 2, 4, v=1024),
+    "debug-gpt-neox-d64": _gpt_neox("debug-gpt-neox-d64", 256, 1024, 2, 4, v=1024),
     "debug-gpt2": dataclasses.replace(_GPT2, vocab_size=512, hidden_size=64, intermediate_size=256,
                                       num_hidden_layers=2, num_attention_heads=2, num_key_value_heads=2,
                                       max_position_embeddings=128, name="debug-gpt2"),
@@ -247,6 +292,8 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
         )
     if mt == "starcoder2":
         return _starcoder2_from_hf_dict(d, name)
+    if mt == "gpt_neox":
+        return _gpt_neox_from_hf_dict(d, name)
     if mt not in ("llama", "mistral", "qwen3", "qwen2", "olmo2"):
         raise ValueError(f"unsupported model_type {mt!r} in {name}")
     if mt == "olmo2":
@@ -355,6 +402,52 @@ def _starcoder2_from_hf_dict(d: dict, name: str) -> ModelConfig:
     )
 
 
+def _gpt_neox_from_hf_dict(d: dict, name: str) -> ModelConfig:
+    """A ``GPTNeoXConfig`` payload, with RoPE settings as ``rotary_pct`` / ``rotary_emb_base`` (the published files) or
+    in transformers 5's ``rope_parameters``.  Every setting the kernel path does not implement is refused, naming its
+    key, rather than dropped."""
+    if d.get("use_parallel_residual", True) is not True:
+        raise ValueError(f"{name}: use_parallel_residual is {d['use_parallel_residual']!r}; only GPT-NeoX's parallel "
+                         "residual is supported")
+    if d.get("hidden_act", "gelu") != "gelu":
+        raise ValueError(f"{name}: hidden_act is {d['hidden_act']!r}; only 'gelu' (exact) is supported")
+    if d.get("attention_bias", True) is not True:
+        raise ValueError(f"{name}: attention_bias is {d['attention_bias']!r}; only GPT-NeoX with biases on every "
+                         "projection is supported")
+    for key in ("hidden_dropout", "attention_dropout"):
+        if d.get(key, 0.0):
+            raise ValueError(f"{name}: {key} is {d[key]!r}; the kernel path has no dropout, set {key} to 0.0 to "
+                             "train without it")
+    rp = d.get("rope_parameters") if isinstance(d.get("rope_parameters"), dict) else None
+    rope = rp if rp is not None else d.get("rope_scaling")
+    if rope and (rope.get("rope_type") or rope.get("type") or "default") != "default":
+        key = "rope_parameters" if rp is not None else "rope_scaling"
+        raise ValueError(f"{name}: {key} has type {rope.get('rope_type') or rope.get('type')!r}; only the default "
+                         "RoPE is supported for GPT-NeoX")
+    theta = d.get("rotary_emb_base", d.get("rope_theta", 1e4))
+    pct = d.get("rotary_pct", d.get("partial_rotary_factor", 0.25))
+    if rp is not None:   # transformers>=5 layout
+        theta = rp.get("rope_theta", theta)
+        pct = rp.get("partial_rotary_factor", pct)
+    h, nh = d["hidden_size"], d["num_attention_heads"]
+    head_dim = h // nh
+    if head_dim not in (64, 128) or head_dim * nh != h:
+        raise ValueError(f"{name}: head_dim (hidden_size / num_attention_heads = {h} / {nh}) is not 64 or 128; the "
+                         "attention kernels serve head_dim 64 and 128")
+    rot = int(head_dim * pct)
+    key = "rope_parameters.partial_rotary_factor" if rp is not None and "partial_rotary_factor" in rp else "rotary_pct"
+    if rot <= 0 or rot % 16:
+        raise ValueError(f"{name}: {key} {pct!r} gives a rotary dim of {rot} of head_dim {head_dim}; the RoPE kernel "
+                         "needs a positive multiple of 16")
+    return ModelConfig(
+        arch="gpt_neox", vocab_size=d["vocab_size"], hidden_size=h, intermediate_size=d["intermediate_size"],
+        num_hidden_layers=d["num_hidden_layers"], num_attention_heads=nh, num_key_value_heads=nh,
+        max_position_embeddings=d.get("max_position_embeddings", 2048), rope_theta=theta,
+        tie_word_embeddings=d.get("tie_word_embeddings", False), layer_norm_epsilon=d.get("layer_norm_eps", 1e-5),
+        partial_rotary_factor=pct, name=name,
+    )
+
+
 def get_config(name: str, **overrides) -> ModelConfig:
     """Resolve ``name`` (registry id, or a directory / file holding an HF ``config.json``)."""
     if name in REGISTRY:
@@ -446,6 +539,17 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
             "hidden_act": "gelu_pytorch_tanh", "use_bias": True, "tie_word_embeddings": cfg.tie_word_embeddings,
             "attention_dropout": 0.0, "residual_dropout": 0.0, "embedding_dropout": 0.0, "bos_token_id": 0,
             "eos_token_id": 0, "torch_dtype": "bfloat16",
+        }
+    if cfg.arch == "gpt_neox":
+        d = {
+            "model_type": "gpt_neox", "architectures": ["GPTNeoXForCausalLM"], "vocab_size": cfg.vocab_size,
+            "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size,
+            "num_hidden_layers": cfg.num_hidden_layers, "num_attention_heads": cfg.num_attention_heads,
+            "max_position_embeddings": cfg.max_position_embeddings, "layer_norm_eps": cfg.layer_norm_epsilon,
+            "rotary_pct": cfg.partial_rotary_factor, "rotary_emb_base": cfg.rope_theta, "hidden_act": "gelu",
+            "use_parallel_residual": True, "attention_bias": True, "hidden_dropout": 0.0, "attention_dropout": 0.0,
+            "tie_word_embeddings": cfg.tie_word_embeddings, "bos_token_id": 0, "eos_token_id": 0,
+            "torch_dtype": "float16",
         }
     if cfg.arch == "llama" and cfg.explicit_head_dim is not None:
         d["head_dim"] = cfg.explicit_head_dim

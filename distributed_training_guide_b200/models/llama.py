@@ -1,7 +1,8 @@
 """Llama-family causal LM built on the sm_90a op layer (Llama; Mistral: Llama plus a sliding attention window; Qwen3:
 Llama plus QK-norm, with a head_dim of its own; Qwen2: Llama plus q/k/v biases; OLMo 2: Llama with a full-width
 QK-norm and RMSNorms after each sublayer instead of before it, ``Olmo2DecoderLayer``; StarCoder2: Llama with
-LayerNorms, a c_fc -> GELU-tanh -> c_proj MLP and a bias on every projection, ``Starcoder2DecoderLayer``).
+LayerNorms, a c_fc -> GELU-tanh -> c_proj MLP and a bias on every projection, ``Starcoder2DecoderLayer``; GPT-NeoX:
+StarCoder2's parameters with a parallel residual, partial rotary embeddings and an exact GELU, ``GPTNeoXDecoderLayer``).
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
 the reference instantiates at e.g. ``02-distributed-data-parallel/train_llm.py:57-58``)
@@ -11,7 +12,8 @@ so checkpoints keep meaningful keys: ``model.embed_tokens.weight``,
 ``model.norm.weight``, ``lm_head.weight``; Qwen3 adds ``...self_attn.{q,k}_norm.weight``, Qwen2
 ``...self_attn.{q,k,v}_proj.bias``; OLMo 2 has ``...self_attn.{q,k}_norm.weight`` ([nh*d], [nkv*d]) and
 ``...post_{attention,feedforward}_layernorm.weight`` and no ``input_layernorm``; StarCoder2 ``...mlp.{c_fc,c_proj}.{weight,bias}``,
-``...self_attn.{q,k,v,o}_proj.bias`` and a ``.bias`` beside every norm gain.
+``...self_attn.{q,k,v,o}_proj.bias`` and a ``.bias`` beside every norm gain; GPT-NeoX StarCoder2's names (its
+checkpoint names and per-head interleaved q|k|v live in ``models/gpt_neox_layout.py``).
 
 What is *different* from the HF module code (SURVEY.md §3.2) is the execution plan:
   * q/k/v (and gate/up) projections run as ONE wgmma GEMM over a fused weight that is
@@ -149,7 +151,7 @@ class RotaryEmbedding(nn.Module):
 
     def __init__(self, config: ModelConfig):
         super().__init__()
-        self.head_dim = config.head_dim
+        self.head_dim = config.rotary_dim   # the rotated share of each head (all of it but for GPT-NeoX)
         self.theta = config.rope_theta
         self.scaling = config.rope_scaling
         self._cache = {}
@@ -404,6 +406,37 @@ class Starcoder2DecoderLayer(LlamaDecoderLayer):
         return down, h
 
 
+class GPTNeoXDecoderLayer(Starcoder2DecoderLayer):
+    """GPT-NeoX's layer: StarCoder2's parameters (names, ``FLAT_ORDER``, fused q|k|v weight and bias) with a parallel
+    residual, ``h' = h + attn(ln1(h)) + mlp(ln2(h))``, RoPE on the first ``rotary_dim`` elements of each q/k head and
+    an exact GELU.  Both norms read the same h (``ops.layer_norm2``); the attention dense and the MLP down-projection
+    write one branch (``ops.parallel_out``), and the residual add stays deferred: the layer returns ``(branch, h)``."""
+
+    def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
+        assert tp_size == 1, "GPT-NeoX layers are not tensor-parallel"
+        super().__init__(config, layer_idx, dtype, device, tp_size)
+        self.rotary_dim = config.rotary_dim
+
+    def forward(self, x, residual, cos, sin, doc_start=None):
+        att = self.self_attn
+        B, S, _ = x.shape
+        fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
+        n1, n2 = self.input_layernorm, self.post_attention_layernorm
+        y1, y2, h = ops.layer_norm2(x, residual, n1.weight, n1.bias, n2.weight, n2.bias, n1.eps)
+        w, owner = self._qkv_weight()
+        b, b_owner = self._qkv_bias()
+        qkv = fused_linear(y1, w, owner, b, b_owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
+        qkv = ops.rope_qkv_(qkv, cos, sin, att.num_heads + att.num_kv_heads, self.rotary_dim)
+        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
+        a = a.reshape(B, S, att.num_heads * att.head_dim)
+        mlp = self.mlp
+        up = ops.fp8_linear(y2, mlp.c_fc.weight, None, mlp.c_fc.bias) if self.fp8 else mlp.c_fc(y2)
+        act = ops.gelu(up)
+        out = ops.parallel_out(a, act, att.o_proj.weight, mlp.c_proj.weight, att.o_proj.bias, mlp.c_proj.bias,
+                               fp8=self.fp8)
+        return out, h
+
+
 class LlamaModel(nn.Module):
     def __init__(self, config: ModelConfig, dtype=None, device=None, tp_size=1):
         super().__init__()
@@ -412,6 +445,7 @@ class LlamaModel(nn.Module):
         # nn.Embedding, 06-tensor-parallel/train_llm.py:82)
         self.embed_tokens = Embedding(config.vocab_size, config.hidden_size // tp_size, dtype, device)
         layer_cls = (Olmo2DecoderLayer if config.post_norm else
+                     GPTNeoXDecoderLayer if config.parallel_residual else
                      Starcoder2DecoderLayer if config.arch == "starcoder2" else LlamaDecoderLayer)
         self.layers = nn.ModuleList(
             [layer_cls(config, i, dtype, device, tp_size) for i in range(config.num_hidden_layers)]

@@ -4,8 +4,9 @@ On CUDA tensors each op calls a hand-written sm_90a kernel from the in-tree
 extension (``csrc/``): wgmma/TMA GEMM (fwd / dgrad / wgrad) in bf16 and, for
 ``fp8_linear``, in fp8 with its amax and cast-transpose kernels, wgmma
 flash-attention, fused residual-add+RMSNorm and norm-then-add (OLMo 2), in-place RoPE on the fused qkv buffer
-(after Qwen3's per-head or OLMo 2's full-width QK-norm in the same kernel), SwiGLU, fused residual-add+LayerNorm
-and GELU-tanh (StarCoder2), in-place
+(after Qwen3's per-head or OLMo 2's full-width QK-norm in the same kernel; partial rotary for GPT-NeoX), SwiGLU,
+fused residual-add+LayerNorm and GELU-tanh (StarCoder2), GPT-NeoX's dual LayerNorm, exact GELU and parallel-residual
+output GEMMs, in-place
 softmax-cross-entropy, embedding gather / scatter-add and flat AdamW.  On CPU tensors the same Functions run the reference math in
 ``ops/reference.py`` (chapter 01's CPU config and the gloo tests).
 
@@ -30,7 +31,7 @@ from . import reference as ref
 __all__ = [
     "linear", "fused_linear", "rms_norm", "add_rms_norm", "rms_norm_add", "rope_qkv_", "qk_norm_rope_",
     "olmo_qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy", "layer_norm",
-    "add_layer_norm", "gelu_tanh",
+    "add_layer_norm", "gelu_tanh", "gelu", "layer_norm2", "parallel_out",
     "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "bias_grad", "ref",
 ]
 
@@ -155,33 +156,41 @@ class _Linear(torch.autograd.Function):
         dy2 = dy.reshape(-1, dy.shape[-1])
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
-        dx = None
-        if ctx.needs_input_grad[0]:
-            gs = getattr(ctx.w_param, "_dtg_gather", None)
-            if gs is not None and dy2.is_cuda and gs.pending():
-                dx = gs.gemm(dy2, False).view(ctx.x_shape)   # FSDP: re-gather the weight inside the dgrad GEMM
-            else:
-                dx = gemm(dy2, w).view(ctx.x_shape)  # [T,N] @ [N,K]
-        dw = None
-        if ctx.needs_input_grad[1] or getattr(ctx.w_param, "_dtg_grad", None) is not None:
-            side = _WGRAD_SIDE["enabled"] and dy2.is_cuda and getattr(ctx.w_param, "_dtg_grad", None) is not None
-            if side:
-                cur, ss = torch.cuda.current_stream(), _wgrad_stream(dy2.device)
-                ss.wait_stream(cur)               # dy2 / x2 were produced on the compute stream
-                dy2.record_stream(ss)             # keep the caching allocator from recycling them too early
-                x2.record_stream(ss)
-                with torch.cuda.stream(ss):
-                    dw = _emit_weight_grad(ctx.w_param,
-                                           lambda out, acc: gemm(dy2, x2, out=out, trans_a=True, accumulate=acc), w)
-                _WGRAD_SIDE["dirty"] = True
-            else:
-                dw = _emit_weight_grad(
-                    ctx.w_param,
-                    lambda out, acc: gemm(dy2, x2, out=out, trans_a=True, accumulate=acc),  # dy^T @ x
-                    w,
-                )
+        dx, dw = _linear_grads(dy2, x2, w, ctx.w_param, ctx.x_shape, ctx.needs_input_grad[0],
+                               ctx.needs_input_grad[1])
         db = _emit_bias_grad(ctx.bias_param, dy2, ctx.bias)
         return dx, dw, None, db, None
+
+
+def _linear_grads(dy2, x2, w, w_param, x_shape, need_dx, need_dw):
+    """(dx, dw) of ``y = x @ w.T`` from the 2-D output gradient ``dy2``: the dgrad GEMM (re-gathering an FSDP weight
+    inside it while its gather is pending) and the wgrad GEMM routed through ``_emit_weight_grad``."""
+    dx = None
+    if need_dx:
+        gs = getattr(w_param, "_dtg_gather", None)
+        if gs is not None and dy2.is_cuda and gs.pending():
+            dx = gs.gemm(dy2, False).view(x_shape)   # FSDP: re-gather the weight inside the dgrad GEMM
+        else:
+            dx = gemm(dy2, w).view(x_shape)  # [T,N] @ [N,K]
+    dw = None
+    if need_dw or getattr(w_param, "_dtg_grad", None) is not None:
+        side = _WGRAD_SIDE["enabled"] and dy2.is_cuda and getattr(w_param, "_dtg_grad", None) is not None
+        if side:
+            cur, ss = torch.cuda.current_stream(), _wgrad_stream(dy2.device)
+            ss.wait_stream(cur)               # dy2 / x2 were produced on the compute stream
+            dy2.record_stream(ss)             # keep the caching allocator from recycling them too early
+            x2.record_stream(ss)
+            with torch.cuda.stream(ss):
+                dw = _emit_weight_grad(w_param,
+                                       lambda out, acc: gemm(dy2, x2, out=out, trans_a=True, accumulate=acc), w)
+            _WGRAD_SIDE["dirty"] = True
+        else:
+            dw = _emit_weight_grad(
+                w_param,
+                lambda out, acc: gemm(dy2, x2, out=out, trans_a=True, accumulate=acc),  # dy^T @ x
+                w,
+            )
+    return dx, dw
 
 
 def linear(x, w, bias=None):
@@ -280,19 +289,28 @@ class _FP8Linear(torch.autograd.Function):
         if not dy2.is_contiguous():
             dy2 = dy2.contiguous()
         dy8, dy8t, sdy = fp8_cast(dy2, torch.float8_e5m2, rowwise=ctx.needs_input_grad[0])
-        dx = None
-        if ctx.needs_input_grad[0]:
-            _, w8t, sw = fp8_cast(w, torch.float8_e4m3fn, rowwise=False, amax=amax_w)
-            dx = gemm_fp8(dy8, sdy, w8t, sw, out_dtype=dy.dtype).view(ctx.x_shape)  # [T,N] . [K,N]^T
-        dw = None
-        if ctx.needs_input_grad[1] or getattr(ctx.w_param, "_dtg_grad", None) is not None:
-            dw = _emit_weight_grad(
-                ctx.w_param,
-                lambda out, acc: gemm_fp8(dy8t, sdy, x8t, sx, out=out, accumulate=acc),  # [N,T] . [K,T]^T
-                ctx.w_param,
-            )
+        dx, dw = _fp8_linear_grads(dy8, dy8t, sdy, x8t, sx, w, amax_w, ctx.w_param, ctx.x_shape, dy.dtype,
+                                   ctx.needs_input_grad[0], ctx.needs_input_grad[1])
         db = _emit_bias_grad(ctx.bias_param, dy2, ctx.bias)   # from the bf16 dy, not its fp8 copy
         return dx, dw, None, db, None
+
+
+def _fp8_linear_grads(dy8, dy8t, sdy, x8t, sx, w, amax_w, w_param, x_shape, dtype, need_dx, need_dw):
+    """(dx, dw) of an fp8 linear from the e5m2 output gradient (both layouts) and the forward's saved transposed
+    e4m3 input: the dgrad GEMM against W8^T re-cast with the forward's amax, and the wgrad GEMM routed through
+    ``_emit_weight_grad``."""
+    dx = None
+    if need_dx:
+        _, w8t, sw = fp8_cast(w, torch.float8_e4m3fn, rowwise=False, amax=amax_w)
+        dx = gemm_fp8(dy8, sdy, w8t, sw, out_dtype=dtype).view(x_shape)  # [T,N] . [K,N]^T
+    dw = None
+    if need_dw or getattr(w_param, "_dtg_grad", None) is not None:
+        dw = _emit_weight_grad(
+            w_param,
+            lambda out, acc: gemm_fp8(dy8t, sdy, x8t, sx, out=out, accumulate=acc),  # [N,T] . [K,T]^T
+            w_param,
+        )
+    return dx, dw
 
 
 def fp8_linear(x, w, owner=None, bias=None, bias_owner=None):
@@ -303,6 +321,100 @@ def fp8_linear(x, w, owner=None, bias=None, bias_owner=None):
     if bias is None:
         return _FP8Linear.apply(x, w, owner if owner is not None else w)
     return _FP8Linear.apply(x, w, owner if owner is not None else w, bias, bias_owner)
+
+
+# --------------------------------------------------------------------------------------
+# parallel-residual branch (GPT-NeoX): x = attn @ Wd^T + act @ W4^T + bd + b4 in one [T, H] buffer
+# --------------------------------------------------------------------------------------
+def _bias_sum(bd, b4):
+    return (bd.float() + b4.float()).to(bd.dtype)
+
+
+def _emit_shared_bias_grad(dy2, bd, b4):
+    """One column sum of ``dy2`` is the gradient of both biases; each is routed like a norm gain's."""
+    db32 = bias_grad(dy2)
+    return (_emit_weight_grad(bd, _norm_dw_into(db32), bd), _emit_weight_grad(b4, _norm_dw_into(db32), b4))
+
+
+class _ParallelOut(torch.autograd.Function):
+    """The dense GEMM writes ``bf16(attn @ Wd^T + bf16(bd + b4))`` (bias epilogue, overwrite mode); the
+    down-projection GEMM adds ``act @ W4^T`` into the same buffer (accumulate mode).  While an FSDP weight's gather is
+    pending, its ``_GatherSpec.gemm`` runs instead and the down-projection's product is added."""
+
+    @staticmethod
+    def forward(ctx, attn, act, wd, w4, bd, b4):
+        a2 = attn.reshape(-1, attn.shape[-1])
+        m2 = act.reshape(-1, act.shape[-1])
+        bias = _bias_sum(bd, b4)
+        gs = getattr(wd, "_dtg_gather", None)
+        if gs is not None and gs.pending():
+            out = gs.gemm(a2 if a2.is_contiguous() else a2.contiguous(), True, bias)
+        else:
+            out = gemm(a2, wd, trans_b=True, bias=bias)
+        gs = getattr(w4, "_dtg_gather", None)
+        if gs is not None and gs.pending():
+            out.add_(gs.gemm(m2 if m2.is_contiguous() else m2.contiguous(), True))
+        else:
+            gemm(m2, w4, out=out, trans_b=True, accumulate=True)
+        ctx.save_for_backward(a2, m2, wd, w4)
+        ctx.params = (bd, b4)
+        ctx.shapes = (attn.shape, act.shape)
+        return out.view(*attn.shape[:-1], wd.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        a2, m2, wd, w4 = ctx.saved_tensors
+        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
+        need = ctx.needs_input_grad
+        dattn, dwd = _linear_grads(dy2, a2, wd, wd, ctx.shapes[0], need[0], need[2])
+        dact, dw4 = _linear_grads(dy2, m2, w4, w4, ctx.shapes[1], need[1], need[3])
+        return (dattn, dact, dwd, dw4) + _emit_shared_bias_grad(dy2, *ctx.params)
+
+
+class _FP8ParallelOut(torch.autograd.Function):
+    """``_ParallelOut`` with both GEMMs in fp8 (``_FP8Linear``'s scheme): the dense GEMM with the summed bias in its
+    epilogue, the down-projection with ``gemm_fp8(..., accumulate=True)``.  The output gradient is cast to e5m2 once
+    for both weights."""
+
+    @staticmethod
+    def forward(ctx, attn, act, wd, w4, bd, b4):
+        a2 = attn.reshape(-1, attn.shape[-1])
+        m2 = act.reshape(-1, act.shape[-1])
+        a8, a8t, sa = fp8_cast(a2, torch.float8_e4m3fn)
+        m8, m8t, sm = fp8_cast(m2, torch.float8_e4m3fn)
+        amax_d, amax_4 = fp8_amax(wd), fp8_amax(w4)
+        wd8, _, swd = fp8_cast(wd, torch.float8_e4m3fn, transposed=False, amax=amax_d)
+        w48, _, sw4 = fp8_cast(w4, torch.float8_e4m3fn, transposed=False, amax=amax_4)
+        out = gemm_fp8(a8, sa, wd8, swd, out_dtype=attn.dtype, bias=_bias_sum(bd, b4))
+        gemm_fp8(m8, sm, w48, sw4, out=out, accumulate=True)
+        ctx.save_for_backward(a8t, sa, m8t, sm, wd, w4, amax_d, amax_4)
+        ctx.params = (bd, b4)
+        ctx.shapes = (attn.shape, act.shape)
+        return out.view(*attn.shape[:-1], wd.shape[0])
+
+    @staticmethod
+    def backward(ctx, dy):
+        a8t, sa, m8t, sm, wd, w4, amax_d, amax_4 = ctx.saved_tensors
+        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
+        need = ctx.needs_input_grad
+        dy8, dy8t, sdy = fp8_cast(dy2, torch.float8_e5m2, rowwise=need[0] or need[1])
+        dattn, dwd = _fp8_linear_grads(dy8, dy8t, sdy, a8t, sa, wd, amax_d, wd, ctx.shapes[0], dy.dtype, need[0],
+                                       need[2])
+        dact, dw4 = _fp8_linear_grads(dy8, dy8t, sdy, m8t, sm, w4, amax_4, w4, ctx.shapes[1], dy.dtype, need[1],
+                                      need[3])
+        return (dattn, dact, dwd, dw4) + _emit_shared_bias_grad(dy2, *ctx.params)
+
+
+def parallel_out(attn, act, wd, w4, bd, b4, fp8=False):
+    """GPT-NeoX's layer branch ``attn @ Wd^T + act @ W4^T + bd + b4`` (attention dense + MLP down-projection) as one
+    [..., H] tensor.  bf16 CUDA tensors run two wgmma GEMMs into one buffer, with no elementwise pass: the first with
+    ``bf16(bd + b4)`` in its epilogue, the second accumulating; backward sums the output gradient once for both
+    biases.  ``fp8``: both GEMMs in fp8 (CPU tensors run the same quantisation through ``ops/reference.py``)."""
+    if fp8:
+        return _FP8ParallelOut.apply(attn, act, wd, w4, bd, b4)
+    if _ext.use_cuda_kernel("gemm", attn, act, wd, w4) and attn.dtype == torch.bfloat16:
+        return _ParallelOut.apply(attn, act, wd, w4, bd, b4)
+    return ref.linear(attn, wd, bd) + ref.linear(act, w4, b4)
 
 
 # --------------------------------------------------------------------------------------
@@ -502,17 +614,84 @@ def gelu_tanh(x):
     return ref.gelu_new(x.float()).to(x.dtype)
 
 
+class _Gelu(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x):
+        ctx.save_for_backward(x)
+        return _ext.load().gelu_fwd(x)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (x,) = ctx.saved_tensors
+        return _ext.load().gelu_bwd(dy.contiguous(), x)
+
+
+def gelu(x):
+    """Exact GELU, ``x/2 * (1 + erf(x / sqrt(2)))`` (``F.gelu(x)``, GPT-NeoX's ``hidden_act: "gelu"``), in fp32 with
+    one rounding.  bf16 CUDA tensors run the sm_90a kernels, which keep the pre-activation for the backward."""
+    if _ext.use_cuda_kernel("gelu", x) and x.dtype == torch.bfloat16:
+        return _Gelu.apply(x.contiguous())
+    return ref.gelu(x)
+
+
+# --------------------------------------------------------------------------------------
+# two LayerNorms over one residual stream (GPT-NeoX's parallel residual)
+# --------------------------------------------------------------------------------------
+class _LayerNorm2(torch.autograd.Function):
+    """(y1, y2[, h]) = (layernorm(h) * w1 + b1, layernorm(h) * w2 + b2[, h]), h = x + r (x without r), one shared
+    statistic.  Backward: one kernel for dx (+ dh as the residual gradient) and the four parameter gradients."""
+
+    @staticmethod
+    def forward(ctx, x, r, w1, b1, w2, b2, eps):
+        C = _ext.load()
+        x2 = x.reshape(-1, x.shape[-1])
+        r2 = r.reshape(-1, r.shape[-1]) if r is not None else None
+        y1, y2, h, mean, rstd = C.layernorm2_fwd(x2, r2, w1, b1, w2, b2, float(eps))
+        ctx.save_for_backward(h if h is not None else x2, w1, w2, mean, rstd)
+        ctx.shape = x.shape
+        ctx.params = (w1, b1, w2, b2)
+        ctx.has_res = r is not None
+        if h is None:
+            return y1.view(x.shape), y2.view(x.shape)
+        return y1.view(x.shape), y2.view(x.shape), h.view(x.shape)
+
+    @staticmethod
+    def backward(ctx, dy1, dy2, dh=None):
+        C = _ext.load()
+        h, w1, w2, mean, rstd = ctx.saved_tensors
+        flat = lambda t: t.reshape(-1, t.shape[-1]).contiguous() if t is not None else torch.zeros_like(h)  # noqa: E731
+        dh2 = dh.reshape(-1, dh.shape[-1]).contiguous() if dh is not None else None
+        dx, d32 = C.layernorm2_bwd(flat(dy1), flat(dy2), h, w1, w2, mean, rstd, dh2)
+        grads = tuple(_emit_weight_grad(p, _norm_dw_into(d32[i]), p) for i, p in enumerate(ctx.params))
+        dx = dx.view(ctx.shape)
+        return (dx, dx if ctx.has_res else None) + grads + (None,)
+
+
+def layer_norm2(x, r, w1, b1, w2, b2, eps):
+    """GPT-NeoX's two pre-norms of one residual stream: ``h = x + r`` (rounded to the input dtype; ``x`` itself when
+    ``r`` is None), then ``(layer_norm(h, w1, b1), layer_norm(h, w2, b2), h)``.  Both norms share one mean and one
+    rstd.  bf16 CUDA tensors run the sm_90a kernels: one read of the row and three writes forward; y1 and y2 are
+    bit-identical to ``layer_norm`` with each (w, b).  The four parameter gradients go through ``_emit_weight_grad``."""
+    if _ext.use_cuda_kernel("layernorm", x, w1, b1, w2, b2) and x.dtype == torch.bfloat16:
+        if r is None:
+            y1, y2 = _LayerNorm2.apply(x.contiguous(), None, w1, b1, w2, b2, eps)
+            return y1, y2, x
+        return _LayerNorm2.apply(x.contiguous(), r.contiguous(), w1, b1, w2, b2, eps)
+    return ref.layer_norm2(x, r, w1, b1, w2, b2, eps)
+
+
 # --------------------------------------------------------------------------------------
 # RoPE, applied in place on the q and k heads of the fused qkv activation
 # --------------------------------------------------------------------------------------
 class _RopeQKV(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, cos, sin, n_rot_heads):
+    def forward(ctx, qkv, cos, sin, n_rot_heads, rotary_dim=None):
         # qkv: [B, S, n_total_heads, d]; the first n_rot_heads heads (q then k) are rotated
         C = _ext.load()
         ctx.save_for_backward(cos, sin)
         ctx.n_rot = n_rot_heads
-        C.rope_inplace(qkv, cos, sin, n_rot_heads, False)
+        ctx.rotary_dim = rotary_dim
+        C.rope_inplace(qkv, cos, sin, n_rot_heads, False, rot_dim=rotary_dim)
         # physically in place, but handed to autograd as a fresh tensor aliasing the same
         # storage: the producer GEMM never re-reads its output, so nothing observes the write
         return qkv.detach()
@@ -523,16 +702,24 @@ class _RopeQKV(torch.autograd.Function):
         cos, sin = ctx.saved_tensors
         if not dqkv.is_contiguous():
             dqkv = dqkv.contiguous()
-        C.rope_inplace(dqkv, cos, sin, ctx.n_rot, True)  # inverse rotation, in place on the grad
-        return dqkv, None, None, None
+        C.rope_inplace(dqkv, cos, sin, ctx.n_rot, True, rot_dim=ctx.rotary_dim)  # inverse rotation, in place
+        return dqkv, None, None, None, None
 
 
-def rope_qkv_(qkv, cos, sin, n_rot_heads):
-    """Rotate heads [0, n_rot_heads) of ``qkv`` [B,S,heads,d] with cos/sin [S,d/2] or [B,S,d/2] (fp32)."""
+def rope_qkv_(qkv, cos, sin, n_rot_heads, rotary_dim=None):
+    """Rotate heads [0, n_rot_heads) of ``qkv`` [B,S,heads,d] with cos/sin [S,r/2] or [B,S,r/2] (fp32), r =
+    ``rotary_dim`` (None: the whole head, r = d).  A partial rotary_dim (GPT-NeoX) rotates the pairs (j, j + r/2),
+    j < r/2, and leaves elements [r, d) of every head untouched; it must be a multiple of 16."""
+    if rotary_dim is not None and rotary_dim == qkv.shape[-1]:
+        rotary_dim = None
     if _ext.use_cuda_kernel("rope", qkv) and qkv.dtype == torch.bfloat16:
         # views produced by a GEMM are fresh tensors, in-place is safe for autograd via mark_dirty
-        return _RopeQKV.apply(qkv, cos.contiguous(), sin.contiguous(), n_rot_heads)
-    rot = ref.rope_apply(qkv[:, :, :n_rot_heads], cos, sin)
+        return _RopeQKV.apply(qkv, cos.contiguous(), sin.contiguous(), n_rot_heads, rotary_dim)
+    if rotary_dim is None:
+        rot = ref.rope_apply(qkv[:, :, :n_rot_heads], cos, sin)
+    else:
+        qk = qkv[:, :, :n_rot_heads]
+        rot = torch.cat([ref.rope_apply(qk[..., :rotary_dim], cos, sin), qk[..., rotary_dim:]], dim=-1)
     return torch.cat([rot, qkv[:, :, n_rot_heads:]], dim=2)
 
 

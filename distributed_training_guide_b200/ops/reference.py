@@ -49,6 +49,13 @@ def layer_norm(x, w, b, eps):
     return F.layer_norm(x.float(), (x.shape[-1],), w.float(), b.float(), eps).to(x.dtype)
 
 
+def layer_norm2(x, r, w1, b1, w2, b2, eps):
+    """GPT-NeoX's two LayerNorms over one residual stream: ``h = x + r`` (``x`` when ``r`` is None), then
+    ``(layer_norm(h, w1, b1), layer_norm(h, w2, b2), h)``."""
+    h = x if r is None else x + r
+    return layer_norm(h, w1, b1, eps), layer_norm(h, w2, b2, eps), h
+
+
 def add_rms_norm(x, residual, w, eps):
     """returns (normed, new_residual) with new_residual = x + residual."""
     h = x + residual
@@ -133,6 +140,11 @@ def swiglu(gu):
 
 def gelu_new(x):
     return 0.5 * x * (1.0 + torch.tanh(math.sqrt(2.0 / math.pi) * (x + 0.044715 * x.pow(3))))
+
+
+def gelu(x):
+    """Exact (erf) GELU, ``x/2 * (1 + erf(x / sqrt(2)))``, in fp32 with one rounding to ``x.dtype``."""
+    return F.gelu(x.float()).to(x.dtype)
 
 
 def shift_labels(labels):

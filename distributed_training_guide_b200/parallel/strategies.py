@@ -431,6 +431,11 @@ class TwoDParallel(Strategy):
                 f"{config.name or config.arch}: tensor parallelism does not support the full-width q/k norm (OLMo 2): "
                 "its statistic spans the q (k) heads that tensor parallelism splits across ranks; train it with the "
                 "single-GPU, DDP or FSDP engines (chapters 01, 02, 04, 05)")
+        if getattr(config, "parallel_residual", False):
+            raise ValueError(
+                f"{config.name or config.arch}: tensor parallelism does not support GPT-NeoX's parallel residual: the "
+                "tensor-parallel layer path runs attention and MLP one after the other on separate norms of the "
+                "updated stream; train it with the single-GPU, DDP or FSDP engines (chapters 01, 02, 04, 05)")
         if getattr(config, "all_bias", False):
             raise ValueError(
                 f"{config.name or config.arch}: tensor parallelism does not support biases on the row-parallel "

@@ -14,7 +14,7 @@ from pathlib import Path
 
 import torch
 
-from ..models import build_model, get_config
+from ..models import build_model, get_config, gpt_neox_layout
 from ..parallel.flat import build_groups
 
 
@@ -45,15 +45,23 @@ def consolidate(exp_dir: str, model_name: str, world: int) -> Path:
             if getattr(cfg, "tie_word_embeddings", False) and "lm_head.weight" in sd:
                 sd["lm_head.weight"].copy_(sd["model.embed_tokens.weight"] if "model.embed_tokens.weight" in sd
                                            else sd["lm_head.weight"])
-        torch.save(sd, out)
+        torch.save(_hf_layout(sd, cfg), out)
         return out
     groups = build_groups(model, "cpu", torch.bfloat16, world_size=world, with_grad=False)
     state = {"model": {g.name: torch.zeros(g.padded_numel, dtype=torch.bfloat16) for g in groups}}
     dcp.load(state, checkpoint_id=str(Path(exp_dir) / "checkpoint"))
     for g in groups:
         g.param.copy_(state["model"][g.name])
-    torch.save(model.state_dict(), out)
+    torch.save(_hf_layout(model.state_dict(), cfg), out)
     return out
+
+
+def _hf_layout(sd, cfg):
+    """GPT-NeoX is written under its own HF names and q|k|v layout (``GPTNeoXForCausalLM`` loads it strictly);
+    every other family already has HF's names."""
+    if cfg.arch == "gpt_neox":
+        return gpt_neox_layout.to_hf_state_dict(sd, cfg.num_attention_heads)
+    return sd
 
 
 def main():

@@ -89,12 +89,23 @@ def maybe_load_pretrained(args, model=None, engine=None, default="never") -> boo
     if rank == 0:
         LOGGER.info(f"Loading pretrained weights from {path}")
     if engine is not None:
-        load_into_fsdp(engine, SafetensorsReader(path) if rank == 0 else None)
+        load_into_fsdp(engine, open_checkpoint(path) if rank == 0 else None)
     else:
-        reader = SafetensorsReader(path)
+        reader = open_checkpoint(path)
         load_state_dict_into_flat(model, {k: reader(k) for k in model.state_dict().keys() if k in reader or
                                           k == "lm_head.weight"})
     return True
+
+
+def open_checkpoint(path: str):
+    """``reader(name) -> tensor`` under this project's parameter names: a ``SafetensorsReader``, seen through
+    ``models.gpt_neox_layout`` when the checkpoint is GPT-NeoX's (other names and layout)."""
+    from ..models import get_config, gpt_neox_layout
+
+    reader = SafetensorsReader(path)
+    if gpt_neox_layout.is_gpt_neox_checkpoint(reader.weight_map):
+        return gpt_neox_layout.HFReader(reader, reader.weight_map, get_config(path).num_attention_heads)
+    return reader
 
 
 def load_into_fsdp(engine, get_tensor: Optional[Callable[[str], torch.Tensor]], src_rank: int = 0):
