@@ -8,10 +8,15 @@
 // other dimension is needed in both layouts; one pass over a 128 x 128 tile staged in shared memory writes both with
 // coalesced stores.  Recipe (what ops/reference.py computes with torch's float8 casts):
 //   scale = amax == 0 ? 1 : FP8_MAX / amax            (correctly rounded fp32 division)
+//   scale = scale > FLT_MAX ? FLT_MAX : scale         (a finite amax below FP8_MAX / FLT_MAX overflows the division)
 //   q     = cvt.rn.satfinite(x * scale)               (round to nearest even, saturate finite values at +-FP8_MAX)
-//   scale_inv = 1 / scale
-// A non-finite amax gives scale 0 or NaN, so the outputs are not all finite and the NaN / Inf reaches the GEMM.
+//   scale_inv = 1 / scale                             (2^-128, a subnormal, for the clamped scale)
+// Without the clamp an Inf scale turns every zero into 0 * Inf = NaN.  The clamp is a comparison, not fminf, so a NaN
+// scale stays NaN: a non-finite amax gives scale 0 or NaN, so the outputs are not all finite and the NaN / Inf
+// reaches the GEMM.
 #include <cuda_fp8.h>
+
+#include <cfloat>
 
 #include "api.h"
 #include "common.cuh"
@@ -73,7 +78,8 @@ __global__ void __launch_bounds__(kCastThreads) cast_transpose_kernel(const __nv
                                                                       float* __restrict__ scale_inv) {
   constexpr float kMax = FMT == 1 ? 448.f : 57344.f;
   const float a = *amax;
-  const float scale = a == 0.f ? 1.f : __fdiv_rn(kMax, a);
+  const float s = a == 0.f ? 1.f : __fdiv_rn(kMax, a);
+  const float scale = s > FLT_MAX ? FLT_MAX : s;
   if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) *scale_inv = __fdiv_rn(1.f, scale);
   __shared__ __align__(16) uint8_t tile[kCastTile * kTilePitch];
   const int r0 = blockIdx.y * kCastTile, c0 = blockIdx.x * kCastTile;

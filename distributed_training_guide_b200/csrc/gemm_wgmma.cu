@@ -791,6 +791,20 @@ void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long 
 // with K contiguous (lda / ldb in elements = bytes), fp32 accumulators, bf16 C with row stride ldc.  A is e4m3, or
 // e5m2 when `a_e5m2` (an output gradient); B is e4m3.  The scales are device pointers, so nothing here waits on the
 // kernels that computed them.
+//
+// With deq = fp32(scale_a[0] * scale_b[0]) and acc the accumulator of A8 . B8^T, every element is
+//   overwrite   bf16(fp32(acc * deq))
+//   accumulate  bf16(fp32(acc * deq + C_old))   one rounding (fmaf)
+//   bias        bf16(fp32(acc * deq + bias))    one rounding (fmaf)
+// acc is summed in ascending K, one k32 wgmma step at a time, and the fp8 wgmma does not accumulate in full fp32.
+// Measured on an H100 over random data at the training shapes:
+//   |C - exact| <= 2^-8 |exact| + 0.62 * 2^-13 * deq * sum_t (|S_(t-1)| + sum_(k in t) |a_k b_k|)
+// with S_t the exact partial sum of the first 32 t products.  Products of two fp8 values are exact, subnormals
+// included (the tensor core does not flush them); a NaN operand makes its row / column of C NaN, an e5m2 +-Inf gives
+// +-Inf (NaN against a zero).  Each element's bits depend only on its row of A and column of B, not on the tile, the
+// variant or ldc.  When deq falls below fp32's normal range (operands cast from a tiny amax, whose scale_inv is
+// 2^-128) the output is finite but deq has lost significant bits, so C is far less precise than the product of the
+// dequantised operands; no test holds it to more than being finite.
 void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
               bool a_e5m2, const float* scale_a, const float* scale_b, bool accumulate, int variant, cudaStream_t s,
               const void* bias) {

@@ -178,16 +178,22 @@ def embedding(ids, w):
 
 def fp8_quantize(t, dtype, amax=None):
     """Per-tensor current scaling of ``t`` to ``dtype`` (``torch.float8_e4m3fn`` or ``torch.float8_e5m2``), as the
-    fp8 cast kernels compute it: ``amax = max|t|``, ``scale = FP8_MAX / amax`` in fp32 (1 when amax is 0),
-    ``t8 = round_to_nearest_even(t * scale)`` saturated at +-FP8_MAX.  torch's cast of an out-of-range value gives
-    NaN (e4m3) or Inf (e5m2) instead of saturating, hence the clamp, which keeps NaN.  A non-finite amax makes the
-    scale 0 or NaN, so ``t8`` holds NaN and the non-finite value reaches whatever consumes it.
+    fp8 cast kernels compute it: ``amax = max|t|``, ``scale = FP8_MAX / amax`` in fp32 (1 when amax is 0) clamped
+    to FLT_MAX, ``t8 = round_to_nearest_even(t * scale)`` saturated at +-FP8_MAX.  The clamp matters for a finite
+    ``0 < amax < FP8_MAX / FLT_MAX`` (about 1.3e-36 for e4m3, 1.7e-34 for e5m2), where the division overflows: an
+    Inf scale would turn every zero into NaN and every other element into +-FP8_MAX; it keeps a NaN scale NaN.
+    torch's cast of an out-of-range value gives NaN (e4m3) or Inf (e5m2) instead of saturating, hence the clamp of
+    ``t * scale``, which keeps NaN.  A non-finite amax makes the scale 0 or NaN, so ``t8`` holds NaN and the
+    non-finite value reaches whatever consumes it.
     ``amax`` (a one-element fp32 tensor) is computed from ``t`` when not given.
-    Returns ``(t8, scale_inv)`` with ``scale_inv = 1 / scale`` as a one-element fp32 tensor."""
+    Returns ``(t8, scale_inv)`` with ``scale_inv = 1 / scale`` as a one-element fp32 tensor (2^-128, a subnormal,
+    for the clamped scale)."""
     fp8_max = torch.finfo(dtype).max
+    flt_max = torch.finfo(torch.float32).max
     tf = t.float()
     amax = tf.abs().max().reshape(1) if amax is None else amax.float().reshape(1)
     scale = torch.where(amax == 0, torch.ones_like(amax), torch.full_like(amax, fp8_max) / amax)
+    scale = torch.where(scale > flt_max, torch.full_like(scale, flt_max), scale)
     t8 = (tf * scale).clamp(-fp8_max, fp8_max).to(dtype)
     return t8, torch.ones_like(scale) / scale
 

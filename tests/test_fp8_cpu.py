@@ -51,6 +51,27 @@ def test_quantize_nonfinite_input_stays_nonfinite(bad, dtype):
     assert not bool(torch.isfinite(deq).all()), "a non-finite input must reach the GEMM output"
 
 
+BF16_MIN_SUBNORMAL = 2.0 ** -133
+
+
+@pytest.mark.parametrize("amax", [1e-37, 1e-36, 1e-34, BF16_MIN_SUBNORMAL], ids=["1e-37", "1e-36", "1e-34", "min"])
+@pytest.mark.parametrize("dtype", [E4M3, E5M2], ids=["e4m3", "e5m2"])
+def test_quantize_tiny_amax_stays_finite(dtype, amax):
+    """FP8_MAX / amax overflows fp32 below amax = FP8_MAX / FLT_MAX (1.3e-36 for e4m3, 1.7e-34 for e5m2): the scale is
+    clamped to FLT_MAX, so zeros stay zero and every element still dequantises to within fp8 rounding of x."""
+    top = torch.tensor(amax, dtype=torch.bfloat16).float().item()
+    x = torch.tensor([[0.0, top, -top, 0.5 * top], [-0.0, 0.3 * top, -0.7 * top, 0.0]]).to(torch.bfloat16)
+    t8, scale_inv = ref.fp8_quantize(x, dtype)
+    q = t8.float()
+    assert not bool(torch.isnan(q).any()), q
+    assert (q[x == 0] == 0).all()
+    assert 0 < scale_inv.item() < float("inf")
+    u, sub = (2.0 ** -4, 2.0 ** -9) if dtype == E4M3 else (2.0 ** -3, 2.0 ** -16)   # unit roundoff, least subnormal
+    xd, deq = x.double(), q.double() * scale_inv.double()
+    tol = (u + 2.0 ** -22) * xd.abs() + 0.5 * sub * scale_inv.double()
+    assert ((deq - xd).abs() <= tol).all(), (deq, xd)
+
+
 def test_quantize_rounds_to_nearest_even():
     # with amax 448 the scale is exactly 1: 17 and 19 lie halfway between e4m3 neighbours (16, 18, 20)
     x = torch.tensor([[448.0, 17.0, 19.0, -17.0]])

@@ -49,17 +49,30 @@ def _input(shape, kind, seed=0, std=1.0):
         x[shape[0] // 3, shape[1] // 2] = float("inf")
     elif kind == "wide":   # 1e-8 .. 1e4: subnormals of both formats and saturation-free tails
         x = x * torch.exp(6 * torch.randn(*shape, device="cuda", generator=g))
-    return x.to(torch.bfloat16)
+    elif kind == "tiny":   # amax ~ 4e-37, below FP8_MAX / FLT_MAX of both formats, with zeros
+        x = x * 1e-37
+        x[:, ::5] = 0
+    x = x.to(torch.bfloat16)
+    # views of a larger buffer: "strided" keeps the 16-byte vector path (ld > C, ld % 8 == 0, aligned base),
+    # "misaligned" (base 2 bytes past a 16-byte boundary) and "odd-ld" (ld = C + 3) take the scalar path
+    pad = {"strided": (8, 16), "misaligned": (1, 7), "odd-ld": (0, 3)}.get(kind)
+    if pad is not None:
+        buf = torch.full((shape[0], pad[0] + shape[1] + pad[1]), float("nan"), device="cuda", dtype=torch.bfloat16)
+        view = buf[:, pad[0]:pad[0] + shape[1]]
+        view.copy_(x)
+        x = view
+    return x
 
 
 # ------------------------------------------------------------------------------------------------------------------
 # amax and cast-transpose
 # ------------------------------------------------------------------------------------------------------------------
 CAST_SHAPES = [(1000, 4104), (4096, 4096), (256, 11008), (7, 33), (129, 130)]
+CAST_KINDS = ["normal", "wide", "zeros", "inf", "tiny", "strided", "misaligned", "odd-ld"]
 
 
 @pytest.mark.parametrize("shape", CAST_SHAPES)
-@pytest.mark.parametrize("kind", ["normal", "wide", "zeros", "inf"])
+@pytest.mark.parametrize("kind", CAST_KINDS)
 def test_amax_exact(shape, kind):
     x = _input(shape, kind)
     got = _C().fp8_amax(x)
@@ -74,13 +87,17 @@ def test_amax_strided_view():
 
 
 @pytest.mark.parametrize("shape", CAST_SHAPES)
-@pytest.mark.parametrize("kind", ["normal", "wide", "zeros", "inf"])
+@pytest.mark.parametrize("kind", CAST_KINDS)
 @pytest.mark.parametrize("dtype", [E4M3, E5M2], ids=["e4m3", "e5m2"])
 def test_cast_transpose_exact(shape, kind, dtype):
     x = _input(shape, kind, seed=1)
     amax = _C().fp8_amax(x)
     x8, x8t, scale_inv = _C().fp8_cast_transpose(x, amax, dtype == E5M2, True, True)
-    want8, want_si = ref.fp8_quantize(x.cpu(), dtype)
+    want8, want_si = ref.fp8_quantize(x.cpu(), dtype)   # a view is gathered into a contiguous copy first
+    if kind != "inf":
+        assert not bool(torch.isnan(x8.float()).any()), "a finite input quantised to NaN"
+    if kind == "tiny":
+        assert bool((x8.float()[x == 0] == 0).all()), "a zero did not stay zero"
     assert x8.dtype == dtype and x8.shape == shape and x8t.shape == shape[::-1]
     _same_bits_nan_aware(x8.cpu(), want8)
     assert torch.equal(_bits(x8t), _bits(x8).t()), "the transposed copy is not the transpose of the row-major copy"
