@@ -8,15 +8,48 @@ namespace dtg {
 
 unsigned long long launch_count();
 
+// ---- norm.cu -------------------------------------------------------------------------------
+// Row norms over bf16 [T, H] rows (H % 8 == 0, H <= norm_max_hidden(kind)) with fp32 statistics:
+//   kRms  y = bf16(h * rstd * w)
+//   kLn   y = bf16((h - mean) * rstd * w + b)                                     (StarCoder2)
+//   kLn2  y1, y2 = the kLn output for (w1, b1) and for (w2, b2), one statistic    (GPT-NeoX)
+// with h = x (kNone), h = bf16(x + r) written to h and normalised (kAddBefore), or, kRms only, h = bf16(r + y)
+// written to h instead of y (kAddAfter, OLMo 2's norm-then-add).  LayerNorm rows whose sums overflow fp32 are
+// normalised scaled by 2^-72.
+enum class NormKind : int { kRms, kLn, kLn2 };
+enum class NormRes : int { kNone, kAddBefore, kAddAfter };
+// fp32 [H] gradient planes of a kind: dw; dw, db; dw1, db1, dw2, db2
+constexpr int norm_grad_planes(NormKind k) { return k == NormKind::kRms ? 1 : k == NormKind::kLn ? 2 : 4; }
+int norm_max_hidden(NormKind k);
+// Operands a variant does not use are null.  mean and rstd are fp32 [T]; mean is LayerNorm's only.
+struct NormFwdArgs {
+  const void* x;
+  const void* r;       // kAddBefore / kAddAfter
+  const void* w[2];    // [H] gains; w[1] for kLn2
+  const void* b[2];    // [H] biases (LayerNorm)
+  void* y[2];          // not written by kAddAfter
+  void* h;             // kAddBefore / kAddAfter
+  float* mean;
+  float* rstd;
+};
+void norm_fwd(NormKind k, NormRes res, const NormFwdArgs& a, int T, int H, float eps, cudaStream_t s);
+// Persistent CTAs of the backward (at most T); partial rows per CTA fix the order of the gradient sums.
+int norm_bwd_grid(NormKind k, int T, int H);
+struct NormBwdArgs {
+  const void* dy[2];   // dy[1] for kLn2
+  const void* h;       // the normalised rows (x itself without a residual)
+  const void* w[2];
+  const float* mean;
+  const float* rstd;
+  const void* dres;    // added to dx when given
+  void* dx;
+  float* partial;      // fp32 [norm_grad_planes(k), norm_bwd_grid(k, T, H), H] scratch
+  float* dparams;      // fp32 [norm_grad_planes(k), H], summed from partial in a fixed order
+};
+// 1 + norm_grad_planes(k) launches: the norm kernel, then one colsum per gradient plane
+void norm_bwd(NormKind k, const NormBwdArgs& a, int T, int H, cudaStream_t s);
+
 // ---- elementwise.cu ------------------------------------------------------------------------
-void rmsnorm_fwd(const void* x, const void* res, const void* w, void* y, void* h_out, float* rstd, int T, int H,
-                 float eps, cudaStream_t s);
-// norm-then-add: h_out = bf16(r + bf16(x * rstd * w)), rstd [T] fp32 (the RMSNorm backward of x takes it as is)
-void rmsnorm_add_fwd(const void* x, const void* res, const void* w, void* h_out, float* rstd, int T, int H, float eps,
-                     cudaStream_t s);
-int rmsnorm_bwd_grid(int T);
-void rmsnorm_bwd(const void* dy, const void* h, const void* w, const float* rstd, const void* dres, void* dx,
-                 float* dw_partial, float* dw, int T, int H, cudaStream_t s);
 // rotates the first rot_dim elements (rot_dim % 16 == 0, <= d; d for the full head) of heads [0, n_rot); cos/sin
 // [S, rot_dim/2] or [T, rot_dim/2]
 void rope_inplace(void* qkv, const float* cos, const float* sin, long long T, int S, int n_heads, int n_rot, int d,
@@ -28,33 +61,12 @@ void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s);
 // colsum then adds in a fixed order: no atomics, bit-identical from run to run.
 int bias_grad_chunks(long long T, int N);
 void bias_grad(const void* dy, long long T, int N, long long ld, float* partial, float* db, cudaStream_t s);
-// LayerNorm (StarCoder2): h_out = bf16(x + res) when res is given (else h = x), y = bf16((h - mean) * rstd * w + b);
-// mean, rstd [T] fp32 for the backward.  H % 8 == 0, H <= 16384.
-void layernorm_fwd(const void* x, const void* res, const void* w, const void* b, void* y, void* h_out, float* mean,
-                   float* rstd, int T, int H, float eps, cudaStream_t s);
-int layernorm_bwd_grid(int T, int H);
-// dx = the LayerNorm backward (+ dres); dw, db [H] fp32 summed through dw_partial / db_partial
-// ([layernorm_bwd_grid(T, H), H] fp32 scratch each) in a fixed order
-void layernorm_bwd(const void* dy, const void* h, const void* w, const float* mean, const float* rstd,
-                   const void* dres, void* dx, float* dw_partial, float* db_partial, float* dw, float* db, int T,
-                   int H, cudaStream_t s);
 // GELU with the tanh approximation on n bf16 elements (n % 8 == 0); the backward from the saved pre-activation x
 void gelu_tanh_fwd(const void* x, void* y, long long n, cudaStream_t s);
 void gelu_tanh_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t s);
 // GELU, exact erf form, likewise
 void gelu_fwd(const void* x, void* y, long long n, cudaStream_t s);
 void gelu_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t s);
-// Two LayerNorms over one residual stream (GPT-NeoX): h_out = bf16(x + res) when res is given (else h = x), one mean
-// and rstd [T] fp32, y1 = bf16(xhat * w1 + b1), y2 = bf16(xhat * w2 + b2).  H % 8 == 0, H <= 8192.
-void layernorm2_fwd(const void* x, const void* res, const void* w1, const void* b1, const void* w2, const void* b2,
-                    void* y1, void* y2, void* h_out, float* mean, float* rstd, int T, int H, float eps,
-                    cudaStream_t s);
-int layernorm2_bwd_grid(int T, int H);
-// dx = the backward of both norms (+ dres); dparams [4, H] fp32 = dw1, db1, dw2, db2, summed through partial
-// ([4, layernorm2_bwd_grid(T, H), H] fp32 scratch) in a fixed order
-void layernorm2_bwd(const void* dy1, const void* dy2, const void* h, const void* w1, const void* w2, const float* mean,
-                    const float* rstd, const void* dres, void* dx, float* partial, float* dparams, int T, int H,
-                    cudaStream_t s);
 void swiglu_fwd(const void* gu, void* h, long long T, int I, cudaStream_t s);
 void swiglu_bwd(const void* dh, const void* gu, void* dgu, long long T, int I, cudaStream_t s);
 void embedding_fwd(const long long* ids, const void* w, void* out, long long T, int H, cudaStream_t s);

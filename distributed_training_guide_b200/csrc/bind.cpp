@@ -125,148 +125,176 @@ std::tuple<c10::optional<Tensor>, c10::optional<Tensor>, Tensor> fp8_cast_transp
   return {out, out_t, scale_inv};
 }
 
+// ---- row norms (norm.cu) ------------------------------------------------------------------------------------------
+// Every norm binding validates its arguments with check_norm before it allocates or launches anything, and returns
+// empty outputs and zero gradients for T == 0 without a launch.
+using Named = std::pair<const Tensor*, const char*>;   // an operand and the name its errors use; null: not given
+
+// x (or dy): bf16 [T, H], contiguous and 16-byte aligned, H a positive multiple of 8 up to the kind's limit.  rows:
+// x's shape; params: bf16 [H]; stats: fp32 [T]; all on x's device.  eps, in a forward: finite, > 0 for LayerNorm and
+// >= 0 for RMSNorm.  Returns H.
+int64_t check_norm(const char* who, dtg::NormKind k, Named x, std::initializer_list<Named> rows,
+                   std::initializer_list<Named> params, std::initializer_list<Named> stats, const double* eps) {
+  const Tensor& x0 = *x.first;
+  check_vec(x0, x.second, at::kBFloat16);
+  TORCH_CHECK(x0.dim() == 2, who, ": ", x.second, " must be 2-D [T, H]");
+  const int64_t T = x0.size(0), H = x0.size(1), max_h = dtg::norm_max_hidden(k);
+  TORCH_CHECK(H > 0 && H % 8 == 0 && H <= max_h, who, ": hidden size must be a positive multiple of 8 and <= ", max_h,
+              ", got ", H);
+  for (const auto& [t, name] : rows) {
+    if (!t) continue;
+    check_vec(*t, name, at::kBFloat16);
+    TORCH_CHECK(t->sizes() == x0.sizes() && t->device() == x0.device(), who, ": ", name, " and ", x.second,
+                " differ in shape or device");
+  }
+  for (const auto& [t, name] : params) {
+    check_vec(*t, name, at::kBFloat16);
+    TORCH_CHECK(t->dim() == 1 && t->size(0) == H, who, ": ", name, " must be [H] = [", H, "]");
+    TORCH_CHECK(t->device() == x0.device(), who, ": ", name, " must be on the device of ", x.second);
+  }
+  for (const auto& [t, name] : stats) {
+    if (!t) continue;
+    check_contig(*t, name, at::kFloat);
+    TORCH_CHECK(t->dim() == 1 && t->size(0) == T && t->device() == x0.device(), who, ": ", name, " must be [T] = [", T,
+                "] on the device of ", x.second);
+  }
+  if (eps) {
+    const bool ln = k != dtg::NormKind::kRms;
+    TORCH_CHECK(std::isfinite(*eps) && (ln ? *eps > 0 : *eps >= 0), who, ": eps must be finite and ",
+                ln ? "> 0" : ">= 0", ", got ", *eps);
+  }
+  return H;
+}
+
+c10::optional<Tensor> optional(const Tensor& t) { return t.defined() ? c10::optional<Tensor>(t) : c10::nullopt; }
+
+struct NormOut {
+  Tensor y1, y2, h, mean, rstd;   // undefined where the variant has no such output
+};
+
+// params: w (RMSNorm), w, b (LayerNorm) or w1, b1, w2, b2 (LayerNorm2); r: the residual, or null
+NormOut norm_fwd(const char* who, dtg::NormKind k, dtg::NormRes mode, const Tensor& x, const Tensor* r,
+                 const char* rname, std::initializer_list<Named> params, double eps) {
+  const int64_t H = check_norm(who, k, {&x, "x"}, {{r, rname}}, params, {}, &eps);
+  const c10::cuda::CUDAGuard guard(x.device());
+  const int64_t T = x.size(0);
+  const bool ln = k != dtg::NormKind::kRms;
+  NormOut o;
+  if (mode != dtg::NormRes::kAddAfter) o.y1 = torch::empty_like(x);
+  if (k == dtg::NormKind::kLn2) o.y2 = torch::empty_like(x);
+  if (r) o.h = torch::empty_like(x);
+  if (ln) o.mean = torch::empty({T}, x.options().dtype(at::kFloat));
+  o.rstd = torch::empty({T}, x.options().dtype(at::kFloat));
+  if (T == 0) return o;
+  auto ptr = [](const Tensor& t) { return t.defined() ? t.data_ptr() : nullptr; };
+  dtg::NormFwdArgs a{};
+  a.x = x.data_ptr();
+  a.r = r ? r->data_ptr() : nullptr;
+  const Named* p = params.begin();
+  for (int q = 0; q < (k == dtg::NormKind::kLn2 ? 2 : 1); ++q) {
+    a.w[q] = (p++)->first->data_ptr();
+    if (ln) a.b[q] = (p++)->first->data_ptr();
+  }
+  a.y[0] = ptr(o.y1);
+  a.y[1] = ptr(o.y2);
+  a.h = ptr(o.h);
+  a.mean = ln ? o.mean.data_ptr<float>() : nullptr;
+  a.rstd = o.rstd.data_ptr<float>();
+  dtg::norm_fwd(k, mode, a, (int)T, (int)H, (float)eps, stream());
+  return o;
+}
+
+// (dx, dparams fp32 [norm_grad_planes(k), H]); dx += dres when dres is given
+std::pair<Tensor, Tensor> norm_bwd(const char* who, dtg::NormKind k, const Tensor& dy1, const char* dyname,
+                                   const Tensor* dy2, const Tensor& h, std::initializer_list<Named> gains,
+                                   const Tensor* mean, const Tensor& rstd, const c10::optional<Tensor>& dres) {
+  const Tensor* dr = dres.has_value() ? &*dres : nullptr;
+  const int64_t H = check_norm(who, k, {&dy1, dyname}, {{dy2, "dy2"}, {&h, "h"}, {dr, "dres"}}, gains,
+                               {{mean, "mean"}, {&rstd, "rstd"}}, nullptr);
+  const c10::cuda::CUDAGuard guard(dy1.device());
+  const int64_t T = dy1.size(0), planes = dtg::norm_grad_planes(k);
+  const auto f32 = dy1.options().dtype(at::kFloat);
+  Tensor dx = torch::empty_like(dy1);
+  if (T == 0) return {dx, torch::zeros({planes, H}, f32)};
+  Tensor dparams = torch::empty({planes, H}, f32);
+  Tensor partial = torch::empty({planes, dtg::norm_bwd_grid(k, (int)T, (int)H), H}, f32);
+  dtg::NormBwdArgs a{};
+  a.dy[0] = dy1.data_ptr();
+  a.dy[1] = dy2 ? dy2->data_ptr() : nullptr;
+  a.h = h.data_ptr();
+  int q = 0;
+  for (const auto& g : gains) a.w[q++] = g.first->data_ptr();
+  a.mean = mean ? mean->data_ptr<float>() : nullptr;
+  a.rstd = rstd.data_ptr<float>();
+  a.dres = dr ? dr->data_ptr() : nullptr;
+  a.dx = dx.data_ptr();
+  a.partial = partial.data_ptr<float>();
+  a.dparams = dparams.data_ptr<float>();
+  dtg::norm_bwd(k, a, (int)T, (int)H, stream());
+  return {dx, dparams};
+}
+
+int norm_bwd_grid(dtg::NormKind k, const char* who, int64_t T, int64_t H) {
+  TORCH_CHECK(T > 0 && H > 0 && H % 8 == 0 && H <= dtg::norm_max_hidden(k), who, ": bad shape");
+  return dtg::norm_bwd_grid(k, (int)T, (int)H);
+}
+
+// (y, rstd, h or None): h = bf16(x + residual) when a residual is given, y = RMSNorm(h) * w
 std::tuple<Tensor, Tensor, c10::optional<Tensor>> rmsnorm_fwd(const Tensor& x, const Tensor& w, double eps,
                                                               const c10::optional<Tensor>& res) {
-  check_vec(x, "x", at::kBFloat16);
-  check_vec(w, "w", at::kBFloat16);
-  const c10::cuda::CUDAGuard guard(x.device());
-  const int T = (int)x.size(0), H = (int)x.size(1);
-  TORCH_CHECK(w.numel() == H, "rmsnorm: w must have one entry per column of x");
-  Tensor y = torch::empty_like(x);
-  Tensor rstd = torch::empty({T}, x.options().dtype(at::kFloat));
-  c10::optional<Tensor> h;
-  const void* rp = nullptr;
-  void* hp = nullptr;
-  if (res.has_value()) {
-    check_vec(*res, "residual", at::kBFloat16);
-    TORCH_CHECK(res->sizes() == x.sizes(), "rmsnorm: residual and x differ in shape");
-    h = torch::empty_like(x);
-    rp = res->data_ptr();
-    hp = h->data_ptr();
-  }
-  dtg::rmsnorm_fwd(x.data_ptr(), rp, w.data_ptr(), y.data_ptr(), hp, rstd.data_ptr<float>(), T, H, (float)eps,
-                   stream());
-  return {y, rstd, h};
+  const Tensor* r = res.has_value() ? &*res : nullptr;
+  const NormOut o = norm_fwd("rmsnorm_fwd", dtg::NormKind::kRms, r ? dtg::NormRes::kAddBefore : dtg::NormRes::kNone,
+                             x, r, "residual", {{&w, "w"}}, eps);
+  return {o.y1, o.rstd, optional(o.h)};
 }
 
 // (h, rstd) with h = bf16(r + bf16(rmsnorm(x) * w)): the norm-then-add of OLMo 2's post-sublayer norms
 std::tuple<Tensor, Tensor> rmsnorm_add_fwd(const Tensor& x, const Tensor& r, const Tensor& w, double eps) {
-  check_vec(x, "x", at::kBFloat16);
-  check_vec(r, "r", at::kBFloat16);
-  check_vec(w, "w", at::kBFloat16);
-  TORCH_CHECK(x.dim() == 2, "rmsnorm_add: x must be 2-D [T, H]");
-  TORCH_CHECK(r.sizes() == x.sizes(), "rmsnorm_add: r and x differ in shape");
-  const int T = (int)x.size(0), H = (int)x.size(1);
-  TORCH_CHECK(w.dim() == 1 && w.numel() == H, "rmsnorm_add: w must have one entry per column of x");
-  TORCH_CHECK(H % 8 == 0 && H <= 16384, "rmsnorm_add: hidden size must be a multiple of 8 and <= 16384, got ", H);
-  TORCH_CHECK(std::isfinite(eps) && eps >= 0, "rmsnorm_add: eps must be finite and >= 0");
-  for (const Tensor* t : {&r, &w})
-    TORCH_CHECK(t->device() == x.device(), "rmsnorm_add: every operand must be on the device of x");
-  const c10::cuda::CUDAGuard guard(x.device());
-  Tensor h = torch::empty_like(x);
-  Tensor rstd = torch::empty({T}, x.options().dtype(at::kFloat));
-  if (T > 0)
-    dtg::rmsnorm_add_fwd(x.data_ptr(), r.data_ptr(), w.data_ptr(), h.data_ptr(), rstd.data_ptr<float>(), T, H,
-                         (float)eps, stream());
-  return {h, rstd};
+  const NormOut o = norm_fwd("rmsnorm_add", dtg::NormKind::kRms, dtg::NormRes::kAddAfter, x, &r, "r", {{&w, "w"}}, eps);
+  return {o.h, o.rstd};
 }
 
+// (dx, dw fp32) of y = RMSNorm(h) * w, with dx += dres when dres is given
 std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& h, const Tensor& w, const Tensor& rstd,
                                        const c10::optional<Tensor>& dres) {
-  check_vec(dy, "dy", at::kBFloat16);
-  check_vec(h, "h", at::kBFloat16);
-  check_vec(w, "w", at::kBFloat16);
-  check_contig(rstd, "rstd", at::kFloat);
-  const c10::cuda::CUDAGuard guard(dy.device());
-  const int T = (int)dy.size(0), H = (int)dy.size(1);
-  TORCH_CHECK(h.sizes() == dy.sizes() && w.numel() == H && rstd.numel() == T, "rmsnorm_bwd: shapes differ");
-  Tensor dx = torch::empty_like(dy);
-  Tensor dw = torch::empty({H}, dy.options().dtype(at::kFloat));
-  Tensor partial = torch::empty({dtg::rmsnorm_bwd_grid(T), H}, dy.options().dtype(at::kFloat));
-  const void* dr = nullptr;
-  if (dres.has_value()) {
-    check_vec(*dres, "dres", at::kBFloat16);
-    TORCH_CHECK(dres->sizes() == dy.sizes(), "rmsnorm_bwd: dres and dy differ in shape");
-    dr = dres->data_ptr();
-  }
-  dtg::rmsnorm_bwd(dy.data_ptr(), h.data_ptr(), w.data_ptr(), rstd.data_ptr<float>(), dr, dx.data_ptr(),
-                   partial.data_ptr<float>(), dw.data_ptr<float>(), T, H, stream());
-  return {dx, dw};
-}
-
-// Shared LayerNorm checks: x (or dy) bf16 [T, H] with H % 8 == 0 and H <= 16384, and a [H] gain; returns H.
-int64_t check_layernorm(const Tensor& x, const char* xname, const Tensor& w, const char* who) {
-  check_vec(x, xname, at::kBFloat16);
-  TORCH_CHECK(x.dim() == 2, who, ": ", xname, " must be 2-D [T, H]");
-  const int64_t H = x.size(1);
-  TORCH_CHECK(H % 8 == 0 && H > 0 && H <= 16384, who, ": hidden size must be a positive multiple of 8 and <= 16384, got ",
-              H);
-  check_vec(w, "w", at::kBFloat16);
-  TORCH_CHECK(w.dim() == 1 && w.size(0) == H, who, ": w must be [H] = [", H, "]");
-  TORCH_CHECK(w.device() == x.device(), who, ": w must be on the device of ", xname);
-  return H;
+  auto [dx, d] = norm_bwd("rmsnorm_bwd", dtg::NormKind::kRms, dy, "dy", nullptr, h, {{&w, "w"}}, nullptr, rstd, dres);
+  return {dx, d[0]};
 }
 
 // (y, h or None, mean, rstd): h = bf16(x + residual) when a residual is given, y = LayerNorm(h) * w + b
 std::tuple<Tensor, c10::optional<Tensor>, Tensor, Tensor> layernorm_fwd(const Tensor& x,
                                                                        const c10::optional<Tensor>& res,
                                                                        const Tensor& w, const Tensor& b, double eps) {
-  const int64_t H = check_layernorm(x, "x", w, "layernorm_fwd");
-  check_vec(b, "b", at::kBFloat16);
-  TORCH_CHECK(b.dim() == 1 && b.size(0) == H, "layernorm_fwd: b must be [H] = [", H, "]");
-  TORCH_CHECK(b.device() == x.device(), "layernorm_fwd: b must be on the device of x");
-  TORCH_CHECK(std::isfinite(eps) && eps > 0, "layernorm_fwd: eps must be finite and > 0, got ", eps);
-  const void* rp = nullptr;
-  if (res.has_value()) {
-    check_vec(*res, "residual", at::kBFloat16);
-    TORCH_CHECK(res->sizes() == x.sizes(), "layernorm_fwd: residual and x differ in shape");
-    TORCH_CHECK(res->device() == x.device(), "layernorm_fwd: residual must be on the device of x");
-    rp = res->data_ptr();
-  }
-  const c10::cuda::CUDAGuard guard(x.device());
-  const int64_t T = x.size(0);
-  Tensor y = torch::empty_like(x);
-  Tensor mean = torch::empty({T}, x.options().dtype(at::kFloat));
-  Tensor rstd = torch::empty({T}, x.options().dtype(at::kFloat));
-  c10::optional<Tensor> h;
-  if (rp) h = torch::empty_like(x);
-  if (T > 0)
-    dtg::layernorm_fwd(x.data_ptr(), rp, w.data_ptr(), b.data_ptr(), y.data_ptr(), h ? h->data_ptr() : nullptr,
-                       mean.data_ptr<float>(), rstd.data_ptr<float>(), (int)T, (int)H, (float)eps, stream());
-  return {y, h, mean, rstd};
+  const Tensor* r = res.has_value() ? &*res : nullptr;
+  const NormOut o = norm_fwd("layernorm_fwd", dtg::NormKind::kLn, r ? dtg::NormRes::kAddBefore : dtg::NormRes::kNone,
+                             x, r, "residual", {{&w, "w"}, {&b, "b"}}, eps);
+  return {o.y1, optional(o.h), o.mean, o.rstd};
 }
 
 // (dx, dw fp32, db fp32) of y = LayerNorm(h) * w + b, with dx += dres when dres is given
 std::tuple<Tensor, Tensor, Tensor> layernorm_bwd(const Tensor& dy, const Tensor& h, const Tensor& w, const Tensor& mean,
                                                  const Tensor& rstd, const c10::optional<Tensor>& dres) {
-  const int64_t H = check_layernorm(dy, "dy", w, "layernorm_bwd");
-  check_vec(h, "h", at::kBFloat16);
-  TORCH_CHECK(h.sizes() == dy.sizes() && h.device() == dy.device(),
-              "layernorm_bwd: h and dy differ in shape or device");
-  const int64_t T = dy.size(0);
-  for (const Tensor* t : {&mean, &rstd}) {
-    check_contig(*t, t == &mean ? "mean" : "rstd", at::kFloat);
-    TORCH_CHECK(t->dim() == 1 && t->size(0) == T && t->device() == dy.device(), "layernorm_bwd: ",
-                t == &mean ? "mean" : "rstd", " must be [T] = [", T, "] on the device of dy");
-  }
-  const void* dr = nullptr;
-  if (dres.has_value()) {
-    check_vec(*dres, "dres", at::kBFloat16);
-    TORCH_CHECK(dres->sizes() == dy.sizes() && dres->device() == dy.device(),
-                "layernorm_bwd: dres and dy differ in shape or device");
-    dr = dres->data_ptr();
-  }
-  const c10::cuda::CUDAGuard guard(dy.device());
-  Tensor dx = torch::empty_like(dy);
-  Tensor dw = torch::zeros({H}, dy.options().dtype(at::kFloat));
-  Tensor db = torch::zeros({H}, dy.options().dtype(at::kFloat));
-  if (T > 0) {
-    Tensor partial = torch::empty({2, dtg::layernorm_bwd_grid((int)T, (int)H), H}, dy.options().dtype(at::kFloat));
-    dtg::layernorm_bwd(dy.data_ptr(), h.data_ptr(), w.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(), dr,
-                       dx.data_ptr(), partial[0].data_ptr<float>(), partial[1].data_ptr<float>(),
-                       dw.data_ptr<float>(), db.data_ptr<float>(), (int)T, (int)H, stream());
-  }
-  return {dx, dw, db};
+  auto [dx, d] = norm_bwd("layernorm_bwd", dtg::NormKind::kLn, dy, "dy", nullptr, h, {{&w, "w"}}, &mean, rstd, dres);
+  return {dx, d[0], d[1]};
+}
+
+// (y1, y2, h or None, mean, rstd): h = bf16(x + residual) when a residual is given, y_i = LayerNorm(h) * w_i + b_i
+std::tuple<Tensor, Tensor, c10::optional<Tensor>, Tensor, Tensor> layernorm2_fwd(
+    const Tensor& x, const c10::optional<Tensor>& res, const Tensor& w1, const Tensor& b1, const Tensor& w2,
+    const Tensor& b2, double eps) {
+  const Tensor* r = res.has_value() ? &*res : nullptr;
+  const NormOut o = norm_fwd("layernorm2_fwd", dtg::NormKind::kLn2, r ? dtg::NormRes::kAddBefore : dtg::NormRes::kNone,
+                             x, r, "residual", {{&w1, "w1"}, {&b1, "b1"}, {&w2, "w2"}, {&b2, "b2"}}, eps);
+  return {o.y1, o.y2, optional(o.h), o.mean, o.rstd};
+}
+
+// (dx, dparams fp32 [4, H] = dw1, db1, dw2, db2) of the two LayerNorms, with dx += dres when dres is given
+std::tuple<Tensor, Tensor> layernorm2_bwd(const Tensor& dy1, const Tensor& dy2, const Tensor& h, const Tensor& w1,
+                                          const Tensor& w2, const Tensor& mean, const Tensor& rstd,
+                                          const c10::optional<Tensor>& dres) {
+  auto [dx, d] = norm_bwd("layernorm2_bwd", dtg::NormKind::kLn2, dy1, "dy1", &dy2, h, {{&w1, "w1"}, {&w2, "w2"}}, &mean,
+                          rstd, dres);
+  return {dx, d};
 }
 
 Tensor gelu_tanh_fwd(const Tensor& x) {
@@ -327,86 +355,6 @@ Tensor gelu_bwd(const Tensor& dy, const Tensor& x) {
   Tensor dx = torch::empty_like(x);
   if (x.numel() > 0) dtg::gelu_bwd(dy.data_ptr(), x.data_ptr(), dx.data_ptr(), x.numel(), stream());
   return dx;
-}
-
-// Checks of the dual LayerNorm: x (or dy1) bf16 [T, H] with H % 8 == 0 and H <= 8192, and [H] bf16 gains / biases
-// on its device; returns H.
-int64_t check_layernorm2(const Tensor& x, const char* xname, std::initializer_list<std::pair<const Tensor*, const char*>> params,
-                         const char* who) {
-  check_vec(x, xname, at::kBFloat16);
-  TORCH_CHECK(x.dim() == 2, who, ": ", xname, " must be 2-D [T, H]");
-  const int64_t H = x.size(1);
-  TORCH_CHECK(H % 8 == 0 && H > 0 && H <= 8192, who, ": hidden size must be a positive multiple of 8 and <= 8192, got ",
-              H);
-  for (const auto& p : params) {
-    check_vec(*p.first, p.second, at::kBFloat16);
-    TORCH_CHECK(p.first->dim() == 1 && p.first->size(0) == H, who, ": ", p.second, " must be [H] = [", H, "]");
-    TORCH_CHECK(p.first->device() == x.device(), who, ": ", p.second, " must be on the device of ", xname);
-  }
-  return H;
-}
-
-// (y1, y2, h or None, mean, rstd): h = bf16(x + residual) when a residual is given, y_i = LayerNorm(h) * w_i + b_i
-std::tuple<Tensor, Tensor, c10::optional<Tensor>, Tensor, Tensor> layernorm2_fwd(
-    const Tensor& x, const c10::optional<Tensor>& res, const Tensor& w1, const Tensor& b1, const Tensor& w2,
-    const Tensor& b2, double eps) {
-  const int64_t H = check_layernorm2(x, "x", {{&w1, "w1"}, {&b1, "b1"}, {&w2, "w2"}, {&b2, "b2"}}, "layernorm2_fwd");
-  TORCH_CHECK(std::isfinite(eps) && eps > 0, "layernorm2_fwd: eps must be finite and > 0, got ", eps);
-  const void* rp = nullptr;
-  if (res.has_value()) {
-    check_vec(*res, "residual", at::kBFloat16);
-    TORCH_CHECK(res->sizes() == x.sizes(), "layernorm2_fwd: residual and x differ in shape");
-    TORCH_CHECK(res->device() == x.device(), "layernorm2_fwd: residual must be on the device of x");
-    rp = res->data_ptr();
-  }
-  const c10::cuda::CUDAGuard guard(x.device());
-  const int64_t T = x.size(0);
-  Tensor y1 = torch::empty_like(x), y2 = torch::empty_like(x);
-  Tensor mean = torch::empty({T}, x.options().dtype(at::kFloat));
-  Tensor rstd = torch::empty({T}, x.options().dtype(at::kFloat));
-  c10::optional<Tensor> h;
-  if (rp) h = torch::empty_like(x);
-  if (T > 0)
-    dtg::layernorm2_fwd(x.data_ptr(), rp, w1.data_ptr(), b1.data_ptr(), w2.data_ptr(), b2.data_ptr(), y1.data_ptr(),
-                        y2.data_ptr(), h ? h->data_ptr() : nullptr, mean.data_ptr<float>(), rstd.data_ptr<float>(),
-                        (int)T, (int)H, (float)eps, stream());
-  return {y1, y2, h, mean, rstd};
-}
-
-// (dx, dparams fp32 [4, H] = dw1, db1, dw2, db2) of the two LayerNorms, with dx += dres when dres is given
-std::tuple<Tensor, Tensor> layernorm2_bwd(const Tensor& dy1, const Tensor& dy2, const Tensor& h, const Tensor& w1,
-                                          const Tensor& w2, const Tensor& mean, const Tensor& rstd,
-                                          const c10::optional<Tensor>& dres) {
-  const int64_t H = check_layernorm2(dy1, "dy1", {{&w1, "w1"}, {&w2, "w2"}}, "layernorm2_bwd");
-  for (const Tensor* t : {&dy2, &h}) {
-    const char* name = t == &dy2 ? "dy2" : "h";
-    check_vec(*t, name, at::kBFloat16);
-    TORCH_CHECK(t->sizes() == dy1.sizes() && t->device() == dy1.device(), "layernorm2_bwd: ", name,
-                " and dy1 differ in shape or device");
-  }
-  const int64_t T = dy1.size(0);
-  for (const Tensor* t : {&mean, &rstd}) {
-    check_contig(*t, t == &mean ? "mean" : "rstd", at::kFloat);
-    TORCH_CHECK(t->dim() == 1 && t->size(0) == T && t->device() == dy1.device(), "layernorm2_bwd: ",
-                t == &mean ? "mean" : "rstd", " must be [T] = [", T, "] on the device of dy1");
-  }
-  const void* dr = nullptr;
-  if (dres.has_value()) {
-    check_vec(*dres, "dres", at::kBFloat16);
-    TORCH_CHECK(dres->sizes() == dy1.sizes() && dres->device() == dy1.device(),
-                "layernorm2_bwd: dres and dy1 differ in shape or device");
-    dr = dres->data_ptr();
-  }
-  const c10::cuda::CUDAGuard guard(dy1.device());
-  Tensor dx = torch::empty_like(dy1);
-  Tensor dparams = torch::zeros({4, H}, dy1.options().dtype(at::kFloat));
-  if (T > 0) {
-    Tensor partial = torch::empty({4, dtg::layernorm2_bwd_grid((int)T, (int)H), H}, dy1.options().dtype(at::kFloat));
-    dtg::layernorm2_bwd(dy1.data_ptr(), dy2.data_ptr(), h.data_ptr(), w1.data_ptr(), w2.data_ptr(),
-                        mean.data_ptr<float>(), rstd.data_ptr<float>(), dr, dx.data_ptr(), partial.data_ptr<float>(),
-                        dparams.data_ptr<float>(), (int)T, (int)H, stream());
-  }
-  return {dx, dparams};
 }
 
 // Shared checks of qk_norm_rope_fwd / _bwd and, with `full`, of the full-width qk_norm_full_rope_fwd / _bwd (gains
@@ -651,10 +599,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("eps"));
   m.def("layernorm_bwd", &layernorm_bwd, py::arg("dy"), py::arg("h"), py::arg("w"), py::arg("mean"),
         py::arg("rstd"), py::arg("dres") = py::none());
-  m.def("layernorm_bwd_grid", [](int64_t T, int64_t H) {
-    TORCH_CHECK(T > 0 && H > 0 && H % 8 == 0 && H <= 16384, "layernorm_bwd_grid: bad shape");
-    return dtg::layernorm_bwd_grid((int)T, (int)H);
-  });
+  m.def("layernorm_bwd_grid",
+        [](int64_t T, int64_t H) { return norm_bwd_grid(dtg::NormKind::kLn, "layernorm_bwd_grid", T, H); });
   m.def("gelu_tanh_fwd", &gelu_tanh_fwd, py::arg("x"));
   m.def("gelu_tanh_bwd", &gelu_tanh_bwd, py::arg("dy"), py::arg("x"));
   m.def("gelu_fwd", &gelu_fwd, py::arg("x"));
@@ -663,10 +609,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("w2"), py::arg("b2"), py::arg("eps"));
   m.def("layernorm2_bwd", &layernorm2_bwd, py::arg("dy1"), py::arg("dy2"), py::arg("h"), py::arg("w1"),
         py::arg("w2"), py::arg("mean"), py::arg("rstd"), py::arg("dres") = py::none());
-  m.def("layernorm2_bwd_grid", [](int64_t T, int64_t H) {
-    TORCH_CHECK(T > 0 && H > 0 && H % 8 == 0 && H <= 8192, "layernorm2_bwd_grid: bad shape");
-    return dtg::layernorm2_bwd_grid((int)T, (int)H);
-  });
+  m.def("layernorm2_bwd_grid",
+        [](int64_t T, int64_t H) { return norm_bwd_grid(dtg::NormKind::kLn2, "layernorm2_bwd_grid", T, H); });
   m.def("swiglu_fwd", &swiglu_fwd);
   m.def("swiglu_bwd", &swiglu_bwd);
   m.def("cross_entropy_fwd_bwd", &cross_entropy_fwd_bwd);

@@ -1,234 +1,13 @@
-// Memory-bound ops of the Llama step, hand-written for sm_90a:
-//   fused (residual add +) RMSNorm fwd / bwd, in-place RoPE on the fused qkv activation,
-//   SwiGLU fwd / bwd, embedding gather / scatter-add, scalar scale, the bias gradient (column sums),
-//   fused (residual add +) LayerNorm fwd / bwd and GELU-tanh fwd / bwd (StarCoder2).
+// Memory-bound ops of the Llama step, hand-written for sm_90a: in-place RoPE on the fused qkv activation,
+//   SwiGLU fwd / bwd, embedding gather / scatter-add, scalar scale, the bias gradient and the fixed-order column
+//   sums the norm backwards share, GELU-tanh (StarCoder2) and exact GELU fwd / bwd.  The row norms are in norm.cu.
 // All are pure-bandwidth kernels: 16-byte vector accesses, fp32 math in registers, one pass
-// over the activations (the row is cached in registers between the statistic and the
-// normalisation).  Replaces the ~6 ATen kernels per RMSNorm / ~10 per RoPE the reference runs
+// over the activations.  Replaces the ~10 ATen kernels per RoPE the reference runs
 // in eager chapters, and Inductor's Triton fusions in compiled ones (SURVEY.md K4-K6, K9, K10).
 #include "api.h"
 #include "common.cuh"
 
 namespace dtg {
-
-// ------------------------------------------------------------------------------------------
-// RMSNorm forward:  h = x (+ r);  y = h * rsqrt(mean(h^2) + eps) * w
-// one CTA per row; each thread keeps its slice of the row in registers (<= kMaxVec 16B vectors)
-// ------------------------------------------------------------------------------------------
-// NV = 16-byte vectors cached per thread, NT = threads per CTA; NV*NT*8 >= H.
-template <int kMaxVec, int kNormThreads, bool HAS_RES>
-__global__ void __launch_bounds__(kNormThreads) rmsnorm_fwd_kernel(
-    const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w,
-    __nv_bfloat16* __restrict__ y, __nv_bfloat16* __restrict__ h_out, float* __restrict__ rstd_out, int H,
-    float eps) {
-  __shared__ float red[32];
-  const int row = blockIdx.x;
-  const int nvec = H >> 3;
-  const __nv_bfloat16* xr = x + (size_t)row * H;
-  const __nv_bfloat16* rr = HAS_RES ? r + (size_t)row * H : nullptr;
-  bf16x8 cache[kMaxVec];
-  float ss = 0.f;
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      bf16x8 v = ld8(xr + i * 8);
-      float f[8];
-      unpack8(v, f);
-      if (HAS_RES) {
-        float g[8];
-        unpack8(ld8(rr + i * 8), g);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] += g[j];
-        v = pack8(f);          // the residual stream is stored (and normalised) in bf16
-        unpack8(v, f);
-        st8(h_out + (size_t)row * H + i * 8, v);
-      }
-      cache[k] = v;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) ss += f[j] * f[j];
-    }
-  }
-  ss = block_sum(ss, red);
-  const float rstd = rsqrtf(ss / (float)H + eps);
-  if (threadIdx.x == 0) rstd_out[row] = rstd;
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      float f[8], g[8];
-      unpack8(cache[k], f);
-      unpack8(ld8(w + i * 8), g);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = f[j] * rstd * g[j];
-      st8(y + (size_t)row * H + i * 8, pack8(f));
-    }
-  }
-}
-
-// Pick (NV, NT) for a hidden size: 128 threads up to H=8192, 256 threads up to 16384.
-#define DTG_NORM_DISPATCH(H, CALL)                                         \
-  do {                                                                     \
-    const int nvec_ = (H) >> 3;                                            \
-    if (nvec_ <= 128) { CALL(1, 128); }                                    \
-    else if (nvec_ <= 256) { CALL(2, 128); }                               \
-    else if (nvec_ <= 512) { CALL(4, 128); }                               \
-    else if (nvec_ <= 1024) { CALL(8, 128); }                              \
-    else if (nvec_ <= 2048) { CALL(8, 256); }                              \
-    else throw std::runtime_error("rmsnorm: hidden size > 16384 unsupported"); \
-  } while (0)
-
-void rmsnorm_fwd(const void* x, const void* res, const void* w, void* y, void* h_out, float* rstd, int T, int H,
-                 float eps, cudaStream_t s) {
-  if (H % 8 != 0) throw std::runtime_error("rmsnorm: hidden size must be a multiple of 8");
-  auto X = (const __nv_bfloat16*)x;
-  auto R = (const __nv_bfloat16*)res;
-  auto W = (const __nv_bfloat16*)w;
-#define CALL_FWD(NV, NT)                                                                                       \
-  if (res)                                                                                                     \
-    rmsnorm_fwd_kernel<NV, NT, true><<<T, NT, 0, s>>>(X, R, W, (__nv_bfloat16*)y, (__nv_bfloat16*)h_out, rstd, H, eps); \
-  else                                                                                                         \
-    rmsnorm_fwd_kernel<NV, NT, false><<<T, NT, 0, s>>>(X, R, W, (__nv_bfloat16*)y, nullptr, rstd, H, eps);
-  DTG_NORM_DISPATCH(H, CALL_FWD);
-#undef CALL_FWD
-  note_launch();
-  DTG_LAUNCH_CHECK();
-}
-
-// ------------------------------------------------------------------------------------------
-// Norm-then-add (OLMo 2's post-sublayer norms):  h = bf16(r + bf16(x * rsqrt(mean(x^2) + eps) * w))
-// The statistic and the normalisation are rmsnorm_fwd_kernel's without a residual, operation for operation, so h is
-// bit-identical to rmsnorm_fwd followed by a bf16 add; y is never written.
-// ------------------------------------------------------------------------------------------
-template <int kMaxVec, int kNormThreads>
-__global__ void __launch_bounds__(kNormThreads) rmsnorm_add_fwd_kernel(
-    const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w,
-    __nv_bfloat16* __restrict__ h_out, float* __restrict__ rstd_out, int H, float eps) {
-  __shared__ float red[32];
-  const int row = blockIdx.x;
-  const int nvec = H >> 3;
-  const __nv_bfloat16* xr = x + (size_t)row * H;
-  bf16x8 cache[kMaxVec];
-  float ss = 0.f;
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      cache[k] = ld8(xr + i * 8);
-      float f[8];
-      unpack8(cache[k], f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) ss += f[j] * f[j];
-    }
-  }
-  ss = block_sum(ss, red);
-  const float rstd = rsqrtf(ss / (float)H + eps);
-  if (threadIdx.x == 0) rstd_out[row] = rstd;
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      float f[8], g[8], fr[8];
-      unpack8(cache[k], f);
-      unpack8(ld8(w + i * 8), g);
-      unpack8(ld8(r + (size_t)row * H + i * 8), fr);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = f[j] * rstd * g[j];
-      unpack8(pack8(f), f);   // the normalised branch is rounded to bf16 before the add
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] += fr[j];
-      st8(h_out + (size_t)row * H + i * 8, pack8(f));
-    }
-  }
-}
-
-void rmsnorm_add_fwd(const void* x, const void* res, const void* w, void* h_out, float* rstd, int T, int H, float eps,
-                     cudaStream_t s) {
-  if (H % 8 != 0) throw std::runtime_error("rmsnorm: hidden size must be a multiple of 8");
-  auto X = (const __nv_bfloat16*)x;
-  auto R = (const __nv_bfloat16*)res;
-  auto W = (const __nv_bfloat16*)w;
-#define CALL_ADD(NV, NT) \
-  rmsnorm_add_fwd_kernel<NV, NT><<<T, NT, 0, s>>>(X, R, W, (__nv_bfloat16*)h_out, rstd, H, eps);
-  DTG_NORM_DISPATCH(H, CALL_ADD);
-#undef CALL_ADD
-  note_launch();
-  DTG_LAUNCH_CHECK();
-}
-
-// ------------------------------------------------------------------------------------------
-// RMSNorm backward.  xhat = h*rstd, g = dy*w:
-//   dx = rstd * (g - xhat * mean(g*xhat)) (+ dres),   dw = sum_rows dy * xhat
-// Persistent CTAs stride over rows and keep their dw partial in registers; partials go to a
-// [grid, H] fp32 scratch reduced by a second kernel (deterministic, no atomics).
-// ------------------------------------------------------------------------------------------
-template <int kMaxVec, int kNormThreads, bool HAS_DRES>
-__global__ void __launch_bounds__(kNormThreads) rmsnorm_bwd_kernel(
-    const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restrict__ w,
-    const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres, __nv_bfloat16* __restrict__ dx,
-    float* __restrict__ dw_partial, int T, int H) {
-  __shared__ float red[32];
-  const int nvec = H >> 3;
-  float dw_acc[kMaxVec][8];
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) dw_acc[k][j] = 0.f;
-
-  for (int row = blockIdx.x; row < T; row += gridDim.x) {
-    const float rs = rstd[row];
-    const size_t base = (size_t)row * H;
-    float dot = 0.f;
-    bf16x8 cg[kMaxVec], cx[kMaxVec];  // g = dy*w (as bf16-rounded dy and fp32 recompute) / h
-#pragma unroll
-    for (int k = 0; k < kMaxVec; ++k) {
-      const int i = threadIdx.x + k * kNormThreads;
-      if (i < nvec) {
-        cg[k] = ld8(dy + base + i * 8);
-        cx[k] = ld8(h + base + i * 8);
-        float fdy[8], fx[8], fw[8];
-        unpack8(cg[k], fdy);
-        unpack8(cx[k], fx);
-        unpack8(ld8(w + i * 8), fw);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float xhat = fx[j] * rs;
-          dot += fdy[j] * fw[j] * xhat;
-          dw_acc[k][j] += fdy[j] * xhat;
-        }
-      }
-    }
-    dot = block_sum(dot, red) / (float)H;
-#pragma unroll
-    for (int k = 0; k < kMaxVec; ++k) {
-      const int i = threadIdx.x + k * kNormThreads;
-      if (i < nvec) {
-        float fdy[8], fx[8], fw[8], out[8];
-        unpack8(cg[k], fdy);
-        unpack8(cx[k], fx);
-        unpack8(ld8(w + i * 8), fw);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) out[j] = rs * (fdy[j] * fw[j] - fx[j] * rs * dot);
-        if (HAS_DRES) {
-          float fr[8];
-          unpack8(ld8(dres + base + i * 8), fr);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) out[j] += fr[j];
-        }
-        st8(dx + base + i * 8, pack8(out));
-      }
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      float4* dst = reinterpret_cast<float4*>(dw_partial + (size_t)blockIdx.x * H + i * 8);
-      dst[0] = make_float4(dw_acc[k][0], dw_acc[k][1], dw_acc[k][2], dw_acc[k][3]);
-      dst[1] = make_float4(dw_acc[k][4], dw_acc[k][5], dw_acc[k][6], dw_acc[k][7]);
-    }
-  }
-}
 
 // out[c] = sum_r partial[r][c]: 32 columns x 8 row lanes per CTA (coalesced 128 B row segments),
 // fixed summation order (deterministic)
@@ -249,10 +28,6 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ p
     out[c] = t;
   }
 }
-
-// enough CTAs in flight to cover HBM latency (each keeps a dw partial in registers; the partials cost
-// grid*H*4 bytes of extra traffic, 19 MB at H=4096)
-int rmsnorm_bwd_grid(int T) { return T < 8 * sm_count() ? T : 8 * sm_count(); }
 
 void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s) {
   colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(partial, out, rows, H);
@@ -326,531 +101,6 @@ void bias_grad(const void* dy, long long T, int N, long long ld, float* partial,
       (const __nv_bfloat16*)dy, T, N, ld, rpc, partial);
   colsum_kernel<<<(N + 31) / 32, 256, 0, s>>>(partial, db, chunks, N);
   note_launch(2);
-  DTG_LAUNCH_CHECK();
-}
-
-void rmsnorm_bwd(const void* dy, const void* h, const void* w, const float* rstd, const void* dres, void* dx,
-                 float* dw_partial, float* dw, int T, int H, cudaStream_t s) {
-  if (H % 8 != 0) throw std::runtime_error("rmsnorm: hidden size must be a multiple of 8");
-  const int grid = rmsnorm_bwd_grid(T);
-  auto DY = (const __nv_bfloat16*)dy;
-  auto HH = (const __nv_bfloat16*)h;
-  auto W = (const __nv_bfloat16*)w;
-  auto DR = (const __nv_bfloat16*)dres;
-#define CALL_BWD(NV, NT)                                                                                          \
-  if (dres)                                                                                                       \
-    rmsnorm_bwd_kernel<NV, NT, true><<<grid, NT, 0, s>>>(DY, HH, W, rstd, DR, (__nv_bfloat16*)dx, dw_partial, T, H); \
-  else                                                                                                            \
-    rmsnorm_bwd_kernel<NV, NT, false><<<grid, NT, 0, s>>>(DY, HH, W, rstd, nullptr, (__nv_bfloat16*)dx, dw_partial, T, H);
-  DTG_NORM_DISPATCH(H, CALL_BWD);
-#undef CALL_BWD
-  colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(dw_partial, dw, grid, H);
-  note_launch(2);
-  DTG_LAUNCH_CHECK();
-}
-
-// ------------------------------------------------------------------------------------------
-// LayerNorm forward (StarCoder2):  h = bf16(x (+ r));  y = bf16((h - mean) * rstd * w + b)
-//   mean = sum(h) / H,  var = sum((h - mean)^2) / H (a second pass over the cached row),  rstd = rsqrt(var + eps)
-// One CTA per row with the row cached in registers, as rmsnorm_fwd_kernel.  A row whose sums overflow fp32 (elements
-// near the bf16 limit) is redone scaled by 2^-72, which is exact for every element above 2^-77; mean and rstd are
-// saved in the row's own units.
-// ------------------------------------------------------------------------------------------
-constexpr float kLnDown = 0x1p-72f, kLnUp = 0x1p72f;
-
-// this thread's sum of h * scale, and of (h * scale - mean)^2, over its cached vectors
-template <int kMaxVec, int kNormThreads>
-__device__ __forceinline__ float ln_sum(const bf16x8 (&cache)[kMaxVec], int nvec, float scale) {
-  float s = 0.f;
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    if (threadIdx.x + k * kNormThreads < nvec) {
-      float f[8];
-      unpack8(cache[k], f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s += f[j] * scale;
-    }
-  }
-  return s;
-}
-template <int kMaxVec, int kNormThreads>
-__device__ __forceinline__ float ln_sq_dev(const bf16x8 (&cache)[kMaxVec], int nvec, float mean, float scale) {
-  float s = 0.f;
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    if (threadIdx.x + k * kNormThreads < nvec) {
-      float f[8];
-      unpack8(cache[k], f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float d = f[j] * scale - mean;
-        s += d * d;
-      }
-    }
-  }
-  return s;
-}
-
-template <int kMaxVec, int kNormThreads, bool HAS_RES>
-__global__ void __launch_bounds__(kNormThreads) layernorm_fwd_kernel(
-    const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w,
-    const __nv_bfloat16* __restrict__ b, __nv_bfloat16* __restrict__ y, __nv_bfloat16* __restrict__ h_out,
-    float* __restrict__ mean_out, float* __restrict__ rstd_out, int H, float eps) {
-  __shared__ float red[32];
-  const int row = blockIdx.x;
-  const int nvec = H >> 3;
-  const __nv_bfloat16* xr = x + (size_t)row * H;
-  const __nv_bfloat16* rr = HAS_RES ? r + (size_t)row * H : nullptr;
-  bf16x8 cache[kMaxVec];
-  float sum = 0.f;
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      bf16x8 v = ld8(xr + i * 8);
-      float f[8];
-      unpack8(v, f);
-      if (HAS_RES) {
-        float g[8];
-        unpack8(ld8(rr + i * 8), g);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] += g[j];
-        v = pack8(f);          // the residual stream is stored (and normalised) in bf16
-        unpack8(v, f);
-        st8(h_out + (size_t)row * H + i * 8, v);
-      }
-      cache[k] = v;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sum += f[j];
-    }
-  }
-  float scale = 1.f;
-  float mean = block_sum(sum, red) / (float)H;
-  float ss = block_sum(ln_sq_dev<kMaxVec, kNormThreads>(cache, nvec, mean, 1.f), red);
-  if (!(isfinite(mean) && isfinite(ss))) {   // uniform over the CTA: block_sum broadcasts
-    scale = kLnDown;
-    mean = block_sum(ln_sum<kMaxVec, kNormThreads>(cache, nvec, kLnDown), red) / (float)H;
-    ss = block_sum(ln_sq_dev<kMaxVec, kNormThreads>(cache, nvec, mean, kLnDown), red);
-  }
-  const float rstd = rsqrtf(ss / (float)H + eps * scale * scale);
-  if (threadIdx.x == 0) {
-    mean_out[row] = scale == 1.f ? mean : mean * kLnUp;
-    rstd_out[row] = scale == 1.f ? rstd : rstd * kLnDown;
-  }
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      float f[8], g[8], c[8];
-      unpack8(cache[k], f);
-      unpack8(ld8(w + i * 8), g);
-      unpack8(ld8(b + i * 8), c);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[j] = (f[j] * scale - mean) * rstd * g[j] + c[j];
-      st8(y + (size_t)row * H + i * 8, pack8(f));
-    }
-  }
-}
-
-void layernorm_fwd(const void* x, const void* res, const void* w, const void* b, void* y, void* h_out, float* mean,
-                   float* rstd, int T, int H, float eps, cudaStream_t s) {
-  if (H % 8 != 0) throw std::runtime_error("layernorm: hidden size must be a multiple of 8");
-  auto X = (const __nv_bfloat16*)x;
-  auto R = (const __nv_bfloat16*)res;
-  auto W = (const __nv_bfloat16*)w;
-  auto B = (const __nv_bfloat16*)b;
-  auto Y = (__nv_bfloat16*)y;
-#define CALL_LN_FWD(NV, NT)                                                                                  \
-  if (res)                                                                                                   \
-    layernorm_fwd_kernel<NV, NT, true><<<T, NT, 0, s>>>(X, R, W, B, Y, (__nv_bfloat16*)h_out, mean, rstd, H, eps); \
-  else                                                                                                       \
-    layernorm_fwd_kernel<NV, NT, false><<<T, NT, 0, s>>>(X, R, W, B, Y, nullptr, mean, rstd, H, eps);
-  DTG_NORM_DISPATCH(H, CALL_LN_FWD);
-#undef CALL_LN_FWD
-  note_launch();
-  DTG_LAUNCH_CHECK();
-}
-
-// ------------------------------------------------------------------------------------------
-// LayerNorm backward.  xhat = (h - mean) * rstd, g = dy * w:
-//   dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dres),   dw = sum_rows dy * xhat,   db = sum_rows dy
-// Persistent CTAs stride over rows as rmsnorm_bwd_kernel does; dw and db partials go to two [grid, H] fp32 scratch
-// rows per CTA, reduced by colsum_kernel in a fixed order (no atomics).  h - mean can only overflow when rstd is below
-// 2^-121, so rows with rstd < 2^-100 recompute xhat from h and mean scaled by 2^-72 (exact powers of two).
-// ------------------------------------------------------------------------------------------
-template <int kMaxVec, int kNormThreads, bool HAS_DRES>
-__global__ void __launch_bounds__(kNormThreads) layernorm_bwd_kernel(
-    const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ h, const __nv_bfloat16* __restrict__ w,
-    const float* __restrict__ mean, const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres,
-    __nv_bfloat16* __restrict__ dx, float* __restrict__ dw_partial, float* __restrict__ db_partial, int T, int H) {
-  __shared__ float red[32];
-  const int nvec = H >> 3;
-  float dw_acc[kMaxVec][8], db_acc[kMaxVec][8];
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) dw_acc[k][j] = db_acc[k][j] = 0.f;
-
-  for (int row = blockIdx.x; row < T; row += gridDim.x) {
-    float rs = rstd[row], mu = mean[row], scale = 1.f;
-    if (rs < 0x1p-100f) {
-      scale = kLnDown;
-      mu *= kLnDown;
-      rs *= kLnUp;
-    }
-    const size_t base = (size_t)row * H;
-    float sg = 0.f, sgx = 0.f;
-    bf16x8 cg[kMaxVec], cx[kMaxVec];
-#pragma unroll
-    for (int k = 0; k < kMaxVec; ++k) {
-      const int i = threadIdx.x + k * kNormThreads;
-      if (i < nvec) {
-        cg[k] = ld8(dy + base + i * 8);
-        cx[k] = ld8(h + base + i * 8);
-        float fdy[8], fx[8], fw[8];
-        unpack8(cg[k], fdy);
-        unpack8(cx[k], fx);
-        unpack8(ld8(w + i * 8), fw);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float xhat = (fx[j] * scale - mu) * rs;
-          const float g = fdy[j] * fw[j];
-          sg += g;
-          sgx += g * xhat;
-          dw_acc[k][j] += fdy[j] * xhat;
-          db_acc[k][j] += fdy[j];
-        }
-      }
-    }
-    sg = block_sum(sg, red) / (float)H;
-    sgx = block_sum(sgx, red) / (float)H;
-    const float rs_out = scale == 1.f ? rs : rs * kLnDown;   // rstd in the row's own units
-#pragma unroll
-    for (int k = 0; k < kMaxVec; ++k) {
-      const int i = threadIdx.x + k * kNormThreads;
-      if (i < nvec) {
-        float fdy[8], fx[8], fw[8], out[8];
-        unpack8(cg[k], fdy);
-        unpack8(cx[k], fx);
-        unpack8(ld8(w + i * 8), fw);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float xhat = (fx[j] * scale - mu) * rs;
-          out[j] = rs_out * (fdy[j] * fw[j] - sg - xhat * sgx);
-        }
-        if (HAS_DRES) {
-          float fr[8];
-          unpack8(ld8(dres + base + i * 8), fr);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) out[j] += fr[j];
-        }
-        st8(dx + base + i * 8, pack8(out));
-      }
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      float4* dst = reinterpret_cast<float4*>(dw_partial + (size_t)blockIdx.x * H + i * 8);
-      dst[0] = make_float4(dw_acc[k][0], dw_acc[k][1], dw_acc[k][2], dw_acc[k][3]);
-      dst[1] = make_float4(dw_acc[k][4], dw_acc[k][5], dw_acc[k][6], dw_acc[k][7]);
-      dst = reinterpret_cast<float4*>(db_partial + (size_t)blockIdx.x * H + i * 8);
-      dst[0] = make_float4(db_acc[k][0], db_acc[k][1], db_acc[k][2], db_acc[k][3]);
-      dst[1] = make_float4(db_acc[k][4], db_acc[k][5], db_acc[k][6], db_acc[k][7]);
-    }
-  }
-}
-
-// The db accumulators double the per-thread partial state of rmsnorm_bwd_kernel, so above H 4096 the row is spread
-// over more threads (at most 4 vectors each) instead of more registers.
-#define DTG_LN_BWD_DISPATCH(H, CALL)                                        \
-  do {                                                                     \
-    const int nvec_ = (H) >> 3;                                            \
-    if (nvec_ <= 128) { CALL(1, 128); }                                    \
-    else if (nvec_ <= 256) { CALL(2, 128); }                               \
-    else if (nvec_ <= 512) { CALL(4, 128); }                               \
-    else if (nvec_ <= 1024) { CALL(4, 256); }                              \
-    else if (nvec_ <= 2048) { CALL(4, 512); }                              \
-    else throw std::runtime_error("layernorm: hidden size > 16384 unsupported"); \
-  } while (0)
-
-// 1024 threads per SM (the CTA size grows with H): enough rows in flight to cover HBM latency while the two [grid, H]
-// fp32 partials stay small (13 MB at H 6144)
-int layernorm_bwd_grid(int T, int H) {
-  const int nvec = H >> 3;
-  const int nt = nvec <= 512 ? 128 : nvec <= 1024 ? 256 : 512;
-  const int g = sm_count() * (1024 / nt);
-  return T < g ? T : g;
-}
-
-void layernorm_bwd(const void* dy, const void* h, const void* w, const float* mean, const float* rstd,
-                   const void* dres, void* dx, float* dw_partial, float* db_partial, float* dw, float* db, int T,
-                   int H, cudaStream_t s) {
-  if (H % 8 != 0) throw std::runtime_error("layernorm: hidden size must be a multiple of 8");
-  const int grid = layernorm_bwd_grid(T, H);
-  auto DY = (const __nv_bfloat16*)dy;
-  auto HH = (const __nv_bfloat16*)h;
-  auto W = (const __nv_bfloat16*)w;
-  auto DR = (const __nv_bfloat16*)dres;
-  auto DX = (__nv_bfloat16*)dx;
-#define CALL_LN_BWD(NV, NT)                                                                                         \
-  if (dres)                                                                                                         \
-    layernorm_bwd_kernel<NV, NT, true><<<grid, NT, 0, s>>>(DY, HH, W, mean, rstd, DR, DX, dw_partial, db_partial, T, H); \
-  else                                                                                                              \
-    layernorm_bwd_kernel<NV, NT, false><<<grid, NT, 0, s>>>(DY, HH, W, mean, rstd, nullptr, DX, dw_partial, db_partial, T, H);
-  DTG_LN_BWD_DISPATCH(H, CALL_LN_BWD);
-#undef CALL_LN_BWD
-  colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(dw_partial, dw, grid, H);
-  colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(db_partial, db, grid, H);
-  note_launch(3);
-  DTG_LAUNCH_CHECK();
-}
-
-// ------------------------------------------------------------------------------------------
-// Two LayerNorms over one residual stream (GPT-NeoX's parallel residual):
-//   h = bf16(x (+ r));  y1 = bf16(xhat * w1 + b1),  y2 = bf16(xhat * w2 + b2),  xhat = (h - mean) * rstd
-// Both norms read the same h, so they share one mean and one rstd: one read of the row, three writes.  The statistic
-// (and its 2^-72 rescaled redo for rows whose sums overflow) and the normalisation are layernorm_fwd_kernel's,
-// operation for operation, so y1 and y2 are bit-identical to layernorm_fwd run with (w1, b1) and with (w2, b2).
-// ------------------------------------------------------------------------------------------
-template <int kMaxVec, int kNormThreads, bool HAS_RES>
-__global__ void __launch_bounds__(kNormThreads) layernorm2_fwd_kernel(
-    const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ r, const __nv_bfloat16* __restrict__ w1,
-    const __nv_bfloat16* __restrict__ b1, const __nv_bfloat16* __restrict__ w2, const __nv_bfloat16* __restrict__ b2,
-    __nv_bfloat16* __restrict__ y1, __nv_bfloat16* __restrict__ y2, __nv_bfloat16* __restrict__ h_out,
-    float* __restrict__ mean_out, float* __restrict__ rstd_out, int H, float eps) {
-  __shared__ float red[32];
-  const int row = blockIdx.x;
-  const int nvec = H >> 3;
-  const __nv_bfloat16* xr = x + (size_t)row * H;
-  const __nv_bfloat16* rr = HAS_RES ? r + (size_t)row * H : nullptr;
-  bf16x8 cache[kMaxVec];
-  float sum = 0.f;
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      bf16x8 v = ld8(xr + i * 8);
-      float f[8];
-      unpack8(v, f);
-      if (HAS_RES) {
-        float g[8];
-        unpack8(ld8(rr + i * 8), g);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) f[j] += g[j];
-        v = pack8(f);          // the residual stream is stored (and normalised) in bf16
-        unpack8(v, f);
-        st8(h_out + (size_t)row * H + i * 8, v);
-      }
-      cache[k] = v;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) sum += f[j];
-    }
-  }
-  float scale = 1.f;
-  float mean = block_sum(sum, red) / (float)H;
-  float ss = block_sum(ln_sq_dev<kMaxVec, kNormThreads>(cache, nvec, mean, 1.f), red);
-  if (!(isfinite(mean) && isfinite(ss))) {   // uniform over the CTA: block_sum broadcasts
-    scale = kLnDown;
-    mean = block_sum(ln_sum<kMaxVec, kNormThreads>(cache, nvec, kLnDown), red) / (float)H;
-    ss = block_sum(ln_sq_dev<kMaxVec, kNormThreads>(cache, nvec, mean, kLnDown), red);
-  }
-  const float rstd = rsqrtf(ss / (float)H + eps * scale * scale);
-  if (threadIdx.x == 0) {
-    mean_out[row] = scale == 1.f ? mean : mean * kLnUp;
-    rstd_out[row] = scale == 1.f ? rstd : rstd * kLnDown;
-  }
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      float f[8], g[8], c[8], o[8];
-      unpack8(cache[k], f);
-      unpack8(ld8(w1 + i * 8), g);
-      unpack8(ld8(b1 + i * 8), c);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = (f[j] * scale - mean) * rstd * g[j] + c[j];
-      st8(y1 + (size_t)row * H + i * 8, pack8(o));
-      unpack8(ld8(w2 + i * 8), g);
-      unpack8(ld8(b2 + i * 8), c);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) o[j] = (f[j] * scale - mean) * rstd * g[j] + c[j];
-      st8(y2 + (size_t)row * H + i * 8, pack8(o));
-    }
-  }
-}
-
-void layernorm2_fwd(const void* x, const void* res, const void* w1, const void* b1, const void* w2, const void* b2,
-                    void* y1, void* y2, void* h_out, float* mean, float* rstd, int T, int H, float eps,
-                    cudaStream_t s) {
-  if (H % 8 != 0 || H > 8192) throw std::runtime_error("layernorm2: hidden size must be a multiple of 8, <= 8192");
-  auto X = (const __nv_bfloat16*)x;
-  auto R = (const __nv_bfloat16*)res;
-  auto W1 = (const __nv_bfloat16*)w1;
-  auto B1 = (const __nv_bfloat16*)b1;
-  auto W2 = (const __nv_bfloat16*)w2;
-  auto B2 = (const __nv_bfloat16*)b2;
-  auto Y1 = (__nv_bfloat16*)y1;
-  auto Y2 = (__nv_bfloat16*)y2;
-#define CALL_LN2_FWD(NV, NT)                                                                                      \
-  if (res)                                                                                                        \
-    layernorm2_fwd_kernel<NV, NT, true><<<T, NT, 0, s>>>(X, R, W1, B1, W2, B2, Y1, Y2, (__nv_bfloat16*)h_out,     \
-                                                         mean, rstd, H, eps);                                     \
-  else                                                                                                            \
-    layernorm2_fwd_kernel<NV, NT, false><<<T, NT, 0, s>>>(X, R, W1, B1, W2, B2, Y1, Y2, nullptr, mean, rstd, H, eps);
-  DTG_NORM_DISPATCH(H, CALL_LN2_FWD);
-#undef CALL_LN2_FWD
-  note_launch();
-  DTG_LAUNCH_CHECK();
-}
-
-__device__ __forceinline__ void st_partial8(float* p, const float (&a)[8]) {
-  float4* dst = reinterpret_cast<float4*>(p);
-  dst[0] = make_float4(a[0], a[1], a[2], a[3]);
-  dst[1] = make_float4(a[4], a[5], a[6], a[7]);
-}
-
-// ------------------------------------------------------------------------------------------
-// Backward of the two LayerNorms.  xhat = (h - mean) * rstd, g = dy1 * w1 + dy2 * w2 (fp32):
-//   dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ dres)
-//   dw1 = sum_rows dy1 * xhat,  db1 = sum_rows dy1,  dw2 = sum_rows dy2 * xhat,  db2 = sum_rows dy2
-// Persistent CTAs as layernorm_bwd_kernel, with its scaled xhat for rows with rstd < 2^-100; the four parameter
-// gradients are fp32 partial rows per CTA ([4, grid, H] scratch) reduced by colsum_kernel in a fixed order.
-// ------------------------------------------------------------------------------------------
-template <int kMaxVec, int kNormThreads, bool HAS_DRES>
-__global__ void __launch_bounds__(kNormThreads) layernorm2_bwd_kernel(
-    const __nv_bfloat16* __restrict__ dy1, const __nv_bfloat16* __restrict__ dy2, const __nv_bfloat16* __restrict__ h,
-    const __nv_bfloat16* __restrict__ w1, const __nv_bfloat16* __restrict__ w2, const float* __restrict__ mean,
-    const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ dres, __nv_bfloat16* __restrict__ dx,
-    float* __restrict__ partial, int T, int H) {
-  __shared__ float red[32];
-  const int nvec = H >> 3;
-  float dw1[kMaxVec][8], db1[kMaxVec][8], dw2[kMaxVec][8], db2[kMaxVec][8];
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) dw1[k][j] = db1[k][j] = dw2[k][j] = db2[k][j] = 0.f;
-
-  for (int row = blockIdx.x; row < T; row += gridDim.x) {
-    float rs = rstd[row], mu = mean[row], scale = 1.f;
-    if (rs < 0x1p-100f) {
-      scale = kLnDown;
-      mu *= kLnDown;
-      rs *= kLnUp;
-    }
-    const size_t base = (size_t)row * H;
-    float sg = 0.f, sgx = 0.f;
-    bf16x8 c1[kMaxVec], c2[kMaxVec];   // h is read again in the second pass: 8 registers fewer, no spill at 512
-#pragma unroll
-    for (int k = 0; k < kMaxVec; ++k) {
-      const int i = threadIdx.x + k * kNormThreads;
-      if (i < nvec) {
-        c1[k] = ld8(dy1 + base + i * 8);
-        c2[k] = ld8(dy2 + base + i * 8);
-        float fd1[8], fd2[8], fx[8], fw1[8], fw2[8];
-        unpack8(c1[k], fd1);
-        unpack8(c2[k], fd2);
-        unpack8(ld8(h + base + i * 8), fx);
-        unpack8(ld8(w1 + i * 8), fw1);
-        unpack8(ld8(w2 + i * 8), fw2);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float xhat = (fx[j] * scale - mu) * rs;
-          const float g = fd1[j] * fw1[j] + fd2[j] * fw2[j];
-          sg += g;
-          sgx += g * xhat;
-          dw1[k][j] += fd1[j] * xhat;
-          db1[k][j] += fd1[j];
-          dw2[k][j] += fd2[j] * xhat;
-          db2[k][j] += fd2[j];
-        }
-      }
-    }
-    sg = block_sum(sg, red) / (float)H;
-    sgx = block_sum(sgx, red) / (float)H;
-    const float rs_out = scale == 1.f ? rs : rs * kLnDown;   // rstd in the row's own units
-#pragma unroll
-    for (int k = 0; k < kMaxVec; ++k) {
-      const int i = threadIdx.x + k * kNormThreads;
-      if (i < nvec) {
-        float fd1[8], fd2[8], fx[8], fw1[8], fw2[8], out[8];
-        unpack8(c1[k], fd1);
-        unpack8(c2[k], fd2);
-        unpack8(ld8(h + base + i * 8), fx);
-        unpack8(ld8(w1 + i * 8), fw1);
-        unpack8(ld8(w2 + i * 8), fw2);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float xhat = (fx[j] * scale - mu) * rs;
-          out[j] = rs_out * (fd1[j] * fw1[j] + fd2[j] * fw2[j] - sg - xhat * sgx);
-        }
-        if (HAS_DRES) {
-          float fr[8];
-          unpack8(ld8(dres + base + i * 8), fr);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) out[j] += fr[j];
-        }
-        st8(dx + base + i * 8, pack8(out));
-      }
-    }
-  }
-  const size_t plane = (size_t)gridDim.x * H;   // partial: [4, grid, H] = dw1, db1, dw2, db2
-#pragma unroll
-  for (int k = 0; k < kMaxVec; ++k) {
-    const int i = threadIdx.x + k * kNormThreads;
-    if (i < nvec) {
-      float* p = partial + (size_t)blockIdx.x * H + i * 8;
-      st_partial8(p, dw1[k]);
-      st_partial8(p + plane, db1[k]);
-      st_partial8(p + 2 * plane, dw2[k]);
-      st_partial8(p + 3 * plane, db2[k]);
-    }
-  }
-}
-
-// Four accumulators per element (dw1, db1, dw2, db2): at most 2 vectors per thread, and the row spread over up to
-// 512 threads, so no variant spills; H <= 8192 (every GPT-NeoX / Pythia width).
-#define DTG_LN2_BWD_DISPATCH(H, CALL)                                       \
-  do {                                                                     \
-    const int nvec_ = (H) >> 3;                                            \
-    if (nvec_ <= 128) { CALL(1, 128); }                                    \
-    else if (nvec_ <= 256) { CALL(2, 128); }                               \
-    else if (nvec_ <= 512) { CALL(2, 256); }                               \
-    else if (nvec_ <= 1024) { CALL(2, 512); }                              \
-    else throw std::runtime_error("layernorm2: hidden size > 8192 unsupported"); \
-  } while (0)
-
-// 1024 threads per SM, as layernorm_bwd_grid
-int layernorm2_bwd_grid(int T, int H) {
-  const int nvec = H >> 3;
-  const int nt = nvec <= 256 ? 128 : nvec <= 512 ? 256 : 512;
-  const int g = sm_count() * (1024 / nt);
-  return T < g ? T : g;
-}
-
-void layernorm2_bwd(const void* dy1, const void* dy2, const void* h, const void* w1, const void* w2, const float* mean,
-                    const float* rstd, const void* dres, void* dx, float* partial, float* dparams, int T, int H,
-                    cudaStream_t s) {
-  if (H % 8 != 0 || H > 8192) throw std::runtime_error("layernorm2: hidden size must be a multiple of 8, <= 8192");
-  const int grid = layernorm2_bwd_grid(T, H);
-  auto D1 = (const __nv_bfloat16*)dy1;
-  auto D2 = (const __nv_bfloat16*)dy2;
-  auto HH = (const __nv_bfloat16*)h;
-  auto W1 = (const __nv_bfloat16*)w1;
-  auto W2 = (const __nv_bfloat16*)w2;
-  auto DR = (const __nv_bfloat16*)dres;
-  auto DX = (__nv_bfloat16*)dx;
-#define CALL_LN2_BWD(NV, NT)                                                                                  \
-  if (dres)                                                                                                   \
-    layernorm2_bwd_kernel<NV, NT, true><<<grid, NT, 0, s>>>(D1, D2, HH, W1, W2, mean, rstd, DR, DX, partial, T, H); \
-  else                                                                                                        \
-    layernorm2_bwd_kernel<NV, NT, false><<<grid, NT, 0, s>>>(D1, D2, HH, W1, W2, mean, rstd, nullptr, DX, partial, T, H);
-  DTG_LN2_BWD_DISPATCH(H, CALL_LN2_BWD);
-#undef CALL_LN2_BWD
-  for (int q = 0; q < 4; ++q)
-    colsum_kernel<<<(H + 31) / 32, 256, 0, s>>>(partial + (size_t)q * grid * H, dparams + (size_t)q * H, grid, H);
-  note_launch(5);
   DTG_LAUNCH_CHECK();
 }
 

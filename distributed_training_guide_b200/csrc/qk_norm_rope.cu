@@ -249,7 +249,7 @@ void qk_norm_rope_bwd(void* dqkv, const void* x_save, const float* rstd, const v
 // Full-width QK-norm + RoPE (OLMo 2) in place on the q and k heads of qkv [T, nh + 2*nkv, 128]:
 //   forward:  y = bf16(x * rstd_r * w),  rstd_r = rsqrt(mean(x^2) + eps) over the token's whole q region (nh * 128
 //             elements) or k region (nkv * 128), w the [nh * 128] q gain or [nkv * 128] k gain, with the one rounding
-//             of rmsnorm_fwd_kernel; then the half-rotation RoPE of rope_inplace_kernel on y, per head.
+//             of the RMSNorm forward (norm.cu); then the half-rotation RoPE of rope_inplace_kernel on y, per head.
 //   backward: inverse rotation, then dx = rstd_r * (g - xhat * mean_r(g * xhat)), g = dy * w, per region;
 //             dw = sum over tokens of dy * xhat over the (nh + nkv) * 128 gain columns, as fp32 per-CTA partial
 //             rows reduced by colsum_kernel in a fixed order (no atomics).

@@ -418,7 +418,7 @@ def parallel_out(attn, act, wd, w4, bd, b4, fp8=False):
 
 
 # --------------------------------------------------------------------------------------
-# RMSNorm (+ fused residual add)
+# Row norms: RMSNorm and LayerNorm (+ fused residual add), OLMo 2's norm-then-add
 # --------------------------------------------------------------------------------------
 def _norm_dw_into(dw32):
     def into(out, acc):
@@ -429,64 +429,60 @@ def _norm_dw_into(dw32):
     return into
 
 
-class _RMSNorm(torch.autograd.Function):
+def _rows(t):
+    return t.reshape(-1, t.shape[-1])
+
+
+def _norm_grads(params, d32):
+    """Route the fp32 gain / bias gradients ``d32[i]`` of ``params[i]`` through ``_emit_weight_grad`` (None for an
+    absent parameter)."""
+    return tuple(None if p is None else _emit_weight_grad(p, _norm_dw_into(d32[i]), p) for i, p in enumerate(params))
+
+
+class _Norm(torch.autograd.Function):
+    """y = norm(h) * w (+ b) with h = x, or (y, h) with h = x + r rounded to bf16, in one pass over the activations.
+    ``b`` None: RMSNorm, else LayerNorm; ``r`` None: no residual.  Backward: dx = the norm's backward + dh, the
+    gradient of both x and r when h is an output."""
+
     @staticmethod
-    def forward(ctx, x, w, eps):
+    def forward(ctx, x, r, w, b, eps):
         C = _ext.load()
-        x2 = x.reshape(-1, x.shape[-1])
-        y, rstd, _ = C.rmsnorm_fwd(x2, w, float(eps), None)
-        ctx.save_for_backward(x2, w, rstd)
+        x2, r2 = _rows(x), (_rows(r) if r is not None else None)
+        if b is None:
+            y, rstd, h = C.rmsnorm_fwd(x2, w, float(eps), r2)
+            stats = (rstd,)
+        else:
+            y, h, mean, rstd = C.layernorm_fwd(x2, r2, w, b, float(eps))
+            stats = (mean, rstd)
+        ctx.save_for_backward(x2 if h is None else h, w, *stats)
         ctx.shape = x.shape
-        ctx.w_param = w
-        return y.view(x.shape)
-
-    @staticmethod
-    def backward(ctx, dy):
-        C = _ext.load()
-        x2, w, rstd = ctx.saved_tensors
-        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
-        dx, dw32 = C.rmsnorm_bwd(dy2, x2, w, rstd, None)
-        dw = _emit_weight_grad(ctx.w_param, _norm_dw_into(dw32), w)
-        return dx.view(ctx.shape), dw, None
-
-
-class _AddRMSNorm(torch.autograd.Function):
-    """(y, h) = (rmsnorm(x + r) * w, x + r) in one pass over the activations."""
-
-    @staticmethod
-    def forward(ctx, x, r, w, eps):
-        C = _ext.load()
-        x2 = x.reshape(-1, x.shape[-1])
-        r2 = r.reshape(-1, r.shape[-1])
-        y, rstd, h = C.rmsnorm_fwd(x2, w, float(eps), r2)
-        ctx.save_for_backward(h, w, rstd)
-        ctx.shape = x.shape
-        ctx.w_param = w
+        ctx.params = (w, b)
+        if h is None:
+            return y.view(x.shape)
         return y.view(x.shape), h.view(x.shape)
 
     @staticmethod
-    def backward(ctx, dy, dh):
+    def backward(ctx, dy, dh=None):
         C = _ext.load()
-        h, w, rstd = ctx.saved_tensors
-        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
-        dh2 = dh.reshape(-1, dh.shape[-1]).contiguous() if dh is not None else None
-        # dx = rmsnorm_bwd(dy) + dh : the gradient of both x and r (h = x + r)
-        dx, dw32 = C.rmsnorm_bwd(dy2, h, w, rstd, dh2)
-        dw = _emit_weight_grad(ctx.w_param, _norm_dw_into(dw32), w)
+        h, w, *stats = ctx.saved_tensors
+        dy2 = _rows(dy).contiguous()
+        dh2 = _rows(dh).contiguous() if dh is not None else None
+        bwd = C.rmsnorm_bwd if ctx.params[1] is None else C.layernorm_bwd
+        dx, *d32 = bwd(dy2, h, w, *stats, dh2)
         dx = dx.view(ctx.shape)
-        return dx, dx, dw, None
+        return (dx, dx if dh is not None else None) + _norm_grads(ctx.params, d32) + (None,)
 
 
 def rms_norm(x, w, eps):
     if _ext.use_cuda_kernel("rmsnorm", x, w) and x.dtype == torch.bfloat16:
-        return _RMSNorm.apply(x, w, eps)
+        return _Norm.apply(x.contiguous(), None, w, None, eps)
     return ref.rms_norm(x, w, eps)
 
 
 def add_rms_norm(x, residual, w, eps):
     """Fused ``h = x + residual; y = rmsnorm(h) * w`` -> (y, h)."""
     if _ext.use_cuda_kernel("rmsnorm", x, residual, w) and x.dtype == torch.bfloat16:
-        return _AddRMSNorm.apply(x, residual, w, eps)
+        return _Norm.apply(x.contiguous(), residual.contiguous(), w, None, eps)
     return ref.add_rms_norm(x, residual, w, eps)
 
 
@@ -497,21 +493,19 @@ class _RMSNormAdd(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, r, w, eps):
         C = _ext.load()
-        x2 = x.reshape(-1, x.shape[-1])
-        h, rstd = C.rmsnorm_add_fwd(x2, r.reshape(-1, r.shape[-1]), w, float(eps))
+        x2 = _rows(x)
+        h, rstd = C.rmsnorm_add_fwd(x2, _rows(r), w, float(eps))
         ctx.save_for_backward(x2, w, rstd)
         ctx.shape = x.shape
-        ctx.w_param = w
+        ctx.params = (w,)
         return h.view(x.shape)
 
     @staticmethod
     def backward(ctx, dh):
         C = _ext.load()
         x2, w, rstd = ctx.saved_tensors
-        dh2 = dh.reshape(-1, dh.shape[-1]).contiguous()
-        dx, dw32 = C.rmsnorm_bwd(dh2, x2, w, rstd, None)
-        dw = _emit_weight_grad(ctx.w_param, _norm_dw_into(dw32), w)
-        return dx.view(ctx.shape), dh, dw, None
+        dx, dw32 = C.rmsnorm_bwd(_rows(dh).contiguous(), x2, w, rstd, None)
+        return (dx.view(ctx.shape), dh) + _norm_grads(ctx.params, (dw32,)) + (None,)
 
 
 def rms_norm_add(x, r, w, eps):
@@ -526,61 +520,12 @@ def rms_norm_add(x, r, w, eps):
 # --------------------------------------------------------------------------------------
 # LayerNorm (+ fused residual add), StarCoder2
 # --------------------------------------------------------------------------------------
-class _LayerNorm(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, x, w, b, eps):
-        C = _ext.load()
-        x2 = x.reshape(-1, x.shape[-1])
-        y, _, mean, rstd = C.layernorm_fwd(x2, None, w, b, float(eps))
-        ctx.save_for_backward(x2, w, mean, rstd)
-        ctx.shape = x.shape
-        ctx.params = (w, b)
-        return y.view(x.shape)
-
-    @staticmethod
-    def backward(ctx, dy):
-        C = _ext.load()
-        x2, w, mean, rstd = ctx.saved_tensors
-        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
-        dx, dw32, db32 = C.layernorm_bwd(dy2, x2, w, mean, rstd, None)
-        dw = _emit_weight_grad(ctx.params[0], _norm_dw_into(dw32), w)
-        db = _emit_weight_grad(ctx.params[1], _norm_dw_into(db32), ctx.params[1])
-        return dx.view(ctx.shape), dw, db, None
-
-
-class _AddLayerNorm(torch.autograd.Function):
-    """(y, h) = (layernorm(x + r) * w + b, x + r) in one pass over the activations."""
-
-    @staticmethod
-    def forward(ctx, x, r, w, b, eps):
-        C = _ext.load()
-        x2 = x.reshape(-1, x.shape[-1])
-        y, h, mean, rstd = C.layernorm_fwd(x2, r.reshape(-1, r.shape[-1]), w, b, float(eps))
-        ctx.save_for_backward(h, w, mean, rstd)
-        ctx.shape = x.shape
-        ctx.params = (w, b)
-        return y.view(x.shape), h.view(x.shape)
-
-    @staticmethod
-    def backward(ctx, dy, dh):
-        C = _ext.load()
-        h, w, mean, rstd = ctx.saved_tensors
-        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
-        dh2 = dh.reshape(-1, dh.shape[-1]).contiguous() if dh is not None else None
-        # dx = layernorm_bwd(dy) + dh : the gradient of both x and r (h = x + r)
-        dx, dw32, db32 = C.layernorm_bwd(dy2, h, w, mean, rstd, dh2)
-        dw = _emit_weight_grad(ctx.params[0], _norm_dw_into(dw32), w)
-        db = _emit_weight_grad(ctx.params[1], _norm_dw_into(db32), ctx.params[1])
-        dx = dx.view(ctx.shape)
-        return dx, dx, dw, db, None
-
-
 def layer_norm(x, w, b, eps):
     """``y = (x - mean) * rsqrt(var + eps) * w + b`` over the last dimension with fp32 statistics and one rounding
     (ATen's bf16 ``layer_norm``).  bf16 CUDA tensors run the sm_90a kernels; the gain and bias gradients go through
     ``_emit_weight_grad`` (overwrite on the first write of a step, accumulate after it)."""
     if _ext.use_cuda_kernel("layernorm", x, w, b) and x.dtype == torch.bfloat16:
-        return _LayerNorm.apply(x.contiguous(), w, b, eps)
+        return _Norm.apply(x.contiguous(), None, w, b, eps)
     return ref.layer_norm(x, w, b, eps)
 
 
@@ -588,7 +533,7 @@ def add_layer_norm(x, residual, w, b, eps):
     """Fused ``h = x + residual; y = layer_norm(h, w, b)`` -> (y, h), with ``h`` rounded to the input dtype before it
     is normalised."""
     if _ext.use_cuda_kernel("layernorm", x, residual, w, b) and x.dtype == torch.bfloat16:
-        return _AddLayerNorm.apply(x.contiguous(), residual.contiguous(), w, b, eps)
+        return _Norm.apply(x.contiguous(), residual.contiguous(), w, b, eps)
     h = x + residual
     return ref.layer_norm(h, w, b, eps), h
 
@@ -644,8 +589,8 @@ class _LayerNorm2(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, r, w1, b1, w2, b2, eps):
         C = _ext.load()
-        x2 = x.reshape(-1, x.shape[-1])
-        r2 = r.reshape(-1, r.shape[-1]) if r is not None else None
+        x2 = _rows(x)
+        r2 = _rows(r) if r is not None else None
         y1, y2, h, mean, rstd = C.layernorm2_fwd(x2, r2, w1, b1, w2, b2, float(eps))
         ctx.save_for_backward(h if h is not None else x2, w1, w2, mean, rstd)
         ctx.shape = x.shape
@@ -659,12 +604,11 @@ class _LayerNorm2(torch.autograd.Function):
     def backward(ctx, dy1, dy2, dh=None):
         C = _ext.load()
         h, w1, w2, mean, rstd = ctx.saved_tensors
-        flat = lambda t: t.reshape(-1, t.shape[-1]).contiguous() if t is not None else torch.zeros_like(h)  # noqa: E731
-        dh2 = dh.reshape(-1, dh.shape[-1]).contiguous() if dh is not None else None
+        flat = lambda t: _rows(t).contiguous() if t is not None else torch.zeros_like(h)  # noqa: E731
+        dh2 = _rows(dh).contiguous() if dh is not None else None
         dx, d32 = C.layernorm2_bwd(flat(dy1), flat(dy2), h, w1, w2, mean, rstd, dh2)
-        grads = tuple(_emit_weight_grad(p, _norm_dw_into(d32[i]), p) for i, p in enumerate(ctx.params))
         dx = dx.view(ctx.shape)
-        return (dx, dx if ctx.has_res else None) + grads + (None,)
+        return (dx, dx if ctx.has_res else None) + _norm_grads(ctx.params, d32) + (None,)
 
 
 def layer_norm2(x, r, w1, b1, w2, b2, eps):

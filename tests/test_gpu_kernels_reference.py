@@ -249,6 +249,28 @@ def test_rmsnorm_rejects_unsupported_hidden_sizes():
         _refused(lambda: C.rmsnorm_fwd(x, w, 1e-5, None), "hidden size")
         rstd = torch.ones(4, device="cuda")
         _refused(lambda: C.rmsnorm_bwd(x, x, w, rstd, None), "hidden size")
+    T, H = 16, 512
+    x = torch.randn(T, H, device="cuda").to(BF16)
+    w = torch.ones(H, device="cuda", dtype=BF16)
+    rstd = torch.ones(T, device="cuda")
+    # a contiguous [B, S, H] tensor with S == H is not B rows of S elements
+    x3 = torch.randn(2, H, H, device="cuda").to(BF16)
+    _refused(lambda: C.rmsnorm_fwd(x3, w, 1e-5, None), "2-D")
+    _refused(lambda: C.rmsnorm_bwd(x3, x3, w, torch.ones(2, device="cuda"), None), "2-D")
+    for eps in (float("nan"), -1e-5, float("inf")):
+        _refused(lambda: C.rmsnorm_fwd(x, w, eps, None), "eps")
+    _refused(lambda: C.rmsnorm_bwd(x, x, w, rstd[:8].contiguous(), None), "rstd")
+    _refused(lambda: C.rmsnorm_bwd(x, x, w, rstd.double(), None), "rstd")
+    _refused(lambda: C.rmsnorm_bwd(x, x, w, rstd, x[:8].contiguous()), "dres")
+    # no rows: empty outputs and zero gradients, without a launch
+    x0 = torch.empty(0, H, device="cuda", dtype=BF16)
+    torch.cuda.synchronize()
+    n0 = _ext.launch_count()
+    y, rstd0, h = C.rmsnorm_fwd(x0, w, 1e-5, x0)
+    dx, dw = C.rmsnorm_bwd(x0, x0, w, rstd0, x0)
+    assert _ext.launch_count() == n0, "a call with no rows launched a kernel"
+    assert y.shape == h.shape == dx.shape == (0, H) and rstd0.shape == (0,)
+    assert dw.shape == (H,) and not dw.any()
 
 
 # ------------------------------------------------------------------------------------------------------------------
