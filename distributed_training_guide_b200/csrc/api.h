@@ -50,10 +50,6 @@ struct NormBwdArgs {
 void norm_bwd(NormKind k, const NormBwdArgs& a, int T, int H, cudaStream_t s);
 
 // ---- elementwise.cu ------------------------------------------------------------------------
-// rotates the first rot_dim elements (rot_dim % 16 == 0, <= d; d for the full head) of heads [0, n_rot); cos/sin
-// [S, rot_dim/2] or [T, rot_dim/2]
-void rope_inplace(void* qkv, const float* cos, const float* sin, long long T, int S, int n_heads, int n_rot, int d,
-                  int rot_dim, bool per_token, bool inverse, cudaStream_t s);
 // out[c] = sum over rows r of partial[r][c] (fp32 [rows, H]), in a fixed order
 void colsum(const float* partial, float* out, int rows, int H, cudaStream_t s);
 // bias gradient: db[n] = sum over t of dy[t, n], dy bf16 [T, N] with row stride ld (elements); N, ld multiples of 8.
@@ -78,7 +74,11 @@ void embedding_bwd_sorted(const void* dout, const long long* ids_sorted, const l
                           bool accumulate, cudaStream_t s);
 void scale_inplace(void* x, const float* scale, long long n, cudaStream_t s);
 
-// ---- qk_norm_rope.cu -----------------------------------------------------------------------
+// ---- rope.cu -------------------------------------------------------------------------------
+// rotates the first rot_dim elements (rot_dim % 16 == 0, <= d; d for the full head) of heads [0, n_rot); cos/sin
+// [S, rot_dim/2] or [T, rot_dim/2]
+void rope_inplace(void* qkv, const float* cos, const float* sin, long long T, int S, int n_heads, int n_rot, int d,
+                  int rot_dim, bool per_token, bool inverse, cudaStream_t s);
 // QK-norm + RoPE (Qwen3) in place on heads [0, nh + nkv) of qkv [T, n_heads, 128] bf16 (n_heads = nh + 2*nkv):
 // per head y = bf16(bf16(x * rstd) * w) with w = q_w (heads < nh) or k_w, then the RoPE of rope_inplace.  cos/sin:
 // fp32 [S, 64] (pos = t % S) or per-token [T, 64].  Writes x_save [T, nh + nkv, 128] bf16 (the pre-norm q|k heads)

@@ -317,22 +317,37 @@ Tensor gelu_tanh_bwd(const Tensor& dy, const Tensor& x) {
   return dx;
 }
 
-void rope_inplace(Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t n_rot, bool inverse,
-                  const c10::optional<int64_t>& rot_dim_arg) {
-  // qkv: [B, S, heads, d] contiguous; cos/sin fp32 [S, rot_dim/2] or [B, S, rot_dim/2]; rot_dim defaults to d
-  check_vec(qkv, "qkv", at::kBFloat16);
+// cos/sin tables of the RoPE kernels, w = rot_dim / 2 floats per row, for qkv [B, S, heads, d]: fp32, 16-byte aligned,
+// both [S, w] (row t % S), [T, w] or [B, S, w] (a row per token), on qkv's device.  Returns per_token.
+bool check_rope_tables(const Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t w, const char* who) {
   check_vec(cos, "cos", at::kFloat);
   check_vec(sin, "sin", at::kFloat);
+  const int64_t B = qkv.size(0), S = qkv.size(1);
+  TORCH_CHECK(sin.sizes() == cos.sizes(), who, ": cos and sin differ in shape");
+  TORCH_CHECK((cos.dim() == 2 || cos.dim() == 3) && cos.size(-1) == w, who, ": cos/sin table has the wrong shape: ",
+              cos.sizes(), " is not [S, ", w, "], [T, ", w, "] or [B, S, ", w, "]");
+  TORCH_CHECK(cos.dim() == 2 || (cos.size(0) == B && cos.size(1) == S), who, ": cos/sin table has the wrong shape: a ",
+              "3-D table must be [B, S, ", w, "] = [", B, ", ", S, ", ", w, "], got ", cos.sizes());
+  const int64_t rows = cos.dim() == 2 ? cos.size(0) : B * S;
+  TORCH_CHECK(rows == S || rows == B * S, who, ": cos/sin table has the wrong shape: its ", rows,
+              " rows match neither S = ", S, " nor T = ", B * S);
+  TORCH_CHECK(cos.device() == qkv.device() && sin.device() == qkv.device(), who,
+              ": cos and sin must be on the device of qkv");
+  return rows != S;
+}
+
+void rope_inplace(Tensor& qkv, const Tensor& cos, const Tensor& sin, int64_t n_rot, bool inverse,
+                  const c10::optional<int64_t>& rot_dim_arg) {
+  // qkv: [B, S, heads, d] contiguous; rot_dim defaults to d
+  check_vec(qkv, "qkv", at::kBFloat16);
   TORCH_CHECK(qkv.dim() == 4, "qkv must be [B,S,heads,d]");
-  const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1), NH = qkv.size(2), d = qkv.size(3);
   const int64_t rot_dim = rot_dim_arg.has_value() ? *rot_dim_arg : d;
   TORCH_CHECK(rot_dim > 0 && rot_dim <= d && rot_dim % 16 == 0,
               "rope: rot_dim must be a positive multiple of 16 and <= head_dim ", d, ", got ", rot_dim);
-  const bool per_token = cos.dim() == 3;
-  TORCH_CHECK(cos.size(-1) == rot_dim / 2 && cos.size(per_token ? 1 : 0) == S, "cos/sin table has the wrong shape");
-  TORCH_CHECK(sin.sizes() == cos.sizes(), "cos and sin differ in shape");
+  const bool per_token = check_rope_tables(qkv, cos, sin, rot_dim / 2, "rope");
   TORCH_CHECK(n_rot >= 0 && n_rot <= NH, "rope: n_rot must be within [0, heads]");
+  const c10::cuda::CUDAGuard guard(qkv.device());
   dtg::rope_inplace(qkv.data_ptr(), cos.data_ptr<float>(), sin.data_ptr<float>(), B * S, (int)S, (int)NH, (int)n_rot,
                     (int)d, (int)rot_dim, per_token, inverse, stream());
 }
@@ -357,105 +372,70 @@ Tensor gelu_bwd(const Tensor& dy, const Tensor& x) {
   return dx;
 }
 
-// Shared checks of qk_norm_rope_fwd / _bwd and, with `full`, of the full-width qk_norm_full_rope_fwd / _bwd (gains
-// [nh * d] and [nkv * d]); returns per_token.  Every refusal happens before any launch.
+// QK-norm + RoPE, per head (Qwen3: gains [d]) or, with FULL, over each token's whole q and k regions (OLMo 2: gains
+// [nh * d] and [nkv * d]).  Every refusal happens before any launch.
+template <bool FULL>
 bool check_qk_norm_rope(const Tensor& qkv, const Tensor& q_w, const Tensor& k_w, const Tensor& cos, const Tensor& sin,
-                        int64_t nh, int64_t nkv, bool full = false) {
+                        int64_t nh, int64_t nkv) {
+  const char* who = FULL ? "qk_norm_full_rope" : "qk_norm_rope";
   check_vec(qkv, "qkv", at::kBFloat16);
-  TORCH_CHECK(qkv.dim() == 4, "qk_norm_rope: qkv must be [B, S, heads, d]");
-  const int64_t B = qkv.size(0), S = qkv.size(1), NH = qkv.size(2), d = qkv.size(3);
-  TORCH_CHECK(d == 128, "qk_norm_rope: head_dim must be 128, got ", d);
-  TORCH_CHECK(nh >= 1 && nkv >= 1 && NH == nh + 2 * nkv, "qk_norm_rope: qkv has ", NH,
+  TORCH_CHECK(qkv.dim() == 4, who, ": qkv must be [B, S, heads, d]");
+  const int64_t NH = qkv.size(2), d = qkv.size(3);
+  TORCH_CHECK(d == 128, who, ": head_dim must be 128, got ", d);
+  TORCH_CHECK(nh >= 1 && nkv >= 1 && NH == nh + 2 * nkv, who, ": qkv has ", NH,
               " heads, expected nh + 2 * nkv with nh, nkv >= 1 (nh = ", nh, ", nkv = ", nkv, ")");
-  if (full)
-    TORCH_CHECK(nh + nkv <= dtg::qk_norm_full_rope_max_heads(), "qk_norm_full_rope: nh + nkv = ", nh + nkv,
-                " exceeds the ", dtg::qk_norm_full_rope_max_heads(), " q + k heads per token the kernel holds");
+  if (FULL)
+    TORCH_CHECK(nh + nkv <= dtg::qk_norm_full_rope_max_heads(), who, ": nh + nkv = ", nh + nkv, " exceeds the ",
+                dtg::qk_norm_full_rope_max_heads(), " q + k heads per token the kernel holds");
   check_vec(q_w, "q_w", at::kBFloat16);
   check_vec(k_w, "k_w", at::kBFloat16);
-  const int64_t qn = full ? nh * d : d, kn = full ? nkv * d : d;
-  TORCH_CHECK(q_w.dim() == 1 && q_w.size(0) == qn, "qk_norm_rope: q_w must be [", qn, "]");
-  TORCH_CHECK(k_w.dim() == 1 && k_w.size(0) == kn, "qk_norm_rope: k_w must be [", kn, "]");
-  check_vec(cos, "cos", at::kFloat);
-  check_vec(sin, "sin", at::kFloat);
-  TORCH_CHECK(sin.sizes() == cos.sizes(), "qk_norm_rope: cos and sin differ in shape");
-  TORCH_CHECK((cos.dim() == 2 || cos.dim() == 3) && cos.size(-1) == d / 2,
-              "qk_norm_rope: cos/sin must be [S, ", d / 2, "], [T, ", d / 2, "] or [B, S, ", d / 2, "]");
-  const int64_t rows = cos.dim() == 2 ? cos.size(0) : cos.size(0) * cos.size(1);
-  TORCH_CHECK(cos.dim() == 2 || (cos.size(0) == B && cos.size(1) == S),
-              "qk_norm_rope: a 3-D cos/sin table must be [B, S, d/2] = [", B, ", ", S, ", ", d / 2, "]");
-  TORCH_CHECK(rows == S || rows == B * S, "qk_norm_rope: cos/sin have ", rows, " rows, which matches neither S = ", S,
-              " nor T = ", B * S);
-  for (const Tensor* t : {&q_w, &k_w, &cos, &sin})
-    TORCH_CHECK(t->device() == qkv.device(), "qk_norm_rope: every operand must be on the device of qkv");
-  return rows != S;
+  const int64_t qn = FULL ? nh * d : d, kn = FULL ? nkv * d : d;
+  TORCH_CHECK(q_w.dim() == 1 && q_w.size(0) == qn, who, ": q_w must be [", qn, "]");
+  TORCH_CHECK(k_w.dim() == 1 && k_w.size(0) == kn, who, ": k_w must be [", kn, "]");
+  TORCH_CHECK(q_w.device() == qkv.device() && k_w.device() == qkv.device(), who,
+              ": q_w and k_w must be on the device of qkv");
+  return check_rope_tables(qkv, cos, sin, d / 2, who);
 }
 
+// returns x_save [B, S, nh + nkv, 128] and rstd: [B, S, nh + nkv] per head, [B, S, 2] (q, k) with FULL
+template <bool FULL>
 std::tuple<Tensor, Tensor> qk_norm_rope_fwd(Tensor& qkv, const Tensor& q_w, const Tensor& k_w, const Tensor& cos,
                                             const Tensor& sin, int64_t nh, int64_t nkv, double eps) {
-  const bool per_token = check_qk_norm_rope(qkv, q_w, k_w, cos, sin, nh, nkv);
-  TORCH_CHECK(std::isfinite(eps) && eps >= 0, "qk_norm_rope: eps must be finite and >= 0");
+  const bool per_token = check_qk_norm_rope<FULL>(qkv, q_w, k_w, cos, sin, nh, nkv);
+  TORCH_CHECK(std::isfinite(eps) && eps >= 0, FULL ? "qk_norm_full_rope" : "qk_norm_rope",
+              ": eps must be finite and >= 0");
   const c10::cuda::CUDAGuard guard(qkv.device());
   const int64_t B = qkv.size(0), S = qkv.size(1);
   Tensor x_save = torch::empty({B, S, nh + nkv, 128}, qkv.options());
-  Tensor rstd = torch::empty({B, S, nh + nkv}, qkv.options().dtype(at::kFloat));
-  dtg::qk_norm_rope_fwd(qkv.data_ptr(), q_w.data_ptr(), k_w.data_ptr(), cos.data_ptr<float>(), sin.data_ptr<float>(),
-                        x_save.data_ptr(), rstd.data_ptr<float>(), B * S, (int)S, (int)qkv.size(2), (int)nh, (int)nkv,
-                        per_token, (float)eps, stream());
+  Tensor rstd = torch::empty({B, S, FULL ? 2 : nh + nkv}, qkv.options().dtype(at::kFloat));
+  (FULL ? dtg::qk_norm_full_rope_fwd : dtg::qk_norm_rope_fwd)(
+      qkv.data_ptr(), q_w.data_ptr(), k_w.data_ptr(), cos.data_ptr<float>(), sin.data_ptr<float>(), x_save.data_ptr(),
+      rstd.data_ptr<float>(), B * S, (int)S, (int)qkv.size(2), (int)nh, (int)nkv, per_token, (float)eps, stream());
   return {x_save, rstd};
 }
 
+// in place on dqkv's q|k heads; returns dw: [2, 128] (q, k) per head, [(nh + nkv) * 128] with FULL
+template <bool FULL>
 Tensor qk_norm_rope_bwd(Tensor& dqkv, const Tensor& x_save, const Tensor& rstd, const Tensor& q_w, const Tensor& k_w,
                         const Tensor& cos, const Tensor& sin, int64_t nh, int64_t nkv) {
-  const bool per_token = check_qk_norm_rope(dqkv, q_w, k_w, cos, sin, nh, nkv);
-  const int64_t B = dqkv.size(0), S = dqkv.size(1), T = B * S;
+  const bool per_token = check_qk_norm_rope<FULL>(dqkv, q_w, k_w, cos, sin, nh, nkv);
+  const char* who = FULL ? "qk_norm_full_rope_bwd" : "qk_norm_rope_bwd";
+  const int64_t B = dqkv.size(0), S = dqkv.size(1), T = B * S, nqk = nh + nkv;
   check_vec(x_save, "x_save", at::kBFloat16);
   check_contig(rstd, "rstd", at::kFloat);
-  TORCH_CHECK(x_save.sizes() == at::IntArrayRef({B, S, nh + nkv, 128}) && x_save.device() == dqkv.device(),
-              "qk_norm_rope_bwd: x_save must be [B, S, nh + nkv, 128] on the device of dqkv");
-  TORCH_CHECK(rstd.sizes() == at::IntArrayRef({B, S, nh + nkv}) && rstd.device() == dqkv.device(),
-              "qk_norm_rope_bwd: rstd must be [B, S, nh + nkv] on the device of dqkv");
+  TORCH_CHECK(x_save.sizes() == at::IntArrayRef({B, S, nqk, 128}) && x_save.device() == dqkv.device(), who,
+              ": x_save must be [B, S, nh + nkv, 128] on the device of dqkv");
+  TORCH_CHECK(rstd.sizes() == at::IntArrayRef({B, S, FULL ? 2 : nqk}) && rstd.device() == dqkv.device(), who,
+              ": rstd must be [B, S, ", FULL ? "2" : "nh + nkv", "] on the device of dqkv");
   const c10::cuda::CUDAGuard guard(dqkv.device());
-  Tensor dw = torch::empty({2, 128}, dqkv.options().dtype(at::kFloat));
-  Tensor partial = torch::empty({dtg::qk_norm_rope_bwd_grid(T, (int)(nh + nkv)), 256}, dqkv.options().dtype(at::kFloat));
-  dtg::qk_norm_rope_bwd(dqkv.data_ptr(), x_save.data_ptr(), rstd.data_ptr<float>(), q_w.data_ptr(), k_w.data_ptr(),
-                        cos.data_ptr<float>(), sin.data_ptr<float>(), partial.data_ptr<float>(), dw.data_ptr<float>(), T,
-                        (int)S, (int)dqkv.size(2), (int)nh, (int)nkv, per_token, stream());
-  return dw;
-}
-
-std::tuple<Tensor, Tensor> qk_norm_full_rope_fwd(Tensor& qkv, const Tensor& q_w, const Tensor& k_w, const Tensor& cos,
-                                                 const Tensor& sin, int64_t nh, int64_t nkv, double eps) {
-  const bool per_token = check_qk_norm_rope(qkv, q_w, k_w, cos, sin, nh, nkv, true);
-  TORCH_CHECK(std::isfinite(eps) && eps >= 0, "qk_norm_full_rope: eps must be finite and >= 0");
-  const c10::cuda::CUDAGuard guard(qkv.device());
-  const int64_t B = qkv.size(0), S = qkv.size(1);
-  Tensor x_save = torch::empty({B, S, nh + nkv, 128}, qkv.options());
-  Tensor rstd = torch::empty({B, S, 2}, qkv.options().dtype(at::kFloat));
-  dtg::qk_norm_full_rope_fwd(qkv.data_ptr(), q_w.data_ptr(), k_w.data_ptr(), cos.data_ptr<float>(),
-                             sin.data_ptr<float>(), x_save.data_ptr(), rstd.data_ptr<float>(), B * S, (int)S,
-                             (int)qkv.size(2), (int)nh, (int)nkv, per_token, (float)eps, stream());
-  return {x_save, rstd};
-}
-
-Tensor qk_norm_full_rope_bwd(Tensor& dqkv, const Tensor& x_save, const Tensor& rstd, const Tensor& q_w,
-                             const Tensor& k_w, const Tensor& cos, const Tensor& sin, int64_t nh, int64_t nkv) {
-  const bool per_token = check_qk_norm_rope(dqkv, q_w, k_w, cos, sin, nh, nkv, true);
-  const int64_t B = dqkv.size(0), S = dqkv.size(1), T = B * S;
-  check_vec(x_save, "x_save", at::kBFloat16);
-  check_contig(rstd, "rstd", at::kFloat);
-  TORCH_CHECK(x_save.sizes() == at::IntArrayRef({B, S, nh + nkv, 128}) && x_save.device() == dqkv.device(),
-              "qk_norm_full_rope_bwd: x_save must be [B, S, nh + nkv, 128] on the device of dqkv");
-  TORCH_CHECK(rstd.sizes() == at::IntArrayRef({B, S, 2}) && rstd.device() == dqkv.device(),
-              "qk_norm_full_rope_bwd: rstd must be [B, S, 2] on the device of dqkv");
-  const c10::cuda::CUDAGuard guard(dqkv.device());
-  const int64_t W = (nh + nkv) * 128;
-  Tensor dw = torch::empty({W}, dqkv.options().dtype(at::kFloat));
-  Tensor partial = torch::empty({T > 0 ? dtg::qk_norm_full_rope_bwd_grid(T, (int)(nh + nkv)) : 1, W},
-                                dqkv.options().dtype(at::kFloat));
-  dtg::qk_norm_full_rope_bwd(dqkv.data_ptr(), x_save.data_ptr(), rstd.data_ptr<float>(), q_w.data_ptr(),
-                             k_w.data_ptr(), cos.data_ptr<float>(), sin.data_ptr<float>(), partial.data_ptr<float>(),
-                             dw.data_ptr<float>(), T, (int)S, (int)dqkv.size(2), (int)nh, (int)nkv, per_token,
-                             stream());
+  Tensor dw = FULL ? torch::empty({nqk * 128}, dqkv.options().dtype(at::kFloat))
+                   : torch::empty({2, 128}, dqkv.options().dtype(at::kFloat));
+  const int grid = (FULL ? dtg::qk_norm_full_rope_bwd_grid : dtg::qk_norm_rope_bwd_grid)(T, (int)nqk);
+  Tensor partial = torch::empty({grid, dw.numel()}, dqkv.options().dtype(at::kFloat));
+  (FULL ? dtg::qk_norm_full_rope_bwd : dtg::qk_norm_rope_bwd)(
+      dqkv.data_ptr(), x_save.data_ptr(), rstd.data_ptr<float>(), q_w.data_ptr(), k_w.data_ptr(),
+      cos.data_ptr<float>(), sin.data_ptr<float>(), partial.data_ptr<float>(), dw.data_ptr<float>(), T, (int)S,
+      (int)dqkv.size(2), (int)nh, (int)nkv, per_token, stream());
   return dw;
 }
 
@@ -586,11 +566,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("rmsnorm_bwd", &rmsnorm_bwd);
   m.def("rope_inplace", &rope_inplace, py::arg("qkv"), py::arg("cos"), py::arg("sin"), py::arg("n_rot"),
         py::arg("inverse"), py::arg("rot_dim") = py::none());
-  m.def("qk_norm_rope_fwd", &qk_norm_rope_fwd);
-  m.def("qk_norm_rope_bwd", &qk_norm_rope_bwd);
+  m.def("qk_norm_rope_fwd", &qk_norm_rope_fwd<false>);
+  m.def("qk_norm_rope_bwd", &qk_norm_rope_bwd<false>);
   m.def("rmsnorm_add_fwd", &rmsnorm_add_fwd);
-  m.def("qk_norm_full_rope_fwd", &qk_norm_full_rope_fwd);
-  m.def("qk_norm_full_rope_bwd", &qk_norm_full_rope_bwd);
+  m.def("qk_norm_full_rope_fwd", &qk_norm_rope_fwd<true>);
+  m.def("qk_norm_full_rope_bwd", &qk_norm_rope_bwd<true>);
   m.def("qk_norm_full_rope_bwd_grid", [](int64_t T, int64_t nqk) {
     TORCH_CHECK(T > 0 && nqk >= 2 && nqk <= dtg::qk_norm_full_rope_max_heads(), "qk_norm_full_rope_bwd_grid: bad shape");
     return dtg::qk_norm_full_rope_bwd_grid(T, (int)nqk);

@@ -35,6 +35,20 @@ inline int sm_count() {
   return n;
 }
 
+// CTAs of 256 threads for a grid-strided elementwise kernel over total_threads work items: at most 16 per SM
+inline int ew_grid(long long total_threads) {
+  long long g = (total_threads + 255) / 256;
+  const long long cap = (long long)sm_count() * 16;
+  if (g > cap) g = cap;
+  if (g < 1) g = 1;
+  return (int)g;
+}
+
+// A sum of squares of bf16 values at or above kSumSqBig (bf16 reaches 2^128) can overflow fp32.  Such values are
+// squared scaled by kSumSqDown, which is exact for every element above 2^-77 (a smaller one is below 2^-94 of the
+// largest square and cannot change the sum) and keeps a sum of 2^16 squares of bf16's largest values finite.
+constexpr float kSumSqBig = 0x1p56f, kSumSqDown = 0x1p-72f, kSumSqUp = 0x1p72f;
+
 // ---- device-side helpers (nvcc only) ----------------------------------------------------------
 #ifdef __CUDACC__
 struct alignas(16) bf16x8 {
@@ -97,6 +111,13 @@ __device__ __forceinline__ float block_max(float v, float* red) {
   float r = (lane < nw) ? red[lane] : -INFINITY;
   r = warp_max(r);
   return r;
+}
+
+// the scale to square values whose largest magnitude is am by, and rsqrt(mean(x^2) + eps) of n values from their sum
+// of squares ss taken at that scale (eps is negligible next to a rescued sum)
+__device__ __forceinline__ float sumsq_scale(float am) { return am >= kSumSqBig ? kSumSqDown : 1.f; }
+__device__ __forceinline__ float sumsq_rstd(float ss, float am, float n, float eps) {
+  return am >= kSumSqBig ? rsqrtf(ss / n) * kSumSqDown : rsqrtf(ss / n + eps);
 }
 
 #endif  // __CUDACC__

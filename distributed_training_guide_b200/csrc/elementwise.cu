@@ -1,9 +1,9 @@
-// Memory-bound ops of the Llama step, hand-written for sm_90a: in-place RoPE on the fused qkv activation,
-//   SwiGLU fwd / bwd, embedding gather / scatter-add, scalar scale, the bias gradient and the fixed-order column
-//   sums the norm backwards share, GELU-tanh (StarCoder2) and exact GELU fwd / bwd.  The row norms are in norm.cu.
+// Memory-bound ops of the Llama step, hand-written for sm_90a: SwiGLU fwd / bwd, embedding gather / scatter-add,
+//   scalar scale, the bias gradient and the fixed-order column sums the norm backwards share, GELU-tanh (StarCoder2)
+//   and exact GELU fwd / bwd.  The row norms are in norm.cu, RoPE and QK-norm in rope.cu.
 // All are pure-bandwidth kernels: 16-byte vector accesses, fp32 math in registers, one pass
-// over the activations.  Replaces the ~10 ATen kernels per RoPE the reference runs
-// in eager chapters, and Inductor's Triton fusions in compiled ones (SURVEY.md K4-K6, K9, K10).
+// over the activations.  Replaces the ATen kernels the reference runs in eager chapters, and Inductor's Triton
+// fusions in compiled ones (SURVEY.md K4-K6, K9, K10).
 #include "api.h"
 #include "common.cuh"
 
@@ -151,8 +151,6 @@ __global__ void gelu_tanh_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const
   }
 }
 
-static int ew_grid(long long total_threads);
-
 void gelu_tanh_fwd(const void* x, void* y, long long n, cudaStream_t s) {
   if (n % 8 != 0) throw std::runtime_error("gelu_tanh: the element count must be a multiple of 8");
   gelu_tanh_fwd_kernel<<<ew_grid(n / 8), 256, 0, s>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, n / 8);
@@ -220,102 +218,6 @@ void gelu_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t
 }
 
 // ------------------------------------------------------------------------------------------
-// RoPE (half-rotation layout) in place on heads [0, n_rot) of qkv [T, n_heads, d].
-// cos/sin: fp32 [S, d/2] (pos = t % S) or per-token [T, d/2].
-// ------------------------------------------------------------------------------------------
-__global__ void rope_inplace_kernel(__nv_bfloat16* __restrict__ qkv, const float* __restrict__ cs,
-                                    const float* __restrict__ sn, long long T, int S, int n_heads, int n_rot, int d,
-                                    int per_token, float sign) {
-  const int d2 = d >> 1;
-  const int vec_per_head = d2 >> 3;  // 8-wide vectors in one half
-  const long long total = T * (long long)n_rot * vec_per_head;
-  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const int v = (int)(idx % vec_per_head);
-    const long long th = idx / vec_per_head;
-    const int head = (int)(th % n_rot);
-    const long long t = th / n_rot;
-    const long long pos = per_token ? t : (t % S);
-    __nv_bfloat16* p = qkv + (t * n_heads + head) * (long long)d + v * 8;
-    float a[8], b[8], c[8], s[8];
-    unpack8(ld8(p), a);
-    unpack8(ld8(p + d2), b);
-    const float4* cp = reinterpret_cast<const float4*>(cs + pos * d2 + v * 8);
-    const float4* sp = reinterpret_cast<const float4*>(sn + pos * d2 + v * 8);
-    float4 c0 = cp[0], c1 = cp[1], s0 = sp[0], s1 = sp[1];
-    c[0] = c0.x; c[1] = c0.y; c[2] = c0.z; c[3] = c0.w; c[4] = c1.x; c[5] = c1.y; c[6] = c1.z; c[7] = c1.w;
-    s[0] = s0.x; s[1] = s0.y; s[2] = s0.z; s[3] = s0.w; s[4] = s1.x; s[5] = s1.y; s[6] = s1.z; s[7] = s1.w;
-    float o1[8], o2[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float sj = s[j] * sign;
-      o1[j] = a[j] * c[j] - b[j] * sj;
-      o2[j] = b[j] * c[j] + a[j] * sj;
-    }
-    st8(p, pack8(o1));
-    st8(p + d2, pack8(o2));
-  }
-}
-
-// Partial rotary (GPT-NeoX): the pairs (j, j + rot_dim/2), j < rot_dim/2, of each head's first rot_dim elements are
-// rotated as rope_inplace_kernel rotates a head of rot_dim; elements [rot_dim, d) are never read or written.
-// cos/sin: [S, rot_dim/2] or [T, rot_dim/2].  A kernel of its own so that the full-width kernel every other family runs
-// is unchanged.
-__global__ void rope_partial_inplace_kernel(__nv_bfloat16* __restrict__ qkv, const float* __restrict__ cs,
-                                            const float* __restrict__ sn, long long T, int S, int n_heads, int n_rot,
-                                            int d, int rot_dim, int per_token, float sign) {
-  const int r2 = rot_dim >> 1;
-  const int vec_per_head = r2 >> 3;
-  const long long total = T * (long long)n_rot * vec_per_head;
-  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const int v = (int)(idx % vec_per_head);
-    const long long th = idx / vec_per_head;
-    const int head = (int)(th % n_rot);
-    const long long t = th / n_rot;
-    const long long pos = per_token ? t : (t % S);
-    __nv_bfloat16* p = qkv + (t * n_heads + head) * (long long)d + v * 8;
-    float a[8], b[8], c[8], s[8];
-    unpack8(ld8(p), a);
-    unpack8(ld8(p + r2), b);
-    const float4* cp = reinterpret_cast<const float4*>(cs + pos * r2 + v * 8);
-    const float4* sp = reinterpret_cast<const float4*>(sn + pos * r2 + v * 8);
-    float4 c0 = cp[0], c1 = cp[1], s0 = sp[0], s1 = sp[1];
-    c[0] = c0.x; c[1] = c0.y; c[2] = c0.z; c[3] = c0.w; c[4] = c1.x; c[5] = c1.y; c[6] = c1.z; c[7] = c1.w;
-    s[0] = s0.x; s[1] = s0.y; s[2] = s0.z; s[3] = s0.w; s[4] = s1.x; s[5] = s1.y; s[6] = s1.z; s[7] = s1.w;
-    float o1[8], o2[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float sj = s[j] * sign;
-      o1[j] = a[j] * c[j] - b[j] * sj;
-      o2[j] = b[j] * c[j] + a[j] * sj;
-    }
-    st8(p, pack8(o1));
-    st8(p + r2, pack8(o2));
-  }
-}
-
-void rope_inplace(void* qkv, const float* cos, const float* sin, long long T, int S, int n_heads, int n_rot, int d,
-                  int rot_dim, bool per_token, bool inverse, cudaStream_t s) {
-  if (d % 16 != 0) throw std::runtime_error("rope: head_dim must be a multiple of 16");
-  if (rot_dim % 16 != 0 || rot_dim <= 0 || rot_dim > d)
-    throw std::runtime_error("rope: rot_dim must be a positive multiple of 16, <= head_dim");
-  const long long total = T * (long long)n_rot * (rot_dim / 16);
-  int grid = (int)((total + 255) / 256);
-  const int cap = sm_count() * 16;
-  if (grid > cap) grid = cap;
-  if (grid < 1) grid = 1;
-  if (rot_dim == d)
-    rope_inplace_kernel<<<grid, 256, 0, s>>>((__nv_bfloat16*)qkv, cos, sin, T, S, n_heads, n_rot, d,
-                                             per_token ? 1 : 0, inverse ? -1.f : 1.f);
-  else
-    rope_partial_inplace_kernel<<<grid, 256, 0, s>>>((__nv_bfloat16*)qkv, cos, sin, T, S, n_heads, n_rot, d, rot_dim,
-                                                     per_token ? 1 : 0, inverse ? -1.f : 1.f);
-  note_launch();
-  DTG_LAUNCH_CHECK();
-}
-
-// ------------------------------------------------------------------------------------------
 // SwiGLU on gu = [gate | up]  ([T, 2I]):  h = silu(g) * u
 // ------------------------------------------------------------------------------------------
 __global__ void swiglu_fwd_kernel(const __nv_bfloat16* __restrict__ gu, __nv_bfloat16* __restrict__ h, long long T,
@@ -357,14 +259,6 @@ __global__ void swiglu_bwd_kernel(const __nv_bfloat16* __restrict__ dh, const __
     st8(dgu + t * 2 * I + v * 8, pack8(dg));
     st8(dgu + t * 2 * I + I + v * 8, pack8(du));
   }
-}
-
-static int ew_grid(long long total_threads) {
-  long long g = (total_threads + 255) / 256;
-  const long long cap = (long long)sm_count() * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
 }
 
 void swiglu_fwd(const void* gu, void* h, long long T, int I, cudaStream_t s) {

@@ -18,10 +18,9 @@ namespace {
 
 constexpr bool is_ln(NormKind k) { return k != NormKind::kRms; }
 
-// A LayerNorm row whose sums overflow fp32 (elements near the bf16 limit) is redone scaled by 2^-72, which is exact
-// for every element above 2^-77; mean and rstd are saved in the row's own units.  In the backward h - mean can only
-// overflow when rstd is below 2^-121, so rows with rstd < 2^-100 recompute xhat from h and mean scaled likewise.
-constexpr float kLnDown = 0x1p-72f, kLnUp = 0x1p72f;
+// A LayerNorm row whose sums overflow fp32 (elements near the bf16 limit) is redone scaled by kSumSqDown (2^-72,
+// common.cuh); mean and rstd are saved in the row's own units.  In the backward h - mean can only overflow when rstd
+// is below 2^-121, so rows with rstd < 2^-100 recompute xhat from h and mean scaled likewise.
 
 // ------------------------------------------------------------------------------------------
 // Launch table: (NV 16-byte vectors per thread, NT threads per CTA); a hidden size H takes the first row with
@@ -155,14 +154,14 @@ __global__ void __launch_bounds__(NT) norm_fwd_kernel(
     mean = block_sum(s, red) / (float)H;
     float ss = block_sum(ln_sq_dev<NV, NT>(cache, nvec, mean, 1.f), red);
     if (!(isfinite(mean) && isfinite(ss))) {   // uniform over the CTA: block_sum broadcasts
-      scale = kLnDown;
-      mean = block_sum(ln_sum<NV, NT>(cache, nvec, kLnDown), red) / (float)H;
-      ss = block_sum(ln_sq_dev<NV, NT>(cache, nvec, mean, kLnDown), red);
+      scale = kSumSqDown;
+      mean = block_sum(ln_sum<NV, NT>(cache, nvec, kSumSqDown), red) / (float)H;
+      ss = block_sum(ln_sq_dev<NV, NT>(cache, nvec, mean, kSumSqDown), red);
     }
     rstd = rsqrtf(ss / (float)H + eps * scale * scale);
     if (threadIdx.x == 0) {
-      mean_out[row] = scale == 1.f ? mean : mean * kLnUp;
-      rstd_out[row] = scale == 1.f ? rstd : rstd * kLnDown;
+      mean_out[row] = scale == 1.f ? mean : mean * kSumSqUp;
+      rstd_out[row] = scale == 1.f ? rstd : rstd * kSumSqDown;
     }
   } else {
     s = block_sum(s, red);
@@ -235,9 +234,9 @@ __global__ void __launch_bounds__(NT) norm_bwd_kernel(
     if constexpr (is_ln(K)) {
       mu = mean[row];
       if (rs < 0x1p-100f) {
-        scale = kLnDown;
-        mu *= kLnDown;
-        rs *= kLnUp;
+        scale = kSumSqDown;
+        mu *= kSumSqDown;
+        rs *= kSumSqUp;
       }
     }
     const size_t base = (size_t)row * H;
@@ -287,7 +286,7 @@ __global__ void __launch_bounds__(NT) norm_bwd_kernel(
     }
     if constexpr (is_ln(K)) sg = block_sum(sg, red) / (float)H;
     sgx = block_sum(sgx, red) / (float)H;
-    const float rs_out = scale == 1.f ? rs : rs * kLnDown;   // rstd in the row's own units
+    const float rs_out = scale == 1.f ? rs : rs * kSumSqDown;   // rstd in the row's own units
 #pragma unroll
     for (int k = 0; k < NV; ++k) {
       const int i = threadIdx.x + k * NT;

@@ -175,6 +175,8 @@ class LlamaAttention(nn.Module):
         self.num_heads = config.num_attention_heads // tp_size
         self.num_kv_heads = config.num_key_value_heads // tp_size
         self.head_dim = d
+        #: the rotated share of each q/k head: all of it but for GPT-NeoX's partial rotary
+        self.rotary_dim = config.rotary_dim
         #: sliding-window attention (Mistral): None, or W >= 1 with query q seeing keys k > q - W only
         self.sliding_window = config.sliding_window
         #: q/k/v biases (Qwen2, StarCoder2), split with their heads under tensor parallelism; an o_proj bias
@@ -198,7 +200,7 @@ class LlamaAttention(nn.Module):
         """RoPE (after QK-norm, when the layer has it) on the q and k heads of ``qkv`` [B,S,heads,d], in place on
         the kernel path."""
         if self.q_norm is None:
-            return ops.rope_qkv_(qkv, cos, sin, self.num_heads + self.num_kv_heads)
+            return ops.rope_qkv_(qkv, cos, sin, self.num_heads + self.num_kv_heads, self.rotary_dim)
         if self.full_qk_norm:
             return ops.olmo_qk_norm_rope_(qkv, self.q_norm.weight, self.k_norm.weight, cos, sin, self.num_heads,
                                           self.num_kv_heads, self.q_norm.eps)
@@ -415,7 +417,6 @@ class GPTNeoXDecoderLayer(Starcoder2DecoderLayer):
     def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
         assert tp_size == 1, "GPT-NeoX layers are not tensor-parallel"
         super().__init__(config, layer_idx, dtype, device, tp_size)
-        self.rotary_dim = config.rotary_dim
 
     def forward(self, x, residual, cos, sin, doc_start=None):
         att = self.self_attn
@@ -426,7 +427,7 @@ class GPTNeoXDecoderLayer(Starcoder2DecoderLayer):
         w, owner = self._qkv_weight()
         b, b_owner = self._qkv_bias()
         qkv = fused_linear(y1, w, owner, b, b_owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
-        qkv = ops.rope_qkv_(qkv, cos, sin, att.num_heads + att.num_kv_heads, self.rotary_dim)
+        qkv = att.position_qk_(qkv, cos, sin)
         a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
         a = a.reshape(B, S, att.num_heads * att.head_dim)
         mlp = self.mlp

@@ -668,12 +668,17 @@ def rope_qkv_(qkv, cos, sin, n_rot_heads, rotary_dim=None):
 
 
 class _QKNormRope(torch.autograd.Function):
+    """QK-norm + RoPE in place on qkv's q|k heads: per head (Qwen3) or, with ``full``, over each token's whole q and k
+    regions (OLMo 2)."""
+
     @staticmethod
-    def forward(ctx, qkv, q_w, k_w, cos, sin, nh, nkv, eps):
+    def forward(ctx, qkv, q_w, k_w, cos, sin, nh, nkv, eps, full):
         C = _ext.load()
-        x_save, rstd = C.qk_norm_rope_fwd(qkv, q_w, k_w, cos, sin, nh, nkv, float(eps))
+        fwd = C.qk_norm_full_rope_fwd if full else C.qk_norm_rope_fwd
+        x_save, rstd = fwd(qkv, q_w, k_w, cos, sin, nh, nkv, float(eps))
         ctx.save_for_backward(x_save, rstd, q_w, k_w, cos, sin)
         ctx.heads = (nh, nkv)
+        ctx.full = full
         ctx.w_params = (q_w, k_w)
         return qkv.detach()   # in place, handed to autograd as a fresh tensor (see _RopeQKV)
 
@@ -683,10 +688,12 @@ class _QKNormRope(torch.autograd.Function):
         x_save, rstd, q_w, k_w, cos, sin = ctx.saved_tensors
         if not dqkv.is_contiguous():
             dqkv = dqkv.contiguous()
-        dw32 = C.qk_norm_rope_bwd(dqkv, x_save, rstd, q_w, k_w, cos, sin, *ctx.heads)   # in place on dqkv's q|k
-        dq = _emit_weight_grad(ctx.w_params[0], _norm_dw_into(dw32[0]), q_w)
-        dk = _emit_weight_grad(ctx.w_params[1], _norm_dw_into(dw32[1]), k_w)
-        return dqkv, dq, dk, None, None, None, None, None
+        bwd = C.qk_norm_full_rope_bwd if ctx.full else C.qk_norm_rope_bwd
+        dw32 = bwd(dqkv, x_save, rstd, q_w, k_w, cos, sin, *ctx.heads).view(-1)   # in place on dqkv's q|k; q then k
+        nq = q_w.numel()
+        dq = _emit_weight_grad(ctx.w_params[0], _norm_dw_into(dw32[:nq]), q_w)
+        dk = _emit_weight_grad(ctx.w_params[1], _norm_dw_into(dw32[nq:]), k_w)
+        return dqkv, dq, dk, None, None, None, None, None, None
 
 
 def qk_norm_rope_(qkv, q_w, k_w, cos, sin, nh, nkv, eps):
@@ -701,34 +708,11 @@ def qk_norm_rope_(qkv, q_w, k_w, cos, sin, nh, nkv, eps):
     on their first use in a step and accumulated on later ones."""
     if (_ext.use_cuda_kernel("qk_norm_rope", qkv, q_w, k_w) and qkv.dtype == torch.bfloat16
             and qkv.shape[-1] == 128):
-        return _QKNormRope.apply(qkv, q_w, k_w, cos.contiguous(), sin.contiguous(), nh, nkv, eps)
+        return _QKNormRope.apply(qkv, q_w, k_w, cos.contiguous(), sin.contiguous(), nh, nkv, eps, False)
     q = ref.rms_norm(qkv[:, :, :nh], q_w, eps)
     k = ref.rms_norm(qkv[:, :, nh:nh + nkv], k_w, eps)
     rot = ref.rope_apply(torch.cat([q, k], dim=2), cos, sin)
     return torch.cat([rot, qkv[:, :, nh + nkv:]], dim=2)
-
-
-class _OlmoQKNormRope(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, qkv, q_w, k_w, cos, sin, nh, nkv, eps):
-        C = _ext.load()
-        x_save, rstd = C.qk_norm_full_rope_fwd(qkv, q_w, k_w, cos, sin, nh, nkv, float(eps))
-        ctx.save_for_backward(x_save, rstd, q_w, k_w, cos, sin)
-        ctx.heads = (nh, nkv)
-        ctx.w_params = (q_w, k_w)
-        return qkv.detach()   # in place, handed to autograd as a fresh tensor (see _RopeQKV)
-
-    @staticmethod
-    def backward(ctx, dqkv):
-        C = _ext.load()
-        x_save, rstd, q_w, k_w, cos, sin = ctx.saved_tensors
-        if not dqkv.is_contiguous():
-            dqkv = dqkv.contiguous()
-        dw32 = C.qk_norm_full_rope_bwd(dqkv, x_save, rstd, q_w, k_w, cos, sin, *ctx.heads)   # in place on q|k
-        nq = q_w.numel()
-        dq = _emit_weight_grad(ctx.w_params[0], _norm_dw_into(dw32[:nq]), q_w)
-        dk = _emit_weight_grad(ctx.w_params[1], _norm_dw_into(dw32[nq:]), k_w)
-        return dqkv, dq, dk, None, None, None, None, None
 
 
 def olmo_qk_norm_rope_(qkv, q_w, k_w, cos, sin, nh, nkv, eps):
@@ -743,7 +727,7 @@ def olmo_qk_norm_rope_(qkv, q_w, k_w, cos, sin, nh, nkv, eps):
     parameters are overwritten on their first use in a step and accumulated on later ones."""
     if (_ext.use_cuda_kernel("qk_norm_rope", qkv, q_w, k_w) and qkv.dtype == torch.bfloat16
             and qkv.shape[-1] == 128):
-        return _OlmoQKNormRope.apply(qkv, q_w, k_w, cos.contiguous(), sin.contiguous(), nh, nkv, eps)
+        return _QKNormRope.apply(qkv, q_w, k_w, cos.contiguous(), sin.contiguous(), nh, nkv, eps, True)
     B, S, _, d = qkv.shape
     q = ref.rms_norm_one_rounding(qkv[:, :, :nh].reshape(B, S, nh * d), q_w, eps).view(B, S, nh, d)
     k = ref.rms_norm_one_rounding(qkv[:, :, nh:nh + nkv].reshape(B, S, nkv * d), k_w, eps).view(B, S, nkv, d)

@@ -162,6 +162,22 @@ def test_rope_rot_dim_default_is_the_head_and_refusals():
             C.rope_inplace(x.clone(), c32, s32, 2, False, rot_dim=rot)
     with pytest.raises(RuntimeError, match="wrong shape"):
         C.rope_inplace(x.clone(), cos, sin, 2, False, rot_dim=32)
+    # a per-token [B', S, r/2] table of another batch, or on another device, is refused before any launch
+    xb = torch.randn(2, 128, 4, 128).bfloat16().cuda()
+    c3, s3 = ref.rope_tables(torch.randint(0, 2048, (3, 128)).cuda(), 32, 1e4)
+    n0 = C.launch_count()
+    for rows in (1, 3):
+        with pytest.raises(RuntimeError, match="wrong shape"):
+            C.rope_inplace(xb.clone(), c3[:rows].contiguous(), s3[:rows].contiguous(), 2, False, rot_dim=32)
+    if torch.cuda.device_count() > 1:
+        with pytest.raises(RuntimeError, match="device"):
+            C.rope_inplace(xb.clone(), c3[:2].to("cuda:1"), s3[:2].to("cuda:1"), 2, False, rot_dim=32)
+    assert C.launch_count() == n0
+    # a [T, r/2] table is the [B, S, r/2] one
+    a, b = xb.clone(), xb.clone()
+    C.rope_inplace(a, c3[:2].contiguous(), s3[:2].contiguous(), 2, False, rot_dim=32)
+    C.rope_inplace(b, c3[:2].reshape(256, 16).contiguous(), s3[:2].reshape(256, 16).contiguous(), 2, False, rot_dim=32)
+    assert torch.equal(a, b) and not torch.equal(a, xb)
 
 
 # ---------------------------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-"""The QK-norm + RoPE kernels (``csrc/qk_norm_rope.cu``) against an fp64 composition, element by element.
+"""The QK-norm + RoPE kernels (``csrc/rope.cu``) against an fp64 composition, element by element.
 
 Forward: each output element may differ from the exact ``rope(rmsnorm(x) * w)`` by the three bf16 roundings the
 kernel makes (``bf16(x * rstd)``, ``bf16(. * w)``, the stored output): 3 * 2^-8 of the terms the rotation sums.
@@ -63,12 +63,16 @@ def _fp64(qkv, q_w, k_w, cos, sin, nh, nkv, dout):
     return out, torch.cat([mag1, mag2], -1), dx, dx_mag, (dwq, dwk), (mq, mk)
 
 
-def _case(B, S, nh, nkv, per_token, seed, scale=1.0, zero_head=False, gains="random"):
+def _case(B, S, nh, nkv, per_token, seed, scale=1.0, zero_head=False, gains="random", bf16_max=False):
     gen = torch.Generator(device="cuda").manual_seed(seed)
     qkv = (torch.randn(B, S, nh + 2 * nkv, 128, generator=gen, device="cuda") * scale).to(torch.bfloat16)
     if zero_head:
         qkv[:, 1, 0] = 0
         qkv[:, -1, nh] = 0
+    if bf16_max:   # a q head with two and a k head with three elements at the bf16 limit, ordinary heads beside them
+        big = torch.finfo(torch.bfloat16).max
+        qkv[:, :, 0, 0], qkv[:, :, 0, 64] = big, -big
+        qkv[:, :, nh, 3], qkv[:, :, nh, 77], qkv[:, :, nh, 100] = big, big, -big
     q_w = torch.randn(128, generator=gen, device="cuda").to(torch.bfloat16)
     k_w = torch.randn(128, generator=gen, device="cuda").to(torch.bfloat16)
     if gains == "zeros-and-negatives":
@@ -89,6 +93,8 @@ CASES = {
     "gains-zero-negative-per-token": dict(B=1, S=300, nh=4, nkv=1, per_token=True, gains="zeros-and-negatives"),
     "all-zero-heads": dict(B=2, S=64, nh=8, nkv=2, per_token=False, zero_head=True),
     "near-bf16-limit": dict(B=1, S=40, nh=4, nkv=1, per_token=False, scale=1e37),
+    # squares whose fp32 sum overflows unless the head is summed scaled down far enough
+    "bf16-max-elements": dict(B=2, S=48, nh=4, nkv=2, per_token=False, bf16_max=True),
     "tiny-inputs": dict(B=1, S=40, nh=4, nkv=1, per_token=False, scale=1e-30),
     "long-qwen3-8b": dict(B=1, S=4096, nh=32, nkv=8, per_token=False),
 }
