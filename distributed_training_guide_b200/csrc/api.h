@@ -65,13 +65,15 @@ void gelu_fwd(const void* x, void* y, long long n, cudaStream_t s);
 void gelu_bwd(const void* dy, const void* x, void* dx, long long n, cudaStream_t s);
 void swiglu_fwd(const void* gu, void* h, long long T, int I, cudaStream_t s);
 void swiglu_bwd(const void* dh, const void* gu, void* dgu, long long T, int I, cudaStream_t s);
-void embedding_fwd(const long long* ids, const void* w, void* out, long long T, int H, cudaStream_t s);
+// Embedding ids follow the vocabulary rule of common.cuh: an id outside [0, V) gets a NaN row from the forward and adds
+// to no row of dw.  out [T,H] = w [V,H] rows.
+void embedding_fwd(const long long* ids, const void* w, void* out, long long T, long long V, int H, cudaStream_t s);
 // dw [V,H] = (or +=) the per-id sum of dout [T,H], in fp32 with one rounding per row.  Scratch: slot [V] uint32 and
 // sums [T,H] fp32, both filled here.  Overwrite mode zeroes the whole table first.
 void embedding_bwd(const void* dout, const long long* ids, void* dw, unsigned int* slot, float* sums, long long T,
                    long long V, int H, bool accumulate, cudaStream_t s);
-void embedding_bwd_sorted(const void* dout, const long long* ids_sorted, const long long* perm, void* dw, long long T, int H,
-                          bool accumulate, cudaStream_t s);
+void embedding_bwd_sorted(const void* dout, const long long* ids_sorted, const long long* perm, void* dw, long long T,
+                          long long V, int H, bool accumulate, cudaStream_t s);
 void scale_inplace(void* x, const float* scale, long long n, cudaStream_t s);
 
 // ---- rope.cu -------------------------------------------------------------------------------

@@ -475,11 +475,10 @@ Tensor swiglu_bwd(const Tensor& dh, const Tensor& gu) {
 }
 
 Tensor cross_entropy_fwd_bwd(Tensor& logits, const Tensor& targets) {
-  check_vec(logits, "logits", at::kBFloat16);
-  check_contig(targets, "targets", at::kLong);
+  dtg::check_loss_args(logits, targets, "cross_entropy");
   const c10::cuda::CUDAGuard guard(logits.device());
   const int T = (int)logits.size(0), V = (int)logits.size(1);
-  TORCH_CHECK(targets.numel() == T, "targets must have one entry per logits row");
+  if (T == 0) return torch::zeros({}, logits.options().dtype(at::kFloat));   // as with every target ignored
   Tensor scratch = torch::empty({T + 2}, logits.options().dtype(at::kFloat));
   float* sp = scratch.data_ptr<float>();
   dtg::cross_entropy_fwd_bwd(logits.data_ptr(), (const long long*)targets.data_ptr<int64_t>(),
@@ -495,23 +494,23 @@ void scale_inplace(Tensor& x, const Tensor& scale) {
 }
 
 Tensor embedding_fwd(const Tensor& ids, const Tensor& w) {
-  check_contig(ids, "ids", at::kLong);
-  check_vec(w, "w", at::kBFloat16);
+  dtg::check_embedding_args(ids, w, "w", "embedding_fwd");
   const c10::cuda::CUDAGuard guard(w.device());
   Tensor out = torch::empty({ids.numel(), w.size(1)}, w.options());
-  dtg::embedding_fwd((const long long*)ids.data_ptr<int64_t>(), w.data_ptr(), out.data_ptr(), ids.numel(),
+  dtg::embedding_fwd((const long long*)ids.data_ptr<int64_t>(), w.data_ptr(), out.data_ptr(), ids.numel(), w.size(0),
                      (int)w.size(1), stream());
   return out;
 }
 void embedding_bwd_sorted(const Tensor& dout, const Tensor& ids_sorted, const Tensor& perm, Tensor& dw, bool accumulate) {
   check_vec(dout, "dout", at::kBFloat16);
-  check_vec(dw, "dw", at::kBFloat16);
-  check_contig(ids_sorted, "ids_sorted", at::kLong);
+  dtg::check_embedding_args(ids_sorted, dw, "dw", "embedding_bwd_sorted");
   check_contig(perm, "perm", at::kLong);
   TORCH_CHECK(perm.numel() == ids_sorted.numel(), "int64 ids / permutation");
+  TORCH_CHECK(dout.dim() == 2 && dout.size(0) == ids_sorted.numel() && dout.size(1) == dw.size(1),
+              "embedding_bwd_sorted: dout must be [T, H] for T ids and dw [V, H]");
   const c10::cuda::CUDAGuard guard(dw.device());
   dtg::embedding_bwd_sorted(dout.data_ptr(), (const long long*)ids_sorted.data_ptr<int64_t>(),
-                            (const long long*)perm.data_ptr<int64_t>(), dw.data_ptr(), ids_sorted.numel(),
+                            (const long long*)perm.data_ptr<int64_t>(), dw.data_ptr(), ids_sorted.numel(), dw.size(0),
                             (int)dw.size(1), accumulate, at::cuda::getCurrentCUDAStream().stream());
 }
 
@@ -519,8 +518,7 @@ void embedding_bwd_sorted(const Tensor& dout, const Tensor& ids_sorted, const Te
 // (the caching allocator keeps them on this stream)
 void embedding_bwd(const Tensor& dout, const Tensor& ids, Tensor& dw, bool accumulate) {
   check_vec(dout, "dout", at::kBFloat16);
-  check_contig(ids, "ids", at::kLong);
-  check_vec(dw, "dw", at::kBFloat16);
+  dtg::check_embedding_args(ids, dw, "dw", "embedding_bwd");
   TORCH_CHECK(dw.dim() == 2 && dout.dim() == 2 && dout.size(1) == dw.size(1) && dout.size(0) == ids.numel(),
               "embedding_bwd: dout must be [T, H] for T ids and dw [V, H]");
   const c10::cuda::CUDAGuard guard(dw.device());
@@ -548,6 +546,28 @@ void adamw_flat(Tensor& p, const Tensor& g, Tensor& m, Tensor& v, double lr, dou
 }
 
 }  // namespace
+
+namespace dtg {
+void check_loss_args(const Tensor& logits, const Tensor& targets, const char* who) {
+  check_vec(logits, "logits", at::kBFloat16);
+  TORCH_CHECK(logits.dim() == 2, who, ": logits must be 2-D [T, V]");
+  TORCH_CHECK(logits.size(1) > 0 && logits.size(1) % 8 == 0, who, ": the vocabulary (logits.size(1)) must be a ",
+              "positive multiple of 8, got ", logits.size(1));
+  TORCH_CHECK(targets.is_cuda() && targets.device() == logits.device(), who, ": targets must be on logits' device");
+  TORCH_CHECK(targets.scalar_type() == at::kLong, who, ": targets must be int64");
+  TORCH_CHECK(targets.is_contiguous(), who, ": targets must be contiguous");
+  TORCH_CHECK(targets.numel() == logits.size(0), who, ": targets must have one entry per logits row (",
+              logits.size(0), "), got ", targets.numel());
+}
+void check_embedding_args(const Tensor& ids, const Tensor& table, const char* table_name, const char* who) {
+  check_vec(table, table_name, at::kBFloat16);
+  TORCH_CHECK(table.dim() == 2 && table.size(1) % 8 == 0, who, ": ", table_name,
+              " must be 2-D [V, H] with H a multiple of 8");
+  TORCH_CHECK(ids.is_cuda() && ids.device() == table.device(), who, ": ids must be on the device of ", table_name);
+  TORCH_CHECK(ids.scalar_type() == at::kLong, who, ": ids must be int64");
+  TORCH_CHECK(ids.is_contiguous(), who, ": ids must be contiguous");
+}
+}  // namespace dtg
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "distributed_training_guide_b200 sm_90a kernels";

@@ -65,10 +65,12 @@ void tp_reduce_mc(const void* part_mc, const void* residual, void* out, long lon
 void vp_ce_stats(const void* logits, const long long* targets, void* stats, int T, int Vl, int v0, cudaStream_t s);
 void vp_ce_grad(void* logits, const long long* targets, const SymmPtrs& stats, float* row_loss, const float* n_valid,
                 int T, int Vl, int v0, int nranks, cudaStream_t s);
-void tp_embed_fwd(const long long* ids, const void* w, const SymmPtrs& dst, long long T, int rpp, int H, int Hl, int rank,
-                  cudaStream_t s);
-void tp_embed_bwd(const long long* ids, const SymmPtrs& dx, void* dw, long long T, int rpp, int H, int Hl, int rank,
-                  cudaStream_t s);
+void tp_embed_fwd(const long long* ids, const void* w, const SymmPtrs& dst, long long T, long long V, int rpp, int H,
+                  int Hl, int rank, cudaStream_t s);
+// dw [V, Hl] = (or +=) the per-id sum of this rank's Hl columns of every token's dx row, pulled from the owning rank
+// into staging [T, Hl] bf16 and summed by embedding_bwd (slot [V] and sums [T, Hl] fp32 are its scratch)
+void tp_embed_bwd(const long long* ids, const SymmPtrs& dx, void* dw, void* staging, unsigned int* slot, float* sums,
+                  long long T, long long V, int rpp, int H, int Hl, int rank, bool accumulate, cudaStream_t s);
 void ce_count_valid(const long long* targets, float* n_valid, int T, cudaStream_t s);
 void ce_finalize(const float* row_loss, const float* n_valid, float* loss, int T, cudaStream_t s);
 

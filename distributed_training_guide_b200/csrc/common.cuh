@@ -49,8 +49,21 @@ inline int ew_grid(long long total_threads) {
 // largest square and cannot change the sum) and keeps a sum of 2^16 squares of bf16's largest values finite.
 constexpr float kSumSqBig = 0x1p56f, kSumSqDown = 0x1p-72f, kSumSqUp = 0x1p72f;
 
+// The one vocabulary rule of every kernel indexed by token id or target (loss, embedding, their TP forms):
+//   kIgnoreIndex        a target that is ignored: zero dlogits row, not counted in n_valid;
+//   0 <= id < V         valid;
+//   anything else       bad: never dereferenced.  A bad target counts in n_valid and gets a NaN row loss and NaN
+//                       dlogits row (a NaN loss is what the log shows, without a host synchronise); a bad embedding
+//                       id gets a NaN forward row and adds to no row in the backward.
+constexpr long long kIgnoreIndex = -100;
+
 // ---- device-side helpers (nvcc only) ----------------------------------------------------------
 #ifdef __CUDACC__
+__device__ __forceinline__ bool in_vocab(long long id, long long V) {
+  return (unsigned long long)id < (unsigned long long)V;   // one compare: a negative id wraps past any V
+}
+__device__ __forceinline__ float nan_f() { return __int_as_float(0x7fffffff); }
+
 struct alignas(16) bf16x8 {
   __nv_bfloat162 v[4];
 };

@@ -3,7 +3,11 @@
 //   pass 2 (same CTA, row now in L2): overwrite the logits with (softmax - onehot) / n_valid
 // so the loss never materialises an fp32 [T,V] copy nor a separate dlogits tensor (the reference
 // path does `.float()` on the logits then log_softmax + nll_loss, SURVEY.md K7).
-// ignore_index = -100 rows get zero gradient and do not count in the mean.
+// Targets follow the vocabulary rule of common.cuh, with V = logits.size(1):
+//   -100 (kIgnoreIndex)   zero dlogits row, not counted in n_valid;
+//   0 <= t < V            the usual loss and gradient;
+//   anything else         counted in n_valid, row loss NaN (so the mean loss is NaN), dlogits row NaN; the logits
+//                         are never indexed with it.
 #include "api.h"
 #include "common.cuh"
 
@@ -14,7 +18,7 @@ constexpr int kCEThreads = 512;
 __global__ void count_valid_kernel(const long long* __restrict__ targets, float* __restrict__ n_valid, int T) {
   __shared__ float red[32];
   float c = 0.f;
-  for (int i = threadIdx.x; i < T; i += blockDim.x) c += (targets[i] >= 0) ? 1.f : 0.f;
+  for (int i = threadIdx.x; i < T; i += blockDim.x) c += (targets[i] != kIgnoreIndex) ? 1.f : 0.f;
   c = block_sum(c, red);
   if (threadIdx.x == 0) *n_valid = c;
 }
@@ -27,6 +31,7 @@ __global__ void __launch_bounds__(kCEThreads) ce_row_kernel(__nv_bfloat16* __res
   const int row = blockIdx.x;
   __nv_bfloat16* lr = logits + (size_t)row * V;
   const long long tgt = targets[row];
+  const bool valid = in_vocab(tgt, V);
   const int nvec = V >> 3;  // V % 8 == 0 enforced by the launcher
   // pass 1: online logsumexp
   float mx = -INFINITY, sum = 0.f;
@@ -48,10 +53,10 @@ __global__ void __launch_bounds__(kCEThreads) ce_row_kernel(__nv_bfloat16* __res
   sum = block_sum(sum, red);
   const float lse = gmx + __logf(sum);
   const float nv = *n_valid;
-  const float inv = (tgt >= 0 && nv > 0.f) ? 1.f / nv : 0.f;
+  const float inv = (tgt == kIgnoreIndex) ? 0.f : valid ? 1.f / nv : nan_f();
   if (threadIdx.x == 0) {
     float l = 0.f;
-    if (tgt >= 0) l = lse - __bfloat162float(lr[tgt]);
+    if (tgt != kIgnoreIndex) l = valid ? lse - __bfloat162float(lr[tgt]) : nan_f();
     row_loss[row] = l;
   }
   __syncthreads();  // the target logit is read before anyone overwrites it
@@ -92,6 +97,7 @@ void ce_finalize(const float* row_loss, const float* n_valid, float* loss, int T
 void cross_entropy_fwd_bwd(void* logits, const long long* targets, float* row_loss, float* n_valid, float* loss,
                            int T, int V, cudaStream_t s) {
   if (V % 8 != 0) throw std::runtime_error("cross_entropy: vocab size must be a multiple of 8");
+  if (T <= 0) return;
   count_valid_kernel<<<1, 1024, 0, s>>>(targets, n_valid, T);
   ce_row_kernel<<<T, kCEThreads, 0, s>>>((__nv_bfloat16*)logits, targets, row_loss, n_valid, V);
   ce_finalize_kernel<<<1, 1024, 0, s>>>(row_loss, n_valid, loss, T);

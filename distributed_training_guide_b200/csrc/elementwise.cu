@@ -278,15 +278,25 @@ void swiglu_bwd(const void* dh, const void* gu, void* dgu, long long T, int I, c
 // ------------------------------------------------------------------------------------------
 // Embedding gather and scatter-add
 // ------------------------------------------------------------------------------------------
+// Ids follow the vocabulary rule of common.cuh: an id outside [0, V) gets a NaN row in the forward and adds to no row
+// in the backward; no kernel dereferences it.
 __global__ void embedding_fwd_kernel(const long long* __restrict__ ids, const __nv_bfloat16* __restrict__ w,
-                                     __nv_bfloat16* __restrict__ out, long long T, int H) {
+                                     __nv_bfloat16* __restrict__ out, long long T, long long V, int H) {
   const int vpr = H >> 3;
   const long long total = T * vpr;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
     const long long t = idx / vpr;
     const int v = (int)(idx % vpr);
-    st8(out + t * H + v * 8, ld8(w + ids[t] * H + v * 8));
+    const long long id = ids[t];
+    bf16x8 r;
+    if (in_vocab(id, V)) {
+      r = ld8(w + id * H + v * 8);
+    } else {
+      const float nan8[8] = {nan_f(), nan_f(), nan_f(), nan_f(), nan_f(), nan_f(), nan_f(), nan_f()};
+      r = pack8(nan8);
+    }
+    st8(out + t * H + v * 8, r);
   }
 }
 
@@ -296,23 +306,29 @@ __global__ void embedding_fwd_kernel(const long long* __restrict__ ids, const __
 //   2. sums[slot[ids[t]]] += dout[t] with fp32 vector atomics, into a zeroed [T, H] fp32 scratch;
 //   3. the token at each id's slot writes dw[id] = bf16(sums[slot] (+ dw[id])).
 // Every shape is fixed by T, H and V, so nothing waits on the host.
-__global__ void embedding_slot_kernel(const long long* __restrict__ ids, unsigned int* __restrict__ slot, long long T) {
-  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < T; t += (long long)gridDim.x * blockDim.x)
-    atomicMin(slot + ids[t], (unsigned int)t);
+// A bad id keeps no slot and is skipped by the two later kernels.
+__global__ void embedding_slot_kernel(const long long* __restrict__ ids, unsigned int* __restrict__ slot, long long T,
+                                      long long V) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < T; t += (long long)gridDim.x * blockDim.x) {
+    const long long id = ids[t];
+    if (in_vocab(id, V)) atomicMin(slot + id, (unsigned int)t);
+  }
 }
 
 __global__ void embedding_sum_kernel(const __nv_bfloat16* __restrict__ dout, const long long* __restrict__ ids,
                                      const unsigned int* __restrict__ slot, float* __restrict__ sums, long long T,
-                                     int H) {
+                                     long long V, int H) {
   const int vpr = H >> 3;
   const long long total = T * vpr;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
     const long long t = idx / vpr;
+    const long long id = ids[t];
+    if (!in_vocab(id, V)) continue;
     const int v = (int)(idx % vpr);
     float g[8];
     unpack8(ld8(dout + t * H + v * 8), g);
-    float4* dst = reinterpret_cast<float4*>(sums + (long long)slot[ids[t]] * H + v * 8);
+    float4* dst = reinterpret_cast<float4*>(sums + (long long)slot[id] * H + v * 8);
     atomicAdd(dst, make_float4(g[0], g[1], g[2], g[3]));
     atomicAdd(dst + 1, make_float4(g[4], g[5], g[6], g[7]));
   }
@@ -320,14 +336,14 @@ __global__ void embedding_sum_kernel(const __nv_bfloat16* __restrict__ dout, con
 
 __global__ void embedding_write_kernel(const float* __restrict__ sums, const long long* __restrict__ ids,
                                        const unsigned int* __restrict__ slot, __nv_bfloat16* __restrict__ dw,
-                                       long long T, int H, int accumulate) {
+                                       long long T, long long V, int H, int accumulate) {
   const int vpr = H >> 3;
   const long long total = T * vpr;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
     const long long t = idx / vpr;
     const long long id = ids[t];
-    if (slot[id] != (unsigned int)t) continue;   // a later occurrence: the first one writes the row
+    if (!in_vocab(id, V) || slot[id] != (unsigned int)t) continue;   // a later occurrence: the first one writes the row
     const int v = (int)(idx % vpr);
     const float4* src = reinterpret_cast<const float4*>(sums + t * H + v * 8);
     const float4 a = src[0], b = src[1];
@@ -347,10 +363,10 @@ __global__ void embedding_write_kernel(const float* __restrict__ sums, const lon
 // fp32 and writes (or accumulates into) the one table row — no atomics, bit-identical from run to run.
 __global__ void embedding_bwd_sorted_kernel(const __nv_bfloat16* __restrict__ dout, const long long* __restrict__ ids_sorted,
                                             const long long* __restrict__ perm, __nv_bfloat16* __restrict__ dw,
-                                            long long T, int H, int accumulate) {
+                                            long long T, long long V, int H, int accumulate) {
   const long long p0 = blockIdx.x;
   const long long id = ids_sorted[p0];
-  if (p0 > 0 && ids_sorted[p0 - 1] == id) return;   // not the start of a run
+  if (!in_vocab(id, V) || (p0 > 0 && ids_sorted[p0 - 1] == id)) return;   // a bad id, or not the start of a run
   for (int c = threadIdx.x; c < (H >> 3); c += blockDim.x) {
     float acc[8];
 #pragma unroll
@@ -365,19 +381,20 @@ __global__ void embedding_bwd_sorted_kernel(const __nv_bfloat16* __restrict__ do
     st8(dw + id * H + c * 8, pack8(acc));
   }
 }
-void embedding_bwd_sorted(const void* dout, const long long* ids_sorted, const long long* perm, void* dw, long long T, int H,
-                          bool accumulate, cudaStream_t s) {
+void embedding_bwd_sorted(const void* dout, const long long* ids_sorted, const long long* perm, void* dw, long long T,
+                          long long V, int H, bool accumulate, cudaStream_t s) {
   if (H % 8 != 0) throw std::runtime_error("embedding: hidden size must be a multiple of 8");
   if (T <= 0) return;
-  embedding_bwd_sorted_kernel<<<(unsigned)T, 128, 0, s>>>((const __nv_bfloat16*)dout, ids_sorted, perm, (__nv_bfloat16*)dw, T, H,
-                                                       accumulate ? 1 : 0);
+  embedding_bwd_sorted_kernel<<<(unsigned)T, 128, 0, s>>>((const __nv_bfloat16*)dout, ids_sorted, perm, (__nv_bfloat16*)dw, T,
+                                                       V, H, accumulate ? 1 : 0);
   note_launch();
   DTG_LAUNCH_CHECK();
 }
 
-void embedding_fwd(const long long* ids, const void* w, void* out, long long T, int H, cudaStream_t s) {
+void embedding_fwd(const long long* ids, const void* w, void* out, long long T, long long V, int H, cudaStream_t s) {
   if (H % 8 != 0) throw std::runtime_error("embedding: hidden size must be a multiple of 8");
-  embedding_fwd_kernel<<<ew_grid(T * (H / 8)), 256, 0, s>>>(ids, (const __nv_bfloat16*)w, (__nv_bfloat16*)out, T, H);
+  if (T <= 0) return;
+  embedding_fwd_kernel<<<ew_grid(T * (H / 8)), 256, 0, s>>>(ids, (const __nv_bfloat16*)w, (__nv_bfloat16*)out, T, V, H);
   note_launch();
   DTG_LAUNCH_CHECK();
 }
@@ -389,9 +406,9 @@ void embedding_bwd(const void* dout, const long long* ids, void* dw, unsigned in
   if (T <= 0) return;
   DTG_CUDA_CHECK(cudaMemsetAsync(slot, 0xFF, (size_t)V * sizeof(unsigned int), s));
   DTG_CUDA_CHECK(cudaMemsetAsync(sums, 0, (size_t)T * H * sizeof(float), s));
-  embedding_slot_kernel<<<ew_grid(T), 256, 0, s>>>(ids, slot, T);
-  embedding_sum_kernel<<<ew_grid(T * (H / 8)), 256, 0, s>>>((const __nv_bfloat16*)dout, ids, slot, sums, T, H);
-  embedding_write_kernel<<<ew_grid(T * (H / 8)), 256, 0, s>>>(sums, ids, slot, (__nv_bfloat16*)dw, T, H,
+  embedding_slot_kernel<<<ew_grid(T), 256, 0, s>>>(ids, slot, T, V);
+  embedding_sum_kernel<<<ew_grid(T * (H / 8)), 256, 0, s>>>((const __nv_bfloat16*)dout, ids, slot, sums, T, V, H);
+  embedding_write_kernel<<<ew_grid(T * (H / 8)), 256, 0, s>>>(sums, ids, slot, (__nv_bfloat16*)dw, T, V, H,
                                                              accumulate ? 1 : 0);
   note_launch(3);
   DTG_LAUNCH_CHECK();

@@ -11,7 +11,10 @@
 //                        logits all-gather + redundant fp32 CE on every TP rank (SURVEY.md N10 / C19).
 //   hidden-parallel embedding   each rank owns H/N columns of the table; the lookup is pushed straight
 //                        into the owning rank's sequence shard (the reference's embedding all-to-all, N9),
-//                        and the backward pulls its column slice of the peers' gradient shards.
+//                        and the backward pulls its column slice of the peers' gradient shards into a local
+//                        staging buffer that the single-GPU embedding backward sums in fp32.
+// Token ids and targets follow the vocabulary rule of common.cuh (V = NR * Vl for the loss, w.size(0) for the
+// embedding).
 #include "api.h"
 #include "comm.cuh"
 #include "comm_device.cuh"
@@ -131,8 +134,8 @@ __global__ void __launch_bounds__(kVpThreads) vp_ce_stats_kernel(const __nv_bflo
   sum = (mx == -INFINITY) ? 0.f : sum * __expf(mx - gmx);
   sum = block_sum(sum, red);
   if (threadIdx.x == 0) {
-    const long long t = targets[row] - v0;
-    const bool mine = targets[row] >= 0 && t >= 0 && t < Vl;
+    const long long t = targets[row] - v0;   // v0 >= 0, so an ignored or negative target is never mine
+    const bool mine = in_vocab(t, Vl);
     stats[row] = make_float4(gmx, sum, mine ? __bfloat162float(lr[t]) : 0.f, mine ? 1.f : 0.f);
   }
 }
@@ -145,6 +148,8 @@ __global__ void __launch_bounds__(kVpThreads) vp_ce_grad_kernel(__nv_bfloat16* _
                                                                const float* __restrict__ n_valid, int Vl, int v0) {
   __shared__ float sh[2];
   const int row = blockIdx.x;
+  const long long tgt = targets[row];
+  const bool valid = in_vocab(tgt, (long long)NR * Vl);
   if (threadIdx.x == 0) {
     float m[NR], s[NR], tl = 0.f;
     float gm = -INFINITY;
@@ -161,13 +166,12 @@ __global__ void __launch_bounds__(kVpThreads) vp_ce_grad_kernel(__nv_bfloat16* _
     for (int k = 0; k < NR; ++k) tot += s[k] * __expf(m[k] - gm);
     const float lse = gm + __logf(tot);
     sh[0] = lse;
-    row_loss[row] = (targets[row] >= 0) ? (lse - tl) : 0.f;
+    row_loss[row] = (tgt == kIgnoreIndex) ? 0.f : valid ? lse - tl : nan_f();
   }
   __syncthreads();
   const float lse = sh[0];
-  const long long tgt = targets[row];
   const float nv = *n_valid;
-  const float inv = (tgt >= 0 && nv > 0.f) ? 1.f / nv : 0.f;
+  const float inv = (tgt == kIgnoreIndex) ? 0.f : valid ? 1.f / nv : nan_f();
   const long long tloc = tgt - v0;
   __nv_bfloat16* lr = logits + (size_t)row * Vl;
   const int nvec = Vl >> 3;
@@ -186,6 +190,7 @@ __global__ void __launch_bounds__(kVpThreads) vp_ce_grad_kernel(__nv_bfloat16* _
 
 void vp_ce_stats(const void* logits, const long long* targets, void* stats, int T, int Vl, int v0, cudaStream_t s) {
   if (Vl % 8) throw std::runtime_error("vocab shard must be a multiple of 8");
+  if (T <= 0) return;
   vp_ce_stats_kernel<<<T, kVpThreads, 0, s>>>((const __nv_bfloat16*)logits, targets, (float4*)stats, Vl, v0);
   note_launch();
   DTG_LAUNCH_CHECK();
@@ -193,6 +198,7 @@ void vp_ce_stats(const void* logits, const long long* targets, void* stats, int 
 
 void vp_ce_grad(void* logits, const long long* targets, const SymmPtrs& stats, float* row_loss, const float* n_valid,
                 int T, int Vl, int v0, int nranks, cudaStream_t s) {
+  if (T <= 0) return;
 #define VP_CASE(NRV)                                                                                         \
   case NRV:                                                                                                  \
     vp_ce_grad_kernel<NRV><<<T, kVpThreads, 0, s>>>((__nv_bfloat16*)logits, targets, stats, row_loss, n_valid, Vl, v0); \
@@ -209,8 +215,10 @@ void vp_ce_grad(void* logits, const long long* targets, const SymmPtrs& stats, f
 // ---- hidden-parallel embedding with the all-to-all fused in ------------------------------------------------
 // fwd: for every token t of the full batch, my H/N columns of its embedding row are written into the
 // sequence shard of the rank that owns token t (dst[owner] + (t % rpp) * H + rank * Hl).
+// An id outside [0, V) writes a NaN row, as the single-GPU forward does.
 __global__ void tp_embed_fwd_kernel(const long long* __restrict__ ids, const __nv_bfloat16* __restrict__ w,
-                                    SymmPtrs dst /*unrotated*/, long long T, int rpp, int H, int Hl, int rank) {
+                                    SymmPtrs dst /*unrotated*/, long long T, long long V, int rpp, int H, int Hl,
+                                    int rank) {
   const int vpr = Hl >> 3;
   const long long total = T * vpr;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
@@ -219,22 +227,31 @@ __global__ void tp_embed_fwd_kernel(const long long* __restrict__ ids, const __n
     const int v = (int)(idx % vpr);
     const int owner = (int)(t / rpp);
     __nv_bfloat16* d = reinterpret_cast<__nv_bfloat16*>(dst.ptr[owner]) + (t % rpp) * H + (long long)rank * Hl + v * 8;
-    st8(d, ld8(w + ids[t] * Hl + v * 8));
+    const long long id = ids[t];
+    bf16x8 r;
+    if (in_vocab(id, V)) {
+      r = ld8(w + id * Hl + v * 8);
+    } else {
+      const float nan8[8] = {nan_f(), nan_f(), nan_f(), nan_f(), nan_f(), nan_f(), nan_f(), nan_f()};
+      r = pack8(nan8);
+    }
+    st8(d, r);
   }
 }
-// bwd: dW_local[ids[t], :] += dx[owner(t)][t % rpp, rank*Hl : (rank+1)*Hl]   (pull from the owner over NVLink)
-__global__ void tp_embed_bwd_kernel(const long long* __restrict__ ids, SymmPtrs dx /*unrotated*/,
-                                    __nv_bfloat16* __restrict__ dw, long long T, int rpp, int H, int Hl, int rank) {
-  const int ppr = Hl >> 1;
-  const long long total = T * ppr;
+// bwd, step 1: staging[t, :] = dx[owner(t)][t % rpp, rank*Hl : (rank+1)*Hl]   (pull from the owner over NVLink).
+// Step 2 is embedding_bwd over the staging rows: one fp32 sum and one bf16 rounding per table row.
+__global__ void tp_embed_pull_kernel(SymmPtrs dx /*unrotated*/, __nv_bfloat16* __restrict__ staging, long long T,
+                                     int rpp, int H, int Hl, int rank) {
+  const int vpr = Hl >> 3;
+  const long long total = T * vpr;
   for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
        idx += (long long)gridDim.x * blockDim.x) {
-    const long long t = idx / ppr;
-    const int c = (int)(idx % ppr);
+    const long long t = idx / vpr;
+    const int v = (int)(idx % vpr);
     const int owner = (int)(t / rpp);
-    const __nv_bfloat162* src = reinterpret_cast<const __nv_bfloat162*>(
-        reinterpret_cast<const __nv_bfloat16*>(dx.ptr[owner]) + (t % rpp) * H + (long long)rank * Hl);
-    atomicAdd(reinterpret_cast<__nv_bfloat162*>(dw + ids[t] * Hl) + c, src[c]);
+    const __nv_bfloat16* src =
+        reinterpret_cast<const __nv_bfloat16*>(dx.ptr[owner]) + (t % rpp) * H + (long long)rank * Hl + v * 8;
+    st8(staging + t * Hl + v * 8, ld8(src));
   }
 }
 
@@ -246,18 +263,23 @@ static int ew_grid2(long long total_threads) {
   return (int)g;
 }
 
-void tp_embed_fwd(const long long* ids, const void* w, const SymmPtrs& dst, long long T, int rpp, int H, int Hl, int rank,
-                  cudaStream_t s) {
+void tp_embed_fwd(const long long* ids, const void* w, const SymmPtrs& dst, long long T, long long V, int rpp, int H,
+                  int Hl, int rank, cudaStream_t s) {
   if (Hl % 8) throw std::runtime_error("hidden shard must be a multiple of 8");
-  tp_embed_fwd_kernel<<<ew_grid2(T * (Hl / 8)), 256, 0, s>>>(ids, (const __nv_bfloat16*)w, dst, T, rpp, H, Hl, rank);
+  if (T <= 0) return;
+  tp_embed_fwd_kernel<<<ew_grid2(T * (Hl / 8)), 256, 0, s>>>(ids, (const __nv_bfloat16*)w, dst, T, V, rpp, H, Hl, rank);
   note_launch();
   DTG_LAUNCH_CHECK();
 }
-void tp_embed_bwd(const long long* ids, const SymmPtrs& dx, void* dw, long long T, int rpp, int H, int Hl, int rank,
-                  cudaStream_t s) {
-  tp_embed_bwd_kernel<<<ew_grid2(T * (Hl / 2)), 256, 0, s>>>(ids, dx, (__nv_bfloat16*)dw, T, rpp, H, Hl, rank);
-  note_launch();
-  DTG_LAUNCH_CHECK();
+void tp_embed_bwd(const long long* ids, const SymmPtrs& dx, void* dw, void* staging, unsigned int* slot, float* sums,
+                  long long T, long long V, int rpp, int H, int Hl, int rank, bool accumulate, cudaStream_t s) {
+  if (Hl % 8) throw std::runtime_error("hidden shard must be a multiple of 8");
+  if (T > 0) {
+    tp_embed_pull_kernel<<<ew_grid2(T * (Hl / 8)), 256, 0, s>>>(dx, (__nv_bfloat16*)staging, T, rpp, H, Hl, rank);
+    note_launch();
+    DTG_LAUNCH_CHECK();
+  }
+  embedding_bwd(staging, ids, dw, slot, sums, T, V, Hl, accumulate, s);
 }
 
 }  // namespace dtg

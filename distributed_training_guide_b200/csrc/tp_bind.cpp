@@ -129,37 +129,80 @@ void py_reduce_mc(uint64_t part_mc, const c10::optional<Tensor>& residual, Tenso
                     err.has_value() ? err->data_ptr<int>() : nullptr, stream());
 }
 
+// the per-row stats buffer of vocab_parallel CE: (max, sum-exp, target logit, mine) as float4 per row
+void check_stats_ptr(uint64_t p, const char* who) {
+  TORCH_CHECK(p != 0 && p % 16 == 0, who, ": every stats buffer must start at a 16-byte aligned address");
+}
+
 void py_vp_ce_stats(const Tensor& logits, const Tensor& targets, Tensor& stats, int64_t v0) {
-  TORCH_CHECK(logits.is_contiguous() && logits.scalar_type() == at::kBFloat16 && stats.scalar_type() == at::kFloat, "bad");
+  check_loss_args(logits, targets, "vp_ce_stats");
+  const int64_t T = logits.size(0), Vl = logits.size(1);
+  TORCH_CHECK(stats.is_cuda() && stats.device() == logits.device(), "vp_ce_stats: stats must be on logits' device");
+  TORCH_CHECK(stats.scalar_type() == at::kFloat && stats.is_contiguous(), "vp_ce_stats: stats must be contiguous fp32");
+  TORCH_CHECK(stats.numel() >= 4 * T, "vp_ce_stats: stats must hold 4 floats per row (", 4 * T, "), got ",
+              stats.numel());
+  check_stats_ptr((uint64_t)stats.data_ptr(), "vp_ce_stats");
+  TORCH_CHECK(v0 >= 0 && v0 % Vl == 0, "vp_ce_stats: v0 must be a non-negative multiple of the shard width ", Vl,
+              ", got ", v0);
   const c10::cuda::CUDAGuard guard(logits.device());
-  dtg::vp_ce_stats(logits.data_ptr(), (const long long*)targets.data_ptr<int64_t>(), stats.data_ptr(), (int)logits.size(0),
-                   (int)logits.size(1), (int)v0, stream());
+  dtg::vp_ce_stats(logits.data_ptr(), (const long long*)targets.data_ptr<int64_t>(), stats.data_ptr(), (int)T, (int)Vl,
+                   (int)v0, stream());
 }
 
 Tensor py_vp_ce_grad(Tensor& logits, const Tensor& targets, const std::vector<uint64_t>& stats_ptrs, int64_t v0) {
+  check_loss_args(logits, targets, "vp_ce_grad");
+  const int64_t T = logits.size(0), Vl = logits.size(1), nr = (int64_t)stats_ptrs.size();
+  TORCH_CHECK(nr == 1 || nr == 2 || nr == 4 || nr == 8, "vp_ce_grad: 1, 2, 4 or 8 ranks, got ", nr);
+  for (uint64_t p : stats_ptrs) check_stats_ptr(p, "vp_ce_grad");
+  TORCH_CHECK(v0 >= 0 && v0 % Vl == 0 && v0 / Vl < nr, "vp_ce_grad: v0 must be a multiple of the shard width ", Vl,
+              " below ", nr, " shards, got ", v0);
   const c10::cuda::CUDAGuard guard(logits.device());
-  const int T = (int)logits.size(0);
+  if (T == 0) return torch::zeros({}, logits.options().dtype(at::kFloat));   // as with every target ignored
   Tensor scratch = torch::empty({T + 2}, logits.options().dtype(at::kFloat));
   float* sp = scratch.data_ptr<float>();
   const long long* tg = (const long long*)targets.data_ptr<int64_t>();
-  dtg::ce_count_valid(tg, sp, T, stream());
-  dtg::vp_ce_grad(logits.data_ptr(), tg, plain(stats_ptrs), sp + 2, sp, T, (int)logits.size(1), (int)v0,
-                  (int)stats_ptrs.size(), stream());
-  dtg::ce_finalize(sp + 2, sp, sp + 1, T, stream());
+  dtg::ce_count_valid(tg, sp, (int)T, stream());
+  dtg::vp_ce_grad(logits.data_ptr(), tg, plain(stats_ptrs), sp + 2, sp, (int)T, (int)Vl, (int)v0, (int)nr, stream());
+  dtg::ce_finalize(sp + 2, sp, sp + 1, (int)T, stream());
   return scratch.slice(0, 1, 2).reshape({});
+}
+
+// the token layout of the hidden-parallel embedding: token t of the full batch lives in row t % rpp of rank t / rpp's
+// [rpp, H] buffer, and this rank owns columns [rank * Hl, (rank + 1) * Hl)
+void check_tp_tokens(int64_t T, const std::vector<uint64_t>& ptrs, int64_t rpp, int64_t H, int64_t Hl, int64_t rank,
+                     const char* who) {
+  const int64_t nr = (int64_t)ptrs.size();
+  TORCH_CHECK(nr >= 1 && nr <= kMaxRanks, who, ": 1..", kMaxRanks, " ranks, got ", nr);
+  for (uint64_t p : ptrs) TORCH_CHECK(p != 0 && p % 16 == 0, who, ": every rank's buffer must be 16-byte aligned");
+  TORCH_CHECK(rank >= 0 && rank < nr, who, ": rank ", rank, " outside the ", nr, " ranks");
+  TORCH_CHECK(rpp >= 1, who, ": rows per rank must be positive");
+  TORCH_CHECK(T <= nr * rpp, who, ": ", T, " tokens do not fit ", nr, " ranks of ", rpp, " rows");
+  TORCH_CHECK(H == nr * Hl, who, ": H (", H, ") must be the ranks times the shard width (", nr, " x ", Hl, ")");
 }
 
 void py_embed_fwd(const Tensor& ids, const Tensor& w, const std::vector<uint64_t>& dst_ptrs, int64_t rpp, int64_t H,
                   int64_t rank) {
+  check_embedding_args(ids, w, "w", "tp_embed_fwd");
+  check_tp_tokens(ids.numel(), dst_ptrs, rpp, H, w.size(1), rank, "tp_embed_fwd");
   const c10::cuda::CUDAGuard guard(w.device());
-  dtg::tp_embed_fwd((const long long*)ids.data_ptr<int64_t>(), w.data_ptr(), plain(dst_ptrs), ids.numel(), (int)rpp,
-                    (int)H, (int)w.size(1), (int)rank, stream());
+  dtg::tp_embed_fwd((const long long*)ids.data_ptr<int64_t>(), w.data_ptr(), plain(dst_ptrs), ids.numel(), w.size(0),
+                    (int)rpp, (int)H, (int)w.size(1), (int)rank, stream());
 }
+// the staging rows and embedding_bwd's scratch live until the call returns (the caching allocator keeps them on this
+// stream)
 void py_embed_bwd(const Tensor& ids, const std::vector<uint64_t>& dx_ptrs, Tensor& dw, int64_t rpp, int64_t H,
-                  int64_t rank) {
+                  int64_t rank, bool accumulate) {
+  check_embedding_args(ids, dw, "dw", "tp_embed_bwd");
+  const int64_t T = ids.numel(), V = dw.size(0), Hl = dw.size(1);
+  check_tp_tokens(T, dx_ptrs, rpp, H, Hl, rank, "tp_embed_bwd");
+  TORCH_CHECK(T < 0xFFFFFFFFLL, "tp_embed_bwd: too many tokens for 32-bit slots");
   const c10::cuda::CUDAGuard guard(dw.device());
-  dtg::tp_embed_bwd((const long long*)ids.data_ptr<int64_t>(), plain(dx_ptrs), dw.data_ptr(), ids.numel(), (int)rpp,
-                    (int)H, (int)dw.size(1), (int)rank, stream());
+  Tensor staging = torch::empty({T, Hl}, dw.options());
+  Tensor slot = torch::empty({V}, dw.options().dtype(at::kInt));
+  Tensor sums = torch::empty({T, Hl}, dw.options().dtype(at::kFloat));
+  dtg::tp_embed_bwd((const long long*)ids.data_ptr<int64_t>(), plain(dx_ptrs), dw.data_ptr(), staging.data_ptr(),
+                    reinterpret_cast<unsigned int*>(slot.data_ptr<int>()), sums.data_ptr<float>(), T, V, (int)rpp,
+                    (int)H, (int)Hl, (int)rank, accumulate, stream());
 }
 }  // namespace
 
@@ -177,6 +220,7 @@ void bind_tp(pybind11::module_& m) {
   m.def("vp_ce_stats", &py_vp_ce_stats);
   m.def("vp_ce_grad", &py_vp_ce_grad);
   m.def("tp_embed_fwd", &py_embed_fwd);
-  m.def("tp_embed_bwd", &py_embed_bwd);
+  m.def("tp_embed_bwd", &py_embed_bwd, py::arg("ids"), py::arg("dx_ptrs"), py::arg("dw"), py::arg("rpp"), py::arg("H"),
+        py::arg("rank"), py::arg("accumulate") = false);
 }
 }  // namespace dtg

@@ -309,10 +309,10 @@ class _HiddenParallelEmbedding(torch.autograd.Function):
         C = _ext.load()
         tp.dx0.local.view(tp.rpp, tp.H).copy_(dx_local)
         tp.barrier()
-        if getattr(w, "_dtg_writes", 0) == 0:
-            g.zero_()
+        # summed in fp32 and rounded once per row; overwrite mode (the first write this step) zeroes absent rows
+        acc = getattr(w, "_dtg_writes", 0) > 0
         w._dtg_writes = getattr(w, "_dtg_writes", 0) + 1
-        C.tp_embed_bwd(ids, tp.dx0.ptrs, g, tp.rpp, tp.H, tp.rank)
+        C.tp_embed_bwd(ids, tp.dx0.ptrs, g, tp.rpp, tp.H, tp.rank, acc)
         return None, None, None
 
 
