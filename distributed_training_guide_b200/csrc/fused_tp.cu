@@ -50,6 +50,7 @@ __global__ void tp_reduce_parts_kernel(const __nv_bfloat16* __restrict__ parts, 
 
 void tp_reduce_parts(const void* parts, const void* residual, void* out, long long n, int nparts, cudaStream_t s) {
   if (n % 8) throw std::runtime_error("tp_reduce_parts: size must be a multiple of 8");
+  if (n <= 0) return;
   long long nvec = n / 8;
   long long grid = (nvec + 255) / 256;
   const long long cap = (long long)sm_count() * 8;

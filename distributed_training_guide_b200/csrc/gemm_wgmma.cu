@@ -847,12 +847,21 @@ void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long l
 //   mode 2  GEMM -> reduce-scatter push : row chunk c of C goes to c_dsts[c] (already offset to my slot)
 //   mode 3  wgrad with B gathered along K : B = concat_p b_srcs[p] ([rows_per_peer, N] each), A MN-major local
 //   mode 4  wgrad with A gathered along K : A = concat_p a_srcs[p] ([rows_per_peer, M] each), B MN-major local
+// Modes 1 and 2 keep the plain GEMM's K order, so their C is bit-identical to gemm_bf16 (variant 2) on the assembled
+// operands; modes 3 and 4 start every tile at this rank's K slice (k_shift), which changes the fp32 summation order.
+//
+// Empty calls, here and in gemm_bf16_ag: with M or N = 0 nothing is launched (and nothing gathered); with K = 0 the
+// product is zero, so overwrite mode writes zeros over C (mode 2: over every owner's rows_per_peer rows) and
+// accumulate mode leaves C unchanged, as in gemm_bf16.  gemm_bf16_bgather refuses empty calls instead: its chunk
+// counters must advance one generation per call, or the next call would wait for chunks that never arrive.
 void gemm_bf16_dist(int mode, const void* const* a_srcs, const void* const* b_srcs, void* const* c_dsts, int M, int N,
                     int K, long long lda, long long ldb, long long ldc, bool b_kmajor, bool accumulate, int nranks,
                     int rank, int rows_per_peer, cudaStream_t s) {
-  if ((N % 8) || (ldc % 8) || (lda % 8) || (ldb % 8))
-    throw std::runtime_error("gemm_bf16_dist: N and the leading dimensions must be multiples of 8 elements");
+  if (mode < 1 || mode > 4) throw std::runtime_error("gemm_bf16_dist: unknown mode");
   if (nranks < 1 || nranks > kMaxRanks) throw std::runtime_error("gemm_bf16_dist: 1..8 ranks");
+  if (rank < 0 || rank >= nranks) throw std::runtime_error("gemm_bf16_dist: rank outside the ranks");
+  if (M < 0 || N < 0 || K < 0) throw std::runtime_error("gemm_bf16_dist: negative extent");
+  if (mode == 2 && accumulate) throw std::runtime_error("gemm_bf16_dist: mode 2 always overwrites");
   GemmDist dist{};
   dist.rows_per_peer = rows_per_peer;
   constexpr int TM = GemmCfg<2>::BM * 2;
@@ -864,6 +873,16 @@ void gemm_bf16_dist(int mode, const void* const* a_srcs, const void* const* b_sr
     if (rows_per_peer % 64 != 0 || rows_per_peer * nranks != K)
       throw std::runtime_error("gemm_bf16_dist: K rows per rank must be a multiple of 64 and sum to K");
     dist.k_shift = rank * (rows_per_peer / 64);
+  }
+  if (M == 0 || N == 0) return;
+  if ((N % 8) || (ldc % 8) || (lda % 8) || (ldb % 8))
+    throw std::runtime_error("gemm_bf16_dist: N and the leading dimensions must be multiples of 8 elements");
+  if (K == 0) {
+    if (mode == 2)
+      for (int p = 0; p < nranks; ++p) gemm_empty_k(c_dsts[p], rows_per_peer, N, ldc, false, s);
+    else
+      gemm_empty_k(c_dsts[0], M, N, ldc, accumulate, s);
+    return;
   }
   for (int p = 0; p < nranks && c_dsts; ++p) dist.c_ptr[p] = (__nv_bfloat16*)c_dsts[p];
   void* C = c_dsts ? c_dsts[0] : nullptr;
@@ -897,8 +916,16 @@ void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int 
   constexpr int TM = GemmCfg<2>::BM * 2;
   if (rows_per_peer % TM != 0 || rows_per_peer * nranks != M) throw std::runtime_error("gemm_bf16_ag: bad row split");
   if ((K * 2LL * TM) % GemmCfg<2>::COMM_PIECE != 0) throw std::runtime_error("gemm_bf16_ag: K must be a multiple of 64");
-  if ((N % 8) || (ldc % 8) || (ldb % 8)) throw std::runtime_error("gemm_bf16_ag: N / leading dims must be multiples of 8");
+  if (nranks < 1 || nranks > kMaxRanks || rank < 0 || rank >= nranks)
+    throw std::runtime_error("gemm_bf16_ag: 1..8 ranks and a rank among them");
+  // the first n_comm CTA pairs copy; at least one pair must be left to multiply
+  if (n_comm < 1 || n_comm >= sm_count() / 2)
+    throw std::runtime_error("gemm_bf16_ag: n_comm must be in [1, " + std::to_string(sm_count() / 2) +
+                             ") (at least one CTA pair copies and one multiplies), got " + std::to_string(n_comm));
   check_bias("gemm_bf16_ag", bias, true, b_kmajor, false, K);
+  if (M == 0 || N == 0) return;
+  if ((N % 8) || (ldc % 8) || (ldb % 8)) throw std::runtime_error("gemm_bf16_ag: N / leading dims must be multiples of 8");
+  if (K == 0) return gemm_empty_k(C, M, N, ldc, false, s);
   GemmDist dist{};
   dist.rows_per_peer = rows_per_peer;
   dist.m_tile_shift = rank * (rows_per_peer / TM);
@@ -907,7 +934,7 @@ void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int 
   dist.ag_flags = flags;
   dist.ag_epoch = ag_epoch;
   dist.bar_epoch = bar_epoch;
-  dist.n_comm = n_comm < 1 ? 1 : n_comm;
+  dist.n_comm = n_comm;
   dist.rank = rank;
   dist.nranks = nranks;
   dist.tile_bytes = (long long)TM * K * 2;
@@ -933,7 +960,13 @@ void gemm_bf16_bgather(const void* A, void* full_base, void* C, int M, int N, in
   if ((N % 8) || (ldc % 8) || (lda % 8) || (ldb % 8))
     throw std::runtime_error("gemm_bf16_bgather: N and the leading dimensions must be multiples of 8 elements");
   check_bias("gemm_bf16_bgather", bias, true, b_kmajor, false, K);
-  if (nranks < 1 || nranks > kMaxRanks) throw std::runtime_error("gemm_bf16_bgather: 1..8 ranks");
+  if (nranks < 1 || nranks > kMaxRanks || rank < 0 || rank >= nranks)
+    throw std::runtime_error("gemm_bf16_bgather: 1..8 ranks and a rank among them");
+  if (M <= 0 || N <= 0 || K <= 0)
+    throw std::runtime_error("gemm_bf16_bgather: empty GEMM (the chunk counters must advance one generation per call)");
+  if (chunk_shift < 14 || chunk_shift > 30) throw std::runtime_error("gemm_bf16_bgather: chunk_shift outside [14, 30]");
+  if (w_off < 0 || w_bytes < 0 || w_off + w_bytes > (long long)nranks * per_bytes)
+    throw std::runtime_error("gemm_bf16_bgather: the weight range must lie inside the shards");
   const long long chunk = 1LL << chunk_shift;
   if (chunk < Cfg::GATHER_PIECE || (w_off % chunk) || (w_bytes % chunk) || (per_bytes % chunk))
     throw std::runtime_error("gemm_bf16_bgather: weight offset / size / shard size must be multiples of the chunk size");

@@ -5,6 +5,8 @@
 #include <pybind11/stl.h>
 #include <torch/extension.h>
 
+#include <tuple>
+
 #include "api.h"
 #include "comm.cuh"
 #include "comm_api.h"
@@ -36,84 +38,148 @@ SymmPtrs plain(const std::vector<uint64_t>& ptrs) {
   return s;
 }
 
+// ---- distributed GEMMs and the partial-sum reduce ----------------------------------------------------------------
+// gemm_dist, gemm_ag, gemm_bgather and tp_reduce_parts validate their arguments with check_dist before anything is
+// launched.  The kernels index their peer-pointer arrays by rank and owner, so a list of the wrong length or a rank
+// out of range would read or write through a pointer nobody passed.
+using PeerList = std::tuple<const std::vector<uint64_t>*, const char*, int64_t>;   // list, name, entries read
+struct Operand {
+  const Tensor* t;   // null: not given
+  const char* name;
+  at::ScalarType dtype;
+  bool flat;         // contiguous; otherwise 2-D with a contiguous last dimension (a row-strided matrix)
+};
+
+// nranks in 1..8 and 0 <= rank < nranks; every list exactly as long as the kernel reads it, each entry a nonzero
+// 16-byte aligned address (TMA bases, bulk copies and 16-byte vectors); every operand on `dev`'s device (the current
+// device when dev is null), of its dtype and layout, 16-byte aligned.
+void check_dist(const char* who, std::initializer_list<PeerList> lists, int64_t nranks, int64_t rank, const Tensor* dev,
+                std::initializer_list<Operand> ops) {
+  TORCH_CHECK(nranks >= 1 && nranks <= kMaxRanks, who, ": 1..", kMaxRanks, " ranks, got ", nranks);
+  TORCH_CHECK(rank >= 0 && rank < nranks, who, ": rank ", rank, " outside the ", nranks, " ranks");
+  for (const auto& [v, name, want] : lists) {
+    TORCH_CHECK((int64_t)v->size() == want, who, ": ", name, " must have ", want, " entries, got ", v->size());
+    for (uint64_t p : *v)
+      TORCH_CHECK(p != 0 && p % 16 == 0, who, ": every entry of ", name, " must be a 16-byte aligned address");
+  }
+  const c10::Device d = dev ? dev->device() : c10::Device(c10::kCUDA, c10::cuda::current_device());
+  for (const auto& o : ops) {
+    if (!o.t) continue;
+    const Tensor& t = *o.t;
+    TORCH_CHECK(t.is_cuda() && t.device() == d, who, ": ", o.name, " must be on ", d);
+    TORCH_CHECK(t.scalar_type() == o.dtype, who, ": ", o.name, " must be ", c10::toString(o.dtype));
+    if (o.flat) {
+      TORCH_CHECK(t.is_contiguous(), who, ": ", o.name, " must be contiguous");
+    } else {
+      TORCH_CHECK(t.dim() == 2 && t.stride(1) == 1, who, ": ", o.name, " must be 2-D with a contiguous last dimension");
+    }
+    TORCH_CHECK(reinterpret_cast<uintptr_t>(t.data_ptr()) % 16 == 0, who, ": ", o.name,
+                " must start at a 16-byte aligned address");
+  }
+}
+
+// mode 1 reads nranks A bases, mode 3 nranks B bases, mode 4 nranks A bases, mode 2 writes nranks C bases (each
+// already offset to this rank's slot); every other list has one entry.  Mode 2 always overwrites its slots.
 void py_gemm_dist(int64_t mode, const std::vector<uint64_t>& a_ptrs, const std::vector<uint64_t>& b_ptrs,
                   const std::vector<uint64_t>& c_ptrs, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb,
                   int64_t ldc, bool b_kmajor, bool accumulate, int64_t nranks, int64_t rank, int64_t rows_per_peer) {
+  TORCH_CHECK(mode >= 1 && mode <= 4, "gemm_dist: mode must be 1..4, got ", mode);
+  const int64_t na = (mode == 1 || mode == 4) ? nranks : 1, nb = mode == 3 ? nranks : 1, nc = mode == 2 ? nranks : 1;
+  check_dist("gemm_dist", {{&a_ptrs, "a_ptrs", na}, {&b_ptrs, "b_ptrs", nb}, {&c_ptrs, "c_ptrs", nc}}, nranks, rank,
+             nullptr, {});
+  TORCH_CHECK(M >= 0 && N >= 0 && K >= 0 && rows_per_peer >= 0, "gemm_dist: negative extent");
+  TORCH_CHECK(mode != 2 || !accumulate, "gemm_dist: mode 2 overwrites the staging slots (accumulate is not supported)");
   const void* as[kMaxRanks] = {nullptr};
   const void* bs[kMaxRanks] = {nullptr};
   void* cs[kMaxRanks] = {nullptr};
-  for (size_t i = 0; i < a_ptrs.size() && i < (size_t)kMaxRanks; ++i) as[i] = (const void*)a_ptrs[i];
-  for (size_t i = 0; i < b_ptrs.size() && i < (size_t)kMaxRanks; ++i) bs[i] = (const void*)b_ptrs[i];
-  for (size_t i = 0; i < c_ptrs.size() && i < (size_t)kMaxRanks; ++i) cs[i] = (void*)c_ptrs[i];
-  if (mode != 2) {  // local C: replicate so dist.c_ptr[0] is valid
-    for (int i = 1; i < kMaxRanks; ++i) cs[i] = cs[0];
-  }
+  for (int64_t i = 0; i < na; ++i) as[i] = (const void*)a_ptrs[i];
+  for (int64_t i = 0; i < nb; ++i) bs[i] = (const void*)b_ptrs[i];
+  for (int64_t i = 0; i < nc; ++i) cs[i] = (void*)c_ptrs[i];
   dtg::gemm_bf16_dist((int)mode, as, bs, cs, (int)M, (int)N, (int)K, lda, ldb, ldc, b_kmajor, accumulate, (int)nranks,
                       (int)rank, (int)rows_per_peer, stream());
 }
 
+// a_bufs and pads: one entry per rank.  The kernel waits for ag_epoch on the tile flags and for bar_epoch on the
+// signal pads, so with more than one rank neither may be 0 (the waits would pass before anything arrived).
 void py_gemm_ag(const std::vector<uint64_t>& a_bufs, const Tensor& b, Tensor& out, bool b_kmajor, int64_t rank,
                 int64_t rows_per_peer, Tensor& flags, int64_t ag_epoch, const std::vector<uint64_t>& pads,
                 int64_t bar_epoch, int64_t n_comm, const c10::optional<Tensor>& bias) {
-  TORCH_CHECK(b.is_cuda() && b.scalar_type() == at::kBFloat16 && b.dim() == 2 && b.stride(1) == 1, "bad B");
-  TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kBFloat16 && out.dim() == 2 && out.stride(1) == 1, "bad out");
-  TORCH_CHECK(flags.scalar_type() == at::kInt && flags.is_cuda(), "flags must be an int32 CUDA tensor");
+  const int64_t nr = (int64_t)a_bufs.size();
+  check_dist("gemm_ag", {{&a_bufs, "a_bufs", nr}, {&pads, "pads", nr}}, nr, rank, &out,
+             {{&b, "b", at::kBFloat16, false}, {&out, "out", at::kBFloat16, false}, {&flags, "flags", at::kInt, true}});
   const void* bp = check_bias(bias, out, b_kmajor, "gemm_ag");
+  TORCH_CHECK(nr == 1 || ((uint32_t)ag_epoch != 0 && (uint32_t)bar_epoch != 0),
+              "gemm_ag: ag_epoch and bar_epoch must be nonzero with more than one rank");
   const c10::cuda::CUDAGuard guard(out.device());
-  const int nr = (int)a_bufs.size();
   const int M = (int)out.size(0), N = (int)out.size(1);
   const int K = (int)(b_kmajor ? b.size(1) : b.size(0));
-  TORCH_CHECK((b_kmajor ? b.size(0) : b.size(1)) == N, "B does not match out");
-  TORCH_CHECK(flags.numel() * 256 >= M, "flags too small");
+  TORCH_CHECK((b_kmajor ? b.size(0) : b.size(1)) == N, "gemm_ag: B does not match out");
+  TORCH_CHECK(flags.numel() * 256 >= M, "gemm_ag: flags must hold one word per 256-row tile");
   const void* as[kMaxRanks] = {nullptr};
   uint32_t* pd[kMaxRanks] = {nullptr};
-  for (int i = 0; i < nr; ++i) {
+  for (int64_t i = 0; i < nr; ++i) {
     as[i] = (const void*)a_bufs[i];
     pd[i] = (uint32_t*)pads[i];
   }
-  dtg::gemm_bf16_ag(as, b.data_ptr(), out.data_ptr(), M, N, K, b.stride(0), out.stride(0), b_kmajor, nr, (int)rank,
+  dtg::gemm_bf16_ag(as, b.data_ptr(), out.data_ptr(), M, N, K, b.stride(0), out.stride(0), b_kmajor, (int)nr, (int)rank,
                     (int)rows_per_peer, (uint32_t*)flags.data_ptr<int>(), (uint32_t)ag_epoch, pd, (uint32_t)bar_epoch,
                     (int)n_comm, stream(), bp);
 }
 
 // C = a @ op(B) with B = a weight inside the flat buffer `full` (element offset w_off, w_numel elements), gathered
-// from the ranks' shards by the kernel itself (FSDP unshard fused into the consuming GEMM)
+// from the ranks' shards by the kernel itself (FSDP unshard fused into the consuming GEMM).  shards and pads: one
+// entry per rank; the weight range must lie inside the shards.  The producer waits for `target` on the chunk
+// counters, so with more than one rank it may not be 0.
 void py_gemm_bgather(const Tensor& a, Tensor& full, Tensor& out, bool b_kmajor, int64_t b_rows, int64_t b_cols,
                      const std::vector<uint64_t>& shards, int64_t per_numel, int64_t w_off, int64_t w_numel,
                      Tensor& counters, int64_t target, int64_t chunk_shift, const std::vector<uint64_t>& pads,
                      int64_t rank, int64_t bar_epoch, const c10::optional<Tensor>& bias) {
-  TORCH_CHECK(a.is_cuda() && a.scalar_type() == at::kBFloat16 && a.dim() == 2 && a.stride(1) == 1, "bad A");
-  TORCH_CHECK(out.is_cuda() && out.scalar_type() == at::kBFloat16 && out.dim() == 2 && out.stride(1) == 1, "bad out");
+  const int64_t nr = (int64_t)shards.size();
+  check_dist("gemm_bgather", {{&shards, "shards", nr}, {&pads, "pads", nr}}, nr, rank, &out,
+             {{&a, "a", at::kBFloat16, false}, {&out, "out", at::kBFloat16, false},
+              {&full, "full", at::kBFloat16, true}, {&counters, "counters", at::kInt, true}});
   const void* bp = check_bias(bias, out, b_kmajor, "gemm_bgather");
-  TORCH_CHECK(full.is_contiguous() && full.scalar_type() == at::kBFloat16, "full must be the flat bf16 buffer");
-  TORCH_CHECK(counters.scalar_type() == at::kInt && counters.is_cuda(), "counters must be an int32 CUDA tensor");
-  TORCH_CHECK(w_off + w_numel <= full.numel() && b_rows * b_cols <= w_numel, "weight outside the flat buffer");
-  TORCH_CHECK(((int64_t)full.numel() * 2) >> chunk_shift <= counters.numel(), "counter array too small");
+  TORCH_CHECK(per_numel >= 1 && w_off >= 0 && w_numel >= 0 && w_off + w_numel <= nr * per_numel,
+              "gemm_bgather: the weight range [", w_off, ", ", w_off + w_numel, ") must lie inside the ", nr,
+              " shards of ", per_numel, " elements");
+  TORCH_CHECK(w_off + w_numel <= full.numel() && b_rows >= 0 && b_cols >= 0 && b_rows * b_cols <= w_numel,
+              "gemm_bgather: weight outside the flat buffer");
+  TORCH_CHECK(chunk_shift >= 14 && chunk_shift <= 30, "gemm_bgather: chunk_shift must be in [14, 30], got ",
+              chunk_shift);
+  TORCH_CHECK(((int64_t)full.numel() * 2) >> chunk_shift <= counters.numel(), "gemm_bgather: counter array too small");
+  TORCH_CHECK(nr == 1 || (uint32_t)target != 0, "gemm_bgather: target must be nonzero with more than one rank");
   const c10::cuda::CUDAGuard guard(out.device());
-  const int nr = (int)shards.size();
-  TORCH_CHECK(nr == (int)pads.size() && nr <= kMaxRanks, "shards / pads per rank");
   const int M = (int)out.size(0), N = (int)out.size(1);
   const int K = (int)a.size(1);
   TORCH_CHECK(a.size(0) == M && (b_kmajor ? (b_rows == N && b_cols == K) : (b_rows == K && b_cols == N)),
-              "shape mismatch");
+              "gemm_bgather: shape mismatch");
   const void* sh[kMaxRanks] = {nullptr};
   uint32_t* pd[kMaxRanks] = {nullptr};
-  for (int i = 0; i < nr; ++i) {
+  for (int64_t i = 0; i < nr; ++i) {
     sh[i] = (const void*)shards[i];
     pd[i] = (uint32_t*)pads[i];
   }
   dtg::gemm_bf16_bgather(a.data_ptr(), full.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b_cols, out.stride(0),
                          b_kmajor, sh, per_numel * 2, w_off * 2, w_numel * 2, (uint32_t*)counters.data_ptr<int>(),
-                         (uint32_t)target, (int)chunk_shift, pd, nr, (int)rank, (uint32_t)bar_epoch, stream(), bp);
+                         (uint32_t)target, (int)chunk_shift, pd, (int)nr, (int)rank, (uint32_t)bar_epoch, stream(), bp);
 }
 
+// out = (residual +) the sum of parts [nparts, *out.shape], nparts in 1..8; every tensor bf16, contiguous and 16-byte
+// aligned on out's device.  An empty out launches nothing.
 void py_reduce_parts(const Tensor& parts, const c10::optional<Tensor>& residual, Tensor& out) {
-  TORCH_CHECK(parts.is_contiguous() && out.is_contiguous() && parts.scalar_type() == at::kBFloat16, "bad tensors");
-  const int64_t nparts = parts.size(0);
-  TORCH_CHECK(parts.numel() == nparts * out.numel(), "parts must be [nparts, *out.shape]");
+  const Tensor* res = residual.has_value() ? &*residual : nullptr;
+  check_dist("tp_reduce_parts", {}, 1, 0, &out,
+             {{&parts, "parts", at::kBFloat16, true}, {&out, "out", at::kBFloat16, true},
+              {res, "residual", at::kBFloat16, true}});
+  TORCH_CHECK(parts.dim() == out.dim() + 1 && parts.size(0) >= 1 && parts.size(0) <= kMaxRanks &&
+                  parts.sizes().slice(1) == out.sizes(),
+              "tp_reduce_parts: parts must be [nparts, *out.shape] with 1..", kMaxRanks, " parts");
+  TORCH_CHECK(!res || res->sizes() == out.sizes(), "tp_reduce_parts: residual must have out's shape");
+  TORCH_CHECK(out.numel() % 8 == 0, "tp_reduce_parts: size must be a multiple of 8");
+  if (out.numel() == 0) return;
   const c10::cuda::CUDAGuard guard(out.device());
-  dtg::tp_reduce_parts(parts.data_ptr(), residual.has_value() ? residual->data_ptr() : nullptr, out.data_ptr(),
-                       out.numel(), (int)nparts, stream());
+  dtg::tp_reduce_parts(parts.data_ptr(), res ? res->data_ptr() : nullptr, out.data_ptr(), out.numel(),
+                       (int)parts.size(0), stream());
 }
 
 void py_reduce_mc(uint64_t part_mc, const c10::optional<Tensor>& residual, Tensor& out, const std::vector<uint64_t>& pads,
