@@ -52,7 +52,8 @@ class TrainEngine:
                cpu_offload: bool = False, checkpoint_activations: bool = False, prefetch_layers: bool = False,
                num_layers: Optional[int] = None, lr_scaling: str = "none", fp8: bool = False,
                document_masking: bool = False, max_grad_norm: Optional[float] = None, **extra):
-        """``fp8=True`` runs the decoder-layer projections in fp8 (``ops.fp8_linear``); single and ddp engines only.
+        """``fp8=True`` runs the decoder-layer projections in fp8 (``ops.linear(..., fp8=True)``); single and ddp
+        engines only.
         ``document_masking=True``: batches that carry ``position_ids`` are packed documents, each starting where its
         position id is 0; attention and targets stay inside each document (single, ddp and fsdp engines, Llama).
         ``max_grad_norm``: clip the gradients by their global L2 norm before AdamW

@@ -1,8 +1,9 @@
 """Llama-family causal LM built on the sm_90a op layer (Llama; Mistral: Llama plus a sliding attention window; Qwen3:
 Llama plus QK-norm, with a head_dim of its own; Qwen2: Llama plus q/k/v biases; OLMo 2: Llama with a full-width
-QK-norm and RMSNorms after each sublayer instead of before it, ``Olmo2DecoderLayer``; StarCoder2: Llama with
-LayerNorms, a c_fc -> GELU-tanh -> c_proj MLP and a bias on every projection, ``Starcoder2DecoderLayer``; GPT-NeoX:
-StarCoder2's parameters with a parallel residual, partial rotary embeddings and an exact GELU, ``GPTNeoXDecoderLayer``).
+QK-norm and RMSNorms after each sublayer instead of before it; StarCoder2: Llama with LayerNorms, a c_fc -> GELU-tanh
+-> c_proj MLP and a bias on every projection; GPT-NeoX: StarCoder2's parameters with a parallel residual, partial
+rotary embeddings and an exact GELU).  One ``LlamaDecoderLayer`` builds every family's layer from its
+``ModelConfig``, and ``decoder_layout`` fixes its flat-buffer layout.
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
 the reference instantiates at e.g. ``02-distributed-data-parallel/train_llm.py:57-58``)
@@ -207,6 +208,14 @@ class LlamaAttention(nn.Module):
         return ops.qk_norm_rope_(qkv, self.q_norm.weight, self.k_norm.weight, cos, sin, self.num_heads,
                                  self.num_kv_heads, self.q_norm.eps)
 
+    def attend(self, qkv, cos, sin, doc_start=None):
+        """Attention from the fused q|k|v projection ``qkv`` [B,S,(nh + 2 nkv) d]: position the q and k heads, then
+        attend.  Returns [B, S, nh d]."""
+        B, S, _ = qkv.shape
+        qkv = self.position_qk_(qkv.view(B, S, self.num_heads + 2 * self.num_kv_heads, self.head_dim), cos, sin)
+        a = ops.attention_qkv(qkv, self.num_heads, self.num_kv_heads, doc_start=doc_start, window=self.sliding_window)
+        return a.reshape(B, S, self.num_heads * self.head_dim)
+
 
 class LlamaMLP(nn.Module):
     def __init__(self, config: ModelConfig, dtype=None, device=None, tp_size=1):
@@ -239,203 +248,134 @@ class FusedWeight:
         self._dtg_ready_hook = None
 
 
+def decoder_layout(config: ModelConfig):
+    """``(flat_order, fused)`` of a decoder layer of ``config``.
+
+    ``flat_order`` is the layer's parameter order in its flat buffer (parallel/flat.py, parallel/fsdp.py), which also
+    fixes FSDP's shard and chunk boundaries and the sharded checkpoint layout; a parameter missing from it would get
+    no gradient buffer and no optimizer update.  The matrices come first (FSDP's chunked layout), with q|k|v and
+    gate|up adjacent so that their fused weights are views of the buffer.  The norms' gains (and LayerNorm biases)
+    follow, then the QK-norm gains, so every replicated gain sits in one run after the matrices (TP sums their
+    gradients over the group in one launch).  Then the q|k|v biases: adjacent, and each a multiple of 8 elements, so
+    they form one [(nh + 2 nkv) d] bias (``fused_view_1d``) next to the fused q|k|v weight.  The o_proj and MLP
+    biases come last.
+
+    ``fused`` maps each fused weight (``qkv``, ``gate_up`` with the SwiGLU MLP, ``qkv_bias`` with q/k/v biases) to
+    its member parameter names."""
+    qkv = ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight")
+    if config.gelu_mlp:
+        mlp, mlp_bias = ("mlp.c_fc.weight", "mlp.c_proj.weight"), ("mlp.c_fc.bias", "mlp.c_proj.bias")
+    else:
+        mlp, mlp_bias = ("mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight"), ()
+    norms = (("post_attention_layernorm", "post_feedforward_layernorm") if config.post_norm else
+             ("input_layernorm", "post_attention_layernorm"))
+    gains = tuple(f"{n}.{p}" for n in norms for p in (("weight", "bias") if config.layer_norm else ("weight",)))
+    qk_norm = ("self_attn.q_norm.weight", "self_attn.k_norm.weight") if config.qk_norm or config.full_qk_norm else ()
+    qkv_bias = (("self_attn.q_proj.bias", "self_attn.k_proj.bias", "self_attn.v_proj.bias")
+                if config.qkv_bias or config.all_bias else ())
+    o_bias = ("self_attn.o_proj.bias",) if config.all_bias else ()
+    fused = {"qkv": qkv}
+    if not config.gelu_mlp:
+        fused["gate_up"] = mlp[:2]
+    if qkv_bias:
+        fused["qkv_bias"] = qkv_bias
+    return qkv + ("self_attn.o_proj.weight",) + mlp + gains + qk_norm + qkv_bias + o_bias + mlp_bias, fused
+
+
 class LlamaDecoderLayer(nn.Module):
-    #: parameter order inside a Llama / Mistral layer's flat buffer; adjacency is what makes fusion free
-    FLAT_ORDER = (
-        "self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight",
-        "self_attn.o_proj.weight", "mlp.gate_proj.weight", "mlp.up_proj.weight",
-        "mlp.down_proj.weight", "input_layernorm.weight", "post_attention_layernorm.weight",
-    )
-    #: appended with QK-norm: after the layer norms, so the matrices stay first (FSDP's chunked layout) and every
-    #: replicated gain sits in one run at the end (TP sums their gradients over the group in one launch)
-    QK_NORM_ORDER = ("self_attn.q_norm.weight", "self_attn.k_norm.weight")
-    #: appended with q/k/v biases (Qwen2), also after the layer norms: adjacent, and each a multiple of 8 elements, so
-    #: they form one [(nh + 2 nkv) d] q|k|v bias (``fused_view_1d``) next to the fused q|k|v weight
-    QKV_BIAS_ORDER = ("self_attn.q_proj.bias", "self_attn.k_proj.bias", "self_attn.v_proj.bias")
-    FUSED = {"qkv": FLAT_ORDER[0:3], "gate_up": FLAT_ORDER[4:6]}
+    """The decoder layer of every family, built from its config: RMSNorms or LayerNorms (``layer_norm``), the SwiGLU
+    ``LlamaMLP`` or the c_fc -> GELU -> c_proj ``Starcoder2MLP`` (``gelu_mlp``), and one of three residual schemes:
+
+      * pre-norm (Llama, Mistral, Qwen2.5, Qwen3, StarCoder2): ``h1 = h + attn(norm_in(h))``,
+        ``h2 = h1 + mlp(norm_pa(h1))``, each add deferred into the next norm's kernel;
+      * ``post_norm`` (OLMo 2): no ``input_layernorm``, ``h1 = h + norm_pa(attn(h))``, ``h2 = h1 + norm_pf(mlp(h1))``;
+      * ``parallel_residual`` (GPT-NeoX): ``h' = h + attn(ln1(h)) + mlp(ln2(h))``, both norms of the same h."""
 
     def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
         super().__init__()
         self.layer_idx = layer_idx
         self.self_attn = LlamaAttention(config, dtype, device, tp_size)
-        self.mlp = LlamaMLP(config, dtype, device, tp_size)
-        self.input_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
-        self.post_attention_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
-        #: this layer's parameter order in its flat buffer (parallel/flat.py, parallel/fsdp.py); a parameter missing
-        #: here would get no gradient buffer and no optimizer update
-        self.flat_order = (self.FLAT_ORDER + (self.QK_NORM_ORDER if config.qk_norm else ())
-                           + (self.QKV_BIAS_ORDER if config.qkv_bias else ()))
-        self._fused = {}  # name -> FusedWeight, installed by parallel.flat.FlatParamGroup
-        self.tp = None  # installed by parallel.tp.apply_tensor_parallel
-        self.fp8 = False  # set through LlamaForCausalLM.fp8: the four projections run ops.fp8_linear
+        if config.gelu_mlp:
+            assert tp_size == 1, f"{config.arch} layers are not tensor-parallel"
+            self.mlp = Starcoder2MLP(config, dtype, device)
+        else:
+            self.mlp = LlamaMLP(config, dtype, device, tp_size)
+        Norm, eps = (LayerNorm, config.layer_norm_epsilon) if config.layer_norm else (RMSNorm, config.rms_norm_eps)
+        if not config.post_norm:
+            self.input_layernorm = Norm(config.hidden_size, eps, dtype, device)
+        self.post_attention_layernorm = Norm(config.hidden_size, eps, dtype, device)
+        if config.post_norm:
+            self.post_feedforward_layernorm = Norm(config.hidden_size, eps, dtype, device)
+        self.post_norm, self.parallel_residual, self.gelu_exact = (config.post_norm, config.parallel_residual,
+                                                                   config.gelu_exact)
+        self.flat_order, self.fused = decoder_layout(config)
+        self._fused = {}  # name -> FusedWeight, installed by parallel.flat.install_fused_views
+        self.tp = None  # set through LlamaForCausalLM.tp: the layer runs TensorParallelRuntime.layer_forward
+        self.fp8 = False  # set through LlamaForCausalLM.fp8: the projections run in fp8
 
-    # fused weights -------------------------------------------------------------------
-    def _qkv_weight(self):
-        f = self._fused.get("qkv")
-        if f is not None and _ext.use_cuda_kernel("gemm", f.data):
-            return f.data, f
-        a = self.self_attn
-        return torch.cat([a.q_proj.weight, a.k_proj.weight, a.v_proj.weight], dim=0), None
-
-    def _qkv_bias(self):
-        """(fused q|k|v bias, its flat-gradient owner) or (None, None) without biases."""
-        a = self.self_attn
-        if a.q_proj.bias is None:
+    def fused_weight(self, name):
+        """(fused weight ``name``, its flat-gradient owner).  That is the ``FusedWeight`` view the flat group
+        installed wherever the projection writes the flat gradient through it: the wgmma GEMM, and the
+        tensor-parallel projections, which route it on the CPU too.  Otherwise it is the members concatenated, with no
+        owner, so that autograd reaches them.  (None, None) for a fused weight the layer does not have."""
+        members = self.fused.get(name)
+        if members is None:
             return None, None
-        f = self._fused.get("qkv_bias")
-        if f is not None and _ext.use_cuda_kernel("gemm", f.data):
+        f = self._fused.get(name)
+        if f is not None and (self.tp is not None or _ext.use_cuda_kernel("gemm", f.data)):
             return f.data, f
-        return torch.cat([a.q_proj.bias, a.k_proj.bias, a.v_proj.bias]), None
+        return torch.cat([self.get_parameter(m) for m in members]), None
 
-    def _gate_up_weight(self):
-        f = self._fused.get("gate_up")
-        if f is not None and _ext.use_cuda_kernel("gemm", f.data):
-            return f.data, f
-        return torch.cat([self.mlp.gate_proj.weight, self.mlp.up_proj.weight], dim=0), None
+    def _proj(self, x, w, bias=None, owner=None, bias_owner=None):
+        """Every projection of the layer, in fp8 or bf16."""
+        return ops.linear(x, w, bias, owner, bias_owner, fp8=self.fp8)
 
-    # forward ---------------------------------------------------------------------------
+    def _attention(self, y, cos, sin, doc_start):
+        """Attention of the normed stream ``y`` [B,S,H] up to the o_proj: [B, S, nh d]."""
+        w, owner = self.fused_weight("qkv")
+        b, b_owner = self.fused_weight("qkv_bias")
+        return self.self_attn.attend(self._proj(y, w, b, owner, b_owner), cos, sin, doc_start)
+
+    def _mlp_act(self, y):
+        """The MLP up to its down-projection: SwiGLU on the fused gate|up, or c_fc -> GELU (exact for GPT-NeoX, the
+        tanh form for StarCoder2)."""
+        if isinstance(self.mlp, LlamaMLP):
+            w, owner = self.fused_weight("gate_up")
+            return ops.swiglu(self._proj(y, w, owner=owner))
+        up = self._proj(y, self.mlp.c_fc.weight, self.mlp.c_fc.bias)
+        return ops.gelu(up) if self.gelu_exact else ops.gelu_tanh(up)
+
+    def _mlp(self, y):
+        down = self.mlp.down_proj if isinstance(self.mlp, LlamaMLP) else self.mlp.c_proj
+        return self._proj(self._mlp_act(y), down.weight, down.bias)
+
     def forward(self, x, residual, cos, sin, doc_start=None):
         """x: [B,S,H] branch output of the previous layer (or the embeddings);
         residual: running residual stream *before* adding x (None for the first layer);
         doc_start: None or int32 [B,S] from ``ops.document_starts`` (attention stays inside each document).
-        Returns (mlp_out, residual) with the final add again deferred to the consumer."""
-        att = self.self_attn
-        B, S, _ = x.shape
-        fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
+        Returns (branch, residual) with the final add again deferred to the consumer."""
+        if self.tp is not None:
+            return self.tp.layer_forward(self, x, residual, cos, sin)
+        o = self.self_attn.o_proj
+        if self.post_norm:
+            # the pending add would need this layer's post_feedforward_layernorm gain, which FSDP may reshard before
+            # the next layer runs, so the layer completes its stream and returns (h2, None): every layer sees
+            # residual = None
+            assert residual is None, "an OLMo 2 layer takes the complete residual stream"
+            n1, n2 = self.post_attention_layernorm, self.post_feedforward_layernorm
+            h1 = ops.rms_norm_add(self._proj(self._attention(x, cos, sin, doc_start), o.weight), x, n1.weight, n1.eps)
+            return ops.rms_norm_add(self._mlp(h1), h1, n2.weight, n2.eps), None
+        if self.parallel_residual:
+            # the attention dense and the MLP down-projection write one branch
+            n1, n2, c_proj = self.input_layernorm, self.post_attention_layernorm, self.mlp.c_proj
+            y1, y2, h = ops.layer_norm2(x, residual, n1.weight, n1.bias, n2.weight, n2.bias, n1.eps)
+            a = self._attention(y1, cos, sin, doc_start)
+            out = ops.parallel_out(a, self._mlp_act(y2), o.weight, c_proj.weight, o.bias, c_proj.bias, fp8=self.fp8)
+            return out, h
         y, h = self.input_layernorm(x, residual)
-        w, owner = self._qkv_weight()
-        b, b_owner = self._qkv_bias()
-        qkv = fused_linear(y, w, owner, b, b_owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
-        qkv = att.position_qk_(qkv, cos, sin)
-        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
-        a = a.reshape(B, S, att.num_heads * att.head_dim)
-        a = ops.fp8_linear(a, att.o_proj.weight) if self.fp8 else att.o_proj(a)
-        y, h = self.post_attention_layernorm(a, h)
-        w, owner = self._gate_up_weight()
-        act = ops.swiglu(fused_linear(y, w, owner))
-        down = ops.fp8_linear(act, self.mlp.down_proj.weight) if self.fp8 else self.mlp.down_proj(act)
-        return down, h
-
-
-class Olmo2DecoderLayer(LlamaDecoderLayer):
-    """OLMo 2's layer: the Llama layer with full-width QK-norm and RMSNorms after each sublayer instead of before it:
-    ``h1 = h + norm_pa(o_proj(attn(h)))``, ``h2 = h1 + norm_pf(mlp(h1))``; there is no ``input_layernorm``."""
-
-    #: matrices first in the Llama order (FSDP's chunked layout; ``FUSED``'s q|k|v and gate|up), then the gains
-    FLAT_ORDER = LlamaDecoderLayer.FLAT_ORDER[:7] + (
-        "post_attention_layernorm.weight", "post_feedforward_layernorm.weight", "self_attn.q_norm.weight",
-        "self_attn.k_norm.weight",
-    )
-
-    def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
-        nn.Module.__init__(self)
-        self.layer_idx = layer_idx
-        self.self_attn = LlamaAttention(config, dtype, device, tp_size)
-        self.mlp = LlamaMLP(config, dtype, device, tp_size)
-        self.post_attention_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
-        self.post_feedforward_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, dtype, device)
-        self.flat_order = self.FLAT_ORDER
-        self._fused = {}
-        self.tp = None
-        self.fp8 = False
-
-    def forward(self, x, residual, cos, sin, doc_start=None):
-        """x: [B,S,H] the residual stream (the embeddings for the first layer); residual: None.  The pending add
-        needs this layer's post_feedforward_layernorm gain, which FSDP may reshard before the next layer runs, so the
-        layer completes its stream and returns (h2, None): every layer sees ``residual = None``."""
-        assert residual is None, "an OLMo 2 layer takes the complete residual stream"
-        att = self.self_attn
-        B, S, _ = x.shape
-        fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
-        w, owner = self._qkv_weight()
-        qkv = fused_linear(x, w, owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
-        qkv = att.position_qk_(qkv, cos, sin)
-        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
-        a = a.reshape(B, S, att.num_heads * att.head_dim)
-        a = ops.fp8_linear(a, att.o_proj.weight) if self.fp8 else att.o_proj(a)
-        n = self.post_attention_layernorm
-        h1 = ops.rms_norm_add(a, x, n.weight, n.eps)
-        w, owner = self._gate_up_weight()
-        act = ops.swiglu(fused_linear(h1, w, owner))
-        down = ops.fp8_linear(act, self.mlp.down_proj.weight) if self.fp8 else self.mlp.down_proj(act)
-        n = self.post_feedforward_layernorm
-        return ops.rms_norm_add(down, h1, n.weight, n.eps), None
-
-
-class Starcoder2DecoderLayer(LlamaDecoderLayer):
-    """StarCoder2's layer: the Llama layer with LayerNorms, a c_fc -> GELU-tanh -> c_proj MLP and a bias on every
-    projection.  The residual add stays deferred: the layer returns ``(c_proj_out, h)``."""
-
-    #: matrices first (FSDP's chunked layout; ``FUSED``'s q|k|v), then the norm gains and biases, then the adjacent
-    #: q|k|v biases (one 1-D view, ``fused_view_1d``), then the o_proj, c_fc and c_proj biases
-    FLAT_ORDER = LlamaDecoderLayer.FLAT_ORDER[:4] + (
-        "mlp.c_fc.weight", "mlp.c_proj.weight", "input_layernorm.weight", "input_layernorm.bias",
-        "post_attention_layernorm.weight", "post_attention_layernorm.bias",
-    ) + LlamaDecoderLayer.QKV_BIAS_ORDER + ("self_attn.o_proj.bias", "mlp.c_fc.bias", "mlp.c_proj.bias")
-    FUSED = {"qkv": FLAT_ORDER[0:3]}
-
-    def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
-        nn.Module.__init__(self)
-        assert tp_size == 1, "StarCoder2 layers are not tensor-parallel"
-        self.layer_idx = layer_idx
-        self.self_attn = LlamaAttention(config, dtype, device)   # q, k, v and o with biases (``all_bias``)
-        h = config.hidden_size
-        self.mlp = Starcoder2MLP(config, dtype, device)
-        self.input_layernorm = LayerNorm(h, config.layer_norm_epsilon, dtype, device)
-        self.post_attention_layernorm = LayerNorm(h, config.layer_norm_epsilon, dtype, device)
-        self.flat_order = self.FLAT_ORDER
-        self._fused = {}
-        self.tp = None
-        self.fp8 = False
-
-    def forward(self, x, residual, cos, sin, doc_start=None):
-        att = self.self_attn
-        B, S, _ = x.shape
-        fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
-        y, h = self.input_layernorm(x, residual)
-        w, owner = self._qkv_weight()
-        b, b_owner = self._qkv_bias()
-        qkv = fused_linear(y, w, owner, b, b_owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
-        qkv = att.position_qk_(qkv, cos, sin)
-        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
-        a = a.reshape(B, S, att.num_heads * att.head_dim)
-        a = ops.fp8_linear(a, att.o_proj.weight, None, att.o_proj.bias) if self.fp8 else att.o_proj(a)
-        y, h = self.post_attention_layernorm(a, h)
-        mlp = self.mlp
-        up = ops.fp8_linear(y, mlp.c_fc.weight, None, mlp.c_fc.bias) if self.fp8 else mlp.c_fc(y)
-        act = ops.gelu_tanh(up)
-        down = ops.fp8_linear(act, mlp.c_proj.weight, None, mlp.c_proj.bias) if self.fp8 else mlp.c_proj(act)
-        return down, h
-
-
-class GPTNeoXDecoderLayer(Starcoder2DecoderLayer):
-    """GPT-NeoX's layer: StarCoder2's parameters (names, ``FLAT_ORDER``, fused q|k|v weight and bias) with a parallel
-    residual, ``h' = h + attn(ln1(h)) + mlp(ln2(h))``, RoPE on the first ``rotary_dim`` elements of each q/k head and
-    an exact GELU.  Both norms read the same h (``ops.layer_norm2``); the attention dense and the MLP down-projection
-    write one branch (``ops.parallel_out``), and the residual add stays deferred: the layer returns ``(branch, h)``."""
-
-    def __init__(self, config: ModelConfig, layer_idx: int, dtype=None, device=None, tp_size=1):
-        assert tp_size == 1, "GPT-NeoX layers are not tensor-parallel"
-        super().__init__(config, layer_idx, dtype, device, tp_size)
-
-    def forward(self, x, residual, cos, sin, doc_start=None):
-        att = self.self_attn
-        B, S, _ = x.shape
-        fused_linear = ops.fp8_linear if self.fp8 else ops.fused_linear
-        n1, n2 = self.input_layernorm, self.post_attention_layernorm
-        y1, y2, h = ops.layer_norm2(x, residual, n1.weight, n1.bias, n2.weight, n2.bias, n1.eps)
-        w, owner = self._qkv_weight()
-        b, b_owner = self._qkv_bias()
-        qkv = fused_linear(y1, w, owner, b, b_owner).view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
-        qkv = att.position_qk_(qkv, cos, sin)
-        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, doc_start=doc_start, window=att.sliding_window)
-        a = a.reshape(B, S, att.num_heads * att.head_dim)
-        mlp = self.mlp
-        up = ops.fp8_linear(y2, mlp.c_fc.weight, None, mlp.c_fc.bias) if self.fp8 else mlp.c_fc(y2)
-        act = ops.gelu(up)
-        out = ops.parallel_out(a, act, att.o_proj.weight, mlp.c_proj.weight, att.o_proj.bias, mlp.c_proj.bias,
-                               fp8=self.fp8)
-        return out, h
+        a = self._attention(y, cos, sin, doc_start)
+        y, h = self.post_attention_layernorm(self._proj(a, o.weight, o.bias), h)
+        return self._mlp(y), h
 
 
 class LlamaModel(nn.Module):
@@ -445,11 +385,8 @@ class LlamaModel(nn.Module):
         # tensor parallel: the table is sharded over the hidden dimension (reference: ColwiseParallel on
         # nn.Embedding, 06-tensor-parallel/train_llm.py:82)
         self.embed_tokens = Embedding(config.vocab_size, config.hidden_size // tp_size, dtype, device)
-        layer_cls = (Olmo2DecoderLayer if config.post_norm else
-                     GPTNeoXDecoderLayer if config.parallel_residual else
-                     Starcoder2DecoderLayer if config.arch == "starcoder2" else LlamaDecoderLayer)
         self.layers = nn.ModuleList(
-            [layer_cls(config, i, dtype, device, tp_size) for i in range(config.num_hidden_layers)]
+            [LlamaDecoderLayer(config, i, dtype, device, tp_size) for i in range(config.num_hidden_layers)]
         )
         if config.layer_norm:
             self.norm = LayerNorm(config.hidden_size, config.layer_norm_epsilon, dtype, device)
@@ -484,8 +421,8 @@ class LlamaForCausalLM(nn.Module):
 
     @property
     def fp8(self) -> bool:
-        """Run the decoder-layer projections (q|k|v, o, gate|up, down) through ``ops.fp8_linear``: fp8 GEMMs with
-        per-tensor current scaling.  The lm_head, embedding, attention, norms and loss stay bf16."""
+        """Run the decoder-layer projections (q|k|v, o, gate|up, down) in fp8 (``ops.linear(..., fp8=True)``): fp8
+        GEMMs with per-tensor current scaling.  The lm_head, embedding, attention, norms and loss stay bf16."""
         return self._fp8
 
     @fp8.setter
@@ -493,6 +430,17 @@ class LlamaForCausalLM(nn.Module):
         self._fp8 = bool(on)
         for layer in self.model.layers:
             layer.fp8 = self._fp8
+
+    @property
+    def tp(self):
+        """The ``parallel.tp.TensorParallelRuntime`` that runs the model's and its layers' forward, or None."""
+        return self._tp
+
+    @tp.setter
+    def tp(self, runtime):
+        self._tp = runtime
+        for layer in self.model.layers:
+            layer.tp = runtime
 
     # -- initialisation -----------------------------------------------------------------
     @torch.no_grad()
@@ -517,26 +465,14 @@ class LlamaForCausalLM(nn.Module):
         return ops.cross_entropy(logits.reshape(-1, logits.shape[-1]), tgt)
 
     # -- forward --------------------------------------------------------------------------
-    def forward(self, input_ids, attention_mask=None, labels=None, position_ids=None, return_logits=None):
-        """``attention_mask`` is accepted for API parity; the data pipeline only produces full
-        (unpadded) chunks so only the causal mask is applied (the reference's all-ones mask
-        collapses to the same thing inside transformers, SURVEY.md K3).  With ``document_masking``
-        and ``position_ids``, attention and targets stay inside each packed document."""
-        if self.tp is not None:
-            return self.tp.model_forward(self, input_ids, labels, position_ids)
-        B, S = input_ids.shape
-        m = self.model
-        if position_ids is None:
-            cos, sin = m.rotary_emb.tables(S, input_ids.device)
-        else:
-            cos, sin = m.rotary_emb(position_ids)
-        doc_start = None
-        if self.document_masking and position_ids is not None:
-            doc_start = ops.document_starts(position_ids)
-        eng = self.engine
+    def decoder(self, input_ids, cos, sin, doc_start=None, embed=None):
+        """The embedding, every decoder layer and the final norm, with the engine's hooks around them and activation
+        checkpointing.  ``embed`` replaces the embedding lookup (tensor parallelism's hidden-parallel one).  Returns
+        the final norm's output."""
+        m, eng = self.model, self.engine
         if eng is not None:
             eng.pre_forward(self)
-        x = m.embed_tokens(input_ids)
+        x = (embed or m.embed_tokens)(input_ids)
         residual = None
         for i, layer in enumerate(m.layers):
             if eng is not None:
@@ -551,7 +487,25 @@ class LlamaForCausalLM(nn.Module):
                 x, residual = eng.post_layer(i, layer, x, residual)
         if eng is not None:
             x, residual = eng.pre_head(x, residual)
-        y, _ = m.norm(x, residual)
+        return m.norm(x, residual)[0]
+
+    def forward(self, input_ids, attention_mask=None, labels=None, position_ids=None, return_logits=None):
+        """``attention_mask`` is accepted for API parity; the data pipeline only produces full
+        (unpadded) chunks so only the causal mask is applied (the reference's all-ones mask
+        collapses to the same thing inside transformers, SURVEY.md K3).  With ``document_masking``
+        and ``position_ids``, attention and targets stay inside each packed document."""
+        B, S = input_ids.shape
+        m = self.model
+        if position_ids is None:
+            cos, sin = m.rotary_emb.tables(S, input_ids.device)
+        else:
+            cos, sin = m.rotary_emb(position_ids)
+        if self.tp is not None:
+            return self.tp.model_forward(self, input_ids, labels, cos, sin)
+        doc_start = None
+        if self.document_masking and position_ids is not None:
+            doc_start = ops.document_starts(position_ids)
+        y = self.decoder(input_ids, cos, sin, doc_start)
         logits = self.lm_head(y.reshape(B * S, -1))  # [T, V], a fresh tensor the loss may consume
         loss = None
         if labels is not None:

@@ -2,7 +2,7 @@
 
 On CUDA tensors each op calls a hand-written sm_90a kernel from the in-tree
 extension (``csrc/``): wgmma/TMA GEMM (fwd / dgrad / wgrad) in bf16 and, for
-``fp8_linear``, in fp8 with its amax and cast-transpose kernels, wgmma
+``linear(..., fp8=True)``, in fp8 with its amax and cast-transpose kernels, wgmma
 flash-attention, fused residual-add+RMSNorm and norm-then-add (OLMo 2), in-place RoPE on the fused qkv buffer
 (after Qwen3's per-head or OLMo 2's full-width QK-norm in the same kernel; partial rotary for GPT-NeoX), SwiGLU,
 fused residual-add+LayerNorm and GELU-tanh (StarCoder2), GPT-NeoX's dual LayerNorm, exact GELU and parallel-residual
@@ -29,10 +29,10 @@ from .. import _ext
 from . import reference as ref
 
 __all__ = [
-    "linear", "fused_linear", "rms_norm", "add_rms_norm", "rms_norm_add", "rope_qkv_", "qk_norm_rope_",
+    "linear", "rms_norm", "add_rms_norm", "rms_norm_add", "rope_qkv_", "qk_norm_rope_",
     "olmo_qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy", "layer_norm",
     "add_layer_norm", "gelu_tanh", "gelu", "layer_norm2", "parallel_out",
-    "embedding", "gemm", "fp8_linear", "fp8_amax", "fp8_cast", "gemm_fp8", "bias_grad", "ref",
+    "embedding", "gemm", "fp8_amax", "fp8_cast", "gemm_fp8", "bias_grad", "ref",
 ]
 
 
@@ -193,24 +193,20 @@ def _linear_grads(dy2, x2, w, w_param, x_shape, need_dx, need_dw):
     return dx, dw
 
 
-def linear(x, w, bias=None):
-    """y = x @ w.T (+ bias).  bf16 CUDA tensors run the wgmma GEMM, the bias in its epilogue."""
-    if _ext.use_cuda_kernel("gemm", x, w) and x.dtype == torch.bfloat16:
-        if bias is None:
-            return _Linear.apply(x, w, w)
-        return _Linear.apply(x, w, w, bias, bias)
-    return ref.linear(x, w, bias)
+def linear(x, w, bias=None, owner=None, bias_owner=None, fp8=False):
+    """y = x @ w.T (+ bias).  bf16 CUDA tensors run the wgmma GEMM, the bias in its epilogue.
 
-
-def fused_linear(x, w, owner=None, bias=None, bias_owner=None):
-    """``linear`` over a fused weight (q|k|v or gate|up).  ``owner`` is the
-    ``models.llama.FusedWeight`` carrying the flat-gradient view, or None when ``w`` is an
-    ordinary autograd tensor (e.g. a ``torch.cat`` of the individual parameters).  ``bias`` /
-    ``bias_owner``: the fused bias (q|k|v, Qwen2) and what carries its flat-gradient view, likewise."""
+    ``owner`` is what carries ``w``'s flat-gradient view: the ``models.llama.FusedWeight`` of a fused weight (q|k|v or
+    gate|up), or None for ``w`` itself (a parameter, or an ordinary autograd tensor such as a ``torch.cat`` of the
+    members).  ``bias_owner`` likewise for ``bias``.  ``fp8``: forward, dgrad and wgrad in fp8 (``_FP8Linear``); the
+    bias gradient is summed from the bf16 output gradient, and CPU tensors run the same quantisation through
+    ``ops/reference.py``."""
+    owner = w if owner is None else owner
+    args = (x, w, owner) if bias is None else (x, w, owner, bias, bias_owner)
+    if fp8:
+        return _FP8Linear.apply(*args)
     if _ext.use_cuda_kernel("gemm", x, w) and x.dtype == torch.bfloat16:
-        if bias is None:
-            return _Linear.apply(x, w, owner if owner is not None else w)
-        return _Linear.apply(x, w, owner if owner is not None else w, bias, bias_owner)
+        return _Linear.apply(*args)
     return ref.linear(x, w, bias)
 
 
@@ -311,16 +307,6 @@ def _fp8_linear_grads(dy8, dy8t, sdy, x8t, sx, w, amax_w, w_param, x_shape, dtyp
             w_param,
         )
     return dx, dw
-
-
-def fp8_linear(x, w, owner=None, bias=None, bias_owner=None):
-    """``linear`` with fp8 GEMMs (forward, dgrad and wgrad).  ``owner`` is what carries the flat-gradient view: the
-    ``models.llama.FusedWeight`` of a fused weight, or the parameter itself; None when ``w`` is an ordinary autograd
-    tensor.  ``bias`` / ``bias_owner`` likewise for a bias added in the forward GEMM's epilogue; its gradient is
-    summed from the bf16 output gradient.  CPU tensors run the same quantisation through ``ops/reference.py``."""
-    if bias is None:
-        return _FP8Linear.apply(x, w, owner if owner is not None else w)
-    return _FP8Linear.apply(x, w, owner if owner is not None else w, bias, bias_owner)
 
 
 # --------------------------------------------------------------------------------------

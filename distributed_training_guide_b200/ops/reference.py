@@ -9,7 +9,7 @@ These serve two roles and are never a second GPU backend:
 Semantics follow what the reference guide gets from ``transformers`` (SURVEY.md §3.2 /
 K1-K9): RMSNorm with fp32 statistics, half-rotation RoPE, causal softmax attention
 with GQA (optionally document-masked and / or sliding-window), SwiGLU, shifted-label mean cross-entropy with ``ignore_index=-100``.  The fp8 functions define the
-quantisation of ``ops.fp8_linear`` (per-tensor current scaling) exactly, so the cast kernels are tested bit for bit.
+quantisation of ``ops.linear(..., fp8=True)`` (per-tensor current scaling) exactly, so the cast kernels are tested bit for bit.
 """
 from __future__ import annotations
 

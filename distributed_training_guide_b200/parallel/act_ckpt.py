@@ -12,11 +12,6 @@ from __future__ import annotations
 import torch
 
 
-def _doc(doc_start):
-    # the tensor-parallel layer adapter takes no doc_start: pass it only when there is one
-    return () if doc_start is None else (doc_start,)
-
-
 class _CheckpointLayer(torch.autograd.Function):
     @staticmethod
     def forward(ctx, layer, cos, sin, doc_start, x, residual):
@@ -24,7 +19,7 @@ class _CheckpointLayer(torch.autograd.Function):
         ctx.has_res = residual is not None
         ctx.save_for_backward(x, *([residual] if residual is not None else []))
         with torch.no_grad():
-            out, res = layer(x, residual, cos, sin, *_doc(doc_start))
+            out, res = layer(x, residual, cos, sin, doc_start)
         return out, res
 
     @staticmethod
@@ -33,7 +28,7 @@ class _CheckpointLayer(torch.autograd.Function):
         x = saved[0].detach().requires_grad_(True)
         residual = saved[1].detach().requires_grad_(True) if ctx.has_res else None
         with torch.enable_grad():
-            out, res = ctx.layer(x, residual, ctx.cos, ctx.sin, *_doc(ctx.doc_start))
+            out, res = ctx.layer(x, residual, ctx.cos, ctx.sin, ctx.doc_start)
         outs, grads = [], []
         for o, g in ((out, d_out), (res, d_res)):
             if g is not None and o.requires_grad:

@@ -119,16 +119,14 @@ class FlatGroup:
 
 
 def install_fused_views(layer, g: FlatGroup, i: int):
-    """Give decoder layer ``i`` its fused weights (its class's ``FUSED``: q|k|v, and gate|up where the layer has
-    one) and, with q/k/v biases, the fused q|k|v bias, as views of its flat group ``g``."""
-    from ..models.llama import FusedWeight, LlamaDecoderLayer
+    """Give decoder layer ``i`` its fused weights (``layer.fused``: q|k|v, gate|up where the layer has one and the
+    q|k|v bias where it has biases) as views of its flat group ``g``."""
+    from ..models.llama import FusedWeight
 
-    for fname, members in type(layer).FUSED.items():
-        data, grad = g.fused_view([f"model.layers.{i}.{m}" for m in members])
+    for fname, members in layer.fused.items():
+        names = [f"model.layers.{i}.{m}" for m in members]
+        data, grad = g.fused_view_1d(names) if fname == "qkv_bias" else g.fused_view(names)
         layer._fused[fname] = g.fused[fname] = FusedWeight(data, grad)
-    if layer.self_attn.q_proj.bias is not None:
-        data, grad = g.fused_view_1d([f"model.layers.{i}.{m}" for m in LlamaDecoderLayer.QKV_BIAS_ORDER])
-        layer._fused["qkv_bias"] = g.fused["qkv_bias"] = FusedWeight(data, grad)
 
 
 def build_groups(model: nn.Module, device, dtype, world_size: int = 1, alloc=None, direct_write=None,

@@ -278,7 +278,7 @@ class FSDPEngine:
         def spec(g, holder, off, numel, rows, cols):
             holder._dtg_gather = _GatherSpec(self, g, off, numel, rows, cols)
 
-        fused_of = {l._flat_group.name: type(l).FUSED for l in self.layers}   # each layer's own fused weights
+        fused_of = {l._flat_group.name: l.fused for l in self.layers}   # each layer's own fused weights
         for g in self.groups:
             g._gathered, g._full_now = set(), False
             if not g.chunk_bytes:

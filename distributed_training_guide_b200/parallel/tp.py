@@ -367,76 +367,35 @@ class _VocabParallelCE(torch.autograd.Function):
 # model / layer forward under tensor parallelism
 # ------------------------------------------------------------------------------------------------
 class TensorParallelRuntime:
-    """Installed as ``model.tp`` and ``layer.tp``: owns the TP forward of the Llama model."""
+    """Installed as ``model.tp`` (and so ``layer.tp``): owns the TP forward of the Llama model."""
 
     def __init__(self, ctx: TPContext):
         self.ctx = ctx
 
-    def fused(self, layer, name, members):
-        f = layer._fused.get(name)
-        if f is not None:
-            return f.data, f
-        return torch.cat([m.weight for m in members], dim=0), None
-
-    def fused_bias(self, layer):
-        """(q|k|v bias slice, its flat-gradient owner); (None, None) without biases."""
-        att = layer.self_attn
-        if att.q_proj.bias is None:
-            return None, None
-        f = layer._fused.get("qkv_bias")
-        if f is not None:
-            return f.data, f
-        return torch.cat([att.q_proj.bias, att.k_proj.bias, att.v_proj.bias]), None
-
-    def layer_forward(self, layer, x, residual, cos, sin, B, S):
+    def layer_forward(self, layer, x, residual, cos, sin):
         """x, residual: sequence shards [T/t, H]; returns (mlp_out_local, residual_local)."""
         tp = self.ctx
         att, mlp = layer.self_attn, layer.mlp
         y, h = layer.input_layernorm(x, residual)
-        w, owner = self.fused(layer, "qkv", (att.q_proj, att.k_proj, att.v_proj))
-        b, b_owner = self.fused_bias(layer)
+        w, owner = layer.fused_weight("qkv")
+        b, b_owner = layer.fused_weight("qkv_bias")
         qkv = _ColumnParallelLinear.apply(y, w, owner, tp, 2 * layer.layer_idx, b, b_owner)
-        qkv = qkv.view(B, S, att.num_heads + 2 * att.num_kv_heads, att.head_dim)
-        qkv = att.position_qk_(qkv, cos, sin)
-        a = ops.attention_qkv(qkv, att.num_heads, att.num_kv_heads, window=att.sliding_window)
-        a = a.reshape(B * S, att.num_heads * att.head_dim)
+        S = cos.shape[-2]   # the tables are [S, d/2], or [B, S, d/2] from position ids
+        a = att.attend(qkv.view(-1, S, qkv.shape[-1]), cos, sin).flatten(0, 1)
         h2 = _RowParallelLinear.apply(a, att.o_proj.weight, att.o_proj.weight, tp, h)   # residual add fused
         y2, _ = layer.post_attention_layernorm(h2, None)
-        w, owner = self.fused(layer, "gate_up", (mlp.gate_proj, mlp.up_proj))
+        w, owner = layer.fused_weight("gate_up")
         gu = _ColumnParallelLinear.apply(y2, w, owner, tp, 2 * layer.layer_idx + 1)
         act = ops.swiglu(gu)
         out = _RowParallelLinear.apply(act, mlp.down_proj.weight, mlp.down_proj.weight, tp, None)
         return out, h2
 
-    def model_forward(self, model, input_ids, labels, position_ids):
+    def model_forward(self, model, input_ids, labels, cos, sin):
         tp = self.ctx
-        B, S = input_ids.shape
-        T = B * S
+        T = input_ids.numel()
         assert T == tp.max_tokens, f"tensor-parallel buffers were sized for {tp.max_tokens} tokens, got {T}"
-        m = model.model
-        if position_ids is None:
-            cos, sin = m.rotary_emb.tables(S, input_ids.device)
-        else:
-            cos, sin = m.rotary_emb(position_ids)
-        eng = model.engine
-        if eng is not None:
-            eng.pre_forward(model)
-        x = _HiddenParallelEmbedding.apply(input_ids, m.embed_tokens.weight, tp)
-        residual = None
-        for i, layer in enumerate(m.layers):
-            if eng is not None:
-                x, residual = eng.pre_layer(i, layer, x, residual)
-            if model.activation_checkpointing and torch.is_grad_enabled():
-                from .act_ckpt import checkpoint_layer
-
-                x, residual = checkpoint_layer(_LayerCall(self, layer, B, S), x, residual, cos, sin)
-            else:
-                x, residual = self.layer_forward(layer, x, residual, cos, sin, B, S)
-            if eng is not None:
-                x, residual = eng.post_layer(i, layer, x, residual)
-        if eng is not None:
-            x, residual = eng.pre_head(x, residual)
-        y, _ = m.norm(x, residual)
+        y = model.decoder(input_ids, cos, sin,
+                          embed=lambda ids: _HiddenParallelEmbedding.apply(ids, model.model.embed_tokens.weight, tp))
         logits = _ColumnParallelLinear.apply(y, model.lm_head.weight, model.lm_head.weight, tp, 2 * tp.n_layers)
         loss = None
         if labels is not None:
@@ -445,13 +404,3 @@ class TensorParallelRuntime:
             loss = _VocabParallelCE.apply(logits, tgt, tp, v0)
             logits = None
         return SimpleNamespace(loss=loss, logits=logits)
-
-
-class _LayerCall:
-    """Adapter so activation checkpointing can re-run a tensor-parallel layer."""
-
-    def __init__(self, rt, layer, B, S):
-        self.rt, self.layer, self.B, self.S = rt, layer, B, S
-
-    def __call__(self, x, residual, cos, sin):
-        return self.rt.layer_forward(self.layer, x, residual, cos, sin, self.B, self.S)

@@ -89,7 +89,7 @@ def test_fp8_linear_forward_and_backward_follow_the_recipe():
     x = torch.randn(2, 16, 64, generator=g).to(torch.bfloat16).requires_grad_()
     w = (0.05 * torch.randn(48, 64, generator=g)).to(torch.bfloat16).requires_grad_()
     dy = (1e-3 * torch.randn(2, 16, 48, generator=g)).to(torch.bfloat16)
-    y = ops.fp8_linear(x, w)
+    y = ops.linear(x, w, fp8=True)
     y.backward(dy)
 
     x8, sx = ref.fp8_quantize(x.detach().reshape(32, 64), E4M3)
@@ -119,11 +119,11 @@ def test_fp8_linear_writes_into_the_flat_gradient_view():
     w._dtg_writes = 0
     x = torch.randn(16, 64, generator=g).to(torch.bfloat16)
     dy = torch.randn(16, 32, generator=g).to(torch.bfloat16)
-    ops.fp8_linear(x.requires_grad_(), w.requires_grad_()).backward(dy)
+    ops.linear(x.requires_grad_(), w.requires_grad_(), fp8=True).backward(dy)
     first = w._dtg_grad.clone()
     assert w.grad is None and w._dtg_writes == 1
     assert torch.equal(buf[:8], torch.full((8,), 7.0, dtype=torch.bfloat16))
-    ops.fp8_linear(x, w).backward(dy)
+    ops.linear(x, w, fp8=True).backward(dy)
     assert w._dtg_writes == 2
     assert torch.allclose(w._dtg_grad.float(), 2 * first.float(), rtol=1e-2)
 
@@ -165,19 +165,19 @@ def test_fp8_is_off_by_default_and_routes_the_projections():
     from distributed_training_guide_b200.engine import TrainEngine
 
     calls = []
-    real = ops.fp8_linear
+    real = ops.linear
     eng = TrainEngine.create("debug-llama", parallelism="single", batch_size=2, seq_length=32, device="cpu")
     assert eng.model.fp8 is False and not any(layer.fp8 for layer in eng.model.model.layers)
     eng_fp8 = TrainEngine.create("debug-llama", parallelism="single", batch_size=2, seq_length=32, device="cpu",
                                  fp8=True)
     assert all(layer.fp8 for layer in eng_fp8.model.model.layers)
     try:
-        ops.fp8_linear = lambda *a, **k: calls.append(a[1].shape) or real(*a, **k)
+        ops.linear = lambda *a, **k: (k.get("fp8") and calls.append(a[1].shape)) or real(*a, **k)
         eng.step(eng.synthetic_batch(seed=0, pinned=False))
         assert calls == []
         eng_fp8.step(eng_fp8.synthetic_batch(seed=0, pinned=False))
     finally:
-        ops.fp8_linear = real
+        ops.linear = real
     assert len(calls) == 4 * eng_fp8.config.num_hidden_layers
 
 

@@ -313,13 +313,22 @@ def test_chapter04_checkpoint_consolidates_to_a_strict_gpt_neox_state_dict(tmp_p
 # flat layout and the layer
 # ---------------------------------------------------------------------------------------------------------------
 def test_flat_order_holds_every_parameter_with_the_matrices_first():
-    from distributed_training_guide_b200.models.llama import GPTNeoXDecoderLayer, Starcoder2DecoderLayer
+    from distributed_training_guide_b200.models.llama import LayerNorm, Starcoder2MLP
     from distributed_training_guide_b200.parallel.flat import build_groups
 
     model = build_model(get_config("debug-gpt-neox"), dtype=torch.bfloat16, device="cpu")
     layer = model.model.layers[0]
-    assert type(layer) is GPTNeoXDecoderLayer and layer.flat_order == Starcoder2DecoderLayer.FLAT_ORDER
+    # StarCoder2's parameters with the parallel residual and the exact GELU
+    assert isinstance(layer.input_layernorm, LayerNorm) and isinstance(layer.post_attention_layernorm, LayerNorm)
+    assert isinstance(layer.mlp, Starcoder2MLP) and layer.gelu_exact
+    assert layer.parallel_residual and not layer.post_norm
     order = layer.flat_order
+    assert order == ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight",
+                     "self_attn.o_proj.weight", "mlp.c_fc.weight", "mlp.c_proj.weight", "input_layernorm.weight",
+                     "input_layernorm.bias", "post_attention_layernorm.weight", "post_attention_layernorm.bias",
+                     "self_attn.q_proj.bias", "self_attn.k_proj.bias", "self_attn.v_proj.bias",
+                     "self_attn.o_proj.bias", "mlp.c_fc.bias", "mlp.c_proj.bias")
+    assert layer.fused == {"qkv": order[:3], "qkv_bias": order[10:13]}
     assert set(order) == {n for n, _ in layer.named_parameters()} and len(order) == len(set(order))
     named = dict(layer.named_parameters())
     dims = [named[n].dim() for n in order]

@@ -225,7 +225,6 @@ def test_pretrained_hf_olmo2_checkpoint_loads(tmp_path):
 # flat layout
 # ---------------------------------------------------------------------------------------------------------------
 def test_flat_order_holds_every_parameter_with_the_matrices_first():
-    from distributed_training_guide_b200.models.llama import LlamaDecoderLayer
     from distributed_training_guide_b200.parallel.flat import build_groups
 
     model = build_model(get_config("debug-olmo2"), dtype=torch.bfloat16, device="cpu")
@@ -236,9 +235,11 @@ def test_flat_order_holds_every_parameter_with_the_matrices_first():
     named = dict(layer.named_parameters())
     dims = [named[n].dim() for n in order]
     assert dims == sorted(dims, reverse=True), "matrices first"
-    assert order[:3] == LlamaDecoderLayer.FUSED["qkv"] and order[4:6] == LlamaDecoderLayer.FUSED["gate_up"]
-    assert order[7:] == ("post_attention_layernorm.weight", "post_feedforward_layernorm.weight",
-                         "self_attn.q_norm.weight", "self_attn.k_norm.weight")
+    assert order == ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight",
+                     "self_attn.o_proj.weight", "mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight",
+                     "post_attention_layernorm.weight", "post_feedforward_layernorm.weight",
+                     "self_attn.q_norm.weight", "self_attn.k_norm.weight")
+    assert layer.fused == {"qkv": order[:3], "gate_up": order[4:6]}
     assert all(named[n].numel() % 8 == 0 for n in order)
     groups = build_groups(model, "cpu", torch.bfloat16)
     assert len({id(p) for g in groups for p in g.params}) == len(list(model.parameters()))
@@ -249,7 +250,10 @@ def test_flat_order_holds_every_parameter_with_the_matrices_first():
     assert layer._fused["gate_up"].data.shape == (2 * 1024, 512)
     # a Llama layer's order is unchanged
     llama = build_model(get_config("debug-llama-gqa"), dtype=torch.bfloat16, device="meta")
-    assert llama.model.layers[0].flat_order == LlamaDecoderLayer.FLAT_ORDER
+    assert llama.model.layers[0].flat_order == (
+        "self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight", "self_attn.o_proj.weight",
+        "mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight", "input_layernorm.weight",
+        "post_attention_layernorm.weight")
 
 
 def test_layers_complete_the_stream_and_model_norm_finishes():

@@ -95,7 +95,7 @@ def test_linear_bias_op_cpu_path():
     g = torch.Generator().manual_seed(0)
     x, w, b = torch.randn(3, 5, 16, generator=g), torch.randn(24, 16, generator=g), torch.randn(24, generator=g)
     torch.testing.assert_close(ops.linear(x, w, b), torch.nn.functional.linear(x, w, b))
-    torch.testing.assert_close(ops.fused_linear(x, w, None, b), torch.nn.functional.linear(x, w, b))
+    torch.testing.assert_close(ops.linear(x, w, b, owner=w, bias_owner=b), torch.nn.functional.linear(x, w, b))
     torch.testing.assert_close(ops.bias_grad(x.reshape(-1, 16)), x.reshape(-1, 16).sum(0))
     out = torch.zeros(15, 24)
     ops.gemm(x.reshape(-1, 16), w, out=out, trans_b=True, bias=b)
@@ -222,7 +222,13 @@ def test_flat_groups_hold_one_qkv_bias_view_after_the_layer_norms():
     tail = [n.split(".", 3)[-1] for n in layer.names[-5:]]
     assert tail == ["input_layernorm.weight", "post_attention_layernorm.weight", "self_attn.q_proj.bias",
                     "self_attn.k_proj.bias", "self_attn.v_proj.bias"]
-    fw = model.model.layers[0]._fused["qkv_bias"]
+    l0 = model.model.layers[0]
+    assert l0.flat_order == ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight",
+                             "self_attn.o_proj.weight", "mlp.gate_proj.weight", "mlp.up_proj.weight",
+                             "mlp.down_proj.weight", "input_layernorm.weight", "post_attention_layernorm.weight",
+                             "self_attn.q_proj.bias", "self_attn.k_proj.bias", "self_attn.v_proj.bias")
+    assert l0.fused == {"qkv": l0.flat_order[:3], "gate_up": l0.flat_order[4:6], "qkv_bias": l0.flat_order[9:]}
+    fw = l0._fused["qkv_bias"]
     nq, nkv = cfg.num_attention_heads * cfg.head_dim, cfg.num_key_value_heads * cfg.head_dim
     assert fw.data.shape == (nq + 2 * nkv,) and fw._dtg_grad.shape == (nq + 2 * nkv,)
     a = model.model.layers[0].self_attn
@@ -235,7 +241,12 @@ def test_flat_groups_hold_one_qkv_bias_view_after_the_layer_norms():
     for name in ("debug-llama-gqa", "debug-mistral", "debug-qwen3"):
         other = build_model(get_config(name), dtype=torch.bfloat16, device="meta")
         l0 = other.model.layers[0]
-        assert l0.flat_order[:9] == l0.FLAT_ORDER and not any(n.endswith(".bias") for n in l0.flat_order)
+        assert l0.flat_order[:9] == ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight",
+                                     "self_attn.o_proj.weight", "mlp.gate_proj.weight", "mlp.up_proj.weight",
+                                     "mlp.down_proj.weight", "input_layernorm.weight",
+                                     "post_attention_layernorm.weight")
+        assert not any(n.endswith(".bias") for n in l0.flat_order)
+        assert "qkv_bias" not in l0.fused
 
 
 def test_tp_shard_spec_splits_the_biases_with_their_heads():

@@ -228,7 +228,14 @@ def test_flat_groups_hold_the_qk_norm_gains_after_the_layer_norms():
     assert len({id(p) for g in groups for p in g.params}) == len(list(model.parameters()))
     # a Llama layer's order is unchanged
     llama = build_model(get_config("debug-llama-gqa"), dtype=torch.bfloat16, device="meta")
-    assert llama.model.layers[0].flat_order == llama.model.layers[0].FLAT_ORDER
+    llama_order = ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight",
+                   "self_attn.o_proj.weight", "mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight",
+                   "input_layernorm.weight", "post_attention_layernorm.weight")
+    assert llama.model.layers[0].flat_order == llama_order
+    assert llama.model.layers[0].fused == {"qkv": llama_order[:3], "gate_up": llama_order[4:6]}
+    l0 = model.model.layers[0]
+    assert l0.flat_order == llama_order + ("self_attn.q_norm.weight", "self_attn.k_norm.weight")
+    assert l0.fused == {"qkv": llama_order[:3], "gate_up": llama_order[4:6]}
 
 
 # ---------------------------------------------------------------------------------------------------------------

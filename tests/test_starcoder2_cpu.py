@@ -273,12 +273,15 @@ def test_chapter04_checkpoint_consolidates_to_hf_names(tmp_path):
 # flat layout
 # ---------------------------------------------------------------------------------------------------------------
 def test_flat_order_holds_every_parameter_with_the_matrices_first():
-    from distributed_training_guide_b200.models.llama import LlamaDecoderLayer, Starcoder2DecoderLayer
+    from distributed_training_guide_b200.models.llama import LayerNorm, Starcoder2MLP
     from distributed_training_guide_b200.parallel.flat import build_groups
 
     model = build_model(get_config("debug-starcoder2"), dtype=torch.bfloat16, device="cpu")
     layer = model.model.layers[0]
-    assert type(layer) is Starcoder2DecoderLayer
+    # LayerNorms, the c_fc -> GELU-tanh -> c_proj MLP and the pre-norm residual with its add deferred
+    assert isinstance(layer.input_layernorm, LayerNorm) and isinstance(layer.post_attention_layernorm, LayerNorm)
+    assert isinstance(layer.mlp, Starcoder2MLP) and not layer.gelu_exact
+    assert not layer.post_norm and not layer.parallel_residual
     order = layer.flat_order
     assert set(order) == {n for n, _ in layer.named_parameters()} and len(order) == len(set(order))
     named = dict(layer.named_parameters())
@@ -288,7 +291,8 @@ def test_flat_order_holds_every_parameter_with_the_matrices_first():
                          "self_attn.o_proj.weight", "mlp.c_fc.weight", "mlp.c_proj.weight")
     assert order[6:10] == ("input_layernorm.weight", "input_layernorm.bias", "post_attention_layernorm.weight",
                            "post_attention_layernorm.bias")
-    assert order[10:13] == LlamaDecoderLayer.QKV_BIAS_ORDER
+    assert order[10:13] == ("self_attn.q_proj.bias", "self_attn.k_proj.bias", "self_attn.v_proj.bias")
+    assert layer.fused == {"qkv": order[:3], "qkv_bias": order[10:13]}
     assert order[13:] == ("self_attn.o_proj.bias", "mlp.c_fc.bias", "mlp.c_proj.bias")
     assert all(named[n].numel() % 8 == 0 for n in order)
     groups = build_groups(model, "cpu", torch.bfloat16)
@@ -302,7 +306,10 @@ def test_flat_order_holds_every_parameter_with_the_matrices_first():
     with pytest.raises(AssertionError, match="outside flat_order"):
         build_groups(model, "cpu", torch.bfloat16)
     llama = build_model(get_config("debug-llama-gqa"), dtype=torch.bfloat16, device="meta")
-    assert llama.model.layers[0].flat_order == LlamaDecoderLayer.FLAT_ORDER
+    assert llama.model.layers[0].flat_order == (
+        "self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight", "self_attn.o_proj.weight",
+        "mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight", "input_layernorm.weight",
+        "post_attention_layernorm.weight")
 
 
 def test_layer_equals_the_reference_ops_and_defers_the_add():
