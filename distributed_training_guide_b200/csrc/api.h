@@ -148,6 +148,36 @@ void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int 
                   bool b_kmajor, int nranks, int rank, int rows_per_peer, uint32_t* flags, uint32_t ag_epoch,
                   uint32_t* const* pads, uint32_t bar_epoch, int n_comm, cudaStream_t s, const void* bias = nullptr);
 
+// Grouped GEMM of the mixture-of-experts layers, one launch for every expert (see gemm_wgmma.cu for the modes);
+// seg [groups + 1] and tile_expert [rows / 128] are the device tables moe_route writes.
+void gemm_bf16_grouped(int mode, const void* A, const void* B, void* C, int M, int N, int K, long long lda,
+                       long long ldb, long long ldc, int groups, const int* seg, const int* tile_expert,
+                       bool accumulate, cudaStream_t s);
+
+// ---- moe.cu --------------------------------------------------------------------------------
+// Routing of T tokens over E <= kMoeMaxExperts experts, top-k (see moe.cu for the layout).  rows_cap = the most
+// permuted rows any routing can need, T * k + E * 127 rounded up to 128; scratch: int32 [moe_route_scratch(T, E)].
+constexpr int kMoeMaxExperts = 256;
+long long moe_rows_cap(long long T, int E, int k);
+long long moe_route_scratch(long long T, int E);
+// From bf16 router logits [T, E] (row stride ldl): p fp32 [T, E] (softmax), idx int32 [T, k], w fp32 [T, k] (the
+// top-k probabilities, ties to the lower expert), pos int32 [T, k], seg int32 [E + 1], tile_expert int32
+// [rows_cap / 128], row_tok int32 [rows_cap] (rows below seg[E]) and counts int32 [E].
+void moe_route(const void* logits, long long ldl, int T, int E, int k, float* p, int* idx, float* w, int* pos,
+               int* seg, int* tile_expert, int* row_tok, int* counts, int* scratch, cudaStream_t s);
+// out [rows_cap, H]: row r < seg[E] is x [T, H]'s row of its token, or zeros on a padding row
+void moe_permute(const void* x, const int* row_tok, const int* seg, int E, int k, int H, long long rows_cap, void* out,
+                 cudaStream_t s);
+// out [T, H] = bf16(sum over slots, in slot order, of w * yp[pos]) in fp32; w null: weights 1 (the input gradient)
+void moe_combine(const void* yp, const int* pos, const float* w, int T, int k, int H, void* out, cudaStream_t s);
+// The combine's backward: dyp [rows_cap, H] row r < seg[E] = bf16(w[a] * dy[t]) (zeros on padding rows) and dw fp32
+// [T, k] = sum_h dy[t, h] * yp[r, h], for a = row_tok[r] and t = a / k
+void moe_combine_bwd(const void* dy, const void* yp, const int* row_tok, const int* seg, const float* w, int E, int k,
+                     int H, long long rows_cap, void* dyp, float* dw, cudaStream_t s);
+// dlogits bf16 [T, E] = bf16(p * (dp - sum_e p dp)) with dp = dw at the selected experts, plus dpsum [E] (null: 0)
+void moe_router_bwd(const float* p, const int* idx, const float* dw, const float* dpsum, int T, int E, int k,
+                    void* dlogits, cudaStream_t s);
+
 // ---- fp8.cu --------------------------------------------------------------------------------
 // amax[0] = max |x| of a bf16 [R, C] matrix with row stride ld (elements), on the device.
 void fp8_amax(const void* x, long long R, int C, long long ld, float* amax, cudaStream_t s);

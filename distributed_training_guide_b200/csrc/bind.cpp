@@ -624,4 +624,5 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   dtg::bind_tp(m);
   dtg::bind_dataloader(m);
   dtg::bind_symm_vmm(m);
+  dtg::bind_moe(m);
 }

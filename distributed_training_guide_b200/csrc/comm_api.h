@@ -18,4 +18,5 @@ void bind_attention(pybind11::module_& m);
 void bind_tp(pybind11::module_& m);
 void bind_dataloader(pybind11::module_& m);
 void bind_symm_vmm(pybind11::module_& m);
+void bind_moe(pybind11::module_& m);
 }  // namespace dtg

@@ -48,15 +48,23 @@ struct TmapSet {
   CUtensorMap m[N];
 };
 
-// Geometry of a tensor-parallel GEMM (all zero / unused for the plain GEMM)
+// Geometry of a tensor-parallel GEMM (all zero / unused for the plain GEMM).  The grouped GEMM of the
+// mixture-of-experts layers (C_MODE 2 / 3) shares the storage of fields it never uses for its routing tables, so the
+// kernels' parameter layout is the same for every mode.
 struct GemmDist {
-  int rows_per_peer;                 // rows (M- or K-direction) each rank contributes / owns
+  union {
+    int rows_per_peer;               // rows (M- or K-direction) each rank contributes / owns
+    int grp_b_rows;                  // grouped forward / dgrad: rows of one expert's slab of B as stored
+  };
   int m_tile_shift;                  // rotate the M tile order so every rank starts on its own rows
   int k_shift;                       // rotate the K block order likewise
   __nv_bfloat16* c_ptr[kMaxRanks];   // C_MODE 1: destination base (already offset to my slot) per owner
   // A_MODE 3 (all-gather by communication CTAs inside the GEMM kernel)
   const char* ag_src[kMaxRanks];     // the symmetric [M, K] buffer on every rank, ROTATED: [0] = mine
-  uint32_t* ag_flags;                // local: one word per 256-row tile, set to ag_epoch once the tile landed
+  union {
+    uint32_t* ag_flags;              // local: one word per 256-row tile, set to ag_epoch once the tile landed
+    const int* grp_tile_expert;      // grouped forward / dgrad: int32 [rows / 128], the expert of each row tile, or -1
+  };
   uint32_t ag_epoch;
   uint32_t* pads[kMaxRanks];         // signal pads (not rotated) for the start-of-kernel barrier
   uint32_t bar_epoch;
@@ -71,7 +79,10 @@ struct GemmDist {
   char* bg_dst;                      // local full (unsharded) flat buffer of the group
   long long bg_per_bytes;            // shard size in bytes
   long long bg_begin, bg_end;        // flat byte range of B (piece aligned; chunk aligned at both ends)
-  uint32_t* bg_cnt;                  // one counter per chunk of the flat buffer (monotonic over generations)
+  union {
+    uint32_t* bg_cnt;                // one counter per chunk of the flat buffer (monotonic over generations)
+    const int* grp_seg;              // grouped: int32 [experts + 1], expert e owns rows [seg[e], seg[e + 1])
+  };
   uint32_t bg_target;                // counter value at which a chunk of this generation is complete
   int bg_chunk_shift;                // log2(chunk bytes)
   int bg_row_bytes;                  // bytes of one row of B as stored (ldb * 2)

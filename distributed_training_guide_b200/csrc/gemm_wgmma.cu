@@ -43,7 +43,7 @@ using namespace ptx;
 //                    acquire the flag before their TMA touches a fetched tile.  Each remote byte crosses NVLink
 //                    exactly once (peer memory bypasses the local L2, so mode 1 re-fetches it per N tile).
 //   C_MODE           0 = local C;  1 = each `rows_per_peer` row chunk of C is stored into its owner's
-//                    staging buffer (GEMM -> reduce-scatter push).
+//                    staging buffer (GEMM -> reduce-scatter push);  2 and 3 = the grouped GEMM (GRP 1 and 2 below).
 //
 // Epilogue.  A local C (C_MODE 0) leaves through shared memory: each consumer warpgroup converts half of its 64 x 256
 // accumulator block at a time into a 32 KB staging area and one thread stores it with two TMA boxes, which clip at M
@@ -52,7 +52,7 @@ using namespace ptx;
 // bounce ring already fills shared memory to within 2 KB of the limit), and so does C_MODE 1 (its rows go to the
 // peers' staging buffers, one base pointer per owner, which one tensor map cannot describe).
 template <int B_MODE, int C_MODE>
-constexpr bool kTmaEpilogue = (B_MODE != 3 && C_MODE == 0);
+constexpr bool kTmaEpilogue = (B_MODE != 3 && C_MODE != 1);
 // B_MODE 3 helpers.  Chunks are waited for in the order the gather warps fetch them: the chunks behind my own slice
 // of [bg_begin, bg_end) first, then the ones in front of it; my own chunks are local and never waited for.
 __device__ __forceinline__ long long bg_clamp(const GemmDist& d, long long x) {
@@ -74,6 +74,17 @@ __device__ __forceinline__ int bg_rotation_chunks(const GemmDist& d) {   // firs
 // accumulator fragment, so it reads one bf16 pair per block j of 8 columns, straight from global memory (L1 / L2
 // serve the 2 N bytes to all CTAs); N is a multiple of 8, so a block is wholly inside or outside [0, N).  Forward
 // layout only (A and B K-major), never together with accumulate.
+//
+// C_MODE 2 / 3 (GRP 1 / 2) is the grouped GEMM of the mixture-of-experts layers: one launch multiplies every
+// expert's rows by that expert's slab of the weights, reading the routing tables (dist.grp_*) from device memory, so
+// nothing waits on the host.  Single CTAs only (CG 1): a 128-row tile never straddles two experts, whose segments
+// start at multiples of 128.  The C tile leaves through the TMA epilogue of C_MODE 0.
+//   GRP 1  fwd / dgrad  C[rows, N] = A[rows, K] . B_e   A K-major; B_e is rows [e * grp_b_rows, (e + 1) * grp_b_rows)
+//                       of B as stored, e the expert of the row tile; tiles of no expert (past the last segment) are
+//                       skipped.
+//   GRP 2  wgrad        C_e[M, N] = A[seg_e, M]^T . B[seg_e, N]   A and B MN-major; the reduction runs over expert
+//                       e's rows only, and C_e is rows [e * M, (e + 1) * M) of C.  Tiles run over (expert, m, n).  An
+//                       expert without rows writes zeros in overwrite mode and leaves C_e untouched in accumulate mode.
 template <bool A_K, bool B_K, int CG, int A_MODE = 0, int B_MODE = 0, int C_MODE = 0, int ET = 0, bool BIAS = false>
 __global__ void __launch_bounds__(GemmCfg<CG>::THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
@@ -84,6 +95,10 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
   static_assert(ET == 0 || (A_K && B_K && A_MODE == 0 && B_MODE == 0 && C_MODE == 0),
                 "the fp8 GEMM takes K-major operands from one tensor map each");
   static_assert(!BIAS || (A_K && B_K && C_MODE == 0), "the bias epilogue serves the forward layout with a local C");
+  constexpr int GRP = C_MODE == 2 ? 1 : (C_MODE == 3 ? 2 : 0);
+  static_assert(GRP == 0 || (CG == 1 && A_MODE == 0 && B_MODE == 0 && ET == 0 && !BIAS &&
+                             (GRP == 1 ? A_K : (!A_K && !B_K))),
+                "the grouped GEMM is a plain bf16 single-CTA GEMM: GRP 1 with A K-major, GRP 2 with both MN-major");
   using Cfg = GemmCfg<CG>;
   constexpr bool TMA_EPI = kTmaEpilogue<B_MODE, C_MODE>;
   constexpr int BK = ET ? 2 * Cfg::BK : Cfg::BK;   // elements of K per stage: one 128-byte span either way
@@ -103,6 +118,23 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
   const int num_clusters = (int)(gridDim.x / CG) - n_comm;
   const int num_kb = (K + BK - 1) / BK;
   const int local_m_tiles = (A_MODE == 3) ? dist.rows_per_peer / (Cfg::BM * CG) : 0;
+  // GRP: tile t -> (m tile, n tile), its expert, the first reduction row (GRP 2) and its K blocks; false: no work
+  [[maybe_unused]] auto grp_tile = [&](int t, int& tm, int& tn, int& e, int& k_row0, int& kbs) -> bool {
+    if constexpr (GRP == 1) {
+      tile_mn(t, num_m_tiles, dist, 0, tm, tn);
+      e = dist.grp_tile_expert[tm];
+      k_row0 = 0;
+      kbs = num_kb;
+      return e >= 0;
+    } else {
+      const int per = num_m_tiles * dist.num_n_tiles;
+      e = t / per;
+      tile_mn(t - e * per, num_m_tiles, dist, 0, tm, tn);
+      k_row0 = dist.grp_seg[e];
+      kbs = (dist.grp_seg[e + 1] - k_row0) / BK;
+      return kbs > 0 || !accumulate;
+    }
+  };
 
   if (threadIdx.x == 0) {
     prefetch_tensormap(&tmAs.m[0]);
@@ -211,9 +243,16 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
       };
       for (int t = cluster_id; t < num_tiles; t += num_clusters) {
         int tm_, tn_;
-        tile_mn(t, num_m_tiles, dist, local_m_tiles, tm_, tn_);
+        [[maybe_unused]] int g_e = 0, g_k0 = 0;
+        int tile_kb = num_kb;
+        if constexpr (GRP != 0) {
+          if (!grp_tile(t, tm_, tn_, g_e, g_k0, tile_kb)) continue;
+        } else {
+          tile_mn(t, num_m_tiles, dist, local_m_tiles, tm_, tn_);
+        }
         const int m0 = tm_ * (Cfg::BM * CG) + (int)cta_rank * Cfg::BM;
-        const int nb = tn_ * Cfg::BN + (int)cta_rank * Cfg::B_ROWS;   // the B rows this CTA loads (for the pair)
+        // the B rows this CTA loads (for the pair); GRP 1 forward: inside the expert's slab
+        const int nb = tn_ * Cfg::BN + (int)cta_rank * Cfg::B_ROWS + ((GRP == 1 && B_K) ? g_e * dist.grp_b_rows : 0);
         const CUtensorMap* tmA_p = &tmAs.m[0];
         int a_m0 = m0;
         if constexpr (A_MODE == 3) {  // fetched tile: wait until the communication CTAs published it
@@ -231,11 +270,16 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
           tmA_p = &tmAs.m[peer];
           a_m0 = m0 - peer * dist.rows_per_peer;
         }
-        for (int kbi = 0; kbi < num_kb; ++kbi) {
+        for (int kbi = 0; kbi < tile_kb; ++kbi) {
           // K-gathered operands start with the local rank's slice of K
           const int kb = (A_MODE == 2 || B_MODE == 2 || (B_MODE == 3 && !B_K)) ? (kbi + dist.k_shift) % num_kb : kbi;
           const int k0 = kb * BK;
           int a_k0 = k0, b_k0 = k0;
+          if constexpr (GRP == 2) {   // the expert's rows of both operands
+            a_k0 += g_k0;
+            b_k0 += g_k0;
+          }
+          if constexpr (GRP == 1 && !B_K) b_k0 += g_e * dist.grp_b_rows;   // dgrad: the expert's slab of B
           const CUtensorMap* tmB_p = &tmBs.m[0];
           if constexpr (A_MODE == 2) {
             const int peer = k0 / dist.rows_per_peer;
@@ -374,9 +418,16 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
     [[maybe_unused]] const int bar_id = 1 + half;   // named barrier of this warpgroup (0 is __syncthreads)
     for (int t = cluster_id; t < num_tiles; t += num_clusters) {
       int tm_, tn_;
-      tile_mn(t, num_m_tiles, dist, local_m_tiles, tm_, tn_);
+      [[maybe_unused]] int g_e = 0, g_k0 = 0;
+      int tile_kb = num_kb;
+      if constexpr (GRP != 0) {
+        if (!grp_tile(t, tm_, tn_, g_e, g_k0, tile_kb)) continue;
+      } else {
+        tile_mn(t, num_m_tiles, dist, local_m_tiles, tm_, tn_);
+      }
       const int m0 = tm_ * (Cfg::BM * CG) + (int)cta_rank * Cfg::BM + half * 64;
       const int n0 = tn_ * Cfg::BN;
+      const int cm0 = m0 + (GRP == 2 ? g_e * M : 0);   // row of C (GRP 2: inside the expert's block)
       // accumulate mode: fetch the first 128 columns of C under the mainloop.  The stores of the previous tile must
       // have read the staging area; every thread finished writing it before they were issued.
       // Boxes entirely outside C (rows >= M, columns >= N) are never loaded or stored.
@@ -385,14 +436,14 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
           const int nbox = n0 + 64 < N ? 2 : 1;
           tma_store_wait_read<0>();
           mbar_arrive_expect_tx(c_bar, nbox * Cfg::EPI_BOX_BYTES);
-          for (int b = 0; b < nbox; ++b) tma_load_2d(&tmC, c_bar, stg + b * Cfg::EPI_BOX_BYTES, n0 + 64 * b, m0);
+          for (int b = 0; b < nbox; ++b) tma_load_2d(&tmC, c_bar, stg + b * Cfg::EPI_BOX_BYTES, n0 + 64 * b, cm0);
         }
       }
       float acc[128];
 #pragma unroll
       for (int i = 0; i < 128; ++i) acc[i] = 0.f;
       int prev = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
+      for (int kb = 0; kb < tile_kb; ++kb) {
         mbar_wait_mma(&full[stage], phase);
         const uint32_t a_base = smem_u32(smem + stage * Cfg::STAGE_BYTES) + (uint32_t)(half * 8192);
         const uint32_t b_base = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
@@ -435,7 +486,7 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
             if (p == 1 && signal) {
               tma_store_wait_read<0>();   // the first half's stores have read the staging area
               mbar_arrive_expect_tx(c_bar, nbox * Cfg::EPI_BOX_BYTES);
-              for (int b = 0; b < nbox; ++b) tma_load_2d(&tmC, c_bar, stg + b * Cfg::EPI_BOX_BYTES, c0 + 64 * b, m0);
+              for (int b = 0; b < nbox; ++b) tma_load_2d(&tmC, c_bar, stg + b * Cfg::EPI_BOX_BYTES, c0 + 64 * b, cm0);
             }
             mbar_wait_mma(c_bar, c_phase);
             c_phase ^= 1;
@@ -487,7 +538,7 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
           fence_proxy_async();            // the generic-proxy writes are visible to the TMA store
           named_bar_sync(bar_id, 128);
           if (signal) {
-            for (int b = 0; b < nbox; ++b) tma_store_2d(&tmC, stg + b * Cfg::EPI_BOX_BYTES, c0 + 64 * b, m0);
+            for (int b = 0; b < nbox; ++b) tma_store_2d(&tmC, stg + b * Cfg::EPI_BOX_BYTES, c0 + 64 * b, cm0);
             tma_store_commit();
           }
         }
@@ -620,13 +671,15 @@ int default_gemm_variant() {
 
 // One launcher for the plain and the tensor-parallel GEMMs.  `a_srcs` / `b_srcs`: base pointer of the
 // operand on every rank (only [0] is used in mode 0); `dist.c_ptr` set by the caller for C_MODE 1.
+// C_MODE 2 and 3 (grouped): `groups` slabs of B (C_MODE 2) or blocks of C (C_MODE 3) follow one another in memory.
 template <bool A_K, bool B_K, int CG, int A_MODE, int B_MODE, int C_MODE, int ET = 0, bool BIAS = false>
 static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, void* C, int M, int N, int K,
                         long long lda, long long ldb, long long ldc, bool accumulate, GemmDist dist, int nranks,
                         cudaStream_t s, const float* scale_a = nullptr, const float* scale_b = nullptr,
-                        const void* bias = nullptr) {
+                        const void* bias = nullptr, int groups = 1) {
   using Cfg = GemmCfg<CG>;
   constexpr int ESIZE = ET ? 1 : 2;   // bytes per operand element
+  constexpr int GRP = C_MODE == 2 ? 1 : (C_MODE == 3 ? 2 : 0);
   TmapSet<(A_MODE ? kMaxRanks : 1)> tmA;
   TmapSet<(B_MODE ? kMaxRanks : 1)> tmB;
   const int rpp = dist.rows_per_peer;
@@ -639,16 +692,20 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
   for (int p = 0; p < ((B_MODE == 1 || B_MODE == 2) ? nranks : 1); ++p) {
     const int ks = (B_MODE == 2) ? rpp : K;
     if constexpr (ET != 0) tmB.m[p] = make_tmap_2d_u8(b_srcs[p], ks, N, ldb, 128, Cfg::B_ROWS);
+    else if constexpr (GRP == 1)   // every expert's slab: the one stacked extent
+      tmB.m[p] = B_K ? make_tmap_2d(b_srcs[p], ks, (uint64_t)N * groups, ldb * 2, 64, Cfg::B_ROWS)
+                     : make_tmap_2d(b_srcs[p], N, (uint64_t)ks * groups, ldb * 2, 64, 64);
     else tmB.m[p] = B_K ? make_tmap_2d(b_srcs[p], ks, N, ldb * 2, 64, Cfg::B_ROWS) : make_tmap_2d(b_srcs[p], N, ks, ldb * 2, 64, 64);
   }
   for (int p = ((A_MODE == 1 || A_MODE == 2) ? nranks : 1); p < (A_MODE ? kMaxRanks : 1); ++p) tmA.m[p] = tmA.m[0];
   for (int p = ((B_MODE == 1 || B_MODE == 2) ? nranks : 1); p < (B_MODE ? kMaxRanks : 1); ++p) tmB.m[p] = tmB.m[0];
   const int num_m_tiles = (M + Cfg::BM * CG - 1) / (Cfg::BM * CG);
   const int num_n_tiles = (N + Cfg::BN - 1) / Cfg::BN;
-  const int num_tiles = num_m_tiles * num_n_tiles;
+  const int num_tiles = num_m_tiles * num_n_tiles * (GRP == 2 ? groups : 1);
   // C in 64 x 64 boxes (the staging layout of the epilogue); the other modes store from registers
   CUtensorMap tmC{};
-  if constexpr (kTmaEpilogue<B_MODE, C_MODE>) tmC = make_tmap_2d(C, N, M, ldc * 2, 64, 64);
+  if constexpr (kTmaEpilogue<B_MODE, C_MODE>)
+    tmC = make_tmap_2d(C, N, (uint64_t)M * (GRP == 2 ? groups : 1), ldc * 2, 64, 64);
   auto kern = gemm_bf16_kernel<A_K, B_K, CG, A_MODE, B_MODE, C_MODE, ET, BIAS>;
   constexpr int kSmem = kTmaEpilogue<B_MODE, C_MODE> ? Cfg::SMEM_BYTES_EPI
                                                      : Cfg::SMEM_BYTES + (B_MODE == 3 ? Cfg::GATHER_BYTES : 0);
@@ -658,7 +715,7 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
     attr_set = true;
   }
   dist.num_n_tiles = num_n_tiles;
-  if constexpr (A_MODE == 0 && B_MODE == 0 && C_MODE == 0) {
+  if constexpr (A_MODE == 0 && B_MODE == 0 && C_MODE != 1) {
     // keep one group's panel of A (group_m x TM x K elements) within ~1/3 of the 50 MB L2; with very long K nothing
     // fits and a squarish block of 8 row tiles by (tiles in flight / 8) column tiles minimises the bytes each
     // wave touches
@@ -1003,6 +1060,48 @@ void gemm_bf16_bgather(const void* A, void* full_base, void* C, int M, int N, in
                                                           nullptr, nullptr, bias);
   else if (b_kmajor) launch_gemm<true, true, 2, 0, 3, 0>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s);
   else launch_gemm<true, false, 2, 0, 3, 0>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s);
+}
+
+// Grouped GEMM of the mixture-of-experts layers (GRP 1 and 2 above), one launch for every expert; the routing tables
+// seg [groups + 1] and tile_expert [rows / 128] are device pointers written by moe_route (moe.cu).
+//   mode 0  forward  C[R, N] = A[R, K] . B_e[N, K]^T       B = [groups * N, K]   R = rows (a multiple of 128)
+//   mode 1  dgrad    C[R, N] = A[R, K] . B_e[K, N]         B = [groups * K, N]   K % 64 == 0
+//   mode 2  wgrad    C_e[M, N] (+)= A[seg_e, M]^T . B[seg_e, N]   A [K, M], B [K, N], C = [groups * M, N]; K is the
+//                    row count of A and B (a multiple of 128), M % 128 == 0
+// Modes 0 and 1 overwrite, and write nothing in row tiles past the last segment.  Every refusal happens before a
+// launch.
+void gemm_bf16_grouped(int mode, const void* A, const void* B, void* C, int M, int N, int K, long long lda,
+                       long long ldb, long long ldc, int groups, const int* seg, const int* tile_expert,
+                       bool accumulate, cudaStream_t s) {
+  if (mode < 0 || mode > 2) throw std::runtime_error("gemm_bf16_grouped: mode must be 0 (forward), 1 (dgrad) or 2 (wgrad)");
+  if (groups < 1) throw std::runtime_error("gemm_bf16_grouped: groups must be >= 1");
+  if (M < 0 || N < 0 || K < 1) throw std::runtime_error("gemm_bf16_grouped: M, N >= 0 and K >= 1");
+  if ((N % 8) || (ldc % 8) || (lda % 8) || (ldb % 8))
+    throw std::runtime_error("gemm_bf16_grouped: N and the leading dimensions must be multiples of 8 elements");
+  if (mode != 2 && accumulate) throw std::runtime_error("gemm_bf16_grouped: the forward and dgrad modes overwrite");
+  if (mode != 2 && M % 128) throw std::runtime_error("gemm_bf16_grouped: the row count must be a multiple of 128");
+  if (mode == 1 && K % 64)
+    throw std::runtime_error("gemm_bf16_grouped: dgrad needs K % 64 == 0 (a K block never reaches the next expert)");
+  if (mode == 2 && (M % 128 || K % 128))
+    throw std::runtime_error("gemm_bf16_grouped: wgrad needs M % 128 == 0 and a row count K that is a multiple of 128");
+  if (!seg || (mode != 2 && !tile_expert)) throw std::runtime_error("gemm_bf16_grouped: missing routing table");
+  check_gemm_bases("gemm_bf16_grouped", A, B, C);
+  if (M == 0 || N == 0) return;
+  const void* as[1] = {A};
+  const void* bs[1] = {B};
+  GemmDist dist{};
+  dist.grp_seg = seg;
+  dist.grp_tile_expert = tile_expert;
+  dist.grp_b_rows = mode == 0 ? N : K;
+  if (mode == 0)
+    launch_gemm<true, true, 1, 0, 0, 2>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, 1, s, nullptr,
+                                                     nullptr, nullptr, groups);
+  else if (mode == 1)
+    launch_gemm<true, false, 1, 0, 0, 2>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, 1, s, nullptr,
+                                                      nullptr, nullptr, groups);
+  else
+    launch_gemm<false, false, 1, 0, 0, 3>(as, bs, C, M, N, K, lda, ldb, ldc, accumulate, dist, 1, s,
+                                                       nullptr, nullptr, nullptr, groups);
 }
 
 }  // namespace dtg

@@ -5,7 +5,7 @@ guide uses (reference: every chapter's ``-m/--model-name`` flag, e.g.
 ``02-distributed-data-parallel/train_llm.py:57``) are resolved from this table
 instead of the hub.  A local directory containing a ``config.json`` is also
 accepted, and tiny ``debug-*`` configs exist for tests.  Families: Llama 2 / 3 / 3.1 / 3.2, Mistral, Qwen3, Qwen2.5,
-OLMo 2 (``allenai/OLMo-2-*``, ``model_type: "olmo2"``), StarCoder2 (``bigcode/starcoder2-*``,
+OLMo 2 (``allenai/OLMo-2-*``, ``model_type: "olmo2"``), OLMoE (``allenai/OLMoE-*``, ``model_type: "olmoe"``), StarCoder2 (``bigcode/starcoder2-*``,
 ``model_type: "starcoder2"``), GPT-NeoX / Pythia (``EleutherAI/pythia-*``, ``model_type: "gpt_neox"``) and GPT-2.
 """
 from __future__ import annotations
@@ -23,7 +23,8 @@ class ModelConfig:
     # biases, olmo2 llama with a full-width QK-norm and post-sublayer norms instead of the pre-norms (``full_qk_norm``,
     # ``post_norm``), starcoder2 llama with LayerNorms, a GELU MLP and biases on every projection (``layer_norm``,
     # ``gelu_mlp``, ``all_bias``), gpt_neox starcoder2's block with a parallel residual, partial rotary embeddings
-    # and an exact GELU (``parallel_residual``, ``rotary_dim``, ``gelu_exact``)
+    # and an exact GELU (``parallel_residual``, ``rotary_dim``, ``gelu_exact``), olmoe llama with OLMo 2's full-width
+    # QK-norm (still pre-norm) and a mixture-of-experts MLP (``moe``)
     vocab_size: int
     hidden_size: int
     intermediate_size: int
@@ -49,6 +50,10 @@ class ModelConfig:
     #: share of each q/k head that RoPE rotates (GPT-NeoX's ``rotary_pct``); read it through ``rotary_dim``
     partial_rotary_factor: float = 1.0
     dropout: float = 0.0
+    #: mixture of experts (OLMoE): ``num_experts`` SwiGLU experts of ``intermediate_size`` each, and the
+    #: ``num_experts_per_tok`` of them with the highest router probability run on each token
+    num_experts: int = 0
+    num_experts_per_tok: int = 0
     name: str = ""
 
     @property
@@ -70,13 +75,19 @@ class ModelConfig:
     @property
     def full_qk_norm(self) -> bool:
         """OLMo 2's QK-norm: one RMSNorm over each token's whole q (nh * head_dim) and one over its whole k (nkv *
-        head_dim), with gains of those lengths.  Exclusive of Qwen3's per-head ``qk_norm``."""
-        return self.arch == "olmo2"
+        head_dim), with gains of those lengths.  Exclusive of Qwen3's per-head ``qk_norm``.  OLMoE has it too."""
+        return self.arch in ("olmo2", "olmoe")
 
     @property
     def post_norm(self) -> bool:
         """OLMo 2's layer: no input_layernorm; h1 = h + norm(attn(h)), h2 = h1 + norm(mlp(h1))."""
         return self.arch == "olmo2"
+
+    @property
+    def moe(self) -> bool:
+        """OLMoE's MLP: a router picks each token's top ``num_experts_per_tok`` of ``num_experts`` SwiGLU experts and
+        sums their outputs weighted by the raw router probabilities (``ops.moe``)."""
+        return self.arch == "olmoe"
 
     @property
     def layer_norm(self) -> bool:
@@ -111,7 +122,8 @@ class ModelConfig:
             per_layer = (h * q + q) + 2 * (kv * h + kv) + (q * h + h) + (h * i + i) + (i * h + h) + 4 * h
             n = v * h + l * per_layer + 2 * h
             return n if self.tie_word_embeddings else n + v * h
-        per_layer = h * q + 2 * kv * h + q * h + 3 * h * i + 2 * h
+        per_layer = h * q + 2 * kv * h + q * h + 2 * h
+        per_layer += self.num_experts * (h + 3 * h * i) if self.moe else 3 * h * i
         if self.qk_norm:
             per_layer += 2 * self.head_dim
         if self.qkv_bias:
@@ -176,6 +188,15 @@ def _olmo2(name, h, i, l, nh, nkv, v=100352, maxpos=4096):
     )
 
 
+def _olmoe(name, h, i, l, nh, nkv, experts, top_k, v=50304, maxpos=4096):
+    return ModelConfig(
+        arch="olmoe", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
+        num_attention_heads=nh, num_key_value_heads=nkv, max_position_embeddings=maxpos,
+        rms_norm_eps=1e-5, rope_theta=1e4, tie_word_embeddings=False, num_experts=experts, num_experts_per_tok=top_k,
+        name=name,
+    )
+
+
 def _starcoder2(name, h, i, l, nh, nkv, theta, tied, v=49152, maxpos=16384, window=4096):
     return ModelConfig(
         arch="starcoder2", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
@@ -237,6 +258,10 @@ REGISTRY = {
     "allenai/OLMo-2-1124-7B": _olmo2("allenai/OLMo-2-1124-7B", 4096, 11008, 32, 32, 32),
     "allenai/OLMo-2-1124-13B": _olmo2("allenai/OLMo-2-1124-13B", 5120, 13824, 40, 40, 40),
     "allenai/OLMo-2-0325-32B": _olmo2("allenai/OLMo-2-0325-32B", 5120, 27648, 64, 40, 8),
+    # OLMoE: 64 experts of intermediate size 1024, top-8, OLMo 2's full-width QK-norm in a pre-norm layer; 6.92B
+    # parameters, about 1.3B active per token.  The shapes are those of the public config.json as recalled when this
+    # table was written; no copy of the file was at hand to check them against.
+    "allenai/OLMoE-1B-7B-0924": _olmoe("allenai/OLMoE-1B-7B-0924", 2048, 1024, 16, 16, 16, 64, 8),
     # StarCoder2: LayerNorms, a GELU MLP, biases on every projection, sliding window 4096; head_dim 128 at every size.
     # Shapes, RoPE theta, window, norm eps and max positions are those of the public config.json files as recalled
     # when this table was written; no copy of those files was at hand to check them against.  transformers'
@@ -267,6 +292,8 @@ REGISTRY = {
     "debug-qwen2": _qwen2("debug-qwen2", 256, 512, 2, 4, 2, False, 1024, 2048),
     # 4 q heads and 2 k heads x 128 over a hidden size of 512: GQA, and a k norm narrower than the q norm
     "debug-olmo2": _olmo2("debug-olmo2", 512, 1024, 2, 4, 2, v=1024, maxpos=2048),
+    # 2 heads x 128 over a hidden size of 256, 8 experts of intermediate size 128, top-2
+    "debug-olmoe": _olmoe("debug-olmoe", 256, 128, 2, 2, 2, 8, 2, v=1024, maxpos=2048),
     # 4 q heads and 2 kv heads x 128 over a hidden size of 512, tied, with StarCoder2's block
     "debug-starcoder2": _starcoder2("debug-starcoder2", 512, 2048, 2, 4, 2, 1e5, True, v=1024, maxpos=2048),
     # 4 heads x 128 over a hidden size of 512 with rotary on 32 of them, and 4 heads x 64 over 256 with rotary on 16,
@@ -294,6 +321,8 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
         return _starcoder2_from_hf_dict(d, name)
     if mt == "gpt_neox":
         return _gpt_neox_from_hf_dict(d, name)
+    if mt == "olmoe":
+        return _olmoe_from_hf_dict(d, name)
     if mt not in ("llama", "mistral", "qwen3", "qwen2", "olmo2"):
         raise ValueError(f"unsupported model_type {mt!r} in {name}")
     if mt == "olmo2":
@@ -399,6 +428,43 @@ def _starcoder2_from_hf_dict(d: dict, name: str) -> ModelConfig:
         max_position_embeddings=d.get("max_position_embeddings", 4096), rope_theta=theta,
         tie_word_embeddings=d.get("tie_word_embeddings", True), sliding_window=d.get("sliding_window"),
         layer_norm_epsilon=d.get("norm_epsilon", 1e-5), name=name,
+    )
+
+
+def _olmoe_from_hf_dict(d: dict, name: str) -> ModelConfig:
+    """An ``OlmoeConfig`` payload.  Every setting the kernel path does not implement is refused, naming its key,
+    rather than dropped; ``router_aux_loss_coef`` and ``output_router_logits`` are training options
+    (``--router-aux-loss-coef``), not part of the model."""
+    if d.get("clip_qkv") is not None:
+        raise ValueError(f"{name}: clip_qkv is {d['clip_qkv']!r}; only clip_qkv null (no clipping) is supported")
+    if d.get("norm_topk_prob", False):
+        raise ValueError(f"{name}: norm_topk_prob is true; only the raw top-k router probabilities are supported")
+    if d.get("attention_bias"):
+        raise ValueError(f"{name}: attention_bias is true; OLMoE projections with a bias are not supported")
+    if d.get("hidden_act", "silu") != "silu":
+        raise ValueError(f"{name}: hidden_act is {d['hidden_act']!r}; only 'silu' (SwiGLU experts) is supported")
+    rp = d.get("rope_parameters") if isinstance(d.get("rope_parameters"), dict) else None
+    rope = rp if rp is not None else d.get("rope_scaling")
+    if rope and (rope.get("rope_type") or rope.get("type") or "default") != "default":
+        key = "rope_parameters" if rp is not None else "rope_scaling"
+        raise ValueError(f"{name}: {key} has type {rope.get('rope_type') or rope.get('type')!r}; only the default "
+                         "RoPE is supported for OLMoE")
+    for key in ("attention_dropout", "hidden_dropout", "dropout"):
+        if d.get(key, 0.0):
+            raise ValueError(f"{name}: {key} is {d[key]!r}; the kernel path has no dropout, set {key} to 0.0 to "
+                             "train without it")
+    if d.get("head_dim") is not None and d["head_dim"] != d["hidden_size"] // d["num_attention_heads"]:
+        raise ValueError(f"{name}: head_dim {d['head_dim']} differs from hidden_size / num_attention_heads = "
+                         f"{d['hidden_size'] // d['num_attention_heads']}; only head_dim = hidden / heads is supported")
+    theta = (rp or {}).get("rope_theta", d.get("rope_theta", 1e4))
+    return ModelConfig(
+        arch="olmoe", vocab_size=d["vocab_size"], hidden_size=d["hidden_size"],
+        intermediate_size=d["intermediate_size"], num_hidden_layers=d["num_hidden_layers"],
+        num_attention_heads=d["num_attention_heads"],
+        num_key_value_heads=d.get("num_key_value_heads", d["num_attention_heads"]),
+        max_position_embeddings=d.get("max_position_embeddings", 4096), rms_norm_eps=d.get("rms_norm_eps", 1e-5),
+        rope_theta=theta, tie_word_embeddings=d.get("tie_word_embeddings", False),
+        num_experts=d.get("num_experts", 64), num_experts_per_tok=d.get("num_experts_per_tok", 8), name=name,
     )
 
 
@@ -550,6 +616,18 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
             "use_parallel_residual": True, "attention_bias": True, "hidden_dropout": 0.0, "attention_dropout": 0.0,
             "tie_word_embeddings": cfg.tie_word_embeddings, "bos_token_id": 0, "eos_token_id": 0,
             "torch_dtype": "float16",
+        }
+    if cfg.arch == "olmoe":
+        d = {
+            "model_type": "olmoe", "architectures": ["OlmoeForCausalLM"], "vocab_size": cfg.vocab_size,
+            "hidden_size": cfg.hidden_size, "intermediate_size": cfg.intermediate_size,
+            "num_hidden_layers": cfg.num_hidden_layers, "num_attention_heads": cfg.num_attention_heads,
+            "num_key_value_heads": cfg.num_key_value_heads, "max_position_embeddings": cfg.max_position_embeddings,
+            "rms_norm_eps": cfg.rms_norm_eps, "rope_theta": cfg.rope_theta, "hidden_act": "silu",
+            "tie_word_embeddings": cfg.tie_word_embeddings, "attention_bias": False, "attention_dropout": 0.0,
+            "clip_qkv": None, "num_experts": cfg.num_experts, "num_experts_per_tok": cfg.num_experts_per_tok,
+            "norm_topk_prob": False, "output_router_logits": False, "router_aux_loss_coef": 0.01,
+            "pad_token_id": 1, "bos_token_id": None, "eos_token_id": 50279, "torch_dtype": "bfloat16",
         }
     if cfg.arch == "llama" and cfg.explicit_head_dim is not None:
         d["head_dim"] = cfg.explicit_head_dim

@@ -2,7 +2,7 @@
 Llama plus QK-norm, with a head_dim of its own; Qwen2: Llama plus q/k/v biases; OLMo 2: Llama with a full-width
 QK-norm and RMSNorms after each sublayer instead of before it; StarCoder2: Llama with LayerNorms, a c_fc -> GELU-tanh
 -> c_proj MLP and a bias on every projection; GPT-NeoX: StarCoder2's parameters with a parallel residual, partial
-rotary embeddings and an exact GELU).  One ``LlamaDecoderLayer`` builds every family's layer from its
+rotary embeddings and an exact GELU; OLMoE: Llama with OLMo 2's full-width QK-norm and a mixture-of-experts MLP).  One ``LlamaDecoderLayer`` builds every family's layer from its
 ``ModelConfig``, and ``decoder_layout`` fixes its flat-buffer layout.
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
@@ -237,6 +237,31 @@ class Starcoder2MLP(nn.Module):
         self.c_proj = Linear(i, h, dtype, device, bias=True)
 
 
+#: the MoE router's parameter name inside a decoder layer (FSDP keeps it out of the GEMM-fused gather)
+MOE_ROUTER = "mlp.gate.weight"
+
+
+class OlmoeExperts(nn.Module):
+    """Every expert's SwiGLU weights in two 3-D parameters (transformers 5's layout): ``gate_up_proj`` [E, 2I, H]
+    (each expert's gate rows, then its up rows) and ``down_proj`` [E, H, I]."""
+
+    def __init__(self, config: ModelConfig, dtype=None, device=None):
+        super().__init__()
+        e, h, i = config.num_experts, config.hidden_size, config.intermediate_size
+        self.gate_up_proj = nn.Parameter(torch.empty(e, 2 * i, h, dtype=dtype, device=device))
+        self.down_proj = nn.Parameter(torch.empty(e, h, i, dtype=dtype, device=device))
+
+
+class OlmoeMoE(nn.Module):
+    """OLMoE's sparse MLP: the router ``gate`` [E, H] and the experts (``ops.moe``)."""
+
+    def __init__(self, config: ModelConfig, dtype=None, device=None):
+        super().__init__()
+        self.top_k = config.num_experts_per_tok
+        self.gate = Linear(config.hidden_size, config.num_experts, dtype, device)
+        self.experts = OlmoeExperts(config, dtype, device)
+
+
 class FusedWeight:
     """A fused [q|k|v] or [gate|up] weight: adjacent parameters of a flat buffer seen as one
     matrix, plus the matching view of the flat gradient buffer (see ops._emit_weight_grad)."""
@@ -265,6 +290,8 @@ def decoder_layout(config: ModelConfig):
     qkv = ("self_attn.q_proj.weight", "self_attn.k_proj.weight", "self_attn.v_proj.weight")
     if config.gelu_mlp:
         mlp, mlp_bias = ("mlp.c_fc.weight", "mlp.c_proj.weight"), ("mlp.c_fc.bias", "mlp.c_proj.bias")
+    elif config.moe:
+        mlp, mlp_bias = (MOE_ROUTER, "mlp.experts.gate_up_proj", "mlp.experts.down_proj"), ()
     else:
         mlp, mlp_bias = ("mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight"), ()
     norms = (("post_attention_layernorm", "post_feedforward_layernorm") if config.post_norm else
@@ -275,7 +302,7 @@ def decoder_layout(config: ModelConfig):
                 if config.qkv_bias or config.all_bias else ())
     o_bias = ("self_attn.o_proj.bias",) if config.all_bias else ()
     fused = {"qkv": qkv}
-    if not config.gelu_mlp:
+    if not config.gelu_mlp and not config.moe:
         fused["gate_up"] = mlp[:2]
     if qkv_bias:
         fused["qkv_bias"] = qkv_bias
@@ -298,6 +325,9 @@ class LlamaDecoderLayer(nn.Module):
         if config.gelu_mlp:
             assert tp_size == 1, f"{config.arch} layers are not tensor-parallel"
             self.mlp = Starcoder2MLP(config, dtype, device)
+        elif config.moe:
+            assert tp_size == 1, f"{config.arch} layers are not tensor-parallel"
+            self.mlp = OlmoeMoE(config, dtype, device)
         else:
             self.mlp = LlamaMLP(config, dtype, device, tp_size)
         Norm, eps = (LayerNorm, config.layer_norm_epsilon) if config.layer_norm else (RMSNorm, config.rms_norm_eps)
@@ -312,6 +342,8 @@ class LlamaDecoderLayer(nn.Module):
         self._fused = {}  # name -> FusedWeight, installed by parallel.flat.install_fused_views
         self.tp = None  # set through LlamaForCausalLM.tp: the layer runs TensorParallelRuntime.layer_forward
         self.fp8 = False  # set through LlamaForCausalLM.fp8: the projections run in fp8
+        #: OLMoE: (assignments per expert int32 [E], router probability column sums fp32 [E]) of the last forward
+        self.router_stats = None
 
     def fused_weight(self, name):
         """(fused weight ``name``, its flat-gradient owner).  That is the ``FusedWeight`` view the flat group
@@ -346,6 +378,11 @@ class LlamaDecoderLayer(nn.Module):
         return ops.gelu(up) if self.gelu_exact else ops.gelu_tanh(up)
 
     def _mlp(self, y):
+        if isinstance(self.mlp, OlmoeMoE):
+            m = self.mlp
+            out, psum, counts = ops.moe(y, m.gate.weight, m.experts.gate_up_proj, m.experts.down_proj, m.top_k)
+            self.router_stats = (counts, psum)
+            return out
         down = self.mlp.down_proj if isinstance(self.mlp, LlamaMLP) else self.mlp.c_proj
         return self._proj(self._mlp_act(y), down.weight, down.bias)
 
@@ -418,6 +455,9 @@ class LlamaForCausalLM(nn.Module):
         #: whose position id is 0 (``ops.document_starts``); attention stays inside each document and the last token
         #: of a document is not trained to predict the first token of the next.  Off: ``position_ids`` only feeds RoPE.
         self.document_masking = False
+        #: OLMoE load balancing (``--router-aux-loss-coef``): loss = CE + coef * ``ref.router_aux_loss`` over every
+        #: layer's tokens; 0 trains on the cross entropy alone
+        self.router_aux_loss_coef = 0.0
 
     @property
     def fp8(self) -> bool:
@@ -505,9 +545,14 @@ class LlamaForCausalLM(nn.Module):
         doc_start = None
         if self.document_masking and position_ids is not None:
             doc_start = ops.document_starts(position_ids)
+        aux = self.router_aux_loss_coef > 0 and labels is not None
+        if aux and self.activation_checkpointing and torch.is_grad_enabled():
+            raise ValueError("the router aux loss needs the router probabilities' graph, which activation "
+                             "checkpointing drops: train with --router-aux-loss-coef 0 or without "
+                             "--checkpoint-activations")
         y = self.decoder(input_ids, cos, sin, doc_start)
         logits = self.lm_head(y.reshape(B * S, -1))  # [T, V], a fresh tensor the loss may consume
-        loss = None
+        loss = aux_loss = None
         if labels is not None:
             tgt = ref.shift_labels(labels)
             if doc_start is not None:
@@ -518,8 +563,15 @@ class LlamaForCausalLM(nn.Module):
             else:
                 loss = ops.cross_entropy(logits, tgt)
                 logits = None  # its storage now holds dlogits (CUDA path)
+            if aux:
+                stats = [layer.router_stats for layer in m.layers]
+                aux_loss = ref.router_aux_loss([c for c, _ in stats], [p for _, p in stats], B * S,
+                                               self.config.num_experts)
+                loss = loss + self.router_aux_loss_coef * aux_loss
         if logits is not None:
             logits = logits.view(B, S, -1)
+        if aux_loss is not None:
+            return SimpleNamespace(loss=loss, logits=logits, aux_loss=aux_loss)
         return SimpleNamespace(loss=loss, logits=logits)
 
 

@@ -32,7 +32,7 @@ __all__ = [
     "linear", "rms_norm", "add_rms_norm", "rms_norm_add", "rope_qkv_", "qk_norm_rope_",
     "olmo_qk_norm_rope_", "attention_qkv", "document_starts", "swiglu", "cross_entropy", "layer_norm",
     "add_layer_norm", "gelu_tanh", "gelu", "layer_norm2", "parallel_out",
-    "embedding", "gemm", "fp8_amax", "fp8_cast", "gemm_fp8", "bias_grad", "ref",
+    "embedding", "gemm", "fp8_amax", "fp8_cast", "gemm_fp8", "bias_grad", "moe", "ref",
 ]
 
 
@@ -820,6 +820,73 @@ def swiglu(gu):
     if _ext.use_cuda_kernel("swiglu", gu) and gu.dtype == torch.bfloat16:
         return _SwiGLU.apply(gu)
     return ref.swiglu(gu)
+
+
+# --------------------------------------------------------------------------------------
+# mixture-of-experts MLP (OLMoE): router top-k, permute, grouped expert GEMMs, SwiGLU, combine
+# --------------------------------------------------------------------------------------
+class _MoE(torch.autograd.Function):
+    """Forward: router logits on the wgmma GEMM; ``moe_route`` (fp32 softmax, top-k, the stable expert-sorted
+    layout); ``moe_permute``; the grouped gate|up GEMM, SwiGLU and the grouped down GEMM over every expert's 128-row
+    padded segment; ``moe_combine``.  Backward mirrors it: ``moe_combine_bwd`` (the permuted output gradient and the
+    routing weights' gradient), grouped dgrad and wgrad GEMMs, ``moe_combine`` with unit weights for the input
+    gradient, then ``moe_router_bwd`` and the router's GEMMs.  No step reads a count back to the host."""
+
+    @staticmethod
+    def forward(ctx, x, gate_w, gate_up, down, k):
+        C = _ext.load()
+        x2 = x.reshape(-1, x.shape[-1])
+        x2 = x2 if x2.is_contiguous() else x2.contiguous()
+        logits = gemm(x2, gate_w, trans_b=True)
+        p, idx, w, pos, seg, tiles, row_tok, counts = C.moe_route(logits, k)
+        xp = C.moe_permute(x2, row_tok, seg, k)
+        R = xp.shape[0]
+        gu = torch.empty(R, gate_up.shape[1], dtype=x.dtype, device=x.device)
+        C.gemm_grouped(0, xp, gate_up, gu, seg, tiles)
+        h = C.swiglu_fwd(gu)
+        yp = torch.empty(R, down.shape[1], dtype=x.dtype, device=x.device)
+        C.gemm_grouped(0, h, down, yp, seg, tiles)
+        y = C.moe_combine(yp, pos, w)
+        psum = C.moe_prob_sums(p)
+        ctx.save_for_backward(x2, gate_w, gate_up, down, p, idx, w, pos, seg, tiles, row_tok, xp, gu, h, yp)
+        ctx.x_shape = x.shape
+        ctx.mark_non_differentiable(counts)
+        return y.view(x.shape), psum, counts
+
+    @staticmethod
+    def backward(ctx, dy, dpsum, _dcounts):
+        C = _ext.load()
+        x2, gate_w, gate_up, down, p, idx, w, pos, seg, tiles, row_tok, xp, gu, h, yp = ctx.saved_tensors
+        dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
+        dyp, dw = C.moe_combine_bwd(dy2, yp, row_tok, seg, w)
+        dh = torch.empty_like(h)
+        C.gemm_grouped(1, dyp, down, dh, seg, tiles)
+        d_down = _emit_weight_grad(down, lambda out, acc: C.gemm_grouped(2, dyp, h, out, seg, None, acc), down)
+        dgu = C.swiglu_bwd(dh, gu)
+        dxp = torch.empty_like(xp)
+        C.gemm_grouped(1, dgu, gate_up, dxp, seg, tiles)
+        d_gate_up = _emit_weight_grad(gate_up, lambda out, acc: C.gemm_grouped(2, dgu, xp, out, seg, None, acc),
+                                      gate_up)
+        dx = C.moe_combine(dxp, pos)
+        dlogits = C.moe_router_bwd(p, idx, dw, dpsum.contiguous() if dpsum is not None else None)
+        gemm(dlogits, gate_w, out=dx, accumulate=True)
+        d_gate = _emit_weight_grad(gate_w, lambda out, acc: gemm(dlogits, x2, out=out, trans_a=True, accumulate=acc),
+                                   gate_w)
+        return dx.view(ctx.x_shape), d_gate, d_gate_up, d_down, None
+
+
+def moe(x, gate_w, gate_up, down, k):
+    """OLMoE's sparse MLP: each token goes through its top-``k`` experts by router probability, weighted by those
+    probabilities (``ref.moe``).  x [..., H], gate_w [E, H], gate_up [E, 2I, H] (gate rows first), down [E, H, I].
+    Returns ``(y, psum, counts)``: y like x; psum fp32 [E], the column sums of the router probabilities (the aux loss
+    differentiates through it); counts int32 [E], the assignments per expert.  bf16 CUDA tensors run the sm_90a
+    kernels; the weight gradients go through ``_emit_weight_grad``."""
+    if _ext.use_cuda_kernel("moe", x, gate_w, gate_up, down) and x.dtype == torch.bfloat16:
+        return _MoE.apply(x, gate_w, gate_up, down, k)
+    x2 = x.reshape(-1, x.shape[-1])
+    y, p = ref.moe(x2, gate_w, gate_up, down, k)
+    counts = torch.bincount(torch.topk(p.detach(), k, dim=-1).indices.reshape(-1), minlength=gate_w.shape[0])
+    return y.view(x.shape), p.sum(0), counts.to(torch.int32)
 
 
 # --------------------------------------------------------------------------------------

@@ -138,6 +138,42 @@ def swiglu(gu):
     return (F.silu(g.float()) * u.float()).to(gu.dtype)
 
 
+def moe_route(x, gate_w, k):
+    """OLMoE's router in fp32: ``(p, w, idx)`` with p = softmax(x @ gate_w.T) [T, E], and w, idx [T, k] the top-k
+    probabilities (kept raw, ``norm_topk_prob: false``) and their experts."""
+    p = torch.softmax(x.float() @ gate_w.float().t(), dim=-1)
+    w, idx = torch.topk(p, k, dim=-1)
+    return p, w, idx
+
+
+def moe(x, gate_w, gate_up, down, k):
+    """OLMoE's sparse MLP in fp32, one expert at a time: ``sum_slot w[t, slot] * expert_idx[t, slot](x_t)`` with
+    ``expert_e(x) = down[e] @ (silu(g) * u)``, ``[g | u] = gate_up[e] @ x``.  x [T, H], gate_w [E, H], gate_up
+    [E, 2I, H], down [E, H, I].  Returns ``(y in x.dtype, p)`` with p the fp32 router probabilities [T, E]."""
+    xf = x.float()
+    p, w, idx = moe_route(xf, gate_w, k)
+    out = torch.zeros_like(xf)
+    for e in range(gate_up.shape[0]):
+        tok, slot = (idx == e).nonzero(as_tuple=True)
+        if tok.numel() == 0:
+            continue
+        g, u = (xf[tok] @ gate_up[e].float().t()).chunk(2, dim=-1)
+        y = (F.silu(g) * u) @ down[e].float().t()
+        out = out.index_add(0, tok, y * w[tok, slot, None])
+    return out.to(x.dtype), p
+
+
+def router_aux_loss(counts, psums, n_tokens, num_experts):
+    """The Switch load-balancing loss of transformers' ``load_balancing_loss_func`` over the concatenated tokens of
+    every layer: ``E * sum_e f_e * P_e`` with f_e = (top-k assignments to e) / tokens and P_e the mean router
+    probability of e.  ``counts`` and ``psums`` hold one [E] tensor per layer (assignment counts and column sums of
+    p); ``n_tokens`` is the token count of one layer."""
+    n = float(n_tokens * len(psums))
+    f = torch.stack([c.float() for c in counts]).sum(0) / n
+    P = torch.stack(list(psums)).sum(0) / n
+    return num_experts * (f * P).sum()
+
+
 def gelu_new(x):
     return 0.5 * x * (1.0 + torch.tanh(math.sqrt(2.0 / math.pi) * (x + 0.044715 * x.pow(3))))
 

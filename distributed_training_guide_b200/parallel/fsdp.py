@@ -36,7 +36,7 @@ import torch
 import torch.distributed as dist
 from torch.autograd import Variable
 
-from ..models.llama import LlamaDecoderLayer, LlamaForCausalLM, init_parameter_
+from ..models.llama import MOE_ROUTER, LlamaDecoderLayer, LlamaForCausalLM, init_parameter_
 from ..ops import reference as ref
 from ..ops import join_wgrad_stream
 from ..utils.timers import nvtx_range
@@ -298,7 +298,9 @@ class FSDPEngine:
                 covered.update(members)
             end_of_matrices = 0
             for n, (p, off, shape) in by_name.items():
-                if len(shape) != 2:
+                # the MoE router is read by ops.moe's own GEMMs, which gather nothing: like the 3-D experts after it,
+                # it stays in the copy-engine tail (the layout puts it right after the attention matrices)
+                if len(shape) != 2 or n.endswith(MOE_ROUTER):
                     continue
                 end_of_matrices = max(end_of_matrices, off + shape[0] * shape[1])
                 if n not in covered:

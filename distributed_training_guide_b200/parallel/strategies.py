@@ -143,6 +143,7 @@ class SingleDevice(Strategy):
         _load_pretrained(args, model=model)
         _apply_fp8(args, model)
         _apply_document_masking(args, model)
+        _apply_router_aux_loss(args, model)
         return model
 
     def build_optimizer(self, args, model, lr):
@@ -176,6 +177,9 @@ def _apply_fp8(args, model):
 
     if not isinstance(model, LlamaForCausalLM):
         raise ValueError(f"fp8 applies to the Llama models' decoder layers, not {type(model).__name__}")
+    if model.config.moe:
+        raise ValueError(f"{model.config.name or model.config.arch}: fp8 does not cover the mixture-of-experts "
+                         "layers (the grouped expert GEMMs are bf16); train it without --fp8")
     model.fp8 = True
 
 
@@ -198,6 +202,18 @@ def _apply_document_masking(args, model):
     if not isinstance(model, LlamaForCausalLM):
         raise ValueError(f"document masking applies to the Llama models, not {type(model).__name__}")
     model.document_masking = True
+
+
+def _apply_router_aux_loss(args, model):
+    """``model.router_aux_loss_coef = args.router_aux_loss_coef`` (mixture-of-experts models only)."""
+    coef = float(getattr(args, "router_aux_loss_coef", 0.0) or 0.0)
+    if coef == 0.0:
+        return
+    if coef < 0:
+        raise ValueError(f"router_aux_loss_coef must be >= 0, got {coef}")
+    if not getattr(getattr(model, "config", None), "moe", False):
+        raise ValueError("router_aux_loss_coef applies to mixture-of-experts models (OLMoE)")
+    model.router_aux_loss_coef = coef
 
 
 def check_document_masking_supported(parallelism: str):
@@ -278,6 +294,7 @@ class DataParallelZero1(Strategy):
                     dist.broadcast(g.param, src=0)
         _apply_fp8(args, model)
         _apply_document_masking(args, model)
+        _apply_router_aux_loss(args, model)
         self.model = model
         return model
 
@@ -333,6 +350,7 @@ class FullyShardedDataParallel(Strategy):
                                  prefetch=True, prefetch_depth=2 if getattr(args, "prefetch_layers", False) else 1)
         model.activation_checkpointing = bool(getattr(args, "checkpoint_activations", False))
         _apply_document_masking(args, model)
+        _apply_router_aux_loss(args, model)
         self.groups = self.engine.groups
         self.model = model
         # chapter 05 (reference 05:76-145): rank 0 reads the checkpoint, every rank keeps its slice of each group
@@ -425,6 +443,10 @@ class TwoDParallel(Strategy):
         from .tp import TensorParallelRuntime, TPContext
 
         env, mesh = self.env, self.mesh
+        if getattr(config, "moe", False):
+            raise ValueError(
+                f"{config.name or config.arch}: tensor parallelism does not support mixture-of-experts layers; train "
+                "it with the single-GPU, DDP or FSDP engines (chapters 01, 02, 04, 05)")
         if getattr(config, "full_qk_norm", False):
             # the layer path below is the tensor-parallel one at every tp size, and it has no full-width norm
             raise ValueError(

@@ -14,7 +14,7 @@ from pathlib import Path
 
 import torch
 
-from ..models import build_model, get_config, gpt_neox_layout
+from ..models import build_model, get_config, gpt_neox_layout, olmoe_layout
 from ..parallel.flat import build_groups
 
 
@@ -57,10 +57,12 @@ def consolidate(exp_dir: str, model_name: str, world: int) -> Path:
 
 
 def _hf_layout(sd, cfg):
-    """GPT-NeoX is written under its own HF names and q|k|v layout (``GPTNeoXForCausalLM`` loads it strictly);
-    every other family already has HF's names."""
+    """GPT-NeoX is written under its own HF names and q|k|v layout (``GPTNeoXForCausalLM`` loads it strictly), OLMoE
+    with one tensor per expert as its published checkpoints are; every other family already has HF's names."""
     if cfg.arch == "gpt_neox":
         return gpt_neox_layout.to_hf_state_dict(sd, cfg.num_attention_heads)
+    if cfg.moe:
+        return olmoe_layout.to_hf_state_dict(sd)
     return sd
 
 

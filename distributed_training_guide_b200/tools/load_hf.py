@@ -99,12 +99,15 @@ def maybe_load_pretrained(args, model=None, engine=None, default="never") -> boo
 
 def open_checkpoint(path: str):
     """``reader(name) -> tensor`` under this project's parameter names: a ``SafetensorsReader``, seen through
-    ``models.gpt_neox_layout`` when the checkpoint is GPT-NeoX's (other names and layout)."""
-    from ..models import get_config, gpt_neox_layout
+    ``models.gpt_neox_layout`` when the checkpoint is GPT-NeoX's (other names and layout), or through
+    ``models.olmoe_layout`` when it stores OLMoE's experts one tensor each."""
+    from ..models import get_config, gpt_neox_layout, olmoe_layout
 
     reader = SafetensorsReader(path)
     if gpt_neox_layout.is_gpt_neox_checkpoint(reader.weight_map):
         return gpt_neox_layout.HFReader(reader, reader.weight_map, get_config(path).num_attention_heads)
+    if olmoe_layout.is_per_expert_checkpoint(reader.weight_map):
+        return olmoe_layout.HFReader(reader, reader.weight_map, get_config(path).num_experts)
     return reader
 
 

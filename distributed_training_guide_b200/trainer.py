@@ -90,6 +90,7 @@ def train(args, strategy):
     timers = {k: LocalTimer(device, name=k) for k in ["data", "forward", "backward", "update"]}
     accum = max(1, getattr(args, "grad_accum_steps", 1))
     running_loss = torch.zeros((), dtype=torch.float32, device=device)
+    running_aux = torch.zeros((), dtype=torch.float32, device=device)   # MoE router aux loss (--router-aux-loss-coef)
     if resumed:
         running_loss += float(state["running_loss"])
     max_steps = getattr(args, "max_steps", None)
@@ -137,6 +138,8 @@ def train(args, strategy):
 
             state["epoch_step"] += 1
             running_loss += outputs.loss.detach().float()
+            if getattr(outputs, "aux_loss", None) is not None:
+                running_aux += outputs.aux_loss.detach().float()
             progress.update(1)
             if not is_boundary:
                 continue
@@ -160,6 +163,8 @@ def train(args, strategy):
                 }
                 if getattr(args, "max_grad_norm", None) is not None:
                     info["grad_norm"] = float(optimizer.last_grad_norm)  # pre-clip norm of this step
+                if getattr(args, "router_aux_loss_coef", 0.0):
+                    info["aux_loss"] = float(running_aux.item()) / (args.log_freq * accum)
                 LOGGER.info(info)
                 strategy.check_health()
                 if tracker is not None:
@@ -167,6 +172,7 @@ def train(args, strategy):
                 last_info = info
                 reset_peak(device)
                 running_loss.zero_()
+                running_aux.zero_()
                 state["running_loss"] = 0
                 for t in timers.values():
                     t.reset()

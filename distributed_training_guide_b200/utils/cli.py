@@ -64,6 +64,10 @@ def get_parser(chapter: str = "01-single-gpu", require_experiment: bool = False)
     p.add_argument("--pretrained", choices=("auto", "require", "never"), default=None,
                    help="load local Hugging Face safetensors for --model-name (chapter 05 defaults to auto: load "
                         "them when they exist on disk; other chapters default to never = random init)")
+    p.add_argument("--router-aux-loss-coef", default=0.0, type=float,
+                   help="mixture-of-experts models (OLMoE): add this times the Switch load-balancing loss of every "
+                        "layer's router to the loss (transformers' load_balancing_loss_func); the log record then "
+                        "carries aux_loss (default: 0, off)")
     if "fp8" in extras:
         p.add_argument("--fp8", default=False, action="store_true",
                        help="run the decoder-layer projections (q|k|v, o, gate|up, down) as fp8 GEMMs with per-tensor "
