@@ -165,15 +165,19 @@ long long moe_route_scratch(long long T, int E);
 // [rows_cap / 128], row_tok int32 [rows_cap] (rows below seg[E]) and counts int32 [E].
 void moe_route(const void* logits, long long ldl, int T, int E, int k, float* p, int* idx, float* w, int* pos,
                int* seg, int* tile_expert, int* row_tok, int* counts, int* scratch, cudaStream_t s);
-// out [rows_cap, H]: row r < seg[E] is x [T, H]'s row of its token, or zeros on a padding row
-void moe_permute(const void* x, const int* row_tok, const int* seg, int E, int k, int H, long long rows_cap, void* out,
+// out [rows_cap, H]: row r < seg[E] is x [T, H]'s row of its token, or zeros on a padding row (NaN where row_tok[r]
+// is outside [-1, T * k))
+void moe_permute(const void* x, int T, const int* row_tok, const int* seg, int E, int k, int H, long long rows_cap,
+                 void* out, cudaStream_t s);
+// out [T, H] = bf16(sum over slots, in slot order, of w * yp[pos]) in fp32; w null: weights 1 (the input gradient).
+// yp has yp_rows >= 1 rows (when T > 0); a token with a pos outside [0, yp_rows) gets a NaN row.
+void moe_combine(const void* yp, long long yp_rows, const int* pos, const float* w, int T, int k, int H, void* out,
                  cudaStream_t s);
-// out [T, H] = bf16(sum over slots, in slot order, of w * yp[pos]) in fp32; w null: weights 1 (the input gradient)
-void moe_combine(const void* yp, const int* pos, const float* w, int T, int k, int H, void* out, cudaStream_t s);
 // The combine's backward: dyp [rows_cap, H] row r < seg[E] = bf16(w[a] * dy[t]) (zeros on padding rows) and dw fp32
-// [T, k] = sum_h dy[t, h] * yp[r, h], for a = row_tok[r] and t = a / k
-void moe_combine_bwd(const void* dy, const void* yp, const int* row_tok, const int* seg, const float* w, int E, int k,
-                     int H, long long rows_cap, void* dyp, float* dw, cudaStream_t s);
+// [T, k] = sum_h dy[t, h] * yp[r, h], for a = row_tok[r] and t = a / k (dy [T, H]; a row whose a is outside
+// [-1, T * k) gets a NaN dyp row and writes no dw)
+void moe_combine_bwd(const void* dy, int T, const void* yp, const int* row_tok, const int* seg, const float* w, int E,
+                     int k, int H, long long rows_cap, void* dyp, float* dw, cudaStream_t s);
 // dlogits bf16 [T, E] = bf16(p * (dp - sum_e p dp)) with dp = dw at the selected experts, plus dpsum [E] (null: 0)
 void moe_router_bwd(const float* p, const int* idx, const float* dw, const float* dpsum, int T, int E, int k,
                     void* dlogits, cudaStream_t s);

@@ -8,6 +8,16 @@
 // permuted activations, seg[0] = 0 and every bound a multiple of 128; its count[e] assignments take the first rows of
 // the segment, in (t, slot) order (a stable counting sort), and the rest of the segment is padding.  pos[a] is the row
 // of assignment a, row_tok[r] the assignment of row r (-1 for a padding row).
+//
+// Ties.  Experts are ranked by their fp32 probability as moe_topk_kernel computes it, ties to the lower expert.  That
+// includes probabilities that underflow to 0 (a row whose logits span more than about 104): they tie, so the lower
+// experts win.
+//
+// Table entries are device data the bindings cannot see, so every kernel that follows one checks it against the
+// extent of what it indexes, in the way of common.cuh's vocabulary rule: a bad entry is never dereferenced.
+//   row_tok[r]  -1 = padding (a zero row); 0 <= a < T * k valid; anything else (a table built for another T or k) is
+//               bad: a NaN row of the permuted output and, in the combine backward, no dw entry (there is none).
+//   pos[a]      0 <= pos[a] < rows of yp valid; anything else gives the token a NaN combined row.
 #include <cuda_bf16.h>
 
 #include "api.h"
@@ -174,18 +184,22 @@ __global__ void moe_pos_kernel(const int* __restrict__ idx, const int* __restric
 // rows of the permuted layout, one CTA per row (rows at or past seg[E] are not touched):
 //   permute  out[r] = x[t(r)], zero on a padding row
 //   dcombine out[r] = bf16(w[a] * dy[t]) and dw[a] = sum_h dy[t, h] * yp[r, h] (fp32, fixed order), zero padding
+// n_assign = T * k of src: a row whose assignment is outside [0, n_assign) gets a NaN row and reads nothing
 template <bool DCOMBINE>
 __global__ void moe_rows_kernel(const __nv_bfloat16* __restrict__ src, const int* __restrict__ row_tok,
-                                const int* __restrict__ seg, int E, int k, int H, const float* __restrict__ w,
-                                const __nv_bfloat16* __restrict__ yp, float* __restrict__ dw,
-                                __nv_bfloat16* __restrict__ out) {
+                                const int* __restrict__ seg, int E, int k, int H, long long n_assign,
+                                const float* __restrict__ w, const __nv_bfloat16* __restrict__ yp,
+                                float* __restrict__ dw, __nv_bfloat16* __restrict__ out) {
   __shared__ float red[32];
   const long long r = blockIdx.x;
   if (r >= seg[E]) return;
   const int a = row_tok[r];
   __nv_bfloat16* orow = out + r * H;
-  if (a < 0) {
-    const bf16x8 z = {};
+  if (a == -1 || (unsigned long long)(long long)a >= (unsigned long long)n_assign) {
+    float f[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) f[i] = a == -1 ? 0.f : nan_f();
+    const bf16x8 z = pack8(f);
     for (int c = threadIdx.x * 8; c < H; c += blockDim.x * 8) st8(orow + c, z);
     return;
   }
@@ -211,17 +225,21 @@ __global__ void moe_rows_kernel(const __nv_bfloat16* __restrict__ src, const int
   }
 }
 
-// one CTA per token: out[t] = bf16(sum over slots, in slot order, of w[a] * yp[pos[a]]) in fp32; w null: weight 1
-__global__ void moe_combine_kernel(const __nv_bfloat16* __restrict__ yp, const int* __restrict__ pos,
+// one CTA per token: out[t] = bf16(sum over slots, in slot order, of w[a] * yp[pos[a]]) in fp32; w null: weight 1.
+// A row pos[a] outside [0, yp_rows) is not read: row 0 (yp_rows >= 1, the binding checks) is read in its place with a
+// NaN weight, so the token's row is NaN, and the loads stay unconditional.
+__global__ void moe_combine_kernel(const __nv_bfloat16* __restrict__ yp, long long yp_rows, const int* __restrict__ pos,
                                    const float* __restrict__ w, int k, int H, __nv_bfloat16* __restrict__ out) {
   const long long t = blockIdx.x;
   for (int c = threadIdx.x * 8; c < H; c += blockDim.x * 8) {
     float acc[8] = {};
     for (int s = 0; s < k; ++s) {
       const long long a = t * k + s;
-      const float wa = w ? w[a] : 1.f;
+      const int row = pos[a];
+      const bool ok = (unsigned long long)(long long)row < (unsigned long long)yp_rows;
+      const float wa = !ok ? nan_f() : (w ? w[a] : 1.f);
       float y[8];
-      unpack8(ld8(yp + (long long)pos[a] * H + c), y);
+      unpack8(ld8(yp + (ok ? (long long)row : 0ll) * H + c), y);
 #pragma unroll
       for (int i = 0; i < 8; ++i) acc[i] = fmaf(wa, y[i], acc[i]);
     }
@@ -282,27 +300,31 @@ void moe_route(const void* logits, long long ldl, int T, int E, int k, float* p,
   note_launch(4);
 }
 
-void moe_permute(const void* x, const int* row_tok, const int* seg, int E, int k, int H, long long rows_cap, void* out,
-                 cudaStream_t s) {
+void moe_permute(const void* x, int T, const int* row_tok, const int* seg, int E, int k, int H, long long rows_cap,
+                 void* out, cudaStream_t s) {
   if (rows_cap == 0) return;
   moe_rows_kernel<false><<<(unsigned)rows_cap, row_threads(H), 0, s>>>(
-      (const __nv_bfloat16*)x, row_tok, seg, E, k, H, nullptr, nullptr, nullptr, (__nv_bfloat16*)out);
+      (const __nv_bfloat16*)x, row_tok, seg, E, k, H, (long long)T * k, nullptr, nullptr, nullptr,
+      (__nv_bfloat16*)out);
   DTG_LAUNCH_CHECK();
   note_launch();
 }
 
-void moe_combine(const void* yp, const int* pos, const float* w, int T, int k, int H, void* out, cudaStream_t s) {
+void moe_combine(const void* yp, long long yp_rows, const int* pos, const float* w, int T, int k, int H, void* out,
+                 cudaStream_t s) {
   if (T == 0) return;
-  moe_combine_kernel<<<T, row_threads(H), 0, s>>>((const __nv_bfloat16*)yp, pos, w, k, H, (__nv_bfloat16*)out);
+  moe_combine_kernel<<<T, row_threads(H), 0, s>>>((const __nv_bfloat16*)yp, yp_rows, pos, w, k, H,
+                                                  (__nv_bfloat16*)out);
   DTG_LAUNCH_CHECK();
   note_launch();
 }
 
-void moe_combine_bwd(const void* dy, const void* yp, const int* row_tok, const int* seg, const float* w, int E, int k,
-                     int H, long long rows_cap, void* dyp, float* dw, cudaStream_t s) {
+void moe_combine_bwd(const void* dy, int T, const void* yp, const int* row_tok, const int* seg, const float* w, int E,
+                     int k, int H, long long rows_cap, void* dyp, float* dw, cudaStream_t s) {
   if (rows_cap == 0) return;
   moe_rows_kernel<true><<<(unsigned)rows_cap, row_threads(H), 0, s>>>(
-      (const __nv_bfloat16*)dy, row_tok, seg, E, k, H, w, (const __nv_bfloat16*)yp, dw, (__nv_bfloat16*)dyp);
+      (const __nv_bfloat16*)dy, row_tok, seg, E, k, H, (long long)T * k, w, (const __nv_bfloat16*)yp, dw,
+      (__nv_bfloat16*)dyp);
   DTG_LAUNCH_CHECK();
   note_launch();
 }

@@ -71,8 +71,8 @@ Tensor moe_permute(const Tensor& x, const Tensor& row_tok, const Tensor& seg, in
   TORCH_CHECK(row_tok.size(0) == rows_cap, who, ": row_tok must have rows_cap = ", rows_cap, " entries");
   const c10::cuda::CUDAGuard guard(x.device());
   Tensor out = torch::empty({rows_cap, H}, x.options());
-  dtg::moe_permute(x.data_ptr(), row_tok.data_ptr<int>(), seg.data_ptr<int>(), (int)E, (int)k, (int)H, rows_cap,
-                   out.data_ptr(), stream());
+  dtg::moe_permute(x.data_ptr(), (int)T, row_tok.data_ptr<int>(), seg.data_ptr<int>(), (int)E, (int)k, (int)H,
+                   rows_cap, out.data_ptr(), stream());
   return out;
 }
 
@@ -83,14 +83,15 @@ Tensor moe_combine(const Tensor& yp, const Tensor& pos, const c10::optional<Tens
   const int64_t T = pos.size(0), k = pos.size(1), H = yp.size(1);
   TORCH_CHECK(H > 0 && H % 8 == 0, who, ": H must be a positive multiple of 8, got ", H);
   TORCH_CHECK(k >= 1, who, ": pos must be [T, k] with k >= 1");
+  TORCH_CHECK(T == 0 || yp.size(0) >= 1, who, ": yp has no rows for pos to name");
   if (w.has_value()) {
     check_t(*w, yp, at::kFloat, 2, who, "w");
     TORCH_CHECK(w->size(0) == T && w->size(1) == k, who, ": w must be [T, k] like pos");
   }
   const c10::cuda::CUDAGuard guard(yp.device());
   Tensor out = torch::empty({T, H}, yp.options());
-  dtg::moe_combine(yp.data_ptr(), pos.data_ptr<int>(), w.has_value() ? w->data_ptr<float>() : nullptr, (int)T, (int)k,
-                   (int)H, out.data_ptr(), stream());
+  dtg::moe_combine(yp.data_ptr(), yp.size(0), pos.data_ptr<int>(), w.has_value() ? w->data_ptr<float>() : nullptr,
+                   (int)T, (int)k, (int)H, out.data_ptr(), stream());
   return out;
 }
 
@@ -110,8 +111,9 @@ std::tuple<Tensor, Tensor> moe_combine_bwd(const Tensor& dy, const Tensor& yp, c
   const c10::cuda::CUDAGuard guard(dy.device());
   Tensor dyp = torch::empty({rows_cap, H}, dy.options());
   Tensor dw = torch::empty({T, k}, w.options());
-  dtg::moe_combine_bwd(dy.data_ptr(), yp.data_ptr(), row_tok.data_ptr<int>(), seg.data_ptr<int>(), w.data_ptr<float>(),
-                       (int)E, (int)k, (int)H, rows_cap, dyp.data_ptr(), dw.data_ptr<float>(), stream());
+  dtg::moe_combine_bwd(dy.data_ptr(), (int)T, yp.data_ptr(), row_tok.data_ptr<int>(), seg.data_ptr<int>(),
+                       w.data_ptr<float>(), (int)E, (int)k, (int)H, rows_cap, dyp.data_ptr(), dw.data_ptr<float>(),
+                       stream());
   return {dyp, dw};
 }
 

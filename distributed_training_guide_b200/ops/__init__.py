@@ -837,6 +837,14 @@ class _MoE(torch.autograd.Function):
         C = _ext.load()
         x2 = x.reshape(-1, x.shape[-1])
         x2 = x2 if x2.is_contiguous() else x2.contiguous()
+        ctx.x_shape = x.shape
+        ctx.empty = x2.shape[0] == 0
+        if ctx.empty:   # no token: nothing to route and no kernel to launch
+            ctx.save_for_backward(gate_w, gate_up, down)
+            E = gate_w.shape[0]
+            counts = torch.zeros(E, dtype=torch.int32, device=x.device)
+            ctx.mark_non_differentiable(counts)
+            return x2.new_empty(x.shape), torch.zeros(E, dtype=torch.float32, device=x.device), counts
         logits = gemm(x2, gate_w, trans_b=True)
         p, idx, w, pos, seg, tiles, row_tok, counts = C.moe_route(logits, k)
         xp = C.moe_permute(x2, row_tok, seg, k)
@@ -849,13 +857,16 @@ class _MoE(torch.autograd.Function):
         y = C.moe_combine(yp, pos, w)
         psum = C.moe_prob_sums(p)
         ctx.save_for_backward(x2, gate_w, gate_up, down, p, idx, w, pos, seg, tiles, row_tok, xp, gu, h, yp)
-        ctx.x_shape = x.shape
         ctx.mark_non_differentiable(counts)
         return y.view(x.shape), psum, counts
 
     @staticmethod
     def backward(ctx, dy, dpsum, _dcounts):
         C = _ext.load()
+        if ctx.empty:   # zero weight gradients: overwrite with zeros, or leave an accumulating buffer as it is
+            zero = lambda out, acc: None if acc else out.zero_()
+            grads = tuple(_emit_weight_grad(t, zero, t) for t in ctx.saved_tensors)
+            return (dy.new_zeros(ctx.x_shape),) + grads + (None,)
         x2, gate_w, gate_up, down, p, idx, w, pos, seg, tiles, row_tok, xp, gu, h, yp = ctx.saved_tensors
         dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
         dyp, dw = C.moe_combine_bwd(dy2, yp, row_tok, seg, w)

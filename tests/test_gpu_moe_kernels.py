@@ -15,45 +15,45 @@ def _C():
 
 
 def _route_ref(logits, k):
-    """fp64 softmax, top-k by probability with ties to the lower expert, stable-sort rows, 128-row segments."""
-    T, E = logits.shape
+    """fp64 softmax and the top-k by probability with ties to the lower expert."""
     p = torch.softmax(logits.double(), -1)
-    order = torch.sort(-p, dim=-1, stable=True).indices[:, :k]
-    counts = torch.bincount(order.reshape(-1), minlength=E)
-    seg = [0]
-    for e in range(E):
-        seg.append(seg[-1] + (int(counts[e]) + 127) // 128 * 128)
-    pos = torch.empty(T, k, dtype=torch.long)
-    fill = list(seg[:-1])
-    for t in range(T):
-        for s in range(k):
-            e = int(order[t, s])
-            pos[t, s] = fill[e]
-            fill[e] += 1
-    return p, order, counts, torch.tensor(seg), pos
+    return p, torch.sort(-p, dim=-1, stable=True).indices[:, :k]
+
+
+def _check_layout(idx, E, pos, seg, tiles, row_tok, counts):
+    """The routing tables of ``moe_route``, exactly, from the experts ``idx`` [T, k] it chose: counts, 128-row padded
+    segments, each assignment's row in a stable counting sort, row_tok (-1 on padding rows) and the expert of every
+    128-row tile up to rows_cap (-1 past the last segment)."""
+    T, k = idx.shape
+    flat = idx.reshape(-1).long().cpu()
+    counts64 = torch.bincount(flat, minlength=E)
+    seg64 = torch.zeros(E + 1, dtype=torch.long)
+    seg64[1:] = torch.cumsum((counts64 + 127) // 128 * 128, 0)
+    order = torch.sort(flat, stable=True).indices                 # assignments grouped by expert, in (t, slot) order
+    first = torch.cumsum(counts64, 0) - counts64                  # index into `order` of each expert's first one
+    pos64 = torch.empty(T * k, dtype=torch.long)
+    pos64[order] = seg64[flat[order]] + torch.arange(T * k) - first[flat[order]]
+    assert torch.equal(counts.cpu().long(), counts64)
+    assert torch.equal(seg.cpu().long(), seg64)
+    assert torch.equal(pos.cpu().long().reshape(-1), pos64)
+    used = int(seg64[-1])
+    want = torch.full((used,), -1, dtype=torch.int32)
+    want[pos64] = torch.arange(T * k, dtype=torch.int32)
+    assert torch.equal(row_tok.cpu()[:used], want)
+    r = torch.arange(tiles.numel()) * 128
+    exp = torch.searchsorted(seg64[1:], r, right=True)            # the expert whose segment holds row r
+    exp[r >= used] = -1
+    assert torch.equal(tiles.cpu().long(), exp)
 
 
 def _check_route(logits, k):
     C = _C()
     p, idx, w, pos, seg, tiles, row_tok, counts = C.moe_route(logits, k)
-    p64, idx64, counts64, seg64, pos64 = _route_ref(logits.cpu(), k)
+    p64, idx64 = _route_ref(logits.cpu(), k)
     assert torch.equal(idx.cpu().long(), idx64)
-    assert torch.equal(counts.cpu().long(), counts64)
-    assert torch.equal(seg.cpu().long(), seg64)
-    assert torch.equal(pos.cpu().long(), pos64)
     torch.testing.assert_close(p.cpu().double(), p64, rtol=2e-6, atol=1e-7)
     torch.testing.assert_close(w.cpu().double(), p64.gather(1, idx64), rtol=2e-6, atol=1e-7)
-    T, E = logits.shape
-    used = int(seg64[-1])
-    rt = row_tok.cpu()[:used]
-    want = torch.full((used,), -1, dtype=torch.int32)
-    want[pos64.reshape(-1)] = torch.arange(T * k, dtype=torch.int32)
-    assert torch.equal(rt, want)
-    te = tiles.cpu()
-    for i in range(te.numel()):
-        r = 128 * i
-        exp = -1 if r >= used else int((seg64[1:] > r).nonzero()[0])
-        assert int(te[i]) == exp, i
+    _check_layout(idx, logits.shape[1], pos, seg, tiles, row_tok, counts)
     return p, idx, w, pos, seg, tiles, row_tok, counts
 
 
