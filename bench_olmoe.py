@@ -6,7 +6,10 @@
   * GB/s of route, permute and combine at that shape;
   * device-timed tokens/s and peak memory of OLMoE-1B-7B training steps (single-GPU engine).
 
-    python bench_olmoe.py [--seq 4096] [--steps 3] [--warmup 1]
+The kernel shapes come from ``--model``'s config (experts, top-k, hidden size, 2 x the expert intermediate size);
+``--layers N`` trains the model truncated to its first N layers (a model too large for one GPU).
+
+    python bench_olmoe.py [--seq 4096] [--steps 3] [--warmup 1] [--model NAME] [--layers N]
 """
 import argparse
 import json
@@ -83,10 +86,11 @@ def kernels(T, E=64, k=8, H=2048, N=2048):
     }
 
 
-def steps(model, seq, n, warmup):
+def steps(model, seq, n, warmup, layers=None):
     from distributed_training_guide_b200.engine import TrainEngine
 
-    eng = TrainEngine.create(model, parallelism="single", batch_size=1, seq_length=seq, lr=1e-4, device="cuda")
+    eng = TrainEngine.create(model, parallelism="single", batch_size=1, seq_length=seq, lr=1e-4, device="cuda",
+                             num_layers=layers)
     try:
         batch = eng.synthetic_batch(seed=0)
         for _ in range(warmup):
@@ -99,7 +103,8 @@ def steps(model, seq, n, warmup):
         b.record()
         b.synchronize()
         dt = a.elapsed_time(b) / 1e3 / n
-        return {"model": model, "seq": seq, "step_s": round(dt, 4), "tokens_per_s": round(seq / dt, 1),
+        return {"model": model + (f"[layers={layers}]" if layers else ""), "seq": seq, "step_s": round(dt, 4),
+                "tokens_per_s": round(seq / dt, 1),
                 "peak_mem_gb": round(torch.cuda.max_memory_allocated() / 2**30, 2),
                 "loss": float(losses[-1])}
     finally:
@@ -112,12 +117,17 @@ def main():
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--model", default="allenai/OLMoE-1B-7B-0924")
+    ap.add_argument("--layers", type=int, default=None, help="train only the first N layers")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("bench_olmoe.py measures on a GPU; none is visible")
-    rec = {"card": _card(), "kernels": kernels(a.seq)}
+    from distributed_training_guide_b200.models.configs import get_config
+
+    cfg = get_config(a.model)
+    rec = {"card": _card(), "kernels": kernels(a.seq, cfg.num_experts, cfg.num_experts_per_tok, cfg.hidden_size,
+                                               2 * cfg.intermediate_size)}
     try:
-        rec["train"] = steps(a.model, a.seq, a.steps, a.warmup)
+        rec["train"] = steps(a.model, a.seq, a.steps, a.warmup, a.layers)
     except torch.OutOfMemoryError as e:
         rec["train"] = {"model": a.model, "error": f"out of memory: {str(e).splitlines()[0]}"}
     print(json.dumps(rec))

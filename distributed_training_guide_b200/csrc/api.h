@@ -161,10 +161,10 @@ constexpr int kMoeMaxExperts = 256;
 long long moe_rows_cap(long long T, int E, int k);
 long long moe_route_scratch(long long T, int E);
 // From bf16 router logits [T, E] (row stride ldl): p fp32 [T, E] (softmax), idx int32 [T, k], w fp32 [T, k] (the
-// top-k probabilities, ties to the lower expert), pos int32 [T, k], seg int32 [E + 1], tile_expert int32
-// [rows_cap / 128], row_tok int32 [rows_cap] (rows below seg[E]) and counts int32 [E].
-void moe_route(const void* logits, long long ldl, int T, int E, int k, float* p, int* idx, float* w, int* pos,
-               int* seg, int* tile_expert, int* row_tok, int* counts, int* scratch, cudaStream_t s);
+// top-k probabilities, ties to the lower expert; norm_topk: divided by their sum), pos int32 [T, k], seg int32
+// [E + 1], tile_expert int32 [rows_cap / 128], row_tok int32 [rows_cap] (rows below seg[E]) and counts int32 [E].
+void moe_route(const void* logits, long long ldl, int T, int E, int k, bool norm_topk, float* p, int* idx, float* w,
+               int* pos, int* seg, int* tile_expert, int* row_tok, int* counts, int* scratch, cudaStream_t s);
 // out [rows_cap, H]: row r < seg[E] is x [T, H]'s row of its token, or zeros on a padding row (NaN where row_tok[r]
 // is outside [-1, T * k))
 void moe_permute(const void* x, int T, const int* row_tok, const int* seg, int E, int k, int H, long long rows_cap,
@@ -178,9 +178,10 @@ void moe_combine(const void* yp, long long yp_rows, const int* pos, const float*
 // [-1, T * k) gets a NaN dyp row and writes no dw)
 void moe_combine_bwd(const void* dy, int T, const void* yp, const int* row_tok, const int* seg, const float* w, int E,
                      int k, int H, long long rows_cap, void* dyp, float* dw, cudaStream_t s);
-// dlogits bf16 [T, E] = bf16(p * (dp - sum_e p dp)) with dp = dw at the selected experts, plus dpsum [E] (null: 0)
+// dlogits bf16 [T, E] = bf16(p * (dp - sum_e p dp)) with dp = dw at the selected experts, plus dpsum [E] (null: 0);
+// norm_topk (w = p_sel / S): dp = (dw - sum_i w_i dw_i) / S at the selected experts, plus dpsum
 void moe_router_bwd(const float* p, const int* idx, const float* dw, const float* dpsum, int T, int E, int k,
-                    void* dlogits, cudaStream_t s);
+                    bool norm_topk, void* dlogits, cudaStream_t s);
 
 // ---- fp8.cu --------------------------------------------------------------------------------
 // amax[0] = max |x| of a bf16 [R, C] matrix with row stride ld (elements), on the device.

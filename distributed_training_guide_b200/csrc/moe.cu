@@ -9,6 +9,10 @@
 // the segment, in (t, slot) order (a stable counting sort), and the rest of the segment is padding.  pos[a] is the row
 // of assignment a, row_tok[r] the assignment of row r (-1 for a padding row).
 //
+// Weights.  w[a] is the raw top-k probability, or with NORM (Qwen3-MoE's norm_topk_prob) p_sel / S, S the fp32 sum of
+// the token's k selected probabilities added in slot order and the quotient correctly rounded (__fdiv_rn).  Only w
+// differs: p, idx and every table are the raw form's bits.  The router backward recomputes S the same way.
+//
 // Ties.  Experts are ranked by their fp32 probability as moe_topk_kernel computes it, ties to the lower expert.  That
 // includes probabilities that underflow to 0 (a row whose logits span more than about 104): they tie, so the lower
 // experts win.
@@ -30,7 +34,10 @@ namespace {
 constexpr int kMaxE = kMoeMaxExperts;
 constexpr int kEPerLane = kMaxE / 32;
 
-// one warp per token: fp32 softmax over the E logits, then k rounds of a warp argmax (ties to the lower expert)
+// one warp per token: fp32 softmax over the E logits, then k rounds of a warp argmax (ties to the lower expert); NORM
+// then divides the token's w row by the sum of its entries (every lane holds the same sum: each round's result is
+// known to all lanes), each lane rescaling the slots lane, lane + 32, ...
+template <bool NORM>
 __global__ void moe_topk_kernel(const __nv_bfloat16* __restrict__ logits, long long ldl, int T, int E, int k,
                                 float* __restrict__ p, int* __restrict__ idx, float* __restrict__ w) {
   const int lane = threadIdx.x & 31;
@@ -65,6 +72,7 @@ __global__ void moe_topk_kernel(const __nv_bfloat16* __restrict__ logits, long l
 #pragma unroll
   for (int j = 0; j < kEPerLane; ++j)
     if (lane + 32 * j < E && v[j] != v[j]) v[j] = -0.5f;
+  float sum = 0.f;   // NORM: the selected probabilities in slot order (NaN for a NaN row)
   for (int slot = 0; slot < k; ++slot) {
     float best = -2.f;
     int be = 0x7fffffff;
@@ -81,9 +89,14 @@ __global__ void moe_topk_kernel(const __nv_bfloat16* __restrict__ logits, long l
       idx[t * k + slot] = be;
       w[t * k + slot] = best == -0.5f ? nan_f() : best;
     }
+    if constexpr (NORM) sum += best == -0.5f ? nan_f() : best;
 #pragma unroll
     for (int j = 0; j < kEPerLane; ++j)
       if (lane + 32 * j == be) v[j] = -1.f;
+  }
+  if constexpr (NORM) {
+    __syncwarp();   // lane 0's w stores are visible to the warp
+    for (int slot = lane; slot < k; slot += 32) w[t * k + slot] = __fdiv_rn(w[t * k + slot], sum);
   }
 }
 
@@ -247,13 +260,31 @@ __global__ void moe_combine_kernel(const __nv_bfloat16* __restrict__ yp, long lo
   }
 }
 
-// one warp per token: dp = dw at the selected experts (+ dpsum[e] everywhere), dlogits = bf16(p * (dp - sum p dp))
+// one warp per token: dp = dw at the selected experts (+ dpsum[e] everywhere), dlogits = bf16(p * (dp - sum p dp)).
+// NORM (w = p_sel / S): the selected experts' dp is (dw_j - sum_i w_i dw_i) / S instead, with S and w recomputed from
+// p and idx as the forward computed them, and the sum over slots in slot order.
+template <bool NORM>
 __global__ void moe_router_bwd_kernel(const float* __restrict__ p, const int* __restrict__ idx,
                                       const float* __restrict__ dw, const float* __restrict__ dpsum, int T, int E,
                                       int k, __nv_bfloat16* __restrict__ dlogits) {
   const int lane = threadIdx.x & 31;
   const long long t = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (t >= T) return;
+  // NORM: S and sum_i w_i dw_i, the same on every lane.  An idx entry outside [0, E) is not followed: its probability
+  // reads as NaN, so the token's row of dlogits is NaN.
+  float S = 1.f, wdw = 0.f;
+  if constexpr (NORM) {
+    S = 0.f;
+    for (int s = 0; s < k; ++s) {
+      const int e = idx[t * k + s];
+      S += (unsigned)e < (unsigned)E ? p[t * E + e] : nan_f();
+    }
+    for (int s = 0; s < k; ++s) {
+      const int e = idx[t * k + s];
+      const float pe = (unsigned)e < (unsigned)E ? p[t * E + e] : nan_f();
+      wdw = fmaf(__fdiv_rn(pe, S), dw[t * k + s], wdw);
+    }
+  }
   float pv[kEPerLane], dp[kEPerLane];
   float dot = 0.f;
 #pragma unroll
@@ -262,7 +293,10 @@ __global__ void moe_router_bwd_kernel(const float* __restrict__ p, const int* __
     pv[j] = e < E ? p[t * E + e] : 0.f;
     dp[j] = (e < E && dpsum) ? dpsum[e] : 0.f;
     for (int s = 0; s < k; ++s)
-      if (idx[t * k + s] == e) dp[j] += dw[t * k + s];
+      if (idx[t * k + s] == e) {
+        if constexpr (NORM) dp[j] += __fdiv_rn(dw[t * k + s] - wdw, S);
+        else dp[j] += dw[t * k + s];
+      }
     dot = fmaf(pv[j], dp[j], dot);
   }
   dot = warp_sum(dot);
@@ -284,10 +318,11 @@ int row_threads(int H) {
 long long moe_rows_cap(long long T, int E, int k) { return ((T * k + (long long)E * 127) + 127) / 128 * 128; }
 long long moe_route_scratch(long long T, int E) { return (T + 31) / 32 * E; }
 
-void moe_route(const void* logits, long long ldl, int T, int E, int k, float* p, int* idx, float* w, int* pos,
-               int* seg, int* tile_expert, int* row_tok, int* counts, int* scratch, cudaStream_t s) {
+void moe_route(const void* logits, long long ldl, int T, int E, int k, bool norm_topk, float* p, int* idx, float* w,
+               int* pos, int* seg, int* tile_expert, int* row_tok, int* counts, int* scratch, cudaStream_t s) {
   const int nchunks = (T + 31) / 32;
-  moe_topk_kernel<<<(T + 7) / 8, 256, 0, s>>>((const __nv_bfloat16*)logits, ldl, T, E, k, p, idx, w);
+  (norm_topk ? moe_topk_kernel<true> : moe_topk_kernel<false>)<<<(T + 7) / 8, 256, 0, s>>>(
+      (const __nv_bfloat16*)logits, ldl, T, E, k, p, idx, w);
   DTG_LAUNCH_CHECK();
   moe_rank_kernel<<<(nchunks + 7) / 8, 256, 0, s>>>(idx, T, E, k, scratch, pos);
   DTG_LAUNCH_CHECK();
@@ -330,9 +365,10 @@ void moe_combine_bwd(const void* dy, int T, const void* yp, const int* row_tok, 
 }
 
 void moe_router_bwd(const float* p, const int* idx, const float* dw, const float* dpsum, int T, int E, int k,
-                    void* dlogits, cudaStream_t s) {
+                    bool norm_topk, void* dlogits, cudaStream_t s) {
   if (T == 0) return;
-  moe_router_bwd_kernel<<<(T + 7) / 8, 256, 0, s>>>(p, idx, dw, dpsum, T, E, k, (__nv_bfloat16*)dlogits);
+  (norm_topk ? moe_router_bwd_kernel<true> : moe_router_bwd_kernel<false>)<<<(T + 7) / 8, 256, 0, s>>>(
+      p, idx, dw, dpsum, T, E, k, (__nv_bfloat16*)dlogits);
   DTG_LAUNCH_CHECK();
   note_launch();
 }

@@ -32,7 +32,9 @@ int64_t check_seg(const Tensor& seg, const Tensor& like, const char* who) {
   return E;
 }
 
-std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> moe_route(const Tensor& logits, int64_t k) {
+// norm_topk: each token's w row is its top-k probabilities divided by their sum (Qwen3-MoE's norm_topk_prob)
+std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> moe_route(const Tensor& logits, int64_t k,
+                                                                                     bool norm_topk) {
   const char* who = "moe_route";
   TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kBFloat16 && logits.dim() == 2 && logits.stride(1) == 1,
               who, ": logits must be a bf16 CUDA [T, E] tensor with a contiguous last dimension");
@@ -54,8 +56,8 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> moe_r
     tile_expert.fill_(-1);
     return {p, idx, w, pos, seg, tile_expert, row_tok, counts};
   }
-  dtg::moe_route(logits.data_ptr(), logits.stride(0), (int)T, (int)E, (int)k, p.data_ptr<float>(), idx.data_ptr<int>(),
-                 w.data_ptr<float>(), pos.data_ptr<int>(), seg.data_ptr<int>(), tile_expert.data_ptr<int>(),
+  dtg::moe_route(logits.data_ptr(), logits.stride(0), (int)T, (int)E, (int)k, norm_topk, p.data_ptr<float>(),
+                 idx.data_ptr<int>(), w.data_ptr<float>(), pos.data_ptr<int>(), seg.data_ptr<int>(), tile_expert.data_ptr<int>(),
                  row_tok.data_ptr<int>(), counts.data_ptr<int>(), scratch.data_ptr<int>(), stream());
   return {p, idx, w, pos, seg, tile_expert, row_tok, counts};
 }
@@ -117,7 +119,9 @@ std::tuple<Tensor, Tensor> moe_combine_bwd(const Tensor& dy, const Tensor& yp, c
   return {dyp, dw};
 }
 
-Tensor moe_router_bwd(const Tensor& p, const Tensor& idx, const Tensor& dw, const c10::optional<Tensor>& dpsum) {
+// norm_topk: the backward of the renormalised weights moe_route(..., norm_topk=True) wrote
+Tensor moe_router_bwd(const Tensor& p, const Tensor& idx, const Tensor& dw, const c10::optional<Tensor>& dpsum,
+                      bool norm_topk) {
   const char* who = "moe_router_bwd";
   check_t(p, p, at::kFloat, 2, who, "p");
   check_t(idx, p, at::kInt, 2, who, "idx");
@@ -133,8 +137,8 @@ Tensor moe_router_bwd(const Tensor& p, const Tensor& idx, const Tensor& dw, cons
   const c10::cuda::CUDAGuard guard(p.device());
   Tensor dlogits = torch::empty({T, E}, p.options().dtype(at::kBFloat16));
   dtg::moe_router_bwd(p.data_ptr<float>(), idx.data_ptr<int>(), dw.data_ptr<float>(),
-                      dpsum.has_value() ? dpsum->data_ptr<float>() : nullptr, (int)T, (int)E, (int)k, dlogits.data_ptr(),
-                      stream());
+                      dpsum.has_value() ? dpsum->data_ptr<float>() : nullptr, (int)T, (int)E, (int)k, norm_topk,
+                      dlogits.data_ptr(), stream());
   return dlogits;
 }
 
@@ -185,14 +189,14 @@ void gemm_grouped(int64_t mode, const Tensor& a, const Tensor& b, Tensor& out, c
 
 namespace dtg {
 void bind_moe(pybind11::module_& m) {
-  m.def("moe_route", &::moe_route, pybind11::arg("logits"), pybind11::arg("k"));
+  m.def("moe_route", &::moe_route, pybind11::arg("logits"), pybind11::arg("k"), pybind11::arg("norm_topk") = false);
   m.def("moe_permute", &::moe_permute, pybind11::arg("x"), pybind11::arg("row_tok"), pybind11::arg("seg"),
         pybind11::arg("k"));
   m.def("moe_combine", &::moe_combine, pybind11::arg("yp"), pybind11::arg("pos"), pybind11::arg("w") = pybind11::none());
   m.def("moe_combine_bwd", &::moe_combine_bwd, pybind11::arg("dy"), pybind11::arg("yp"), pybind11::arg("row_tok"),
         pybind11::arg("seg"), pybind11::arg("w"));
   m.def("moe_router_bwd", &::moe_router_bwd, pybind11::arg("p"), pybind11::arg("idx"), pybind11::arg("dw"),
-        pybind11::arg("dpsum") = pybind11::none());
+        pybind11::arg("dpsum") = pybind11::none(), pybind11::arg("norm_topk") = false);
   m.def("gemm_grouped", &::gemm_grouped, pybind11::arg("mode"), pybind11::arg("a"), pybind11::arg("b"),
         pybind11::arg("out"), pybind11::arg("seg"), pybind11::arg("tile_expert") = pybind11::none(),
         pybind11::arg("accumulate") = false);

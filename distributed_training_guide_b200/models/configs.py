@@ -5,7 +5,8 @@ guide uses (reference: every chapter's ``-m/--model-name`` flag, e.g.
 ``02-distributed-data-parallel/train_llm.py:57``) are resolved from this table
 instead of the hub.  A local directory containing a ``config.json`` is also
 accepted, and tiny ``debug-*`` configs exist for tests.  Families: Llama 2 / 3 / 3.1 / 3.2, Mistral, Qwen3, Qwen2.5,
-OLMo 2 (``allenai/OLMo-2-*``, ``model_type: "olmo2"``), OLMoE (``allenai/OLMoE-*``, ``model_type: "olmoe"``), StarCoder2 (``bigcode/starcoder2-*``,
+OLMo 2 (``allenai/OLMo-2-*``, ``model_type: "olmo2"``), OLMoE (``allenai/OLMoE-*``, ``model_type: "olmoe"``), Qwen3-MoE
+(``Qwen/Qwen3-30B-A3B``, ``Qwen/Qwen3-235B-A22B``, ``model_type: "qwen3_moe"``), StarCoder2 (``bigcode/starcoder2-*``,
 ``model_type: "starcoder2"``), GPT-NeoX / Pythia (``EleutherAI/pythia-*``, ``model_type: "gpt_neox"``) and GPT-2.
 """
 from __future__ import annotations
@@ -18,13 +19,15 @@ from typing import Optional
 
 @dataclasses.dataclass
 class ModelConfig:
-    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "olmo2" | "starcoder2" | "gpt_neox" | "gpt2"; mistral is
+    arch: str  # "llama" | "mistral" | "qwen3" | "qwen2" | "olmo2" | "olmoe" | "qwen3_moe" | "starcoder2" | "gpt_neox" |
+    # "gpt2"; mistral is
     # llama with a sliding attention window, qwen3 llama with QK-norm and a head_dim of its own, qwen2 llama with q/k/v
     # biases, olmo2 llama with a full-width QK-norm and post-sublayer norms instead of the pre-norms (``full_qk_norm``,
     # ``post_norm``), starcoder2 llama with LayerNorms, a GELU MLP and biases on every projection (``layer_norm``,
     # ``gelu_mlp``, ``all_bias``), gpt_neox starcoder2's block with a parallel residual, partial rotary embeddings
     # and an exact GELU (``parallel_residual``, ``rotary_dim``, ``gelu_exact``), olmoe llama with OLMo 2's full-width
-    # QK-norm (still pre-norm) and a mixture-of-experts MLP (``moe``)
+    # QK-norm (still pre-norm) and a mixture-of-experts MLP (``moe``), qwen3_moe qwen3 with olmoe's MLP
+    # (``intermediate_size`` is then each expert's, HF's ``moe_intermediate_size``)
     vocab_size: int
     hidden_size: int
     intermediate_size: int
@@ -54,6 +57,8 @@ class ModelConfig:
     #: ``num_experts_per_tok`` of them with the highest router probability run on each token
     num_experts: int = 0
     num_experts_per_tok: int = 0
+    #: Qwen3-MoE: each token's routing weights are its top-k probabilities divided by their sum, not the raw ones
+    norm_topk_prob: bool = False
     name: str = ""
 
     @property
@@ -85,9 +90,10 @@ class ModelConfig:
 
     @property
     def moe(self) -> bool:
-        """OLMoE's MLP: a router picks each token's top ``num_experts_per_tok`` of ``num_experts`` SwiGLU experts and
-        sums their outputs weighted by the raw router probabilities (``ops.moe``)."""
-        return self.arch == "olmoe"
+        """OLMoE's and Qwen3-MoE's MLP: a router picks each token's top ``num_experts_per_tok`` of ``num_experts``
+        SwiGLU experts and sums their outputs weighted by the router probabilities, raw or renormalised
+        (``norm_topk_prob``) (``ops.moe``)."""
+        return self.arch in ("olmoe", "qwen3_moe")
 
     @property
     def layer_norm(self) -> bool:
@@ -197,6 +203,11 @@ def _olmoe(name, h, i, l, nh, nkv, experts, top_k, v=50304, maxpos=4096):
     )
 
 
+def _qwen3_moe(name, h, i, l, nh, nkv, experts, top_k, v=151936, maxpos=40960, norm_topk_prob=True):
+    return dataclasses.replace(_qwen3(name, h, i, l, nh, nkv, False, v=v, maxpos=maxpos), arch="qwen3_moe",
+                               num_experts=experts, num_experts_per_tok=top_k, norm_topk_prob=norm_topk_prob)
+
+
 def _starcoder2(name, h, i, l, nh, nkv, theta, tied, v=49152, maxpos=16384, window=4096):
     return ModelConfig(
         arch="starcoder2", vocab_size=v, hidden_size=h, intermediate_size=i, num_hidden_layers=l,
@@ -262,6 +273,13 @@ REGISTRY = {
     # parameters, about 1.3B active per token.  The shapes are those of the public config.json as recalled when this
     # table was written; no copy of the file was at hand to check them against.
     "allenai/OLMoE-1B-7B-0924": _olmoe("allenai/OLMoE-1B-7B-0924", 2048, 1024, 16, 16, 16, 64, 8),
+    # Qwen3-MoE: Qwen3's per-head QK-norm at head_dim 128, 128 experts, top-8 with renormalised weights, untied; the
+    # intermediate size is each expert's (moe_intermediate_size).  30,532,122,624 and 235,093,634,560 parameters, as
+    # transformers' Qwen3MoeForCausalLM counts them.  The shapes are those of the public config.json files as recalled
+    # when this table was written; no copy of those files was at hand to check them against.
+    "Qwen/Qwen3-30B-A3B": _qwen3_moe("Qwen/Qwen3-30B-A3B", 2048, 768, 48, 32, 4, 128, 8),
+    "Qwen/Qwen3-30B-A3B-Base": _qwen3_moe("Qwen/Qwen3-30B-A3B-Base", 2048, 768, 48, 32, 4, 128, 8),
+    "Qwen/Qwen3-235B-A22B": _qwen3_moe("Qwen/Qwen3-235B-A22B", 4096, 1536, 94, 64, 4, 128, 8),
     # StarCoder2: LayerNorms, a GELU MLP, biases on every projection, sliding window 4096; head_dim 128 at every size.
     # Shapes, RoPE theta, window, norm eps and max positions are those of the public config.json files as recalled
     # when this table was written; no copy of those files was at hand to check them against.  transformers'
@@ -294,6 +312,9 @@ REGISTRY = {
     "debug-olmo2": _olmo2("debug-olmo2", 512, 1024, 2, 4, 2, v=1024, maxpos=2048),
     # 2 heads x 128 over a hidden size of 256, 8 experts of intermediate size 128, top-2
     "debug-olmoe": _olmoe("debug-olmoe", 256, 128, 2, 2, 2, 8, 2, v=1024, maxpos=2048),
+    # 4 q heads and 2 kv heads x 128 = 512 over a hidden size of 256, 16 experts of intermediate size 128, top-4 with
+    # renormalised weights
+    "debug-qwen3-moe": _qwen3_moe("debug-qwen3-moe", 256, 128, 2, 4, 2, 16, 4, v=1024, maxpos=2048),
     # 4 q heads and 2 kv heads x 128 over a hidden size of 512, tied, with StarCoder2's block
     "debug-starcoder2": _starcoder2("debug-starcoder2", 512, 2048, 2, 4, 2, 1e5, True, v=1024, maxpos=2048),
     # 4 heads x 128 over a hidden size of 512 with rotary on 32 of them, and 4 heads x 64 over 256 with rotary on 16,
@@ -323,6 +344,8 @@ def _from_hf_dict(d: dict, name: str) -> ModelConfig:
         return _gpt_neox_from_hf_dict(d, name)
     if mt == "olmoe":
         return _olmoe_from_hf_dict(d, name)
+    if mt == "qwen3_moe":
+        return _qwen3_moe_from_hf_dict(d, name)
     if mt not in ("llama", "mistral", "qwen3", "qwen2", "olmo2"):
         raise ValueError(f"unsupported model_type {mt!r} in {name}")
     if mt == "olmo2":
@@ -465,6 +488,55 @@ def _olmoe_from_hf_dict(d: dict, name: str) -> ModelConfig:
         max_position_embeddings=d.get("max_position_embeddings", 4096), rms_norm_eps=d.get("rms_norm_eps", 1e-5),
         rope_theta=theta, tie_word_embeddings=d.get("tie_word_embeddings", False),
         num_experts=d.get("num_experts", 64), num_experts_per_tok=d.get("num_experts_per_tok", 8), name=name,
+    )
+
+
+def _qwen3_moe_from_hf_dict(d: dict, name: str) -> ModelConfig:
+    """A ``Qwen3MoeConfig`` payload: every layer sparse, routing weights raw or renormalised (``norm_topk_prob``,
+    false by default as in ``Qwen3MoeConfig``).  Every setting the kernel path does not implement is refused, naming
+    its key, rather than dropped; ``router_aux_loss_coef`` and ``output_router_logits`` are training options
+    (``--router-aux-loss-coef``), not part of the model."""
+    if d.get("mlp_only_layers"):
+        raise ValueError(f"{name}: mlp_only_layers is {d['mlp_only_layers']!r}; dense layers between the sparse ones "
+                         "are not supported, only [] (every layer sparse)")
+    if d.get("decoder_sparse_step", 1) != 1:
+        raise ValueError(f"{name}: decoder_sparse_step is {d['decoder_sparse_step']!r}; dense layers between the "
+                         "sparse ones are not supported, only 1 (every layer sparse)")
+    if d.get("use_sliding_window"):
+        raise ValueError(f"{name}: use_sliding_window is true; Qwen3-MoE sliding-window layers are not supported")
+    if "sliding_attention" in (d.get("layer_types") or ()):
+        raise ValueError(f"{name}: layer_types contains 'sliding_attention'; Qwen3-MoE sliding-window layers are not "
+                         "supported")
+    if d.get("attention_bias"):
+        raise ValueError(f"{name}: attention_bias is true; q/k/v/o projections with a bias are not supported")
+    if d.get("hidden_act", "silu") != "silu":
+        raise ValueError(f"{name}: hidden_act is {d['hidden_act']!r}; only 'silu' (SwiGLU experts) is supported")
+    rp = d.get("rope_parameters") if isinstance(d.get("rope_parameters"), dict) else None
+    rope = rp if rp is not None else d.get("rope_scaling")
+    if rope and (rope.get("rope_type") or rope.get("type") or "default") != "default":
+        key = "rope_parameters" if rp is not None else "rope_scaling"
+        raise ValueError(f"{name}: {key} has type {rope.get('rope_type') or rope.get('type')!r}; only the default "
+                         "RoPE is supported for Qwen3-MoE")
+    for key in ("attention_dropout", "hidden_dropout", "dropout"):
+        if d.get(key, 0.0):
+            raise ValueError(f"{name}: {key} is {d[key]!r}; the kernel path has no dropout, set {key} to 0.0 to "
+                             "train without it")
+    experts = d.get("num_experts", d.get("num_local_experts", 128))
+    if experts > 256:
+        raise ValueError(f"{name}: num_experts is {experts}; the routing kernels serve at most 256 experts")
+    head_dim = d.get("head_dim") or d["hidden_size"] // d["num_attention_heads"]
+    if head_dim != 128:
+        raise ValueError(f"{name}: head_dim is {head_dim}; Qwen3-MoE's per-head QK-norm kernel serves head_dim 128")
+    theta = (rp or {}).get("rope_theta", d.get("rope_theta", 1e6))
+    return ModelConfig(
+        arch="qwen3_moe", vocab_size=d["vocab_size"], hidden_size=d["hidden_size"],
+        intermediate_size=d.get("moe_intermediate_size", 768), num_hidden_layers=d["num_hidden_layers"],
+        num_attention_heads=d["num_attention_heads"],
+        num_key_value_heads=d.get("num_key_value_heads", d["num_attention_heads"]),
+        max_position_embeddings=d.get("max_position_embeddings", 32768), rms_norm_eps=d.get("rms_norm_eps", 1e-6),
+        rope_theta=theta, tie_word_embeddings=d.get("tie_word_embeddings", False), explicit_head_dim=128,
+        qk_norm=True, num_experts=experts, num_experts_per_tok=d.get("num_experts_per_tok", 8),
+        norm_topk_prob=bool(d.get("norm_topk_prob", False)), name=name,
     )
 
 
@@ -628,6 +700,19 @@ def to_hf_config_dict(cfg: ModelConfig) -> dict:
             "clip_qkv": None, "num_experts": cfg.num_experts, "num_experts_per_tok": cfg.num_experts_per_tok,
             "norm_topk_prob": False, "output_router_logits": False, "router_aux_loss_coef": 0.01,
             "pad_token_id": 1, "bos_token_id": None, "eos_token_id": 50279, "torch_dtype": "bfloat16",
+        }
+    if cfg.arch == "qwen3_moe":
+        d = {
+            "model_type": "qwen3_moe", "architectures": ["Qwen3MoeForCausalLM"], "vocab_size": cfg.vocab_size,
+            "hidden_size": cfg.hidden_size, "moe_intermediate_size": cfg.intermediate_size,
+            "num_hidden_layers": cfg.num_hidden_layers, "num_attention_heads": cfg.num_attention_heads,
+            "num_key_value_heads": cfg.num_key_value_heads, "head_dim": cfg.head_dim,
+            "max_position_embeddings": cfg.max_position_embeddings, "rms_norm_eps": cfg.rms_norm_eps,
+            "rope_theta": cfg.rope_theta, "hidden_act": "silu", "tie_word_embeddings": cfg.tie_word_embeddings,
+            "attention_bias": False, "attention_dropout": 0.0, "use_sliding_window": False, "decoder_sparse_step": 1,
+            "mlp_only_layers": [], "num_experts": cfg.num_experts, "num_experts_per_tok": cfg.num_experts_per_tok,
+            "norm_topk_prob": cfg.norm_topk_prob, "output_router_logits": False, "router_aux_loss_coef": 0.001,
+            "bos_token_id": 151643, "eos_token_id": 151645, "torch_dtype": "bfloat16",
         }
     if cfg.arch == "llama" and cfg.explicit_head_dim is not None:
         d["head_dim"] = cfg.explicit_head_dim

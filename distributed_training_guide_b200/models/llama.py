@@ -2,7 +2,8 @@
 Llama plus QK-norm, with a head_dim of its own; Qwen2: Llama plus q/k/v biases; OLMo 2: Llama with a full-width
 QK-norm and RMSNorms after each sublayer instead of before it; StarCoder2: Llama with LayerNorms, a c_fc -> GELU-tanh
 -> c_proj MLP and a bias on every projection; GPT-NeoX: StarCoder2's parameters with a parallel residual, partial
-rotary embeddings and an exact GELU; OLMoE: Llama with OLMo 2's full-width QK-norm and a mixture-of-experts MLP).  One ``LlamaDecoderLayer`` builds every family's layer from its
+rotary embeddings and an exact GELU; OLMoE: Llama with OLMo 2's full-width QK-norm and a mixture-of-experts MLP; Qwen3-MoE: Qwen3 with OLMoE's
+mixture-of-experts MLP, its routing weights optionally renormalised).  One ``LlamaDecoderLayer`` builds every family's layer from its
 ``ModelConfig``, and ``decoder_layout`` fixes its flat-buffer layout.
 
 Same module tree and parameter names as ``transformers``' ``LlamaForCausalLM`` (what
@@ -253,11 +254,13 @@ class OlmoeExperts(nn.Module):
 
 
 class OlmoeMoE(nn.Module):
-    """OLMoE's sparse MLP: the router ``gate`` [E, H] and the experts (``ops.moe``)."""
+    """The sparse MLP of OLMoE and Qwen3-MoE (the same parameters): the router ``gate`` [E, H] and the experts
+    (``ops.moe``); Qwen3-MoE may renormalise each token's routing weights (``norm_topk_prob``)."""
 
     def __init__(self, config: ModelConfig, dtype=None, device=None):
         super().__init__()
         self.top_k = config.num_experts_per_tok
+        self.norm_topk_prob = config.norm_topk_prob
         self.gate = Linear(config.hidden_size, config.num_experts, dtype, device)
         self.experts = OlmoeExperts(config, dtype, device)
 
@@ -380,7 +383,8 @@ class LlamaDecoderLayer(nn.Module):
     def _mlp(self, y):
         if isinstance(self.mlp, OlmoeMoE):
             m = self.mlp
-            out, psum, counts = ops.moe(y, m.gate.weight, m.experts.gate_up_proj, m.experts.down_proj, m.top_k)
+            out, psum, counts = ops.moe(y, m.gate.weight, m.experts.gate_up_proj, m.experts.down_proj, m.top_k,
+                                        m.norm_topk_prob)
             self.router_stats = (counts, psum)
             return out
         down = self.mlp.down_proj if isinstance(self.mlp, LlamaMLP) else self.mlp.c_proj

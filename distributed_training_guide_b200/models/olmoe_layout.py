@@ -1,6 +1,6 @@
-"""OLMoE's published checkpoint layout and ours.
+"""The published mixture-of-experts checkpoint layout of OLMoE and Qwen3-MoE, and ours.
 
-Published OLMoE checkpoints store one tensor per expert: ``model.layers.{i}.mlp.experts.{j}.{gate,up,down}_proj.weight``
+Published OLMoE and Qwen3-MoE checkpoints (the same expert parameter names) store one tensor per expert: ``model.layers.{i}.mlp.experts.{j}.{gate,up,down}_proj.weight``
 ([I, H], [I, H], [H, I]).  The model here (and transformers 5 in memory) holds each layer's experts as two 3-D
 parameters, ``mlp.experts.gate_up_proj`` [E, 2I, H] (expert j's gate rows, then its up rows) and ``mlp.experts.down_proj``
 [E, H, I].  Every other name is shared.  This module is the one place that knows the mapping: ``HFReader`` serves our

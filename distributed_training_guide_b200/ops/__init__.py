@@ -823,7 +823,7 @@ def swiglu(gu):
 
 
 # --------------------------------------------------------------------------------------
-# mixture-of-experts MLP (OLMoE): router top-k, permute, grouped expert GEMMs, SwiGLU, combine
+# mixture-of-experts MLP (OLMoE, Qwen3-MoE): router top-k, permute, grouped expert GEMMs, SwiGLU, combine
 # --------------------------------------------------------------------------------------
 class _MoE(torch.autograd.Function):
     """Forward: router logits on the wgmma GEMM; ``moe_route`` (fp32 softmax, top-k, the stable expert-sorted
@@ -833,11 +833,12 @@ class _MoE(torch.autograd.Function):
     gradient, then ``moe_router_bwd`` and the router's GEMMs.  No step reads a count back to the host."""
 
     @staticmethod
-    def forward(ctx, x, gate_w, gate_up, down, k):
+    def forward(ctx, x, gate_w, gate_up, down, k, norm_topk_prob):
         C = _ext.load()
         x2 = x.reshape(-1, x.shape[-1])
         x2 = x2 if x2.is_contiguous() else x2.contiguous()
         ctx.x_shape = x.shape
+        ctx.norm_topk_prob = norm_topk_prob
         ctx.empty = x2.shape[0] == 0
         if ctx.empty:   # no token: nothing to route and no kernel to launch
             ctx.save_for_backward(gate_w, gate_up, down)
@@ -846,7 +847,7 @@ class _MoE(torch.autograd.Function):
             ctx.mark_non_differentiable(counts)
             return x2.new_empty(x.shape), torch.zeros(E, dtype=torch.float32, device=x.device), counts
         logits = gemm(x2, gate_w, trans_b=True)
-        p, idx, w, pos, seg, tiles, row_tok, counts = C.moe_route(logits, k)
+        p, idx, w, pos, seg, tiles, row_tok, counts = C.moe_route(logits, k, norm_topk_prob)
         xp = C.moe_permute(x2, row_tok, seg, k)
         R = xp.shape[0]
         gu = torch.empty(R, gate_up.shape[1], dtype=x.dtype, device=x.device)
@@ -866,7 +867,7 @@ class _MoE(torch.autograd.Function):
         if ctx.empty:   # zero weight gradients: overwrite with zeros, or leave an accumulating buffer as it is
             zero = lambda out, acc: None if acc else out.zero_()
             grads = tuple(_emit_weight_grad(t, zero, t) for t in ctx.saved_tensors)
-            return (dy.new_zeros(ctx.x_shape),) + grads + (None,)
+            return (dy.new_zeros(ctx.x_shape),) + grads + (None, None)
         x2, gate_w, gate_up, down, p, idx, w, pos, seg, tiles, row_tok, xp, gu, h, yp = ctx.saved_tensors
         dy2 = dy.reshape(-1, dy.shape[-1]).contiguous()
         dyp, dw = C.moe_combine_bwd(dy2, yp, row_tok, seg, w)
@@ -879,23 +880,24 @@ class _MoE(torch.autograd.Function):
         d_gate_up = _emit_weight_grad(gate_up, lambda out, acc: C.gemm_grouped(2, dgu, xp, out, seg, None, acc),
                                       gate_up)
         dx = C.moe_combine(dxp, pos)
-        dlogits = C.moe_router_bwd(p, idx, dw, dpsum.contiguous() if dpsum is not None else None)
+        dlogits = C.moe_router_bwd(p, idx, dw, dpsum.contiguous() if dpsum is not None else None, ctx.norm_topk_prob)
         gemm(dlogits, gate_w, out=dx, accumulate=True)
         d_gate = _emit_weight_grad(gate_w, lambda out, acc: gemm(dlogits, x2, out=out, trans_a=True, accumulate=acc),
                                    gate_w)
-        return dx.view(ctx.x_shape), d_gate, d_gate_up, d_down, None
+        return dx.view(ctx.x_shape), d_gate, d_gate_up, d_down, None, None
 
 
-def moe(x, gate_w, gate_up, down, k):
-    """OLMoE's sparse MLP: each token goes through its top-``k`` experts by router probability, weighted by those
-    probabilities (``ref.moe``).  x [..., H], gate_w [E, H], gate_up [E, 2I, H] (gate rows first), down [E, H, I].
+def moe(x, gate_w, gate_up, down, k, norm_topk_prob=False):
+    """OLMoE's and Qwen3-MoE's sparse MLP: each token goes through its top-``k`` experts by router probability,
+    weighted by those probabilities, or with ``norm_topk_prob`` (Qwen3-MoE) by those probabilities divided by their
+    sum (``ref.moe``).  x [..., H], gate_w [E, H], gate_up [E, 2I, H] (gate rows first), down [E, H, I].
     Returns ``(y, psum, counts)``: y like x; psum fp32 [E], the column sums of the router probabilities (the aux loss
     differentiates through it); counts int32 [E], the assignments per expert.  bf16 CUDA tensors run the sm_90a
     kernels; the weight gradients go through ``_emit_weight_grad``."""
     if _ext.use_cuda_kernel("moe", x, gate_w, gate_up, down) and x.dtype == torch.bfloat16:
-        return _MoE.apply(x, gate_w, gate_up, down, k)
+        return _MoE.apply(x, gate_w, gate_up, down, k, bool(norm_topk_prob))
     x2 = x.reshape(-1, x.shape[-1])
-    y, p = ref.moe(x2, gate_w, gate_up, down, k)
+    y, p = ref.moe(x2, gate_w, gate_up, down, k, norm_topk_prob)
     counts = torch.bincount(torch.topk(p.detach(), k, dim=-1).indices.reshape(-1), minlength=gate_w.shape[0])
     return y.view(x.shape), p.sum(0), counts.to(torch.int32)
 

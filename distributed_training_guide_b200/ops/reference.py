@@ -138,20 +138,23 @@ def swiglu(gu):
     return (F.silu(g.float()) * u.float()).to(gu.dtype)
 
 
-def moe_route(x, gate_w, k):
-    """OLMoE's router in fp32: ``(p, w, idx)`` with p = softmax(x @ gate_w.T) [T, E], and w, idx [T, k] the top-k
-    probabilities (kept raw, ``norm_topk_prob: false``) and their experts."""
+def moe_route(x, gate_w, k, norm_topk_prob=False):
+    """The MoE router in fp32: ``(p, w, idx)`` with p = softmax(x @ gate_w.T) [T, E], and w, idx [T, k] the top-k
+    probabilities and their experts.  w is kept raw (OLMoE, ``norm_topk_prob: false``) or divided by its row sum in
+    fp32 (Qwen3-MoE's ``norm_topk_prob: true``, as ``Qwen3MoeTopKRouter`` does it)."""
     p = torch.softmax(x.float() @ gate_w.float().t(), dim=-1)
     w, idx = torch.topk(p, k, dim=-1)
+    if norm_topk_prob:
+        w = w / w.sum(dim=-1, keepdim=True)
     return p, w, idx
 
 
-def moe(x, gate_w, gate_up, down, k):
-    """OLMoE's sparse MLP in fp32, one expert at a time: ``sum_slot w[t, slot] * expert_idx[t, slot](x_t)`` with
+def moe(x, gate_w, gate_up, down, k, norm_topk_prob=False):
+    """The sparse MLP of OLMoE and Qwen3-MoE in fp32, one expert at a time: ``sum_slot w[t, slot] * expert_idx[t, slot](x_t)`` with
     ``expert_e(x) = down[e] @ (silu(g) * u)``, ``[g | u] = gate_up[e] @ x``.  x [T, H], gate_w [E, H], gate_up
     [E, 2I, H], down [E, H, I].  Returns ``(y in x.dtype, p)`` with p the fp32 router probabilities [T, E]."""
     xf = x.float()
-    p, w, idx = moe_route(xf, gate_w, k)
+    p, w, idx = moe_route(xf, gate_w, k, norm_topk_prob)
     out = torch.zeros_like(xf)
     for e in range(gate_up.shape[0]):
         tok, slot = (idx == e).nonzero(as_tuple=True)

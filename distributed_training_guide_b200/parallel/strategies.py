@@ -212,7 +212,7 @@ def _apply_router_aux_loss(args, model):
     if coef < 0:
         raise ValueError(f"router_aux_loss_coef must be >= 0, got {coef}")
     if not getattr(getattr(model, "config", None), "moe", False):
-        raise ValueError("router_aux_loss_coef applies to mixture-of-experts models (OLMoE)")
+        raise ValueError("router_aux_loss_coef applies to mixture-of-experts models (OLMoE, Qwen3-MoE)")
     model.router_aux_loss_coef = coef
 
 

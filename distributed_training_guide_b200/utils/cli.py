@@ -65,7 +65,7 @@ def get_parser(chapter: str = "01-single-gpu", require_experiment: bool = False)
                    help="load local Hugging Face safetensors for --model-name (chapter 05 defaults to auto: load "
                         "them when they exist on disk; other chapters default to never = random init)")
     p.add_argument("--router-aux-loss-coef", default=0.0, type=float,
-                   help="mixture-of-experts models (OLMoE): add this times the Switch load-balancing loss of every "
+                   help="mixture-of-experts models (OLMoE, Qwen3-MoE): add this times the Switch load-balancing loss of every "
                         "layer's router to the loss (transformers' load_balancing_loss_func); the log record then "
                         "carries aux_loss (default: 0, off)")
     if "fp8" in extras:
