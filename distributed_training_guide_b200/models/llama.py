@@ -345,7 +345,8 @@ class LlamaDecoderLayer(nn.Module):
         self._fused = {}  # name -> FusedWeight, installed by parallel.flat.install_fused_views
         self.tp = None  # set through LlamaForCausalLM.tp: the layer runs TensorParallelRuntime.layer_forward
         self.fp8 = False  # set through LlamaForCausalLM.fp8: the projections run in fp8
-        #: OLMoE: (assignments per expert int32 [E], router probability column sums fp32 [E]) of the last forward
+        #: OLMoE: (assignments per expert int32 [E], router probability column sums fp32 [E]) of the forward in flight;
+        #: the model's forward takes them and sets this back to None
         self.router_stats = None
 
     def fused_weight(self, name):
@@ -555,6 +556,13 @@ class LlamaForCausalLM(nn.Module):
                              "checkpointing drops: train with --router-aux-loss-coef 0 or without "
                              "--checkpoint-activations")
         y = self.decoder(input_ids, cos, sin, doc_start)
+        # the router statistics are read here and nowhere else: a layer must not keep them past its forward, because
+        # their autograd graph reaches the engine's boundaries, whose callbacks hold the engine and so the model, and
+        # that cycle runs through autograd nodes the garbage collector cannot see (the model would never be freed)
+        stats = [layer.router_stats for layer in m.layers] if self.config.moe else None
+        if stats is not None:
+            for layer in m.layers:
+                layer.router_stats = None
         logits = self.lm_head(y.reshape(B * S, -1))  # [T, V], a fresh tensor the loss may consume
         loss = aux_loss = None
         if labels is not None:
@@ -568,7 +576,6 @@ class LlamaForCausalLM(nn.Module):
                 loss = ops.cross_entropy(logits, tgt)
                 logits = None  # its storage now holds dlogits (CUDA path)
             if aux:
-                stats = [layer.router_stats for layer in m.layers]
                 aux_loss = ref.router_aux_loss([c for c, _ in stats], [p for _, p in stats], B * S,
                                                self.config.num_experts)
                 loss = loss + self.router_aux_loss_coef * aux_loss

@@ -1,4 +1,8 @@
-"""NVLink symmetric-memory collectives vs torch.distributed (NCCL) results — needs >= 2 GPUs."""
+"""NVLink symmetric-memory collectives vs torch.distributed (NCCL) results — needs >= 2 GPUs.
+
+The numerics of the plain-DDP and FSDP engines at world size 1 (loss, every gradient as AdamW consumed it and the
+update, against an fp32 model and bit for bit against the single-GPU engine) are checked on one GPU by
+``test_gpu_engines_reference.py``; this file remains the check over real NVLink."""
 import math
 
 import pytest

@@ -1,5 +1,9 @@
 """Tensor-parallel fused kernels (AG->GEMM, GEMM->RS, K-gathered wgrad, vocab-parallel CE, hidden-parallel
-embedding) on 2 GPUs vs a single-GPU run with the same seed and batch."""
+embedding) on 2 GPUs vs a single-GPU run with the same seed and batch.
+
+The numerics of the tensor-parallel and FSDP engines at world size 1 (loss, every gradient as AdamW consumed it and
+the update, against an fp32 model) are checked on one GPU by ``test_gpu_engines_reference.py``; this file remains
+the check over real NVLink."""
 import pytest
 import torch
 

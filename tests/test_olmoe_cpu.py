@@ -294,3 +294,41 @@ def test_router_aux_loss_flag():
     with pytest.raises(ValueError, match="mixture-of-experts"):
         _apply_router_aux_loss(a, build_llama(get_config("debug-llama"), dtype=torch.float32, device="meta",
                                               init=False))
+
+
+@pytest.mark.parametrize("coef", [0.0, 0.01])
+def test_model_under_an_engine_is_freed(coef):
+    """A layer must not keep its router statistics past the forward: their autograd graph reaches the engine's
+    boundaries, whose callbacks hold the engine and so the model, and a reference from the layer would close a cycle
+    through autograd nodes that the garbage collector cannot see (the model, and with FSDP the symmetric gradient
+    slots its parameters point into, would never be freed)."""
+    import gc
+    import weakref
+
+    from distributed_training_guide_b200.parallel.ddp import boundary
+
+    class Hooks:   # the engines' hook protocol, with a boundary in front of every layer bound to the engine
+        def pre_forward(self, model):
+            pass
+
+        def pre_layer(self, i, layer, x, residual):
+            return boundary(lambda: self.model, x, residual)
+
+        def post_layer(self, i, layer, x, residual):
+            return x, residual
+
+        def pre_head(self, x, residual):
+            return x, residual
+
+    cfg = get_config("debug-olmoe")
+    model = build_llama(cfg, dtype=torch.float32)
+    model.router_aux_loss_coef = coef
+    model.engine = Hooks()
+    model.engine.model = model
+    ids = torch.randint(0, cfg.vocab_size, (1, 32), generator=torch.Generator().manual_seed(0))
+    model(input_ids=ids, labels=ids).loss.backward()
+    assert all(layer.router_stats is None for layer in model.model.layers)
+    alive = weakref.ref(model.model.layers[0].mlp.gate.weight)
+    del model
+    gc.collect()
+    assert alive() is None, "the model outlived its last reference"
