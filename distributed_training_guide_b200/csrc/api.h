@@ -124,7 +124,7 @@ void adamw_flat(void* p, const void* g, void* m, void* v, long long n, float lr,
 //   a_kmajor: A stored [M,K] (else [K,M]);  b_kmajor: B stored [N,K] (else [K,N]).
 // lda/ldb/ldc are row strides in elements.  variant: 0 = auto, 1 = 1-CTA 128x256, 2 = 2-CTA cluster 256x256
 // bias: null, or bf16 [N] added to every row before the rounding to bf16 (forward layout, a_kmajor and b_kmajor,
-// overwrite mode only; 16-byte aligned).  The same holds for the bias of gemm_fp8 (e4m3 A), _ag and _bgather.
+// overwrite mode only; 16-byte aligned).  The same holds for the bias of gemm_fp8 (e4m3 A) and gemm_bf16_ag.
 void gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, long long lda, long long ldb, long long ldc,
                bool a_kmajor, bool b_kmajor, bool accumulate, int variant, cudaStream_t s, const void* bias = nullptr);
 
@@ -140,10 +140,6 @@ void gemm_bf16_dist(int mode, const void* const* a_srcs, const void* const* b_sr
                     int K, long long lda, long long ldb, long long ldc, bool b_kmajor, bool accumulate, int nranks,
                     int rank, int rows_per_peer, cudaStream_t s);
 
-void gemm_bf16_bgather(const void* A, void* full_base, void* C, int M, int N, int K, long long lda, long long ldb,
-                       long long ldc, bool b_kmajor, const void* const* shards, long long per_bytes, long long w_off,
-                       long long w_bytes, uint32_t* counters, uint32_t target, int chunk_shift, uint32_t* const* pads,
-                       int nranks, int rank, uint32_t bar_epoch, cudaStream_t s, const void* bias = nullptr);
 void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int N, int K, long long ldb, long long ldc,
                   bool b_kmajor, int nranks, int rank, int rows_per_peer, uint32_t* flags, uint32_t ag_epoch,
                   uint32_t* const* pads, uint32_t bar_epoch, int n_comm, cudaStream_t s, const void* bias = nullptr);

@@ -212,24 +212,6 @@ void comm_allgather_ce(const SymmPtrs& shards, void* full, const SymmPads& pads,
   }
 }
 
-// full[begin, end) <- the same flat element range from the ranks' shards (NOT rotated pointers: shards.ptr[p] is rank p)
-void comm_gather_range_ce(const SymmPtrs& shards, void* full, const SymmPads& pads, size_t begin, size_t end, size_t per,
-                          int rank, int nranks, uint32_t epoch, int* err, bool barrier, cudaStream_t s) {
-  if (barrier) {
-    barrier_kernel<<<1, 32, 0, s>>>(pads, rank, nranks, epoch, err);
-    note_launch();
-    DTG_LAUNCH_CHECK();
-  }
-  for (int p = 0; p < nranks; ++p) {
-    const size_t lo = begin > (size_t)p * per ? begin : (size_t)p * per;
-    const size_t hi = end < (size_t)(p + 1) * per ? end : (size_t)(p + 1) * per;
-    if (lo >= hi) continue;
-    DTG_CUDA_CHECK(cudaMemcpyAsync((char*)full + lo * sizeof(__nv_bfloat16),
-                                   shards.ptr[p] + (lo - (size_t)p * per) * sizeof(__nv_bfloat16),
-                                   (hi - lo) * sizeof(__nv_bfloat16), cudaMemcpyDeviceToDevice, s));
-  }
-}
-
 void comm_reduce_scatter(const SymmPtrs& grads, void* out, const SymmPads& pads, size_t elem_off, size_t n, float scale,
                          int rank, int nranks, uint32_t epoch, int* err, int blocks, cudaStream_t s) {
   check_geometry(n, nranks, blocks);

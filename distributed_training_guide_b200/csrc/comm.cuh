@@ -32,8 +32,6 @@ void comm_allgather(const SymmPtrs& shards, void* full, const SymmPads& pads, si
                     int nranks, uint32_t epoch, int* err, bool barrier, int blocks, cudaStream_t s);
 void comm_allgather_ce(const SymmPtrs& shards, void* full, const SymmPads& pads, size_t shard_off, size_t per, int rank,
                        int nranks, uint32_t epoch, int* err, bool barrier, cudaStream_t s);
-void comm_gather_range_ce(const SymmPtrs& shards, void* full, const SymmPads& pads, size_t begin, size_t end, size_t per,
-                          int rank, int nranks, uint32_t epoch, int* err, bool barrier, cudaStream_t s);
 void comm_reduce_scatter(const SymmPtrs& grads, void* out, const SymmPads& pads, size_t elem_off, size_t n, float scale,
                          int rank, int nranks, uint32_t epoch, int* err, int blocks, cudaStream_t s);
 void comm_barrier(const SymmPads& pads, int rank, int nranks, uint32_t epoch, int* err, cudaStream_t s);

@@ -227,23 +227,6 @@ void allgather(const std::vector<uint64_t>& shards, Tensor& full, const std::vec
                  (int)shards.size(), (uint32_t)epoch, e, barrier, (int)blocks, stream());
 }
 
-void gather_range(const std::vector<uint64_t>& shards, Tensor& full, const std::vector<uint64_t>& pads, int64_t begin,
-                  int64_t end, int64_t per, int64_t rank, int64_t epoch, const c10::optional<Tensor>& err, bool barrier) {
-  const char* who = "comm_gather_range";
-  check_peers(who, shards, "shards", pads, rank);
-  check_count(who, "per", per);
-  check_count(who, "begin", begin);
-  check_local(who, "full", full, at::kBFloat16);
-  TORCH_CHECK(begin <= end && end <= full.numel(), who, ": bad range [", begin, ", ", end, ") of a full buffer of ",
-              full.numel(), " elements");
-  TORCH_CHECK(end <= per * (int64_t)shards.size(), who, ": range end ", end, " lies past the ", shards.size(),
-              " shards of ", per, " elements");
-  SymmPtrs sp{};
-  for (size_t k = 0; k < shards.size(); ++k) sp.ptr[k] = (char*)shards[k];
-  comm_gather_range_ce(sp, full.data_ptr(), pads_of(pads), (size_t)begin, (size_t)end, (size_t)per, (int)rank,
-                       (int)shards.size(), (uint32_t)epoch, err_ptr(who, err), barrier, stream());
-}
-
 void reduce_scatter(const std::vector<uint64_t>& grads, Tensor& out, const std::vector<uint64_t>& pads, int64_t elem_off,
                     int64_t n, double scale, int64_t rank, int64_t epoch, const c10::optional<Tensor>& err,
                     int64_t blocks) {
@@ -357,7 +340,6 @@ void bind_comm(pybind11::module_& m) {
   m.def("comm_nvls_allreduce_scale", &nvls_allreduce_scale);
   m.def("comm_nvls_rs_adamw", &nvls_rs_adamw);
   m.def("comm_reduce_scatter", &reduce_scatter);
-  m.def("comm_gather_range", &gather_range);
   m.def("comm_barrier", &barrier);
   m.def("comm_reduce_sumsq", &reduce_sumsq);
   m.def("comm_nvls_reduce_sumsq", &nvls_reduce_sumsq);

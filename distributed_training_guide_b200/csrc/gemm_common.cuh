@@ -28,10 +28,7 @@ struct GemmCfg {
   // A_MODE 3 communication CTAs reuse the pipeline smem as a ring of COMM_SLOTS pieces
   static constexpr int COMM_PIECE = 32768;
   static constexpr int COMM_SLOTS = STAGES * STAGE_BYTES / COMM_PIECE;
-  // B_MODE 3 (operand B gathered from the ranks' FSDP shards by warp 1 of every CTA): a 2-slot bounce ring
-  static constexpr int GATHER_PIECE = 16384;
-  static constexpr int GATHER_BYTES = 2 * GATHER_PIECE;
-  // TMA-store epilogue (every mode but B_MODE 3 and C_MODE 1): each consumer warpgroup stages half of its 64 x 256
+  // TMA-store epilogue (every mode but C_MODE 1): each consumer warpgroup stages half of its 64 x 256
   // output rows at a time, as two 64 x 64 boxes of 128B-swizzled bf16, behind the barrier area rounded up to 1 KB
   static constexpr int EPI_BOX_BYTES = 64 * 64 * 2;
   static constexpr int EPI_WG_BYTES = 2 * EPI_BOX_BYTES;
@@ -71,23 +68,7 @@ struct GemmDist {
   int n_comm;                        // clusters (CTA pairs) that copy instead of multiplying
   int rank, nranks;
   long long tile_bytes;              // bytes of one 256-row tile of A (contiguous: lda == K)
-  // B_MODE 3 (FSDP unshard inside the consuming GEMM): operand B is a weight whose bytes [bg_begin, bg_end) of the
-  // group's flat layout are spread over the ranks' shards (rank p owns flat bytes [p*per, (p+1)*per)).  Warp 1 of
-  // every CTA bounces 16 KB pieces shard -> smem -> local full buffer and counts them per `1 << bg_chunk_shift`
-  // byte chunk; the TMA producer acquires the counters of the chunks under a B box before loading it.
-  const char* bg_src[kMaxRanks];     // shard base per rank (NOT rotated; [rank] is my own shard)
-  char* bg_dst;                      // local full (unsharded) flat buffer of the group
-  long long bg_per_bytes;            // shard size in bytes
-  long long bg_begin, bg_end;        // flat byte range of B (piece aligned; chunk aligned at both ends)
-  union {
-    uint32_t* bg_cnt;                // one counter per chunk of the flat buffer (monotonic over generations)
-    const int* grp_seg;              // grouped: int32 [experts + 1], expert e owns rows [seg[e], seg[e + 1])
-  };
-  uint32_t bg_target;                // counter value at which a chunk of this generation is complete
-  int bg_chunk_shift;                // log2(chunk bytes)
-  int bg_row_bytes;                  // bytes of one row of B as stored (ldb * 2)
-  int bg_rows;                       // rows of B as stored
-  int n_tile_shift;                  // rotate the N tile order so every rank starts on the rows it owns
+  const int* grp_seg;                // grouped: int32 [experts + 1], expert e owns rows [seg[e], seg[e + 1])
   // L2-aware rasterisation of the plain GEMM: tiles run M-fastest inside groups of `group_m` row tiles (0 = one
   // group = the whole M extent); `num_n_tiles` is set by the launcher.
   int group_m, num_n_tiles;
@@ -118,8 +99,7 @@ __host__ __device__ __forceinline__ void tile_mn(int t, int num_m_tiles, const G
       return;
     }
     m = tile_m(t, num_m_tiles, d);
-    n = t / num_m_tiles + d.n_tile_shift;
-    if (n >= d.num_n_tiles && d.n_tile_shift) n -= d.num_n_tiles;
+    n = t / num_m_tiles;
     return;
   }
   const int num_n = d.k_shift;  // reused field: number of N tiles (K is never gathered in this mode)

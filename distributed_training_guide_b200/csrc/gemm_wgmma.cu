@@ -2,7 +2,6 @@
 // TMA into 128B-swizzled shared memory), persistent and warp-specialised, 384 threads:
 //
 //   warpgroup 0   warp 0  TMA producer     (one elected lane)   smem ring: full/empty mbarriers
-//                 warp 1  B_MODE 3 gather  (one elected lane)   FSDP unshard inside the GEMM
 //   warpgroups 1-2        consumers        64 rows of the 128 x 256 tile each: wgmma m64n256k16 from shared
 //                                          memory, then registers -> bf16 -> shared -> TMA store (optionally
 //                                          C += ..., with C TMA-loaded into the same staging area)
@@ -37,7 +36,7 @@ using namespace ptx;
 //                    (all-gather -> GEMM);  2 = the reduction dimension K gathered from the ranks (wgrad
 //                    over a sequence-sharded activation).  Tiles are fetched from the owning peer by TMA
 //                    over NVLink, so the transfer streams under the MMA pipeline.
-//                    3 = all-gather by COMMUNICATION CTAs of this same kernel: the first `n_comm` CTA pairs
+//   A_MODE           3 = all-gather by COMMUNICATION CTAs of this same kernel: the first `n_comm` CTA pairs
 //                    bulk-copy (cp.async.bulk, NVLink -> smem -> local HBM) the peers' row tiles into the
 //                    local [M, K] buffer and publish a per-tile flag; the GEMM CTAs start on the local rows and
 //                    acquire the flag before their TMA touches a fetched tile.  Each remote byte crosses NVLink
@@ -48,19 +47,10 @@ using namespace ptx;
 // Epilogue.  A local C (C_MODE 0) leaves through shared memory: each consumer warpgroup converts half of its 64 x 256
 // accumulator block at a time into a 32 KB staging area and one thread stores it with two TMA boxes, which clip at M
 // and N, so no element needs a bounds test and the writes are whole 128-byte lines.  Accumulate mode TMA-loads the C
-// boxes into the same staging area first and adds them there.  B_MODE 3 keeps the register epilogue (its gather
-// bounce ring already fills shared memory to within 2 KB of the limit), and so does C_MODE 1 (its rows go to the
-// peers' staging buffers, one base pointer per owner, which one tensor map cannot describe).
-template <int B_MODE, int C_MODE>
-constexpr bool kTmaEpilogue = (B_MODE != 3 && C_MODE != 1);
-// B_MODE 3 helpers.  Chunks are waited for in the order the gather warps fetch them: the chunks behind my own slice
-// of [bg_begin, bg_end) first, then the ones in front of it; my own chunks are local and never waited for.
-__device__ __forceinline__ long long bg_clamp(const GemmDist& d, long long x) {
-  return x < d.bg_begin ? d.bg_begin : (x > d.bg_end ? d.bg_end : x);
-}
-__device__ __forceinline__ int bg_rotation_chunks(const GemmDist& d) {   // first chunk (relative) behind my slice
-  return (int)((bg_clamp(d, (long long)(d.rank + 1) * d.bg_per_bytes) - d.bg_begin) >> d.bg_chunk_shift);
-}
+// boxes into the same staging area first and adds them there.  C_MODE 1 keeps the register epilogue: its rows go to
+// the peers' staging buffers, one base pointer per owner, which one tensor map cannot describe.
+template <int C_MODE>
+constexpr bool kTmaEpilogue = (C_MODE != 1);
 
 // ET selects the operand element type: 0 = bf16 (every mode above); 1 = fp8, A e4m3 and B e4m3; 2 = fp8, A e5m2 and B
 // e4m3.  The fp8 forms take both operands K-major and plain (mode 0): the fp8 wgmma has no transposed operands, so
@@ -100,14 +90,14 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
                              (GRP == 1 ? A_K : (!A_K && !B_K))),
                 "the grouped GEMM is a plain bf16 single-CTA GEMM: GRP 1 with A K-major, GRP 2 with both MN-major");
   using Cfg = GemmCfg<CG>;
-  constexpr bool TMA_EPI = kTmaEpilogue<B_MODE, C_MODE>;
+  constexpr bool TMA_EPI = kTmaEpilogue<C_MODE>;
   constexpr int BK = ET ? 2 * Cfg::BK : Cfg::BK;   // elements of K per stage: one 128-byte span either way
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
-  uint64_t* comm_bar = bars + 2 * Cfg::STAGES;  // [COMM_SLOTS] (A_MODE 3) or [2] (B_MODE 3)
+  uint64_t* comm_bar = bars + 2 * Cfg::STAGES;  // [COMM_SLOTS] (A_MODE 3)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -149,8 +139,6 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
     }
     if constexpr (A_MODE == 3)
       for (int i = 0; i < Cfg::COMM_SLOTS; ++i) mbar_init(&comm_bar[i], 1);
-    if constexpr (B_MODE == 3)
-      for (int i = 0; i < 2; ++i) mbar_init(&comm_bar[i], 1);
     fence_barrier_init();
   }
   if (CG == 2) cluster_sync(); else __syncthreads();
@@ -209,38 +197,6 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
     if (elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
-      // B_MODE 3: chunks of B complete (roughly) in the order the gather warps copy them — starting at my own shard.
-      // `bg_wm` = how many chunks, in that order, this CTA has already seen complete; a B box is readable once the
-      // watermark has passed the last chunk under its rows.  Every chunk counter is polled at most once per CTA.
-      [[maybe_unused]] int bg_wm = 0;
-      [[maybe_unused]] const int bg_nch = (B_MODE == 3) ? (int)((dist.bg_end - dist.bg_begin) >> dist.bg_chunk_shift) : 0;
-      [[maybe_unused]] const int bg_rot = (B_MODE == 3) ? bg_rotation_chunks(dist) : 0;
-      [[maybe_unused]] const int bg_my0 = (B_MODE == 3)
-          ? (int)((bg_clamp(dist, (long long)dist.rank * dist.bg_per_bytes) - dist.bg_begin) >> dist.bg_chunk_shift) : 0;
-      [[maybe_unused]] const int bg_tail = bg_nch - bg_rot;          // remote chunks behind my slice: fetched first
-      [[maybe_unused]] auto bg_wait_rows = [&](int r0, int r1) {   // rows [r0, r1) of B as stored
-        if (r1 > dist.bg_rows) r1 = dist.bg_rows;
-        if (r0 >= r1) return;
-        const int c0 = (int)(((long long)r0 * dist.bg_row_bytes) >> dist.bg_chunk_shift);
-        const int c1 = (int)((((long long)r1 * dist.bg_row_bytes) - 1) >> dist.bg_chunk_shift);
-        int need = 0;                                  // highest fetch-order index under the rows, + 1
-        for (int c = c0; c <= c1; ++c) {
-          if (c >= bg_my0 && c < bg_rot) continue;     // my own chunk: already local
-          const int ci = c >= bg_rot ? c - bg_rot : bg_tail + c;
-          need = ci + 1 > need ? ci + 1 : need;
-        }
-        if (need <= bg_wm) return;
-        const uint32_t* cnt = dist.bg_cnt + (dist.bg_begin >> dist.bg_chunk_shift);
-        while (bg_wm < need) {
-          const int c = bg_wm < bg_tail ? bg_rot + bg_wm : bg_wm - bg_tail;
-          const unsigned long long t0 = global_timer_ns();
-          while ((int32_t)(ld_acquire_gpu(cnt + c) - dist.bg_target) < 0)
-            if (global_timer_ns() - t0 > kWaitTimeoutNs)
-              __trap();  // FSDP gather GEMM: a weight chunk never arrived
-          ++bg_wm;
-        }
-        fence_proxy_async_all();                       // the chunk was written through the async proxy (bulk stores)
-      };
       for (int t = cluster_id; t < num_tiles; t += num_clusters) {
         int tm_, tn_;
         [[maybe_unused]] int g_e = 0, g_k0 = 0;
@@ -264,7 +220,6 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
             fence_proxy_async_all();
           }
         }
-        if constexpr (B_MODE == 3 && B_K) bg_wait_rows(nb, nb + Cfg::B_ROWS);   // forward: B rows are output features
         if constexpr (A_MODE == 1) {  // this row block lives on rank m0 / rows_per_peer
           const int peer = m0 / dist.rows_per_peer;
           tmA_p = &tmAs.m[peer];
@@ -272,7 +227,7 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
         }
         for (int kbi = 0; kbi < tile_kb; ++kbi) {
           // K-gathered operands start with the local rank's slice of K
-          const int kb = (A_MODE == 2 || B_MODE == 2 || (B_MODE == 3 && !B_K)) ? (kbi + dist.k_shift) % num_kb : kbi;
+          const int kb = (A_MODE == 2 || B_MODE == 2) ? (kbi + dist.k_shift) % num_kb : kbi;
           const int k0 = kb * BK;
           int a_k0 = k0, b_k0 = k0;
           if constexpr (GRP == 2) {   // the expert's rows of both operands
@@ -291,7 +246,6 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
             tmB_p = &tmBs.m[peer];
             b_k0 = k0 - peer * dist.rows_per_peer;
           }
-          if constexpr (B_MODE == 3 && !B_K) bg_wait_rows(k0, k0 + Cfg::BK);      // dgrad: B rows are the reduction index
           const CUtensorMap& tmA = *tmA_p;
           const CUtensorMap& tmB = *tmB_p;
           mbar_wait_mma(&empty[stage], phase ^ 1);   // (CG 2: the peer's consumers released it too)
@@ -323,74 +277,6 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
             }
           }
           if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1 && !is_comm) {
-    // ===================== B_MODE 3: gather warp (FSDP unshard inside the consuming GEMM) =====================
-    if constexpr (B_MODE == 3) {
-      if (elect_one()) {
-        constexpr uint32_t PIECE = Cfg::GATHER_PIECE;
-        uint8_t* gs = smem + Cfg::STAGES * Cfg::STAGE_BYTES + Cfg::BAR_BYTES;
-        const int ch = (int)blockIdx.x, nr = dist.nranks, rk = dist.rank;
-        // Optional entry barrier (bar_epoch != 0): every peer has started its copy of this kernel.  The FSDP engine
-        // does not need it: shards only change inside the fused reduce-scatter+AdamW kernels, whose exit barrier
-        // every rank's compute stream joins before the next step's first GEMM.
-        for (int p = 0; p < nr && dist.bar_epoch; ++p)
-          st_release_sys(dist.pads[p] + ch * kMaxRanks + rk, dist.bar_epoch);
-        for (int p = 0; p < nr && dist.bar_epoch; ++p) {
-          const uint32_t* mine = dist.pads[rk] + ch * kMaxRanks + p;
-          const unsigned long long t0 = global_timer_ns();
-          while ((int32_t)(ld_acquire_sys(mine) - dist.bar_epoch) < 0)
-            if (global_timer_ns() - t0 > kWaitTimeoutNs)
-              __trap();  // FSDP gather GEMM: peer did not arrive at the entry barrier
-        }
-        // pieces of [bg_begin, bg_end) that live on OTHER ranks, visited starting right after my own slice (the
-        // local slice was copied into the full buffer before this kernel started: engine-side D2D prefetch)
-        static_assert(PIECE == (1u << 14), "16 KB pieces");
-        const long long my_lo = bg_clamp(dist, (long long)rk * dist.bg_per_bytes);
-        const long long my_hi = bg_clamp(dist, (long long)(rk + 1) * dist.bg_per_bytes);
-        const long long total = (dist.bg_end - dist.bg_begin) / PIECE;
-        const long long mine = (my_hi - my_lo) / PIECE;
-        const long long np = total - mine;                               // remote pieces
-        const long long after = (dist.bg_end - my_hi) / PIECE;           // remote pieces behind my slice
-        uint32_t* const cnt = dist.bg_cnt;
-        auto flat_of = [&](long long i) {                                // i-th remote piece in visiting order
-          return i < after ? my_hi + i * (long long)PIECE : dist.bg_begin + (i - after) * (long long)PIECE;
-        };
-        auto issue = [&](long long i, uint32_t it) {
-          const long long flat = flat_of(i);
-          const int owner = (int)(flat / dist.bg_per_bytes);
-          const char* src = dist.bg_src[owner] + (flat - (long long)owner * dist.bg_per_bytes);
-          const uint32_t slot = it & 1;
-          mbar_arrive_expect_tx(&comm_bar[slot], PIECE);
-          bulk_load_g2s(gs + slot * PIECE, src, PIECE, &comm_bar[slot]);
-        };
-        const long long first = blockIdx.x, stride = gridDim.x;
-        uint32_t it = 0;
-        long long prev_flat = -1;
-        if (first < np) issue(first, 0);
-        for (long long i = first; i < np; i += stride, ++it) {
-          if (i + stride < np) {
-            bulk_wait_group_read<0>();   // the store that last read the other slot (piece it-1) is done with it
-            issue(i + stride, it + 1);
-          }
-          const uint32_t slot = it & 1;
-          mbar_wait_mma(&comm_bar[slot], (it >> 1) & 1);
-          const long long flat = flat_of(i);
-          bulk_store_s2g(dist.bg_dst + flat, gs + slot * PIECE, PIECE);
-          bulk_commit_group();
-          if (prev_flat >= 0) {          // piece it-1 is complete in local memory once only this store is pending
-            bulk_wait_group<1>();
-            fence_proxy_async_all();
-            red_release_gpu_add(cnt + (prev_flat >> dist.bg_chunk_shift), 1u);
-          }
-          prev_flat = flat;
-        }
-        if (prev_flat >= 0) {
-          bulk_wait_group<0>();
-          fence_proxy_async_all();
-          red_release_gpu_add(cnt + (prev_flat >> dist.bg_chunk_shift), 1u);
         }
       }
     }
@@ -472,7 +358,7 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
       fence_regs(acc);
       if (prev >= 0) release(prev);
       // epilogue: accumulator fragment (x dequantisation scale, fp8) -> bf16 pairs -> staging area -> TMA store
-      // (B_MODE 3 and C_MODE 1: -> global from registers)
+      // (C_MODE 1: -> global from registers)
       [[maybe_unused]] float deq = 1.f;
       if constexpr (ET != 0) deq = scale_a[0] * scale_b[0];
       if constexpr (TMA_EPI) {
@@ -565,11 +451,7 @@ gemm_bf16_kernel(const __grid_constant__ TmapSet<(A_MODE ? kMaxRanks : 1)> tmAs,
               y *= deq;
             }
             __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(crow + col);
-            if constexpr (BIAS) {
-              const float2 g = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(bias + col));
-              x += g.x;
-              y += g.y;
-            } else if (accumulate) {
+            if (accumulate) {
               const float2 g = __bfloat1622float2(*p);
               x += g.x;
               y += g.y;
@@ -704,11 +586,10 @@ static void launch_gemm(const void* const* a_srcs, const void* const* b_srcs, vo
   const int num_tiles = num_m_tiles * num_n_tiles * (GRP == 2 ? groups : 1);
   // C in 64 x 64 boxes (the staging layout of the epilogue); the other modes store from registers
   CUtensorMap tmC{};
-  if constexpr (kTmaEpilogue<B_MODE, C_MODE>)
+  if constexpr (kTmaEpilogue<C_MODE>)
     tmC = make_tmap_2d(C, N, (uint64_t)M * (GRP == 2 ? groups : 1), ldc * 2, 64, 64);
   auto kern = gemm_bf16_kernel<A_K, B_K, CG, A_MODE, B_MODE, C_MODE, ET, BIAS>;
-  constexpr int kSmem = kTmaEpilogue<B_MODE, C_MODE> ? Cfg::SMEM_BYTES_EPI
-                                                     : Cfg::SMEM_BYTES + (B_MODE == 3 ? Cfg::GATHER_BYTES : 0);
+  constexpr int kSmem = kTmaEpilogue<C_MODE> ? Cfg::SMEM_BYTES_EPI : Cfg::SMEM_BYTES;
   static bool attr_set = false;
   if (!attr_set) {
     DTG_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
@@ -909,8 +790,7 @@ void gemm_fp8(const void* A, const void* B, void* C, int M, int N, int K, long l
 //
 // Empty calls, here and in gemm_bf16_ag: with M or N = 0 nothing is launched (and nothing gathered); with K = 0 the
 // product is zero, so overwrite mode writes zeros over C (mode 2: over every owner's rows_per_peer rows) and
-// accumulate mode leaves C unchanged, as in gemm_bf16.  gemm_bf16_bgather refuses empty calls instead: its chunk
-// counters must advance one generation per call, or the next call would wait for chunks that never arrive.
+// accumulate mode leaves C unchanged, as in gemm_bf16.
 void gemm_bf16_dist(int mode, const void* const* a_srcs, const void* const* b_srcs, void* const* c_dsts, int M, int N,
                     int K, long long lda, long long ldb, long long ldc, bool b_kmajor, bool accumulate, int nranks,
                     int rank, int rows_per_peer, cudaStream_t s) {
@@ -1003,64 +883,6 @@ void gemm_bf16_ag(const void* const* a_bufs, const void* B, void* C, int M, int 
   else launch_gemm<true, false, 2, 3, 0, 0>(as, bs, C, M, N, K, K, ldb, ldc, false, dist, nranks, s);
 }
 
-
-// FSDP unshard fused into the consuming GEMM (B_MODE 3): C[M,N] = A . op(B) where B is a weight of a flat parameter
-// group whose bytes are spread over the ranks' shards.  `full_base` is the local unsharded flat buffer of the group
-// (B = full_base + w_off bytes, row-major with leading dimension ldb); `shards[p]` rank p's shard (per_bytes each,
-// rank p owns flat bytes [p*per, (p+1)*per)).  The kernel's gather warps copy [w_off, w_off + w_bytes) out of the
-// shards into the full buffer while its tensor cores consume the rows that have already arrived.
-void gemm_bf16_bgather(const void* A, void* full_base, void* C, int M, int N, int K, long long lda, long long ldb,
-                       long long ldc, bool b_kmajor, const void* const* shards, long long per_bytes, long long w_off,
-                       long long w_bytes, uint32_t* counters, uint32_t target, int chunk_shift, uint32_t* const* pads,
-                       int nranks, int rank, uint32_t bar_epoch, cudaStream_t s, const void* bias) {
-  using Cfg = GemmCfg<2>;
-  if ((N % 8) || (ldc % 8) || (lda % 8) || (ldb % 8))
-    throw std::runtime_error("gemm_bf16_bgather: N and the leading dimensions must be multiples of 8 elements");
-  check_bias("gemm_bf16_bgather", bias, true, b_kmajor, false, K);
-  if (nranks < 1 || nranks > kMaxRanks || rank < 0 || rank >= nranks)
-    throw std::runtime_error("gemm_bf16_bgather: 1..8 ranks and a rank among them");
-  if (M <= 0 || N <= 0 || K <= 0)
-    throw std::runtime_error("gemm_bf16_bgather: empty GEMM (the chunk counters must advance one generation per call)");
-  if (chunk_shift < 14 || chunk_shift > 30) throw std::runtime_error("gemm_bf16_bgather: chunk_shift outside [14, 30]");
-  if (w_off < 0 || w_bytes < 0 || w_off + w_bytes > (long long)nranks * per_bytes)
-    throw std::runtime_error("gemm_bf16_bgather: the weight range must lie inside the shards");
-  const long long chunk = 1LL << chunk_shift;
-  if (chunk < Cfg::GATHER_PIECE || (w_off % chunk) || (w_bytes % chunk) || (per_bytes % chunk))
-    throw std::runtime_error("gemm_bf16_bgather: weight offset / size / shard size must be multiples of the chunk size");
-  const int b_rows = b_kmajor ? N : K;                 // rows of B as stored
-  const int b_cols = b_kmajor ? K : N;
-  if (ldb != b_cols || (long long)b_rows * b_cols * 2 > w_bytes)
-    throw std::runtime_error("gemm_bf16_bgather: B must be a dense row-major weight inside the gathered range");
-  if (sm_count() > 256 /* kMaxChannels of the signal pad (comm.cuh) */) throw std::runtime_error("gemm_bf16_bgather: more CTAs than signal-pad channels");
-  GemmDist dist{};
-  for (int p = 0; p < nranks; ++p) {
-    dist.bg_src[p] = (const char*)shards[p];
-    dist.pads[p] = pads[p];
-  }
-  dist.bg_dst = (char*)full_base;
-  dist.bg_per_bytes = per_bytes;
-  dist.bg_begin = w_off;
-  dist.bg_end = w_off + w_bytes;
-  dist.bg_cnt = counters;
-  dist.bg_target = target;
-  dist.bg_chunk_shift = chunk_shift;
-  dist.bg_row_bytes = (int)(ldb * 2);
-  dist.bg_rows = b_rows;
-  dist.rank = rank;
-  dist.nranks = nranks;
-  dist.bar_epoch = bar_epoch;
-  // start on the rows this rank owns (their copy is local): rotate the N tiles (forward) / K blocks (dgrad)
-  long long my_row = ((long long)rank * per_bytes - w_off) / (ldb * 2);
-  if (my_row < 0 || my_row >= b_rows) my_row = 0;
-  if (b_kmajor) dist.n_tile_shift = (int)(my_row / Cfg::BN);
-  else dist.k_shift = (int)(my_row / Cfg::BK);
-  const void* as[1] = {A};
-  const void* bs[1] = {(const char*)full_base + w_off};
-  if (bias) launch_gemm<true, true, 2, 0, 3, 0, 0, true>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s,
-                                                          nullptr, nullptr, bias);
-  else if (b_kmajor) launch_gemm<true, true, 2, 0, 3, 0>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s);
-  else launch_gemm<true, false, 2, 0, 3, 0>(as, bs, C, M, N, K, lda, ldb, ldc, false, dist, nranks, s);
-}
 
 // Grouped GEMM of the mixture-of-experts layers (GRP 1 and 2 above), one launch for every expert; the routing tables
 // seg [groups + 1] and tile_expert [rows / 128] are device pointers written by moe_route (moe.cu).

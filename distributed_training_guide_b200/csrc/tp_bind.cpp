@@ -16,7 +16,7 @@ namespace {
 using torch::Tensor;
 inline cudaStream_t stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
-// bias [N] of the all-gather / gather GEMMs' forward (b_kmajor) form: each refusal names the argument
+// bias [N] of the all-gather GEMM's forward (b_kmajor) form: each refusal names the argument
 const void* check_bias(const c10::optional<Tensor>& bias, const Tensor& out, bool b_kmajor, const char* who) {
   if (!bias.has_value()) return nullptr;
   const Tensor& b = *bias;
@@ -39,7 +39,7 @@ SymmPtrs plain(const std::vector<uint64_t>& ptrs) {
 }
 
 // ---- distributed GEMMs and the partial-sum reduce ----------------------------------------------------------------
-// gemm_dist, gemm_ag, gemm_bgather and tp_reduce_parts validate their arguments with check_dist before anything is
+// gemm_dist, gemm_ag and tp_reduce_parts validate their arguments with check_dist before anything is
 // launched.  The kernels index their peer-pointer arrays by rank and owner, so a list of the wrong length or a rank
 // out of range would read or write through a pointer nobody passed.
 using PeerList = std::tuple<const std::vector<uint64_t>*, const char*, int64_t>;   // list, name, entries read
@@ -124,44 +124,6 @@ void py_gemm_ag(const std::vector<uint64_t>& a_bufs, const Tensor& b, Tensor& ou
   dtg::gemm_bf16_ag(as, b.data_ptr(), out.data_ptr(), M, N, K, b.stride(0), out.stride(0), b_kmajor, (int)nr, (int)rank,
                     (int)rows_per_peer, (uint32_t*)flags.data_ptr<int>(), (uint32_t)ag_epoch, pd, (uint32_t)bar_epoch,
                     (int)n_comm, stream(), bp);
-}
-
-// C = a @ op(B) with B = a weight inside the flat buffer `full` (element offset w_off, w_numel elements), gathered
-// from the ranks' shards by the kernel itself (FSDP unshard fused into the consuming GEMM).  shards and pads: one
-// entry per rank; the weight range must lie inside the shards.  The producer waits for `target` on the chunk
-// counters, so with more than one rank it may not be 0.
-void py_gemm_bgather(const Tensor& a, Tensor& full, Tensor& out, bool b_kmajor, int64_t b_rows, int64_t b_cols,
-                     const std::vector<uint64_t>& shards, int64_t per_numel, int64_t w_off, int64_t w_numel,
-                     Tensor& counters, int64_t target, int64_t chunk_shift, const std::vector<uint64_t>& pads,
-                     int64_t rank, int64_t bar_epoch, const c10::optional<Tensor>& bias) {
-  const int64_t nr = (int64_t)shards.size();
-  check_dist("gemm_bgather", {{&shards, "shards", nr}, {&pads, "pads", nr}}, nr, rank, &out,
-             {{&a, "a", at::kBFloat16, false}, {&out, "out", at::kBFloat16, false},
-              {&full, "full", at::kBFloat16, true}, {&counters, "counters", at::kInt, true}});
-  const void* bp = check_bias(bias, out, b_kmajor, "gemm_bgather");
-  TORCH_CHECK(per_numel >= 1 && w_off >= 0 && w_numel >= 0 && w_off + w_numel <= nr * per_numel,
-              "gemm_bgather: the weight range [", w_off, ", ", w_off + w_numel, ") must lie inside the ", nr,
-              " shards of ", per_numel, " elements");
-  TORCH_CHECK(w_off + w_numel <= full.numel() && b_rows >= 0 && b_cols >= 0 && b_rows * b_cols <= w_numel,
-              "gemm_bgather: weight outside the flat buffer");
-  TORCH_CHECK(chunk_shift >= 14 && chunk_shift <= 30, "gemm_bgather: chunk_shift must be in [14, 30], got ",
-              chunk_shift);
-  TORCH_CHECK(((int64_t)full.numel() * 2) >> chunk_shift <= counters.numel(), "gemm_bgather: counter array too small");
-  TORCH_CHECK(nr == 1 || (uint32_t)target != 0, "gemm_bgather: target must be nonzero with more than one rank");
-  const c10::cuda::CUDAGuard guard(out.device());
-  const int M = (int)out.size(0), N = (int)out.size(1);
-  const int K = (int)a.size(1);
-  TORCH_CHECK(a.size(0) == M && (b_kmajor ? (b_rows == N && b_cols == K) : (b_rows == K && b_cols == N)),
-              "gemm_bgather: shape mismatch");
-  const void* sh[kMaxRanks] = {nullptr};
-  uint32_t* pd[kMaxRanks] = {nullptr};
-  for (int64_t i = 0; i < nr; ++i) {
-    sh[i] = (const void*)shards[i];
-    pd[i] = (uint32_t*)pads[i];
-  }
-  dtg::gemm_bf16_bgather(a.data_ptr(), full.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b_cols, out.stride(0),
-                         b_kmajor, sh, per_numel * 2, w_off * 2, w_numel * 2, (uint32_t*)counters.data_ptr<int>(),
-                         (uint32_t)target, (int)chunk_shift, pd, (int)nr, (int)rank, (uint32_t)bar_epoch, stream(), bp);
 }
 
 // out = (residual +) the sum of parts [nparts, *out.shape], nparts in 1..8; every tensor bf16, contiguous and 16-byte
@@ -277,10 +239,6 @@ void bind_tp(pybind11::module_& m) {
   m.def("gemm_ag", &py_gemm_ag, py::arg("a_bufs"), py::arg("b"), py::arg("out"), py::arg("b_kmajor"), py::arg("rank"),
         py::arg("rows_per_peer"), py::arg("flags"), py::arg("ag_epoch"), py::arg("pads"), py::arg("bar_epoch"),
         py::arg("n_comm"), py::arg("bias") = py::none());
-  m.def("gemm_bgather", &py_gemm_bgather, py::arg("a"), py::arg("full"), py::arg("out"), py::arg("b_kmajor"),
-        py::arg("b_rows"), py::arg("b_cols"), py::arg("shards"), py::arg("per_numel"), py::arg("w_off"),
-        py::arg("w_numel"), py::arg("counters"), py::arg("target"), py::arg("chunk_shift"), py::arg("pads"),
-        py::arg("rank"), py::arg("bar_epoch"), py::arg("bias") = py::none());
   m.def("tp_reduce_parts", &py_reduce_parts);
   m.def("tp_reduce_mc", &py_reduce_mc);
   m.def("vp_ce_stats", &py_vp_ce_stats);

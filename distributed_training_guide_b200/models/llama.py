@@ -238,10 +238,6 @@ class Starcoder2MLP(nn.Module):
         self.c_proj = Linear(i, h, dtype, device, bias=True)
 
 
-#: the MoE router's parameter name inside a decoder layer (FSDP keeps it out of the GEMM-fused gather)
-MOE_ROUTER = "mlp.gate.weight"
-
-
 class OlmoeExperts(nn.Module):
     """Every expert's SwiGLU weights in two 3-D parameters (transformers 5's layout): ``gate_up_proj`` [E, 2I, H]
     (each expert's gate rows, then its up rows) and ``down_proj`` [E, H, I]."""
@@ -280,10 +276,10 @@ def decoder_layout(config: ModelConfig):
     """``(flat_order, fused)`` of a decoder layer of ``config``.
 
     ``flat_order`` is the layer's parameter order in its flat buffer (parallel/flat.py, parallel/fsdp.py), which also
-    fixes FSDP's shard and chunk boundaries and the sharded checkpoint layout; a parameter missing from it would get
-    no gradient buffer and no optimizer update.  The matrices come first (FSDP's chunked layout), with q|k|v and
-    gate|up adjacent so that their fused weights are views of the buffer.  The norms' gains (and LayerNorm biases)
-    follow, then the QK-norm gains, so every replicated gain sits in one run after the matrices (TP sums their
+    fixes FSDP's shard boundaries and the sharded checkpoint layout; a parameter missing from it would get
+    no gradient buffer and no optimizer update.  The matrices come first, with q|k|v and gate|up adjacent so that
+    their fused weights are views of the buffer.  The norms' gains (and LayerNorm biases) follow, then the QK-norm
+    gains, so every replicated gain sits in one run after the matrices (TP sums their
     gradients over the group in one launch).  Then the q|k|v biases: adjacent, and each a multiple of 8 elements, so
     they form one [(nh + 2 nkv) d] bias (``fused_view_1d``) next to the fused q|k|v weight.  The o_proj and MLP
     biases come last.
@@ -294,7 +290,7 @@ def decoder_layout(config: ModelConfig):
     if config.gelu_mlp:
         mlp, mlp_bias = ("mlp.c_fc.weight", "mlp.c_proj.weight"), ("mlp.c_fc.bias", "mlp.c_proj.bias")
     elif config.moe:
-        mlp, mlp_bias = (MOE_ROUTER, "mlp.experts.gate_up_proj", "mlp.experts.down_proj"), ()
+        mlp, mlp_bias = ("mlp.gate.weight", "mlp.experts.gate_up_proj", "mlp.experts.down_proj"), ()
     else:
         mlp, mlp_bias = ("mlp.gate_proj.weight", "mlp.up_proj.weight", "mlp.down_proj.weight"), ()
     norms = (("post_attention_layernorm", "post_feedforward_layernorm") if config.post_norm else

@@ -143,11 +143,7 @@ class _Linear(torch.autograd.Function):
         ctx.bias = bias
         ctx.bias_param = (bias_param if bias_param is not None else bias) if bias is not None else None
         ctx.x_shape = x.shape
-        gs = getattr(ctx.w_param, "_dtg_gather", None)   # FSDP: the weight may still have to be gathered
-        if gs is not None and x2.is_cuda and gs.pending():
-            y = gs.gemm(x2 if x2.is_contiguous() else x2.contiguous(), True, bias)   # unshard fused into this GEMM
-        else:
-            y = gemm(x2, w, trans_b=True, bias=bias)
+        y = gemm(x2, w, trans_b=True, bias=bias)
         return y.view(*x.shape[:-1], w.shape[0])
 
     @staticmethod
@@ -163,15 +159,11 @@ class _Linear(torch.autograd.Function):
 
 
 def _linear_grads(dy2, x2, w, w_param, x_shape, need_dx, need_dw):
-    """(dx, dw) of ``y = x @ w.T`` from the 2-D output gradient ``dy2``: the dgrad GEMM (re-gathering an FSDP weight
-    inside it while its gather is pending) and the wgrad GEMM routed through ``_emit_weight_grad``."""
+    """(dx, dw) of ``y = x @ w.T`` from the 2-D output gradient ``dy2``: the dgrad GEMM and the wgrad GEMM routed
+    through ``_emit_weight_grad``."""
     dx = None
     if need_dx:
-        gs = getattr(w_param, "_dtg_gather", None)
-        if gs is not None and dy2.is_cuda and gs.pending():
-            dx = gs.gemm(dy2, False).view(x_shape)   # FSDP: re-gather the weight inside the dgrad GEMM
-        else:
-            dx = gemm(dy2, w).view(x_shape)  # [T,N] @ [N,K]
+        dx = gemm(dy2, w).view(x_shape)  # [T,N] @ [N,K]
     dw = None
     if need_dw or getattr(w_param, "_dtg_grad", None) is not None:
         side = _WGRAD_SIDE["enabled"] and dy2.is_cuda and getattr(w_param, "_dtg_grad", None) is not None
@@ -324,24 +316,15 @@ def _emit_shared_bias_grad(dy2, bd, b4):
 
 class _ParallelOut(torch.autograd.Function):
     """The dense GEMM writes ``bf16(attn @ Wd^T + bf16(bd + b4))`` (bias epilogue, overwrite mode); the
-    down-projection GEMM adds ``act @ W4^T`` into the same buffer (accumulate mode).  While an FSDP weight's gather is
-    pending, its ``_GatherSpec.gemm`` runs instead and the down-projection's product is added."""
+    down-projection GEMM adds ``act @ W4^T`` into the same buffer (accumulate mode)."""
 
     @staticmethod
     def forward(ctx, attn, act, wd, w4, bd, b4):
         a2 = attn.reshape(-1, attn.shape[-1])
         m2 = act.reshape(-1, act.shape[-1])
         bias = _bias_sum(bd, b4)
-        gs = getattr(wd, "_dtg_gather", None)
-        if gs is not None and gs.pending():
-            out = gs.gemm(a2 if a2.is_contiguous() else a2.contiguous(), True, bias)
-        else:
-            out = gemm(a2, wd, trans_b=True, bias=bias)
-        gs = getattr(w4, "_dtg_gather", None)
-        if gs is not None and gs.pending():
-            out.add_(gs.gemm(m2 if m2.is_contiguous() else m2.contiguous(), True))
-        else:
-            gemm(m2, w4, out=out, trans_b=True, accumulate=True)
+        out = gemm(a2, wd, trans_b=True, bias=bias)
+        gemm(m2, w4, out=out, trans_b=True, accumulate=True)
         ctx.save_for_backward(a2, m2, wd, w4)
         ctx.params = (bd, b4)
         ctx.shapes = (attn.shape, act.shape)

@@ -36,7 +36,7 @@ import torch
 import torch.distributed as dist
 from torch.autograd import Variable
 
-from ..models.llama import MOE_ROUTER, LlamaDecoderLayer, LlamaForCausalLM, init_parameter_
+from ..models.llama import LlamaDecoderLayer, LlamaForCausalLM, init_parameter_
 from ..ops import reference as ref
 from ..ops import join_wgrad_stream
 from ..utils.timers import nvtx_range
@@ -69,21 +69,6 @@ def _zero_counters(self):
 FlatGroup.zero_grad_counters = _zero_counters
 
 
-class _GatherSpec:
-    """Handle on a weight matrix of an FSDP group for ``ops._Linear``: where it sits in the group's flat buffer."""
-
-    def __init__(self, eng, g, off, numel, rows, cols):
-        self.eng, self.g, self.off, self.numel, self.rows, self.cols = eng, g, off, numel, rows, cols
-
-    def pending(self) -> bool:
-        return self.eng.gather_pending(self)
-
-    def gemm(self, a, b_kmajor: bool, bias=None):
-        """a @ W^T (+ bias) (``b_kmajor``: forward) or a @ W (dgrad) with W gathered from the ranks' shards by the GEMM
-        itself.  The bias is a 1-D parameter of the group's prefetched tail, already local."""
-        return self.eng._gather_gemm(self, a, b_kmajor, bias)
-
-
 class FSDPEngine:
     N_FULL_SLOTS = 3
     N_GRAD_SLOTS = 2
@@ -109,41 +94,12 @@ class FSDPEngine:
         self.direct_write = self.use_kernels and self.is_llama
         self.tied = bool(getattr(model.config, "tie_word_embeddings", False))
         assert self.is_llama or init_fn is None, "tensor-parallel slices are implemented for the Llama family"
-        esize = torch.empty((), dtype=dtype).element_size()
-        # Unshard fused into the consuming GEMMs (csrc/gemm_wgmma.cu, B_MODE 3): the big matrices of a group are
-        # gathered by the GEMM kernel that reads them; only the small tail (norm gains) keeps a prefetched copy.
-        # Needs every matrix to start and end on a chunk boundary of the flat layout and every shard to be a whole
-        # number of chunks.  Selected with DTG_FSDP_GATHER=gemm; the DEFAULT is the copy-engine unshard of whole groups
-        # ("ce"): one 16 KB x 2 bounce ring per CTA does not keep enough NVLink bytes in flight to feed a GEMM that consumes
-        # 7/8 remote weights, while the copy engines prefetch a whole layer ahead for free.
-        self.fused_gather = (self.use_kernels and self.is_llama and world_size > 1 and esize == 2 and init_fn is None
-                             and os.environ.get("DTG_FSDP_GATHER", "ce") == "gemm")
-
-        def pick_chunk(named):
-            """largest power-of-two chunk (16 KB .. 512 KB) that tiles every matrix of the group; 0 = not eligible"""
-            mats = [p.numel() * esize for _, p in named if p.dim() == 2]
-            seen_small = False
-            for _, p in named:              # matrices first, small tensors last (so matrix offsets stay aligned)
-                if p.dim() == 2 and seen_small:
-                    return 0
-                seen_small = seen_small or p.dim() != 2
-            c = 512 << 10
-            while mats and c >= (16 << 10):
-                if all(m % c == 0 for m in mats):
-                    return c
-                c >>= 1
-            return 0
-
-        def pad_of(named):
-            c = pick_chunk(named) if self.fused_gather else 0
-            base = ALIGN * world_size * 16
-            return max(base, world_size * c // esize) if c else base
+        pad = ALIGN * world_size * 16
 
         def layout(named):
             off = 0
             for _, p in named:
                 off = _round_up(off + p.numel(), ALIGN)
-            pad = pad_of(named)
             return _round_up(max(off, pad), pad)
 
         layer_named = []
@@ -155,7 +111,7 @@ class FSDPEngine:
             embed_named = [("model.embed_tokens.weight", core.embed_tokens.weight)]
             head_named = [(f"model.norm.{n}", p) for n, p in core.norm.named_parameters()]   # gain (+ bias)
             if not self.tied:  # a tied lm_head IS the embedding parameter (it lives in the embed group)
-                head_named.insert(0, ("lm_head.weight", model.lm_head.weight))  # matrix first: chunk-aligned
+                head_named.insert(0, ("lm_head.weight", model.lm_head.weight))
             default_init = lambda p, n: init_parameter_(p, n, seed)  # noqa: E731
         else:
             from ..models.gpt2 import init_parameter_ as gpt2_init
@@ -166,7 +122,7 @@ class FSDPEngine:
             head_named = [(f"transformer.ln_f.{n}", p) for n, p in core.ln_f.named_parameters()]
             assert self.tied and model.lm_head.weight is core.wte.weight, "GPT-2 layout expects a tied lm_head"
             default_init = lambda p, n: gpt2_init(p, n, seed, L)  # noqa: E731
-        max_layer = max(layout(n) for n in layer_named) if layer_named else ALIGN * world_size * 16
+        max_layer = max(layout(n) for n in layer_named) if layer_named else pad
 
         def local(n):
             return torch.zeros(n, dtype=dtype, device=self.device)
@@ -194,10 +150,9 @@ class FSDPEngine:
             def alloc(n, dt):
                 return bufs.pop(0)[:n]
 
-            g = FlatGroup(name, named, self.device, dtype, pad_multiple=pad_of(named), alloc=alloc, with_grad=True,
+            g = FlatGroup(name, named, self.device, dtype, pad_multiple=pad, alloc=alloc, with_grad=True,
                           direct_write=self.direct_write)
             assert g.padded_numel == n_pad
-            g.chunk_bytes = pick_chunk(named) if (self.fused_gather and name != "embed") else 0
             # deterministic init of the whole group inside the slot, then keep only my shard
             for n, p in named:
                 if init_fn is not None:
@@ -224,8 +179,6 @@ class FSDPEngine:
         self.head = make_group("head", head_named, local(layout(head_named)), symmetric(layout(head_named)))
         self.layer_groups = self.groups[1:1 + L]
         self.shard_of = {s.name: s for s in self.shards}
-        if self.fused_gather:
-            self._install_gather_specs(model)
         model._flat_groups = self.groups
         model.engine = self
 
@@ -254,79 +207,6 @@ class FSDPEngine:
         if world_size > 1 and dist.is_initialized():
             dist.barrier(group=pg)
 
-    # -- unshard fused into the consuming GEMMs ------------------------------------------------------------
-    def _install_gather_specs(self, model):
-        """Give every matrix that a linear op reads (fused q|k|v and gate|up, o_proj, down_proj, lm_head) a
-        ``_dtg_gather`` handle: ``ops._Linear`` then runs the GEMM that also gathers the weight from the ranks'
-        shards (first use after the group became live) or the plain GEMM (already gathered).
-
-        Reference: FSDP2's per-layer all-gather in front of the layer's first matmul and again in backward
-        (``fully_shard(layer, reshard_after_forward=True)``, ``04-fully-sharded-data-parallel/train_llm.py:83-90``) and
-        the root ``model.unshard()`` prefetch (``04:187-188``): there three NCCL-side kernels per gather (copy-in,
-        all_gather_into_tensor, copy-out), here none — the bytes move inside the consuming wgmma GEMM."""
-        self.gather_pads = self.symm.new_pad_set()   # these kernels run on the compute stream: own pad + epochs
-        self._counters, self._ngather = {}, {}
-        esize = 2
-
-        def counters_for(full):
-            key = full.data_ptr()
-            if key not in self._counters:
-                self._counters[key] = torch.zeros(max(64, full.numel() * esize // (16 << 10) + 1), dtype=torch.int32,
-                                                  device=self.device)
-            return self._counters[key]
-
-        def spec(g, holder, off, numel, rows, cols):
-            holder._dtg_gather = _GatherSpec(self, g, off, numel, rows, cols)
-
-        fused_of = {l._flat_group.name: l.fused for l in self.layers}   # each layer's own fused weights
-        for g in self.groups:
-            g._gathered, g._full_now = set(), False
-            if not g.chunk_bytes:
-                g.tail = None
-                continue
-            counters_for(g.param)
-            by_name = dict(zip(g.names, zip(g.params, g.offsets, g.shapes)))
-            covered = set()
-            for fname, fw in g.fused.items():
-                if fw.data.dim() != 2:   # the fused q|k|v bias (Qwen2): 1-D, it lives in the prefetched tail
-                    continue
-                members = [n for n in g.names if any(n.endswith(m) for m in fused_of[g.name][fname])]
-                off = by_name[members[0]][1]
-                rows = sum(by_name[n][2][0] for n in members)
-                cols = by_name[members[0]][2][1]
-                spec(g, fw, off, rows * cols, rows, cols)
-                covered.update(members)
-            end_of_matrices = 0
-            for n, (p, off, shape) in by_name.items():
-                # the MoE router is read by ops.moe's own GEMMs, which gather nothing: like the 3-D experts after it,
-                # it stays in the copy-engine tail (the layout puts it right after the attention matrices)
-                if len(shape) != 2 or n.endswith(MOE_ROUTER):
-                    continue
-                end_of_matrices = max(end_of_matrices, off + shape[0] * shape[1])
-                if n not in covered:
-                    spec(g, p, off, shape[0] * shape[1], shape[0], shape[1])
-            # what is left after the matrices (norm gains): a prefetched copy-engine gather of that flat range
-            g.tail = (end_of_matrices, g.numel) if g.numel > end_of_matrices else None
-
-    def _gather_gemm(self, sp, a, b_kmajor, bias=None):
-        g = sp.g
-        C = self.symm.C
-        full = g.param
-        sh = self.shard_of[g.name]
-        M = a.shape[0]
-        out = torch.empty(M, sp.rows if b_kmajor else sp.cols, dtype=a.dtype, device=a.device)
-        key = (full.data_ptr(), sp.off)
-        n = self._ngather.get(key, 0) + 1
-        self._ngather[key] = n
-        shift = g.chunk_bytes.bit_length() - 1
-        ppc = g.chunk_bytes // (16 << 10)
-        with nvtx_range(f"gather_gemm:{g.name}"):
-            C.gemm_bgather(a, full, out, b_kmajor, sp.rows, sp.cols, self._symm_of[sh.param.data_ptr()].ptrs,
-                           sh.padded_numel, sp.off, sp.numel, self._counters[full.data_ptr()], n * ppc, shift,
-                           self.gather_pads.ptrs, self.rank, 0, bias)   # epoch 0: no entry barrier (see the kernel)
-        g._gathered.add(sp.off)
-        return out
-
     # -- optimizer ---------------------------------------------------------------------------------
     def build_optimizer(self, lr):
         state_device = torch.device("cpu") if self.cpu_offload else None
@@ -351,15 +231,11 @@ class FSDPEngine:
             return g.name in self._unsharded
         return self.slot_owner[self.slot_of[g.name]] == g.name
 
-    def unshard(self, g: FlatGroup, force_full: bool = False):
-        """Make ``g``'s parameters available in its full buffer.  Copy-engine path: the whole group is gathered now
-        (asynchronously on the comm stream).  Fused path (``g.chunk_bytes``): only the small tail is copied now; every
-        matrix is gathered by the first GEMM that reads it (``_gather_gemm``)."""
+    def unshard(self, g: FlatGroup):
+        """Make ``g``'s parameters available in its full buffer: the whole group is gathered now (asynchronously on
+        the comm stream)."""
         if self._is_live(g):
-            if force_full and self.use_kernels and getattr(g, "chunk_bytes", 0) and not g._full_now:
-                self._set_dead(g)
-            else:
-                return
+            return
         sh = self.shard_of[g.name]
         if g.name in ("embed", "head"):
             self._unsharded.add(g.name)
@@ -373,9 +249,6 @@ class FSDPEngine:
             else:
                 g.param.copy_(sh.param)
             return
-        lazy = bool(getattr(g, "chunk_bytes", 0)) and not force_full
-        g._gathered = set()
-        g._full_now = not lazy
         with torch.cuda.stream(self.comm_stream):
             if g.name not in ("embed", "head"):
                 ev = self.slot_free[self.slot_of[g.name]]
@@ -383,43 +256,15 @@ class FSDPEngine:
                     self.comm_stream.wait_event(ev)  # the slot's previous layer has finished computing
             t0 = self._trace_begin()
             with nvtx_range(f"unshard:{g.name}"):
-                if lazy:
-                    # what the GEMMs do not fetch themselves: my own slice (a local copy) and the small tail
-                    per = sh.padded_numel
-                    # (raw copies, not tensor ops: an in-place torch op on the slot would bump the autograd version
-                    # of every weight view another layer saved for its backward)
-                    self.symm.gather_range_(self._symm_of[sh.param.data_ptr()], g.param, self.rank * per,
-                                            (self.rank + 1) * per, per, barrier=False)
-                    # the device barrier in front of the tail copies is also what orders every later read of the
-                    # peers' shards (by the gather warps of this group's GEMMs, which wait for `ag_done`) behind
-                    # the peers' previous optimizer work on their communication streams
-                    if g.tail is not None:
-                        self.symm.gather_range_(self._symm_of[sh.param.data_ptr()], g.param, g.tail[0], g.tail[1],
-                                                sh.padded_numel)
-                    else:
-                        self.symm.barrier_()
-                else:
-                    if getattr(g, "chunk_bytes", 0):
-                        g._gathered = {"all"}
-                    self.symm.allgather_(self._symm_of[sh.param.data_ptr()], g.param, 0, sh.padded_numel,
-                                         copy_engine=self.ag_copy_engine)
+                self.symm.allgather_(self._symm_of[sh.param.data_ptr()], g.param, 0, sh.padded_numel,
+                                     copy_engine=self.ag_copy_engine)
             self._trace_end("unshard", t0)
             ev = torch.cuda.Event()
             ev.record(self.comm_stream)
             self.ag_done[g.name] = ev
 
-    def _set_dead(self, g):
-        if g.name in ("embed", "head"):
-            self._unsharded.discard(g.name)
-        else:
-            self.slot_owner[self.slot_of[g.name]] = None
-
-    def gather_pending(self, sp) -> bool:
-        g = sp.g
-        return bool(g.chunk_bytes) and self._is_live(g) and "all" not in g._gathered and sp.off not in g._gathered
-
-    def wait_unsharded(self, g: FlatGroup, force_full: bool = False):
-        self.unshard(g, force_full)
+    def wait_unsharded(self, g: FlatGroup):
+        self.unshard(g)
         if self.use_kernels:
             t0 = self._trace_begin()
             torch.cuda.current_stream().wait_event(self.ag_done[g.name])
@@ -724,7 +569,7 @@ class FSDPEngine:
                 self.slot_owner[self.slot_of[g.name]] = None
             else:
                 self._unsharded.discard(g.name)
-            self.wait_unsharded(g, force_full=True)
+            self.wait_unsharded(g)
             if self.use_kernels:
                 torch.cuda.synchronize(self.device)
             for n, p in zip(g.names, g.params):

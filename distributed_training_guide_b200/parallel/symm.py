@@ -282,23 +282,6 @@ class SymmGroup:
 
         return alloc
 
-    def new_pad_set(self):
-        """A second signal pad + epoch counter for kernels that run on ANOTHER stream than this group's usual one:
-        epochs are handed out in host order, so two streams sharing one pad could write a lower epoch over a
-        higher one.  Returns an object with ``ptrs`` and ``next_epoch()``."""
-        buf = self.alloc_bytes(int(self.C.SYMM_PAD_BYTES))
-
-        class _Pads:
-            ptrs = buf.ptrs
-            _buf = buf
-            _e = 0
-
-            def next_epoch(self):
-                self._e += 1
-                return self._e
-
-        return _Pads()
-
     def reserved_bytes(self) -> int:
         return sum(c.size for c in self._chunks)
 
@@ -336,14 +319,6 @@ class SymmGroup:
         peer copies (zero SM time: the right choice for a prefetch that runs under GEMMs)."""
         self.C.comm_allgather(shards.ptrs, full, self.pad_ptrs, shard_off, per, self.rank, self._epochs(1), self.err,
                               barrier, 0 if copy_engine else (blocks or self.comm_blocks))
-
-    def gather_range_(self, shards: SymmBuffer, full: torch.Tensor, begin: int, end: int, per: int,
-                      barrier: bool = True):
-        """``full[begin:end]`` = the same element range of the group's flat layout, copied from whichever ranks' shards
-        hold it (rank p owns flat elements [p*per, (p+1)*per)): a 1-warp device barrier + peer copies on the copy
-        engines.  The small "tail" gather of the fused FSDP path."""
-        self.C.comm_gather_range(shards.ptrs, full, self.pad_ptrs, begin, end, per, self.rank, self._epochs(1), self.err,
-                                 barrier)
 
     def reduce_scatter_(self, grads: SymmBuffer, out: torch.Tensor, elem_off: int, n: int, scale: float,
                         blocks: Optional[int] = None):

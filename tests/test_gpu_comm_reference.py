@@ -503,7 +503,7 @@ def test_rs_adamw_check_rejects_a_dropped_rank():
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# allgather and gather_range
+# allgather
 # ------------------------------------------------------------------------------------------------------------------
 # (blocks, shard_off, barrier): on SMs (blocks >= 1, grid-stride at 1 and 3) and on the copy engines (0)
 AG_CASES = [(1, 0, True), (3, 88, True), (96, 0, False), (256, 88, False), (0, 0, True), (0, 88, False)]
@@ -531,47 +531,6 @@ def test_allgather_copies_the_shards_in_rank_order(nr):
             assert _same(full.view[:nr * per], data.reshape(-1)), f"{t}: not the shards in rank order"
             assert bool(torch.isnan(full.view[nr * per:].float()).all()) and full.intact(), f"{t}: wrote past NR·per"
             shards.check(t)
-
-
-@pytest.mark.parametrize("nr", [1, 2, 4, 8])
-def test_gather_range_copies_exactly_the_range(nr):
-    C = _C()
-    per = 1000
-    total = nr * per
-    data = _randn((nr, per), nr).to(BF16)
-    shards = _Replicas(nr, per, 0, seed=nr)
-    shards.load(data)
-    flat = data.reshape(-1)
-    ranges = [(5, 5), (per // 4, per // 4 + 37), (total - per, total), (0, total), (total - 40, total),
-              (total - per // 2 - 8, total - 16),        # a tail range after the matrices, short of the padded end
-              (8 * (total // 16), 8 * (total // 16) + 3)]
-    if nr > 1:
-        ranges += [(per - 3, per + 5), (per, 2 * per)]   # crossing two shards; exactly shard 1
-    for b, e in ranges:
-        for barrier in (True, False):
-            rig = _Rig(nr, seed=b + e)
-            rig.arm(21, 1)
-            for r in sorted({0, nr - 1}):
-                full = _Guarded(total, seed=r + b)
-                before = _bits(full.view).clone()
-                t = f"gather_range nr{nr} [{b}, {e}) {'barrier' if barrier else 'no barrier'} rank {r}"
-                rig.run(t, r, 20, 1, 1 if barrier else 0,
-                        lambda: C.comm_gather_range(shards.ptrs(), full.view, rig.pad_ptrs(), b, e, per, r, 20,
-                                                    rig.err.view, barrier),
-                        launches=1 if barrier else 0)
-                assert _same(full.view[b:e], flat[b:e]), f"{t}: range differs from the flat layout"
-                keep = torch.ones(total, dtype=torch.bool, device="cuda")
-                keep[b:e] = False
-                assert torch.equal(_bits(full.view)[keep], before[keep]) and full.intact(), f"{t}: wrote outside"
-                shards.check(t)
-    # own shard without a barrier, as the fused FSDP unshard copies it
-    for r in range(nr):
-        rig = _Rig(nr, seed=r)
-        full = _Guarded(total, seed=r)
-        rig.run(f"own shard rank {r}", r, 1, 1, 0,
-                lambda: C.comm_gather_range(shards.ptrs(), full.view, rig.pad_ptrs(), r * per, (r + 1) * per, per, r,
-                                            1, rig.err.view, False), launches=0)
-        assert _same(full.view[r * per:(r + 1) * per], data[r])
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -798,7 +757,7 @@ def test_rs_adamw_refusals(push):
     assert all(g.intact() for g in (mg, vg, pg, pl))
 
 
-def test_allgather_and_gather_range_refusals():
+def test_allgather_refusals():
     C = _C()
     nr, per = 2, 64
     shards, pads, err, _keep = _base(nr, per, 8)     # each rank's shard: `per` elements at element 8
@@ -815,21 +774,6 @@ def test_allgather_and_gather_range_refusals():
         _refused(ag(full=full.view[1:nr * per + 1]), "full must start at a 16-byte aligned")
         _refused(ag(full=full.view[:nr * per].float()), "full must be BFloat16")
         _refused(ag(full=full.view[:nr * per - 8]), "full buffer too small")
-    base = dict(shards=shards.ptrs(), full=full.view[:4 * per], pads=pads, begin=0, end=nr * per, per=per, rank=0,
-                err=err)
-
-    def gr(**kw):
-        a = {**base, **kw}
-        return lambda: C.comm_gather_range(a["shards"], a["full"], a["pads"], a["begin"], a["end"], a["per"],
-                                           a["rank"], 1, a["err"], True)
-    _bad_common(gr, "shards", shards.ptrs(), pads, err, None, "per")
-    _refused(gr(end=nr * per + 8), "lies past the 2 shards")      # inside `full`, past the last shard
-    _refused(gr(begin=-8), "begin must not be negative")
-    _refused(gr(begin=0, end=-8), "bad range")
-    _refused(gr(begin=16, end=8), "bad range")
-    _refused(gr(end=4 * per + 8), "bad range")
-    _refused(gr(full=full.view[:4 * per].to(CPU)), "full must be on")
-    _refused(gr(full=full.view[1:4 * per + 1]), "full must start at a 16-byte aligned")
     shards.check("refusals")
     assert full.intact() and bool((full.view == 0).all())
 

@@ -1,4 +1,4 @@
-"""The tensor-parallel and FSDP modes of the wgmma GEMM and the partial-sum reduce, on one GPU, against the plain GEMM
+"""The tensor-parallel modes of the wgmma GEMM and the partial-sum reduce, on one GPU, against the plain GEMM
 bit for bit and against fp64.
 
 Ranks are emulated as in ``test_gpu_vocab_reference.py``: every rank's buffer is a separate tensor on the same device,
@@ -7,12 +7,12 @@ pads are plain int32 tensors of ``SYMM_MAX_CHANNELS x 8``.  One GPU cannot test 
 ``multigpu`` tests stay the check over real NVLink.
 
 Contracts (the launcher comment in ``gemm_wgmma.cu``):
-- ``gemm_ag`` (all-gather by communication CTAs, then the GEMM), ``gemm_dist`` modes 1 and 2 and ``gemm_bgather``'s
-  forward keep the plain GEMM's K order, so they are bit-identical to ``gemm(..., variant=2)`` on the assembled
-  operands, with the same bias or accumulate.
-- ``gemm_dist`` modes 3 and 4 and ``gemm_bgather``'s dgrad start every tile at this rank's K slice.  They must be within
-  the fp64 element bound of ``test_gpu_gemm_reference.py`` (``2^-8 |exact| + ELEM_C K 2^-24 (|A| @ |B|)``), and
-  bit-identical where the rotation is 0.
+- ``gemm_ag`` (all-gather by communication CTAs, then the GEMM) and ``gemm_dist`` modes 1 and 2 keep the plain GEMM's
+  K order, so they are bit-identical to ``gemm(..., variant=2)`` on the assembled operands, with the same bias or
+  accumulate.
+- ``gemm_dist`` modes 3 and 4 start every tile at this rank's K slice.  They must be within the fp64 element bound of
+  ``test_gpu_gemm_reference.py`` (``2^-8 |exact| + ELEM_C K 2^-24 (|A| @ |B|)``), and bit-identical where the rotation
+  is 0.
 - ``tp_reduce_parts`` is bit-identical to an fp32 sum of the parts in part order, then the residual, then one bf16
   rounding.  Against fp64 the reduced rows must be within (1 + 2^-8) x (2^-8 |exact| + the partials' GEMM element
   bounds + t 2^-24 sum |terms|): the final rounding, each pushed partial's rounding and accumulation, and the fp32 sum
@@ -20,12 +20,12 @@ Contracts (the launcher comment in ``gemm_wgmma.cu``):
   GEMMs actually pushed: that half sees a 2-ulp error in one element.
 
 Every operand sits where a wrong read or write shows: a peer's rows or bytes outside its owner's slice are NaN at the
-call, staging slots, outputs and full buffers are views inside allocations whose outside bits must not change, and an
-overwritten output starts out NaN.
+call, staging slots and outputs are views inside allocations whose outside bits must not change, and an overwritten
+output starts out NaN.
 
-The kernels spin on flags, counters and pads, and trap after 8 s.  No test here can reach that: before each launch
-the test asserts that every emulated peer's arrival is already in ``pads[rank]`` and every counter the kernel waits on
-is exactly one generation below its target, and ``gemm_bgather`` runs with ``bar_epoch`` 0.
+The kernels spin on flags and pads, and trap after 8 s.  No test here can reach that: before each launch the test
+asserts that every emulated peer's arrival is already in ``pads[rank]``, and the only flags the kernel waits on are
+the ones its own communication CTAs set.
 """
 import pytest
 import torch
@@ -404,111 +404,9 @@ def test_gemm_dist_modes3_and_4_against_fp64(t, rpp):
     print(f"\nmodes 3/4 t{t} rpp{rpp}: element bound c used {worst:.3g} of {ELEM_C}")
 
 
-# ------------------------------------------------------------------------------------------------------------------
-# gemm_bgather: FSDP's unshard inside the consuming GEMM (B_MODE 3)
-# ------------------------------------------------------------------------------------------------------------------
-CHUNK16, CHUNK512 = 14, 19   # chunk_shift: 16 KB and 512 KB chunks (16 KB pieces: 1 and 32 per chunk)
-
-# name: (t, per (elements per shard), w_off, b_rows, b_cols, w_numel (None: b_rows * b_cols), chunk_shift, ranks).
-# The layout is t * per elements; rank r owns [r * per, (r + 1) * per).  Forward reads B [N, K] = [b_rows, b_cols],
-# dgrad reads B [K, N] = [b_rows, b_cols].
-BG_LAYOUTS = {
-    "whole": (4, 131072, 0, 1024, 512, None, CHUNK16, (0, 1, 3)),
-    "mid_shard_straddles_4": (4, 131072, 65536, 768, 512, None, CHUNK16, (0, 2, 3)),
-    "in_one_remote_shard": (8, 262144, 3 * 262144, 512, 512, None, CHUNK512, (0, 5)),
-    "in_own_shard": (2, 262144, 262144 + 8192, 256, 512, None, CHUNK16, (1,)),
-    "k1376_rows_across_chunks": (2, 196608, 16384, 256, 1376, None, CHUNK16, (0, 1)),
-    "n1376_dgrad_rows": (4, 196608, 0, 512, 1376, None, CHUNK16, (1, 2)),
-    "chunks_512k_padded_range": (4, 524288, 262144, 1024, 768, 1048576, CHUNK512, (0, 1, 3)),
-}
-
-
-def _bg_remote_chunks(t, per, w_off, w_numel, shift, r):
-    cb = 1 << shift
-    c0, c1 = (w_off * 2) // cb, ((w_off + w_numel) * 2) // cb
-    return [c for c in range(c0, c1) if (c * cb) // (per * 2) != r]
-
-
-def _bg_run(name, b_kmajor, with_bias):
-    C = _C()
-    t, per, w_off, b_rows, b_cols, w_numel, shift, ranks = BG_LAYOUTS[name]
-    w_numel = w_numel or b_rows * b_cols
-    assert (w_off * 2) % (1 << shift) == 0 and (w_numel * 2) % (1 << shift) == 0 and (per * 2) % (1 << shift) == 0
-    total = t * per
-    ppc = (1 << shift) // 16384
-    nch = (total * 2) >> shift
-    M = 520
-    K = b_cols if b_kmajor else b_rows
-    N = b_rows if b_kmajor else b_cols
-    worst = 0.0
-    for r in ranks:
-        seed = sum(map(ord, name)) + 97 * r
-        shards = [_Guarded(per, fill=None, seed=seed + p) for p in range(t)]
-        full = _Guarded(total, seed=seed + 20)
-        counters = _Guarded(nch + 8, dtype=torch.int32, fill=None, seed=seed + 21)
-        remote = _bg_remote_chunks(t, per, w_off, w_numel, shift, r)
-        counters.view.fill_(777)          # own and out-of-range chunks: never waited for, never counted
-        if remote:
-            counters.view[torch.tensor(remote, device="cuda")] = 0
-        pads = _pads(t)
-        A = _randn((M, K), seed + 30)
-        bias = _randn((N,), seed + 31) if with_bias else None
-        for gen in (1, 2):
-            flat = _randn((total,), seed + 40 + gen, std=K ** -0.5)   # the next generation's weights
-            for p in range(t):
-                shards[p].view.copy_(flat[p * per:(p + 1) * per])
-            full.view.fill_(NAN)
-            full.view[r * per:(r + 1) * per].copy_(shards[r].view)   # the engine copies the local slice first
-            full_before = _bits(full.view).clone()
-            cnt_before = counters.view.clone()
-            og, out = _out(M, N)
-            target = gen * ppc
-            if remote:   # every chunk the kernel waits on is exactly one generation below the target
-                assert bool((counters.view[torch.tensor(remote, device="cuda")] == target - ppc).all())
-            C.gemm_bgather(A, full.view, out, b_kmajor, b_rows, b_cols, [s.view.data_ptr() for s in shards], per,
-                           w_off, w_numel, counters.view, target, shift, [p.data_ptr() for p in pads], r, 0, bias)
-            torch.cuda.synchronize()
-            tag = f"{name} r{r} {'fwd' if b_kmajor else 'dgrad'}{' bias' if bias is not None else ''} gen{gen}"
-            rng = slice(w_off, w_off + w_numel)
-            assert _same(full.view[rng], flat[rng]), f"{tag}: the gathered range is not the flat layout"
-            keep = torch.ones(total, dtype=torch.bool, device="cuda")
-            keep[rng] = False
-            assert torch.equal(_bits(full.view)[keep], full_before[keep]), f"{tag}: wrote outside the weight range"
-            assert full.intact() and _out_intact(og), f"{tag}: wrote outside its views"
-            want_cnt = cnt_before.clone()
-            if remote:
-                want_cnt[torch.tensor(remote, device="cuda")] = target
-            assert torch.equal(counters.view, want_cnt) and counters.intact(), f"{tag}: chunk counters"
-            assert all(bool((p == 0).all()) for p in pads), f"{tag}: bar_epoch 0 must not touch the pads"
-            assert all(s.intact() for s in shards), f"{tag}: wrote outside a shard"
-            B = flat[w_off:w_off + b_rows * b_cols].view(b_rows, b_cols)
-            if b_kmajor:
-                assert _same(out, _plain(A, B, True, bias)), f"{tag}: differs from the plain GEMM"
-            else:
-                worst = max(worst, _check_fp64(tag, A, B, out))
-                my_row = (r * per - w_off) // b_cols
-                if not 0 <= my_row < b_rows:
-                    my_row = 0
-                if my_row // 64 == 0:
-                    assert _same(out, _plain(A, B, False)), f"{tag}: K rotation 0 but differs from the plain GEMM"
-    return worst
-
-
-@pytest.mark.parametrize("name", list(BG_LAYOUTS))
-def test_gemm_bgather_forward_matches_plain_gemm(name):
-    _bg_run(name, True, False)
-    _bg_run(name, True, True)
-
-
-@pytest.mark.parametrize("name", list(BG_LAYOUTS))
-def test_gemm_bgather_dgrad_against_fp64(name):
-    c = _bg_run(name, False, False)
-    print(f"\n{name}: dgrad element bound c used {c:.3g} of {ELEM_C}")
-
-
-def test_bgather_dgrad_bound_rejects_wrong_chunk_dropped_chunk_and_two_ulps():
-    """The element bound the dgrad is held to sees a K block of B taken from the wrong place, a K block that never
-    arrived (zero) and a 2-ulp error in one element."""
+def test_k_rotated_bound_rejects_wrong_block_dropped_block_and_two_ulps():
+    """The element bound modes 3 and 4 are held to sees a K block of B taken from the wrong place, a K block that
+    never arrived (zero) and a 2-ulp error in one element."""
     M, K, N = 520, 1376, 512
     A = _randn((M, K), 1)
     B = _randn((K, N), 2, std=K ** -0.5)
@@ -518,7 +416,7 @@ def test_bgather_dgrad_bound_rejects_wrong_chunk_dropped_chunk_and_two_ulps():
     wrong[640:704] = B[704:768]
     dropped = B.clone()
     dropped[640:704] = 0
-    for what, Bx in (("wrong chunk", wrong), ("dropped chunk", dropped)):
+    for what, Bx in (("wrong block", wrong), ("dropped block", dropped)):
         assert _evaluate(A, B, {"k": _plain(A, Bx, False)})["k"][1] > ELEM_C, f"{what} not rejected"
     i = int(good.float().abs().argmax())
     g2 = good.clone().view(-1)
@@ -529,9 +427,9 @@ def test_bgather_dgrad_bound_rejects_wrong_chunk_dropped_chunk_and_two_ulps():
 # ------------------------------------------------------------------------------------------------------------------
 # empty calls
 # ------------------------------------------------------------------------------------------------------------------
-def test_empty_calls_launch_nothing_and_k0_writes_zeros():
-    """M or N = 0 launches nothing; K = 0 writes zeros in overwrite mode and leaves C in accumulate mode, as the
-    plain GEMM does.  gemm_bgather refuses an empty call (its counters must advance one generation per call)."""
+def test_tp_empty_calls_launch_nothing_and_k0_writes_zeros():
+    """gemm_ag, gemm_dist and tp_reduce_parts: M or N = 0 launches nothing; K = 0 writes zeros in overwrite mode and
+    leaves C in accumulate mode, as the plain GEMM does."""
     C = _C()
     t, rpp, N = 2, 256, 264
     bufs = [_Guarded(t * rpp * 64, seed=p) for p in range(t)]
@@ -579,12 +477,6 @@ def test_empty_calls_launch_nothing_and_k0_writes_zeros():
             torch.cuda.synchronize()
             want = old if acc else torch.zeros_like(old)
             assert _same(out, want) and _out_intact(og), (mode, acc)
-    # gemm_bgather: refused
-    shard = torch.zeros(8192, device="cuda", dtype=BF16)
-    cnt = torch.zeros(8, device="cuda", dtype=torch.int32)
-    _refused(lambda: C.gemm_bgather(torch.empty(0, 64, device="cuda", dtype=BF16), shard, torch.empty(0, 128,
-                                    device="cuda", dtype=BF16), True, 128, 64, [shard.data_ptr()], 8192, 0, 8192, cnt,
-                                    1, CHUNK16, [pads[0].data_ptr()], 0, 0), "empty")
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -658,39 +550,6 @@ def test_gemm_dist_refusals():
     _refused(call(mode=3, a_ptrs=(ap,), b_ptrs=(wp,), c_ptrs=(cp[0],)), "b_ptrs must have 2 entries")
     _refused(call(mode=4, a_ptrs=(ap, ap, ap), c_ptrs=(cp[0],)), "a_ptrs must have 2 entries")
     _refused(call(mode=1, a_ptrs=(ap, ap), c_ptrs=(cp[0],), M=-256), "negative")
-
-
-def test_gemm_bgather_refusals():
-    C = _C()
-    t, per, shift = 2, 65536, CHUNK16
-    N, K, M = 256, 256, 128
-    shards = [_Guarded(per, fill=0.0, seed=p) for p in range(t)]
-    full = _Guarded(4 * per, fill=0.0)                  # room past the last shard
-    cnt = _Guarded((4 * per * 2 >> shift) + 8, dtype=torch.int32, fill=0)
-    pads = _pads(t)
-    base = dict(a=_randn((M, K), 1), full=full.view, out=_out(M, N)[1], b_kmajor=True, b_rows=N, b_cols=K,
-                shards=[s.view.data_ptr() for s in shards], per_numel=per, w_off=0, w_numel=N * K,
-                counters=cnt.view, target=1, chunk_shift=shift, pads=[p.data_ptr() for p in pads], rank=0,
-                bar_epoch=0)
-
-    def call(**kw):
-        return lambda: C.gemm_bgather(**{**base, **kw})
-    cpu = torch.device("cpu")
-    _refused(call(rank=2), "rank 2 outside")
-    _refused(call(rank=-1), "rank -1 outside")
-    _refused(call(w_off=2 * per - 8192, w_numel=N * K), "must lie inside the 2 shards")   # owner 2 had no shard
-    _refused(call(w_off=-8192), "must lie inside")
-    _refused(call(a=base["a"].to(cpu)), "a must be on")
-    _refused(call(full=full.view.to(cpu)), "full must be on")
-    _refused(call(counters=cnt.view.to(cpu)), "counters must be on")
-    _refused(call(counters=cnt.view[::2]), "counters must be contiguous")
-    _refused(call(counters=cnt.view.long()), "counters must be Int")
-    _refused(call(pads=base["pads"][:1]), "pads must have 2 entries")
-    _refused(call(shards=base["shards"] * 5, pads=base["pads"] * 5), "1..8 ranks")
-    _refused(call(shards=[base["shards"][0], base["shards"][1] + 2]), "16-byte aligned")
-    _refused(call(target=0), "target must be nonzero")
-    _refused(call(chunk_shift=63), "chunk_shift")
-    _refused(call(full=full.view[1:1 + 2 * per]), "full must start at a 16-byte")
 
 
 def test_reduce_parts_refusals():

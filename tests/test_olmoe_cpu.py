@@ -269,19 +269,6 @@ def test_distributed_olmoe_matches_single_process(parallelism, ckpt):
     assert want[-1] < want[0], want   # the steps train: the comparison is not of three untouched models
 
 
-def test_fsdp_keeps_the_router_in_the_copy_engine_tail():
-    """The router is read by ops.moe's GEMMs, which do not gather: it must lie in the tail the copy engines fetch, with
-    the experts, and never get a GEMM-fused gather spec."""
-    from distributed_training_guide_b200.parallel import fsdp
-
-    src = open(fsdp.__file__).read()
-    assert "n.endswith(MOE_ROUTER)" in src
-    order, _ = decoder_layout(get_config("allenai/OLMoE-1B-7B-0924"))
-    i = order.index(fsdp.MOE_ROUTER)
-    assert order[i - 1] == "self_attn.o_proj.weight" and order[i + 1:i + 3] == ("mlp.experts.gate_up_proj",
-                                                                              "mlp.experts.down_proj")
-
-
 def test_router_aux_loss_flag():
     from distributed_training_guide_b200.parallel.strategies import _apply_router_aux_loss
     from distributed_training_guide_b200.utils.cli import get_parser
